@@ -9,8 +9,9 @@ weights are `loftr.functional_state_dict(noise=1e-3)`: full-shape layers that im
 a dense Gaussian perturbation on every conv / linear weight so that no tensor-core operand is structurally zero (a
 chip multiplying zeros draws less power and clocks higher than one running a trained checkpoint).
 
-A "step" = `--micro` engine batches of `--batch` pairs (default 5 x 32 = 160 pairs) through matcher + solver on one
-GPU, so that the driver's 20 steps time >= 5 s of steady state. With N GPUs every rank runs its own pairs (weak
+A "step" = `--micro` engine batches of `--batch` pairs (default 5 x 16 = 80 pairs) through matcher + solver on one
+GPU. Engine batches of 16: creating the engine for batches of 32 fails to allocate its buffers on an 80 GB H100.
+`--dump-outputs DIR` writes the poses of the headline run's last engine batch. With N GPUs every rank runs its own pairs (weak
 scaling); one NCCL gather of the pose records at the end of the stream.
 
   python bench.py --gpus N --steps K --warmup W            # our arm (one process per GPU, torchrun for N > 1)
@@ -47,7 +48,7 @@ def parse():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--batch", type=int, default=int(os.environ.get("MFR_BENCH_BATCH", 32)), help="pairs per engine batch")
+    ap.add_argument("--batch", type=int, default=int(os.environ.get("MFR_BENCH_BATCH", 16)), help="pairs per engine batch")
     ap.add_argument("--micro", type=int, default=int(os.environ.get("MFR_BENCH_MICRO", 5)), help="engine batches per step")
     ap.add_argument("--hyp", type=int, default=1024, help="5-point hypotheses per pair")
     ap.add_argument("--match-thr", type=float, default=0.2, help="LoFTR coarse confidence threshold (reference: 0.2)")
@@ -60,6 +61,9 @@ def parse():
     ap.add_argument("--configs", default=os.environ.get("MFR_BENCH_CONFIGS", "C1,C3,C4,C5"), help="extra BASELINE configs to measure ('' = none)")
     ap.add_argument("--stream-pairs", type=int, default=10000, help="length of the C4 pair stream")
     ap.add_argument("--no-siblings", action="store_true", help="skip the tf32 / fp32x3 runs of the headline workload")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps of the headline run, write the poses of its last engine batch (the last --batch pairs "
+                         "of the last step: R [B,3,3], metric t [B,3], inliers [B]) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -162,10 +166,10 @@ WEIGHTS_NOTE = {
                          "normalised cross-correlation (a working matcher: ~1-3.6 k matches per pair), plus seeded Gaussian noise on every conv / "
                          "linear weight so that all tensor-core operands are dense; the reference does not ship its checkpoints"),
     "functional": "loftr.functional_state_dict(): the same without the perturbation (99.8 % of the weights are zero)"}
-WORKLOAD = "LoFTR coarse-to-fine + 5-pt essential (EssentialMatrixMetric, scale from depth), 540x720 (720x544 padded), 1xB200 per rank"
-DTYPE = {"bf16": ("bf16 (ResNet-FPN maps, token-GEMM / correlation / linear-attention operands: bf16 storage, kind::f16 MMA, fp32 accumulate; "
+WORKLOAD = "LoFTR coarse-to-fine + 5-pt essential (EssentialMatrixMetric, scale from depth), 540x720 (720x544 padded), 1xH100 per rank"
+DTYPE = {"bf16": ("bf16 (ResNet-FPN maps, token-GEMM / correlation / linear-attention operands: bf16 storage, bf16 wgmma, fp32 accumulate; "
                   "token residual stream, LayerNorm, similarity matrix, dual softmax, fine matching fp32; pose solve fp64/fp32)"),
-         "tf32": "tf32 (fp32 storage, kind::tf32 MMA inputs in every GEMM, fp32 accumulate; attention / LayerNorm / softmax fp32; pose solve fp64/fp32)",
+         "tf32": "tf32 (fp32 storage, tf32 wgmma inputs in every GEMM, fp32 accumulate; attention / LayerNorm / softmax fp32; pose solve fp64/fp32)",
          "fp32x3": "fp32 via 3xTF32 split GEMMs (fp32 storage, hi/lo operand split, fp32 accumulate; everything else fp32; pose solve fp64/fp32)"}
 
 
@@ -173,19 +177,8 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), "measured", d.get("bf16_tflops_sustained")
-    return 6650.0, 1590.0, "fallback", 1400.0
-
-
-def load_traffic(precision, batch):
-    """DRAM bytes of the ResNet-FPN conv launches of one engine batch, from the committed ncu capture of this
-    workload (profiles/README.md); None when no capture exists for the configuration."""
-    for rnd in ("r02", "r01"):
-        p = os.path.join(ROOT, "profiles", f"{rnd}_conv_gemm_metrics_{precision}_B{batch}.json")
-        if os.path.exists(p):
-            d = json.load(open(p))["backbone"]
-            return int(d["dram_read"] + d["dram_write"]), os.path.relpath(p, ROOT)
-    return None, None
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops", 989.0), "measured", d.get("bf16_tflops_sustained")
+    return 3350.0, 989.0, "data-sheet (H100 SXM dense)", None
 
 
 # ------------------------------------------------------------------------------------------------
@@ -329,6 +322,14 @@ def decomposition(hs, be, eng_matches, label):
     return out
 
 
+def dump_outputs(out_dir, last):
+    """The arrays the timed path hands its caller for its last engine batch: R [B, 3, 3], t [B, 3], inliers [B]."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, x in zip(("R", "t", "inliers"), last):
+        a = np.asarray(x.cpu().numpy() if hasattr(x, "cpu") else x)
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float64 if a.dtype == np.float64 else np.float32))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -348,6 +349,8 @@ def run_ours(args):
     out_bytes = int(pipe.slots[0]["rec_host"].numel() * 4) * micro
     clk, clk2 = ClockSampler(hs.local_rank), ClockSampler(hs.local_rank)
     ms_res, last = hs.timed(pipe, eng, lambda b: hs.submit_resident(pipe, eng, b), K * micro, Wm * micro, gather_at_end=True, sampler=clk)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     clocks = clk.summary()
     ms_e2e, _ = hs.timed(pipe, eng, lambda b: hs.submit_host(pipe, b), K * micro, Wm * micro, sampler=clk2)
     clocks_e2e = clk2.summary()
@@ -369,10 +372,9 @@ def run_ours(args):
     result = None
     if rank == 0:
         hbm, bf16, how, bf16_sus = load_peaks()
-        # ---- roofline of the dominant kernel (tcgen05 conv/GEMM), per-launch device times by CUDA events
+        # ---- roofline of the dominant kernel (wgmma conv/GEMM), per-launch device times by CUDA events
         prof = eng.profile(hs.dres["g0"][hs.idx_cache[0]], hs.dres["g1"][hs.idx_cache[0]])
         tot_ms = sum(p[2] for p in prof)
-        traffic, traffic_src = load_traffic(args.precision, B)
         is_bb = lambda p: p[1] == 1 and p[0].startswith("layer")          # ResNet-FPN implicit-GEMM convs
         bb = [p for p in prof if is_bb(p)]
         og = [p for p in prof if p[1] == 1 and not is_bb(p)]             # transformer / correlation / fine-level GEMMs
@@ -382,18 +384,17 @@ def run_ours(args):
         peak = bf16 if args.precision == "bf16" else bf16 / 2.0
         peak_sus = (bf16_sus if args.precision == "bf16" else bf16_sus / 2.0) if bf16_sus else None
         achieved = bb_fl / (bb_ms * 1e-3) / 1e12
-        roofline = {"kernel": f"conv_gemm_tf32_kernel, ResNet-FPN convs (tcgen05 kind::{kind}, {len(bb)} launches per engine batch)",
+        roofline = {"kernel": f"conv_gemm_kernel, ResNet-FPN convs (wgmma {kind}, {len(bb)} launches per engine batch)",
                     "bound": "tensor", "achieved": round(achieved, 1), "peak": round(peak, 1), "unit": "TFLOP/s",
                     "frac": round(achieved / peak, 4),
-                    "peak_note": f"{how} cuBLAS bf16 burst {bf16} TFLOP/s" + ("" if args.precision == "bf16" else " / 2 (kind::tf32 issues at half the bf16 rate)") +
+                    "peak_note": f"{how} cuBLAS bf16 burst {bf16} TFLOP/s" + ("" if args.precision == "bf16" else " / 2 (tf32 issues at half the bf16 rate)") +
                                  "; the per-launch times behind `achieved` come from an eager pass with an event pair per launch (a kernel timed alone: burst peak)",
                     "frac_of_sustained_peak": round(achieved / peak_sus, 4) if peak_sus else None,
                     "sustained_peak_note": f"cuBLAS bf16 sustained {bf16_sus} TFLOP/s (back to back for 4 s, power-capped clocks): the denominator that matches the multi-second timed region",
                     "algorithmic_flops_per_launch_avg": bb_fl / max(1, len(bb)), "avg_launch_ms": round(bb_ms / max(1, len(bb)), 4),
-                    "share_of_step": round(bb_ms / tot_ms, 3), "flops_per_engine_batch": bb_fl, "traffic": traffic,
-                    "traffic_note": (f"dram__bytes_read.sum + dram__bytes_write.sum summed over the {len(bb)} launches of one engine batch, {traffic_src}"
-                                     if traffic else "no ncu capture committed for this precision / batch"),
-                    "other_gemms": {"what": "token (q|k|v, merge, MLP), correlation and fine-level GEMMs of the same kernel", "launches": len(og),
+                    "share_of_step": round(bb_ms / tot_ms, 3), "flops_per_engine_batch": bb_fl, "traffic": None,
+                    "traffic_note": "DRAM traffic not measured",
+                    "other_gemms": {"what": "token (q|k|v; merge / MLP: the fused encoder-tail kernel in bf16 mode), correlation and fine-level GEMMs", "launches": len(og),
                                     "achieved": round(og_fl / (og_ms * 1e-3) / 1e12, 1), "peak": round(peak, 1),
                                     "frac": round(og_fl / (og_ms * 1e-3) / 1e12 / peak, 4), "share_of_step": round(og_ms / tot_ms, 3)},
                     "whole_step_tflops": round((bb_fl + og_fl) * K * micro / (ms_res * 1e-3) / 1e12, 1)}
@@ -458,7 +459,7 @@ def run_ours(args):
             "config": {"workload": WORKLOAD, "pairs_per_step_per_gpu": B * micro, "engine_batch": B, "engine_batches_per_step": micro,
                        "precision": args.precision, "hypotheses_per_pair": args.hyp, "match_thr": args.match_thr,
                        "matches_last_batch": m_last, "weights": WEIGHTS_NOTE[args.weights], "timed_region_s": round(ms_res / 1e3, 2),
-                       "l2": "per-batch working set (activations + 150 MB similarity matrix per pair) far exceeds the 126 MB L2; inputs rotate over %d distinct pairs" % hs.n_pool},
+                       "l2": "per-batch working set (activations + 150 MB similarity matrix per pair) far exceeds the 50 MB L2; inputs rotate over %d distinct pairs" % hs.n_pool},
             "e2e": {"value": round(e2e_value, 2), "unit": "pairs/s", "h2d_bytes_per_step": in_bytes,
                     "d2h_bytes_per_step": out_bytes, "ms_per_step": round(ms_e2e / K, 3), "clocks": clocks_e2e,
                     "api": "mfr_b200.pipeline.RelocPipeline.submit_host (copy / matcher / RANSAC stages of consecutive batches overlap)"},
@@ -616,12 +617,12 @@ def config_c3(hs, args):
     eng.close(); be.close()
     return {"workload": "SuperPoint + SuperGlue (1024 keypoints, matchers.py:65-71) + PnPSolver (P3P RANSAC 3 px + LM refine), 540x720",
             "weights": wnote, "value": round(B * nb / (ms_res * 1e-3), 2), "unit": "pairs/s", "pairs_per_batch": B, "ms_per_batch": round(ms_res / nb, 3),
-            "dtype": "tf32 (fp32 storage, kind::tf32 MMA inputs; softmax / Sinkhorn / NMS fp32; pose solve fp64/fp32)",
+            "dtype": "tf32 (fp32 storage, tf32 wgmma inputs; softmax / Sinkhorn / NMS fp32; pose solve fp64/fp32)",
             "e2e": {"value": round(B * nb / (ms_e2e * 1e-3), 2), "unit": "pairs/s",
                     "h2d_bytes_per_batch": int(sum(np.prod(hs.h[k].shape[1:]) * 4 for k in stage) * B), "d2h_bytes_per_batch": B * 13 * 4},
             "keypoints_per_image": round(float(np.mean(kp)), 1), "matches_per_pair": round(float(np.mean(mt)), 1),
             "gpu_launches_per_batch": n_launch,
-            "roofline": {"kernel": "conv_gemm_tf32_kernel (SuperPoint convs, SuperGlue linears + attention GEMMs); whole-step figure", "bound": "tensor",
+            "roofline": {"kernel": "conv_gemm_kernel (SuperPoint convs, SuperGlue linears + attention GEMMs); whole-step figure", "bound": "tensor",
                          "achieved": round(achieved, 1), "peak": round(bf16 / 2, 1), "unit": "TFLOP/s", "frac": round(achieved / (bf16 / 2), 4),
                          "algorithmic_flops_per_pair": flops_pair, "traffic": None},
             "accuracy": {"pairs": len(errs), "solved": len(fin([e[0] for e in errs])), "median_rot_err_deg": med(fin([e[0] for e in errs])),
@@ -831,7 +832,7 @@ def cpu_baseline(args, hs, sample):
         tn, ts = cpu_pairs(sample, args.match_thr, args.weights, pool=pool, device="cuda")
         out["torch_eager_on_this_gpu"] = {"loftr_ms_per_pair": round(tn / sample * 1e3, 1), "opencv_solver_ms_per_pair": round(ts / sample * 1e3, 1),
                                           "pairs_per_s": round(sample / (tn + ts), 2),
-                                          "note": "oracle LoFTR as torch eager fp32 on the B200 (one pair per forward, the reference's batch size) + OpenCV solver on the host: "
+                                          "note": "oracle LoFTR as torch eager fp32 on the GPU (one pair per forward, the reference's batch size) + OpenCV solver on the host: "
                                                   "the deployment the reference documents (offline GPU matcher + online CPU solver), serialised"}
     except Exception as e:
         out["torch_eager_on_this_gpu"] = {"error": f"{type(e).__name__}: {e}"}

@@ -1,4 +1,4 @@
-/* mfr_b200 — C ABI of the B200-native feature-matching + scale-from-depth hot path.
+/* mfr_b200 — C ABI of the H100-native feature-matching + scale-from-depth hot path.
  *
  * Drop-in boundary for nianticlabs/map-free-reloc (reference paths are relative to that repo):
  * the reference has no FFI of its own (pure Python over torch / OpenCV wheels), so each entry
@@ -30,7 +30,7 @@ extern "C" {
 int mfr_version(void);
 int mfr_device_sm_count(void);
 
-/* Implicit-GEMM convolution on tcgen05 tensor cores (TF32 inputs, fp32 accumulate), NHWC.
+/* Implicit-GEMM convolution on the Hopper tensor cores (wgmma, TF32 inputs, fp32 accumulate), NHWC.
  * Replaces torch's cuDNN conv2d / cuBLAS linear / einsum calls of the matcher networks:
  *   etc/feature_matching_baselines/LoFTR/src/loftr/backbone/resnet_fpn.py:5-12 (conv1x1/conv3x3),
  *   .../loftr_module/transformer.py:22-32 (Linear), .../utils/coarse_matching.py:113 (einsum).
@@ -43,11 +43,10 @@ int mfr_conv2d_nhwc_tf32(const float* x, int N, int H, int W, int Cin, long long
                          int b_batched, const float* bias, const float* residual, long long ldr,
                          int act, float alpha, float* out, long long ldo, void* stream);
 
-/* Same op with bf16 operands (x, w as bf16 bits; tcgen05 kind::f16, fp32 accumulate). ldx / ldw are
+/* Same op with bf16 operands (x, w as bf16 bits; bf16 wgmma, fp32 accumulate). ldx / ldw are
  * element strides with ldx*2 and ldw*2 multiples of 16 bytes (ldw = per-tap row stride of w, >= Cin).
  * out / residual are bf16 when out_bf16 != 0 (then Cout % 4 == 0), else fp32. bias is fp32.
- * bf16 output rows whose stride ldo is exactly Cout rounded up to a multiple of 8 own their padding: the
- * (at most 7) elements past Cout of every pixel may be overwritten with zeros (16-byte store units). */
+ * Elements past Cout of an output row are not written. */
 int mfr_conv2d_nhwc_bf16(const void* x, int N, int H, int W, int Cin, long long ldx, const void* w,
                          long long ldw, int Cout, int R, int S, int stride, int pad, const float* bias,
                          const void* residual, long long ldr, int act, float alpha, void* out,
@@ -104,7 +103,7 @@ int mfr_loftr_debug_tensor(mfr_loftr* h, const char* name, float** ptr, long lon
 int mfr_loftr_num_kernels(const mfr_loftr* h);  /* steps of the launch list per forward */
 int mfr_loftr_num_launches(const mfr_loftr* h); /* kernel launches per forward */
 /* Eager run with a CUDA-event pair around every step of the launch list (host arrays out):
- * ms[i] device time, flops[i] algorithmic FLOPs, kinds[i] 1 = tcgen05 conv/GEMM, names 32 bytes each.
+ * ms[i] device time, flops[i] algorithmic FLOPs, kinds[i] 1 = tensor-core conv/GEMM, names 32 bytes each.
  * Returns the number of steps (or a negative MFR_ERR_*). */
 int mfr_loftr_profile(mfr_loftr* h, const float* img0, const float* img1, int src_h, int src_w,
                       void* stream, int max_steps, float* ms, double* flops, int* kinds, char* names);
@@ -240,14 +239,9 @@ int mfr_host_p3p(const double* X, const double* f, double* R_out, double* t_out)
 int mfr_host_poly_real_roots(const double* coef, int deg, double* roots);
 int mfr_host_decompose_essential(const double* E, double* R1, double* R2, double* t);
 
-/* Debug probes (microbenchmarks used by scripts/, not part of the product path): microseconds per
- * launch of an empty / TMEM-allocating kernel with the GEMM's launch shape, and of a prebuilt
- * conv/GEMM op launched back to back. */
-float mfr_debug_probe_overhead(int mode, int smem_bytes, int grid, int iters);
-/* tensor-pipe probe: ns per tcgen05.mma (128 x BN x 32 B of K, operands resident in shared memory) when one
- * thread issues n_per_commit MMAs per tcgen05.commit, optionally waiting for each commit */
-float mfr_debug_mma_probe(int n_per_commit, int BN, int bf16, int wait_each, int iters, int grid, int two_commits);
-/* flags: bit 0 = x/w are bf16, bit 1 = out/residual are bf16, bit 2 = channel strides padded to multiples of 8 elements;
+/* Debug probe (microbenchmark used by scripts/, not part of the product path): microseconds per
+ * launch of a prebuilt conv/GEMM op launched back to back.
+ * flags: bit 0 = x/w are bf16, bit 1 = out/residual are bf16, bit 2 = channel strides padded to multiples of 8 elements;
  * residual may be NULL */
 float mfr_debug_time_conv(const float* x, int N, int H, int W, int Cin, const float* w, int Cout, int R,
                           int stride, float* out, int iters, int flags, const float* residual);
@@ -262,7 +256,7 @@ int mfr_linear_attention(const void* q, const void* k, const void* v, void* msg,
 
 /* Stage entry for tests: the backbone stem, conv 7x7 stride 2 pad 3, 1 -> 128 channels, folded-BN bias, ReLU
  * (LoFTR/src/loftr/backbone/resnet_fpn.py:52-62,102). img fp32 [NI][H][W]; w fp32 [128][49]; out [NI][H/2][W/2][128], bf16 when
- * out_bf16 != 0 (the tcgen05 kernel; MFR_STEM_TC=0 selects the mma.sync one), else fp32; exact_fp32: plain FMA kernel. */
+ * out_bf16 != 0, else fp32 (both on mma.sync); exact_fp32: plain FMA kernel. */
 int mfr_stem_conv7x7(const float* img, const float* w, const float* bias, void* out, int NI, int H, int W, int out_bf16,
                      int exact_fp32, void* stream);
 
@@ -301,13 +295,14 @@ int mfr_resize_linear(const void* src, int src_is_u8, int src_w, int src_h, long
 int mfr_pose_metrics(const double* q_gt, const double* t_gt, const double* q_est, const double* t_est, const double* K, int W,
                      int H, int n, double* trans_err, double* rot_err, double* reproj_err, void* stream);
 
-/* Stage entry: the fused tail of one LoFTREncoderLayer (loftr_module/transformer.py:52-58),
+/* Stage entry: the tail of one LoFTREncoderLayer (loftr_module/transformer.py:52-58),
  *   x += norm2(mlp2(relu(mlp0([x | norm1(merge(msg))])))),  bf16 tensor-core operands, fp32 accumulate / LayerNorm / residual,
  * for n_blocks row blocks of rows_cap token rows (live rows per block: *dyn_rows when non-null). Device pointers:
  * msg bf16 [rows][C]; xb bf16 [rows][2C] (columns [0, C) = shadow of x: read, then rewritten with the new x);
  * x fp32 [rows][2C] (columns [0, C) in / out); w_merge [C][C], w_mlp0 [2C][2C], w_mlp2 [C][2C] bf16 row-major
- * ([out][in], the reference's nn.Linear layout); g1 / b1 / g2 / b2 fp32 [C]. C = 256 or 128. `iters` launches back to
- * back (timing); note that every launch applies the residual update again. */
+ * ([out][in], the reference's nn.Linear layout); g1 / b1 / g2 / b2 fp32 [C]. C = 256 or 128. One fused wgmma kernel
+ * launch (csrc/encoder_tail.cu, the engine's bf16 path). `iters` launches back to back (timing); note that every launch
+ * applies the residual update again. */
 int mfr_encoder_tail(const void* msg, void* xb, float* x, const void* w_merge, const void* w_mlp0, const void* w_mlp2,
                      const float* g1, const float* b1, const float* g2, const float* b2, int C, int n_blocks,
                      long long rows_cap, const int* dyn_rows, int iters, void* stream);

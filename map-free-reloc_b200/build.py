@@ -1,7 +1,7 @@
-"""Builds libmfr_b200.so (hand-written sm_100a CUDA behind a C ABI) in-tree with nvcc.
+"""Builds libmfr_b200.so (hand-written sm_90a CUDA behind a C ABI) in-tree with nvcc.
 
 Usage: python map-free-reloc_b200/build.py [--force]
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so and the object files are build products (git-ignored).
 """
 import os
 import subprocess
@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libmfr_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xptxas", "-v",
 ]
 
@@ -55,7 +55,7 @@ def build(force=False, verbose=True):
                     print(os.path.basename(src), line.strip())
     if not ok:
         raise RuntimeError("nvcc failed")
-    cmd = [NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", OUT, *objs, "-lcudart", "-lnvjpeg"]
+    cmd = [NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", OUT, *objs, "-lcudart", "-lnvjpeg"]
     subprocess.check_call(cmd)
     return OUT
 

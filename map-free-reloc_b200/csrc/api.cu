@@ -5,9 +5,9 @@
 #include <cstdlib>
 #include "common.cuh"
 #include "conv_gemm.cuh"
+#include "encoder_tail.cuh"
 #include "loftr_engine.cuh"
 #include "loftr_ops.cuh"
-#include "encoder_tail.cuh"
 #include "spsg_engine.cuh"
 #include "geometry_solvers.cuh"
 #include "geometry.cuh"
@@ -251,13 +251,6 @@ int mfr_host_decompose_essential(const double* E, double* R1, double* R2, double
 }
 
 // ------------------------------------------------------------------------------------------ debug probes
-float mfr_debug_probe_overhead(int mode, int smem_bytes, int grid, int iters) {
-  return mfr::conv_gemm_probe_overhead(mode, smem_bytes, grid, iters, nullptr);
-}
-float mfr_debug_mma_probe(int n_per_commit, int BN, int bf16, int wait_each, int iters, int grid, int two_commits) {
-  return mfr::conv_gemm_mma_probe(n_per_commit, BN, bf16, wait_each, iters, grid, two_commits);
-}
-
 float mfr_debug_time_conv(const float* x, int N, int H, int W, int Cin, const float* w, int Cout, int R,
                           int stride, float* out, int iters, int flags, const float* residual) {
   mfr::ConvGemmDesc d{};
@@ -306,7 +299,7 @@ int mfr_linear_attention(const void* q, const void* k, const void* v, void* msg,
     return r;
   }
   if (L <= 0 || S <= 0) return MFR_ERR_ARG;
-  const int splits = std::max(1, std::min((S + 63) / 64, (2 * 148 + n - 1) / n));
+  const int splits = std::max(1, std::min((S + 63) / 64, (2 * mfr::sm_count() + n - 1) / n));
   float *kv_part = nullptr, *kv = nullptr;
   if (cudaMalloc(&kv_part, static_cast<size_t>(n) * splits * 8448 * sizeof(float)) != cudaSuccess) return MFR_ERR_CUDA;
   if (cudaMalloc(&kv, static_cast<size_t>(n) * 8448 * sizeof(float)) != cudaSuccess) { cudaFree(kv_part); return MFR_ERR_CUDA; }
@@ -354,28 +347,7 @@ int mfr_encoder_tail(const void* msg, void* xb, float* x, const void* w_merge, c
   d.dyn_rows = dyn_rows;
   mfr::EncoderTailParams p;
   int rc = mfr::encoder_tail_build(d, &p);
-  if (rc != MFR_OK) return rc;
   for (int i = 0; i < iters && rc == MFR_OK; ++i) rc = mfr::encoder_tail_launch(p, static_cast<cudaStream_t>(stream));
-  if (rc == MFR_OK && getenv("MFR_TAIL_DEBUG") != nullptr) {   // timeline of block 0 (one extra launch)
-    long long* d = nullptr;
-    cudaMalloc(&d, 256 * sizeof(long long));
-    cudaMemset(d, 0, 256 * sizeof(long long));
-    p.dbg = d;
-    mfr::encoder_tail_launch(p, static_cast<cudaStream_t>(stream));
-    cudaStreamSynchronize(static_cast<cudaStream_t>(stream));
-    long long h[256];
-    cudaMemcpy(h, d, sizeof(h), cudaMemcpyDeviceToHost);
-    cudaFree(d);
-    long long t0 = 0;
-    for (int r = 0; r < 4; ++r)
-      if (h[r * 64 + 1] && (t0 == 0 || h[r * 64 + 1] < t0)) t0 = h[r * 64 + 1];
-    const char* names[4] = {"mma", "front", "tma", "back"};
-    for (int r = 0; r < 4; ++r) {
-      fprintf(stderr, "[encoder_tail C=%d %s]", C, names[r]);
-      for (int k = 0; k < 32 && h[r * 64 + 2 * k + 1]; ++k) fprintf(stderr, " %lld@%lld", h[r * 64 + 2 * k], h[r * 64 + 2 * k + 1] - t0);
-      fprintf(stderr, "\n");
-    }
-  }
   return rc;
 }
 

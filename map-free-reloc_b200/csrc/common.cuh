@@ -1,7 +1,7 @@
-// Shared device/host helpers for the mfr_b200 CUDA library (sm_100a only).
+// Shared device/host helpers for the mfr_b200 CUDA library (sm_90a).
 //
-// PTX wrappers for the Blackwell async machinery used by the tensor-core kernels:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld).
+// PTX wrappers for the Hopper async machinery used by the tensor-core kernels: mbarrier and TMA
+// (cp.async.bulk.tensor); the warpgroup MMA wrappers are in wgmma.cuh.
 // Everything here is hand-written inline PTX; no CUTLASS/CuTe types are used.
 #pragma once
 
@@ -36,6 +36,17 @@ inline bool first_call_on_device(bool (&seen)[64]) {
 }
 
 namespace mfr {
+
+// SMs of the current device (launch-size heuristics); 132 (H100 SXM) when no device can be queried
+inline int sm_count() {
+  static int sms = 0;
+  if (sms == 0) {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 132;
+    sms = n;
+  }
+  return sms;
+}
 
 // ---------------------------------------------------------------------------------------------
 // generic
@@ -100,7 +111,18 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int tag
   if (mbar_try_wait(bar, parity)) return;
   mbar_wait_slow(bar, parity, tag);
 }
-// One lane of a converged warp (elect.sync): lets ptxas emit a single UTMALDG / UTCHMMA instead of the
+// Barrier wait for kernels that issue wgmma: spin loop inlined and without printf. Any function call (mbar_wait's
+// out-of-line slow path, vprintf) in such a kernel makes ptxas serialise the wgmma pipeline. A wait that exceeds the
+// bound traps (`tag` names the wait site for a debugger).
+__device__ __forceinline__ void mbar_wait_inl(uint32_t bar, uint32_t parity, int tag) {
+  (void)tag;
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity))
+    if (clock64() - t0 > MFR_SPIN_TIMEOUT_CYCLES) __trap();
+}
+
+// One lane of a converged warp (elect.sync): lets ptxas emit a single UTMALDG instead of the
 // per-active-thread loop it wraps around uniform-datapath instructions in divergent code.
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred;
@@ -143,208 +165,6 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm,
       " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(dst),
       "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
-}
-
-// TMA load multicast to the CTAs of `cta_mask` in the cluster: data and complete_tx land at the same shared-memory
-// offsets (dst, bar) in every destination CTA
-__device__ __forceinline__ void tma_load_3d_mcast(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1,
-                                                  int c2, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"(cta_mask)
-      : "memory");
-}
-// CTA-pair (cta_group::2) loads: the bytes land in THIS CTA's shared memory, the complete_tx goes to `bar`, a
-// shared::cluster address that may belong to the peer (the pair's leader collects both CTAs' transactions on its barrier)
-__device__ __forceinline__ void tma_load_3d_2sm(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2,
-                                                int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-// shared::cluster address of the location `addr` (a shared::cta address of this CTA) in the CTA of rank `rank`
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-// arrive on an mbarrier anywhere in the cluster (shared::cluster address)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// TMA store: shared -> global (tiled tensor map), completion tracked by the issuing thread's bulk groups
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* tm, uint32_t src, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
-          reinterpret_cast<uint64_t>(tm)),
-      "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// wait until at most N of this thread's bulk groups still READ their shared-memory source
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N>
-__device__ __forceinline__ void tma_store_wait() {
-  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------
-// tcgen05 : tensor memory + 5th-gen tensor-core MMA
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// MMA completion -> mbarrier arrive (implies tcgen05.fence::before_thread_sync).
-// commit that arrives on the barrier at the same offset in every CTA of `cta_mask`
-__device__ __forceinline__ void tc_commit_mcast(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   bar),
-               "h"(cta_mask)
-               : "memory");
-}
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   bar)
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], TF32 inputs (fp32 bits in smem), fp32 accumulate.
-__device__ __forceinline__ void tc_mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// BF16 inputs, fp32 accumulate.
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// ---- CTA-pair variants (cta_group::2): one instruction works on the tensor memory / barriers of both CTAs of a pair.
-// alloc / dealloc: one warp of EACH CTA (same warp index) executes them; mma / commit: the leader CTA (rank 0) only.
-__device__ __forceinline__ void tmem_alloc2(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// completion of the pair's MMAs -> arrive on the barrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void tc_commit2_mcast(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"(cta_mask)
-               : "memory");
-}
-// D[tmem of both CTAs, 128 rows each] (+)= A[256 rows: 128 from each CTA's smem] * B[N rows: N/2 from each CTA's smem]
-__device__ __forceinline__ void tc_mma_tf32_2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16_2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns: thread t of the warp gets row (lane base + t).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle (rows are 128 B, 8-row
-// swizzle atoms are 1024 B apart). Field layout follows the sm_100 "matrix descriptor":
-//   [0,14)  start address >> 4      [16,30) leading byte offset >> 4 (ignored for SW128 K-major)
-//   [32,46) stride byte offset >> 4 [46,48) version = 1            [61,64) layout: 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t umma_desc_sw128_kmajor(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
-// Instruction descriptor for kind::tf32 / kind::f16 with fp32 accumulation, both operands K-major.
-//   [4,6) D format (1 = f32)  [7,10) A format  [10,13) B format  (0 f16, 1 bf16, 2 tf32)
-//   [17,23) N >> 3            [24,29) M >> 4
-__host__ __device__ constexpr uint32_t umma_idesc(uint32_t ab_format, uint32_t M, uint32_t N) {
-  return (1u << 4) | (ab_format << 7) | (ab_format << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
 }
 
 }  // namespace mfr

@@ -1,24 +1,25 @@
-// tcgen05 implicit-GEMM convolution kernel (sm_100a). See conv_gemm.cuh for the op definition.
+// wgmma implicit-GEMM convolution kernel (sm_90a). See conv_gemm.cuh for the op definition.
 //
-// Structure (one persistent CTA per SM, 192 threads):
-//   warp 0      : TMA producer. Per k-block it loads a [TH x TW pixels] x [32 channels] activation
-//                 box (rank-4 tensor map over NHWC; halo / padding comes back as zeros through the
-//                 TMA out-of-bounds fill, stride-2 through the map's traversal stride) and a
-//                 [BN filters] x [32 channels] weight box, both 128B-swizzled, into a 4-stage ring.
-//   warp 1      : MMA issuer. One elected lane issues 4 x tcgen05.mma (128 x BN x 8, kind::tf32)
-//                 per stage into one of two TMEM accumulators (2 x 256 columns), then
-//                 tcgen05.commit frees the stage / publishes the accumulator.
-//   warps 2..5  : epilogue. tcgen05.ld the accumulator (thread = output pixel, 32 channels per
-//                 load), apply alpha / bias / residual / activation, write NHWC fp32.
-// The epilogue of tile i overlaps the main loop of tile i+1 through the double-buffered TMEM.
+// Structure (one persistent CTA per SM, 384 threads = three warpgroups):
+//   warp 0          : TMA producer. Per k-block it loads a [TH x TW pixels] x [32 fp32 | 64 bf16 channels] activation
+//                     box (rank-4 tensor map over NHWC; halo / padding comes back as zeros through the TMA
+//                     out-of-bounds fill, stride-2 through the map's traversal stride) and a [BN filters] x [same
+//                     channels] weight box, both 128B-swizzled, into the operand rings.
+//   warps 1..3      : idle (they complete the producer's warpgroup, so that the MMA warpgroups start on a warpgroup
+//                     boundary as wgmma requires).
+//   warpgroups 1, 2 : MMA + epilogue. Warpgroup g owns rows 64g..64g+63 of every 128-pixel sub-tile: per k-step it
+//                     issues one m64nBNk(32 B) wgmma per sub-tile, accumulating in registers; one wgmma group stays in
+//                     flight while the slots of the previous one are handed back to the producer. The epilogue
+//                     applies alpha / bias / residual / activation straight from the accumulator registers.
+// The producer runs ahead by the depth of the rings, so the loads of tile i+1 overlap the epilogue of tile i.
 #include "conv_gemm.cuh"
+#include "wgmma.cuh"
 
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <mutex>
-#include <type_traits>
 
 namespace mfr {
 
@@ -26,466 +27,141 @@ namespace {
 
 constexpr int kMaxSlots = 8;                    // slots per operand ring (A ring and B ring)
 constexpr int kBlockK = 32;                     // fp32 elements per k-block = 128 B = swizzle span
-constexpr int kUmmaK = 8;                       // tf32: 32 B of K per instruction
 constexpr int kTileM = 128;
 constexpr int kMaxBN = 256;
 constexpr int kAStage = kTileM * kBlockK * 4;   // 16 KB
-constexpr int kRingBytes = 204 * 1024;          // operand rings (A slots + B slots)
-constexpr int kStgStride = 36;                  // floats per staged row (144 B: conflict-free 128-bit access)
-constexpr int kStgBytes4 = 4 * 32 * kStgStride * 4;  // epilogue transpose buffers, one per epilogue warp (18 KB with 4 warps)
-constexpr int kSmemBytes = kRingBytes + kStgBytes4 + 1024 /*align slack*/;
-// with 8 epilogue warps the second 18 KB of staging comes out of the ring (token GEMMs with K <= 512 do not need its depth)
-constexpr int kRingBytes8 = kRingBytes - kStgBytes4;
-// Two MMA-issuing warps that alternate commit groups hide the commit stall (profiles/r01_mma_probe2.txt) and were
-// measured 3 % faster on the backbone, but the two instruction streams interleave in the pipe in a timing-dependent
-// order, so the fp32 accumulation order — and with it the last bits of the result — changes from run to run. The
-// engine promises bit-identical replays (tests/test_loftr_gpu.py), so the second issuer is compiled out.
-constexpr bool kDualIssue = false;
-constexpr int kThreads = 64 + 32 * 4;   // TMA producer, MMA issuer, 4 epilogue warps (the 8-warp instantiation: 64 + 32 * 8)
-static_assert(!kDualIssue, "the second MMA issuer was removed from the warp layout");
-constexpr int kTmemCols = 512;
+constexpr int kRingBytes = 212 * 1024;          // operand rings (A slots + B slots)
+constexpr int kZeroBytes = kMaxBN * 32;         // zero page: operand of the unused k-steps of a 32-byte channel-tail group
+constexpr int kSmemBytes = kRingBytes + kZeroBytes + 1024 /*align slack*/;
+constexpr int kMmaWarps = 8;                    // two MMA warpgroups
+constexpr int kThreads = 128 + 32 * kMmaWarps;
 
-__device__ __forceinline__ long long gtime() {
-  long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-#define MFR_STAMP(i) do { if (p.dbg != nullptr && blockIdx.x == 0) p.dbg[i] = gtime(); } while (0)
-// debug launches only (p.dbg set): SM cycles block 0 spends inside a barrier wait, summed into `acc`
-#define MFR_TIMED_WAIT(acc, bar, parity, tag)                 \
-  do {                                                        \
-    if (dbg_on) {                                             \
-      const long long t0_ = clock64();                        \
-      mbar_wait(bar, parity, tag);                            \
-      acc += clock64() - t0_;                                 \
-    } else {                                                  \
-      mbar_wait(bar, parity, tag);                            \
-    }                                                         \
-  } while (0)
-
-__device__ __forceinline__ float apply_act(float v, int act) {
+__device__ __forceinline__ float act_fn(float v, int act, bool fast) {
   if (act == ACT_RELU) return fmaxf(v, 0.f);
   if (act == ACT_LEAKY) return v > 0.f ? v : 0.01f * v;
-  if (act == ACT_ELU1) return v > 0.f ? v + 1.f : __expf(v);
-  return v;
-}
-// FAST (bf16 outputs only): elu(x) + 1 for x <= 0 is exp(x) in (0, 1] — a bare ex2.approx on the pre-scaled argument (2
-// instructions) instead of __expf with its range fix-ups (~9); its 2-ulp error is far below the bf16 rounding that follows.
-template <int ACT, bool FAST = false>
-__device__ __forceinline__ float act_fn(float v) {
-  if constexpr (ACT == ACT_RELU) return fmaxf(v, 0.f);
-  if constexpr (ACT == ACT_LEAKY) return v > 0.f ? v : 0.01f * v;
-  if constexpr (ACT == ACT_ELU1) {
-    if constexpr (FAST) {   // max(v, 0) + 2^min(v log2 e, 0): the same bits as the select form in five instructions
+  if (act == ACT_ELU1) {
+    // bf16 outputs: elu(x) + 1 for x <= 0 is exp(x) in (0, 1] — a bare ex2.approx on the pre-scaled argument; its 2-ulp
+    // error is far below the bf16 rounding that follows
+    if (fast) {
       float e;
       asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(fminf(v * 1.4426950408889634f, 0.f)));
       return fmaxf(v, 0.f) + e;
-    } else {
-      return v > 0.f ? v + 1.f : __expf(v);
     }
+    return v > 0.f ? v + 1.f : __expf(v);
   }
   return v;
 }
 
-// Coalesced part of the epilogue for one 32-channel chunk: 8 x (LDS.128 -> alpha/bias/residual/act ->
-// STG.128); lane (sub_r, sub_c) handles staged row k*4+sub_r, channels sub_c..sub_c+3.
-__device__ __forceinline__ float4 bf16x4_to_float4(uint2 u) {
-  float4 f;
-  f.x = __uint_as_float(u.x << 16); f.y = __uint_as_float(u.x & 0xffff0000u);
-  f.z = __uint_as_float(u.y << 16); f.w = __uint_as_float(u.y & 0xffff0000u);
-  return f;
-}
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }
+__device__ __forceinline__ float bf16_to_float(uint16_t u) { return __uint_as_float(static_cast<uint32_t>(u) << 16); }
 
-// Epilogue of one 128-pixel sub-tile, run by the 4 epilogue warps (warp q owns TMEM lanes 32q..32q+31):
-// per 32-channel chunk  tcgen05.ld (thread = pixel) -> per-warp shared-memory transpose -> 8 x
-// (LDS.128 -> alpha/bias/residual/act -> coalesced STG); lane (sub_r, sub_c) handles staged rows
-// k*4+sub_r, channels sub_c..sub_c+3. The residual of chunk c+1 is fetched before chunk c is stored
-// (and the first one before the accumulator wait), so its HBM latency never sits in front of a store.
-template <int ACT, bool RES, bool OBF, int EPI>
-__device__ __forceinline__ void epilogue_subtile(const ConvGemmParams& p, uint32_t taddr, float* stg, int lane,
-                                                 int n0, const long long (&off_o)[8], const long long (&off_r)[8],
-                                                 uint32_t okmask, uint32_t wait_bar, uint32_t wait_phase,
-                                                 bool do_wait, int c_begin) {
-  using RT = typename std::conditional<OBF, uint2, float4>::type;
-  const int sub_r = lane >> 3, sub_c = (lane & 7) * 4;
-  RT rnext[8];
-  auto issue_res = [&](int c0) {
-    const int n = n0 + c0 + sub_c;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      if constexpr (OBF) rnext[k] = make_uint2(0u, 0u);
-      else rnext[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (((okmask >> k) & 1u) && n < p.Cout && c0 + sub_c < p.BN) {
-        if constexpr (OBF)
-          rnext[k] = __ldg(reinterpret_cast<const uint2*>(reinterpret_cast<const uint16_t*>(p.residual) + off_r[k] + n));
-        else
-          rnext[k] = __ldg(reinterpret_cast<const float4*>(p.residual + off_r[k] + n));
-      }
-    }
-  };
-  constexpr int kStep = 32 * (EPI / 4);   // this warp's chunks: c_begin, c_begin + kStep, ...
-  if constexpr (RES) issue_res(c_begin);
-  if (do_wait) {
-    mbar_wait(wait_bar, wait_phase, 4);
-    tc_fence_after();
-  }
-  const float alpha = p.alpha;
-  for (int c0 = c_begin; c0 < p.BN; c0 += kStep) {
-    uint32_t r[32];
-    tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>(c0), r);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-      *reinterpret_cast<uint4*>(stg + lane * kStgStride + j * 4) =
-          make_uint4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-    __syncwarp();
-    RT rcur[8];
-    if constexpr (RES) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) rcur[k] = rnext[k];
-      if (c0 + kStep < p.BN) issue_res(c0 + kStep);
-    }
-    const int n = n0 + c0 + sub_c;
-    const uint32_t okm = (n < p.Cout && c0 + sub_c < p.BN) ? okmask : 0u;   // BN need not be a multiple of 32
-    float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (p.bias != nullptr && okm) b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n));
-    const bool do_act = n < p.act_cols;   // n..n+3 never straddle act_cols (multiple of 4)
-    const float* stg_rd = stg + sub_r * kStgStride + sub_c;
-    float4 vv[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) vv[k] = *reinterpret_cast<const float4*>(stg_rd + k * (4 * kStgStride));
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      float4 v = vv[k];
-      if (okm & (1u << k)) {
-        v.x = fmaf(v.x, alpha, b4.x); v.y = fmaf(v.y, alpha, b4.y);
-        v.z = fmaf(v.z, alpha, b4.z); v.w = fmaf(v.w, alpha, b4.w);
-        if constexpr (RES) {
-          float4 r4;
-          if constexpr (OBF) r4 = bf16x4_to_float4(rcur[k]);
-          else r4 = rcur[k];
-          v.x += r4.x; v.y += r4.y; v.z += r4.z; v.w += r4.w;
-        }
-        if (do_act) {
-          v.x = act_fn<ACT, OBF>(v.x); v.y = act_fn<ACT, OBF>(v.y); v.z = act_fn<ACT, OBF>(v.z); v.w = act_fn<ACT, OBF>(v.w);
-        }
-        if constexpr (OBF)
-          *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(p.out) + off_o[k] + n) =
-              make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
-        else
-          *reinterpret_cast<float4*>(p.out + off_o[k] + n) = v;
-      }
-    }
-    __syncwarp();
-  }
-}
+// 64-bit wgmma shared-memory matrix descriptor = constant high part | ((address >> 4) & 0x3fff). K-major, 128-byte rows,
+// 128B swizzle: 8-row swizzle atoms 1024 B apart (stride byte offset), layout type 1 in bits [62,64).
+constexpr uint64_t kDescHi = (1ull << 16) | (64ull << 32) | (1ull << 62);
+// same for 32-byte rows with the 32B swizzle (8-row groups 256 B apart, layout type 3): the narrow channel-tail tiles
+constexpr uint64_t kDescHi32 = (1ull << 16) | (16ull << 32) | (3ull << 62);
 
-// TMA-store epilogue of one 128-pixel sub-tile (fp32 output, no residual, TW a power of two): the thread that
-// holds a pixel's 32 channels applies alpha / bias / activation in registers, writes them as the 128-byte row
-// `lane` of a 128B-swizzled 32 x 32 staging tile, and one elected lane hands the tile to the TMA engine. Edge
-// clipping (ragged tiles, channel tail) is the tensor map's bounds check; no per-thread global stores.
-template <int ACT>
-__device__ __forceinline__ void epilogue_subtile_tma(const ConvGemmParams& p, uint32_t taddr, uint32_t stg_addr, int lane,
-                                                     int n0, int x0, int y0, int img, uint32_t wait_bar,
-                                                     uint32_t wait_phase, bool do_wait) {
-  if (do_wait) {
-    mbar_wait(wait_bar, wait_phase, 4);
-    tc_fence_after();
-  }
+// Epilogue of one accumulator fragment: rows (pixels) r0 and r0 + 8 of sub-tile m, columns 8j + 2(lane % 4) + {0, 1}.
+template <int BN_T>
+__device__ __forceinline__ void epilogue_subtile(const ConvGemmParams& p, const float (&acc)[BN_T / 2], int row0, int lane, int n0,
+                                                 int tx, int ty, int img, int m, int tile_rows, int w_lim, bool vec2) {
+  const bool obf = p.out_bf16 != 0;
   const float alpha = p.alpha;
-  const uint32_t row_addr = stg_addr + static_cast<uint32_t>(lane) * 128u;
-  const uint32_t sw = static_cast<uint32_t>(lane & 7);
-  for (int c0 = 0; c0 < p.BN; c0 += 32) {
-    uint32_t r[32];
-    tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>(c0), r);
-    tmem_ld_wait();
-    const int n = n0 + c0;
-    const bool do_act = n < p.act_cols;                 // act_cols is a multiple of 32 on this path
-    float v[32];
 #pragma unroll
-    for (int j4 = 0; j4 < 8; ++j4) {
-      float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (p.bias != nullptr && n + 4 * j4 < p.Cout) b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n + 4 * j4));
-      v[4 * j4] = fmaf(__uint_as_float(r[4 * j4]), alpha, b4.x);
-      v[4 * j4 + 1] = fmaf(__uint_as_float(r[4 * j4 + 1]), alpha, b4.y);
-      v[4 * j4 + 2] = fmaf(__uint_as_float(r[4 * j4 + 2]), alpha, b4.z);
-      v[4 * j4 + 3] = fmaf(__uint_as_float(r[4 * j4 + 3]), alpha, b4.w);
-    }
-    if (do_act) {
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + 8 * h;
+    const int ly = row / p.TW, lx = row - ly * p.TW;
+    const int y = ty * tile_rows + m * p.TH + ly, x = tx * p.TW + lx;
+    if (row >= p.TW * p.TH || y >= p.Ho || x >= w_lim) continue;
+    const long long o_off = img * p.out_img_stride + static_cast<long long>(y) * p.out_y_stride + static_cast<long long>(x) * p.ldo;
+    const long long r_off = img * p.res_img_stride + (static_cast<long long>(y) * p.Wo + x) * p.ldr;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = act_fn<ACT>(v[j]);
-    }
-    // the previous chunk's store must have finished reading the staging tile
-    if (elect_one_sync()) tma_store_wait_read<0>();
-    __syncwarp();
-#pragma unroll
-    for (int j4 = 0; j4 < 8; ++j4) {
-      const uint32_t a = row_addr + ((static_cast<uint32_t>(j4) ^ sw) << 4);
-      asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a), "f"(v[4 * j4]), "f"(v[4 * j4 + 1]),
-                   "f"(v[4 * j4 + 2]), "f"(v[4 * j4 + 3])
-                   : "memory");
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (elect_one_sync()) {
-      tma_store_4d(&p.tmC, stg_addr, n, x0, y0, img);
-      tma_store_commit();
-    }
-  }
-}
-
-// The same for bf16 outputs: 64 channels (two tcgen05.ld) per staged tile, rows of 64 packed bf16 = 128 bytes.
-// With 8 epilogue warps the two warps of a TMEM lane quadrant alternate 64-channel groups (c_begin = 0 / 64), each with its own
-// staging tile: one warp converts while the other's store drains.
-template <int ACT, int EPI>
-__device__ __forceinline__ void epilogue_subtile_tma_bf16(const ConvGemmParams& p, uint32_t taddr, uint32_t stg_addr, int lane,
-                                                          int n0, int x0, int y0, int img, uint32_t wait_bar,
-                                                          uint32_t wait_phase, bool do_wait, int c_begin) {
-  if (do_wait) {
-    mbar_wait(wait_bar, wait_phase, 4);
-    tc_fence_after();
-  }
-  const float alpha = p.alpha;
-  const bool plain = p.bias == nullptr && alpha == 1.f;
-  const uint32_t row_addr = stg_addr + static_cast<uint32_t>(lane) * 128u;
-  const uint32_t sw = static_cast<uint32_t>(lane & 7);
-  for (int c0 = c_begin; c0 < p.BN; c0 += 64 * (EPI / 4)) {
-    uint32_t o[32];
-    uint32_t ra[2][32];
-    const bool has2 = c0 + 32 < p.BN;                     // BN is a multiple of 16: the second half may not exist
-    tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>(c0), ra[0]);        // both halves in flight before the wait
-    tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>(has2 ? c0 + 32 : c0), ra[1]);   // (no second half: re-read, ignored)
-    tmem_ld_wait();
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int n = n0 + c0 + 32 * h;
-      if (h == 0 || has2) {
-        const uint32_t (&r)[32] = ra[h];
-        const bool do_act = n < p.act_cols;               // act_cols is a multiple of 32 on this path
-#pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-          float v0 = __uint_as_float(r[4 * j4]), v1 = __uint_as_float(r[4 * j4 + 1]);
-          float v2 = __uint_as_float(r[4 * j4 + 2]), v3 = __uint_as_float(r[4 * j4 + 3]);
-          if (!plain) {                                     // (uniform) plain: alpha = 1, no bias — fma(v, 1, 0) = v
-            float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p.bias != nullptr && n + 4 * j4 < p.Cout) b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n + 4 * j4));
-            v0 = fmaf(v0, alpha, b4.x); v1 = fmaf(v1, alpha, b4.y); v2 = fmaf(v2, alpha, b4.z); v3 = fmaf(v3, alpha, b4.w);
+    for (int j = 0; j < BN_T / 8; ++j) {
+      const int c = 8 * j + 2 * (lane & 3);
+      const int n = n0 + c;
+      if (c >= p.BN || n >= p.Cout) continue;
+      float v[2] = {acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]};
+      const bool two = n + 1 < p.Cout;
+      if (vec2 && two) {
+        float b0 = 0.f, b1 = 0.f;
+        if (p.bias != nullptr) { b0 = __ldg(p.bias + n); b1 = __ldg(p.bias + n + 1); }
+        v[0] = fmaf(v[0], alpha, b0);
+        v[1] = fmaf(v[1], alpha, b1);
+        if (p.residual != nullptr) {
+          if (obf) {
+            const uint32_t r = __ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.residual) + r_off + n));
+            v[0] += __uint_as_float(r << 16);
+            v[1] += __uint_as_float(r & 0xffff0000u);
+          } else {
+            const float2 r = __ldg(reinterpret_cast<const float2*>(p.residual + r_off + n));
+            v[0] += r.x;
+            v[1] += r.y;
           }
-          if (do_act) {
-            v0 = act_fn<ACT, true>(v0); v1 = act_fn<ACT, true>(v1); v2 = act_fn<ACT, true>(v2); v3 = act_fn<ACT, true>(v3);
-          }
-          o[16 * h + 2 * j4] = pack_bf16x2(v0, v1);
-          o[16 * h + 2 * j4 + 1] = pack_bf16x2(v2, v3);
         }
+        if (n < p.act_cols) v[0] = act_fn(v[0], p.act, obf);
+        if (n + 1 < p.act_cols) v[1] = act_fn(v[1], p.act, obf);
+        if (obf) *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out) + o_off + n) = pack_bf16x2(v[0], v[1]);
+        else *reinterpret_cast<float2*>(p.out + o_off + n) = make_float2(v[0], v[1]);
       } else {
 #pragma unroll
-        for (int j = 0; j < 16; ++j) o[16 * h + j] = 0u;  // channels >= Cout: clipped by the tensor map
-      }
-    }
-    // the previous group's store must have finished reading the staging tile
-    if (elect_one_sync()) tma_store_wait_read<0>();
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(row_addr + ((static_cast<uint32_t>(j) ^ sw) << 4)), "r"(o[4 * j]),
-                   "r"(o[4 * j + 1]), "r"(o[4 * j + 2]), "r"(o[4 * j + 3])
-                   : "memory");
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (elect_one_sync()) {
-      tma_store_4d(&p.tmC, stg_addr, n0 + c0, x0, y0, img);
-      tma_store_commit();
-    }
-  }
-}
-
-// Epilogue of the swapped-operand mode: TMEM lane = output channel (warp q owns channels 32q..32q+31), TMEM column
-// = pixel of the 256-pixel tile. Per 32-pixel chunk: tcgen05.ld (thread = channel, 32 pixels) -> transposing
-// shared-memory write (element (pixel, channel): consecutive lanes hit consecutive banks) -> the same coalesced
-// store phase as the normal mode (lane (sub_r, sub_c): pixels k*4+sub_r of the chunk, channels sub_c..sub_c+3).
-template <int ACT, bool RES, bool OBF>
-__device__ __forceinline__ void epilogue_tile_swap(const ConvGemmParams& p, uint32_t taddr, float* stg, int lane, int q,
-                                                   int tx, int ty, int img, int tile_rows, int w_lim, uint32_t wait_bar,
-                                                   uint32_t wait_phase) {
-  using RT = typename std::conditional<OBF, uint2, float4>::type;
-  const int sub_r = lane >> 3, sub_c = (lane & 7) * 4;
-  const int n = q * 32 + sub_c;                       // first of this lane's 4 output channels
-  const bool n_ok = n < p.Cout;
-  float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (p.bias != nullptr && n_ok) b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n));
-  const float alpha = p.alpha;
-  const int tw_shift = 31 - __clz(p.TW);              // TW is a power of two in halo mode
-  // pixel k*4+sub_r of chunk c0 -> its index inside the image (y*Wo + x, fits 32 bits), or -1 when it is not stored
-  auto pix_of = [&](int c0, int k) -> int {
-    const int pr = c0 + k * 4 + sub_r;                // pixel of the tile, (y, x) order over TW columns
-    const int ly = pr >> tw_shift, lx = pr & (p.TW - 1);
-    const int y = ty * tile_rows + ly, x = tx * p.TW + lx;
-    return (n_ok && y < p.Ho && x < w_lim) ? y * p.Wo + x : -1;
-  };
-  const int ldo = static_cast<int>(p.ldo), ldr = static_cast<int>(p.ldr);      // per-image offsets fit 32 bits
-  float* out_img = OBF ? reinterpret_cast<float*>(reinterpret_cast<uint16_t*>(p.out) + img * p.out_img_stride + n)
-                       : p.out + img * p.out_img_stride + n;
-  const float* res_img = nullptr;
-  if constexpr (RES)
-    res_img = OBF ? reinterpret_cast<const float*>(reinterpret_cast<const uint16_t*>(p.residual) + img * p.res_img_stride + n)
-                  : p.residual + img * p.res_img_stride + n;
-  RT rnext[8];
-  int pnext[8];
-  auto prefetch = [&](int c0) {                       // pixel indices (and residual) of chunk c0, one chunk ahead of its use
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      pnext[k] = pix_of(c0, k);
-      if constexpr (RES) {
-        if constexpr (OBF) rnext[k] = make_uint2(0u, 0u);
-        else rnext[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (pnext[k] >= 0) {
-          if constexpr (OBF) rnext[k] = __ldg(reinterpret_cast<const uint2*>(reinterpret_cast<const uint16_t*>(res_img) + pnext[k] * ldr));
-          else rnext[k] = __ldg(reinterpret_cast<const float4*>(res_img + pnext[k] * ldr));
-        }
-      }
-    }
-  };
-  prefetch(0);
-  mbar_wait(wait_bar, wait_phase, 4);
-  tc_fence_after();
-  for (int c0 = 0; c0 < 2 * kTileM; c0 += 32) {
-    uint32_t r[32];
-    tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>(c0), r);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 32; ++j) stg[j * kStgStride + lane] = __uint_as_float(r[j]);
-    __syncwarp();
-    RT rcur[8];
-    int pcur[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      pcur[k] = pnext[k];
-      if constexpr (RES) rcur[k] = rnext[k];
-    }
-    if (c0 + 32 < 2 * kTileM) prefetch(c0 + 32);
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      if (pcur[k] < 0) continue;
-      float4 v = *reinterpret_cast<const float4*>(stg + (k * 4 + sub_r) * kStgStride + sub_c);
-      v.x = fmaf(v.x, alpha, b4.x); v.y = fmaf(v.y, alpha, b4.y);
-      v.z = fmaf(v.z, alpha, b4.z); v.w = fmaf(v.w, alpha, b4.w);
-      if constexpr (RES) {
-        float4 r4;
-        if constexpr (OBF) r4 = bf16x4_to_float4(rcur[k]);
-        else r4 = rcur[k];
-        v.x += r4.x; v.y += r4.y; v.z += r4.z; v.w += r4.w;
-      }
-      v.x = act_fn<ACT, OBF>(v.x); v.y = act_fn<ACT, OBF>(v.y); v.z = act_fn<ACT, OBF>(v.z); v.w = act_fn<ACT, OBF>(v.w);
-      if constexpr (OBF)
-        *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(out_img) + pcur[k] * ldo) = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
-      else
-        *reinterpret_cast<float4*>(out_img + pcur[k] * ldo) = v;
-    }
-    __syncwarp();
-  }
-}
-
-// Scalar epilogue for shapes the vector path cannot take (Cout or strides not multiples of 4); fp32 only.
-template <int EPI>
-__device__ __forceinline__ void epilogue_subtile_scalar(const ConvGemmParams& p, uint32_t taddr, int n0, bool row_ok,
-                                                        long long o_off, long long r_off, int c_begin) {
-  for (int c0 = c_begin; c0 < p.BN; c0 += 32 * (EPI / 4)) {
-    uint32_t r[32];
-    tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>(c0), r);
-    tmem_ld_wait();
-    if (row_ok) {
-      float* orow = p.out + o_off;
-      const float* rrow = p.residual ? p.residual + r_off : nullptr;
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int n = n0 + c0 + j;
-        if (n < p.Cout && c0 + j < p.BN) {
-          float v = __uint_as_float(r[j]) * p.alpha;
-          if (p.bias) v += __ldg(p.bias + n);
-          if (rrow) v += __ldg(rrow + n);
-          orow[n] = n < p.act_cols ? apply_act(v, p.act) : v;
+        for (int e = 0; e < 2; ++e) {
+          const int ne = n + e;
+          if (ne >= p.Cout || c + e >= p.BN) continue;
+          float t = v[e] * alpha;
+          if (p.bias != nullptr) t += __ldg(p.bias + ne);
+          if (p.residual != nullptr)
+            t += obf ? bf16_to_float(reinterpret_cast<const uint16_t*>(p.residual)[r_off + ne]) : __ldg(p.residual + r_off + ne);
+          if (ne < p.act_cols) t = act_fn(t, p.act, obf);
+          if (obf) reinterpret_cast<uint16_t*>(p.out)[o_off + ne] = static_cast<uint16_t>(pack_bf16x2(t, 0.f) & 0xffffu);
+          else p.out[o_off + ne] = t;
         }
       }
     }
   }
 }
 
-// 64-bit shared-memory matrix descriptor = constant high part | ((address >> 4) & 0x3fff)
-constexpr uint64_t kDescHi = (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-__device__ __forceinline__ uint64_t desc_at(uint32_t addr) { return kDescHi | ((addr >> 4) & 0x3fffu); }
-// same for 32-byte rows with the 32B swizzle (8-row groups 256 B apart): the narrow channel-tail tiles
-constexpr uint64_t kDescHi32 = (1ull << 16) | (16ull << 32) | (1ull << 46) | (6ull << 61);
-__device__ __forceinline__ uint64_t desc32_at(uint32_t addr) { return kDescHi32 | ((addr >> 4) & 0x3fffu); }
-
-// EPI = number of epilogue warps: 4 (one per TMEM lane quadrant) or 8 (two per quadrant, alternating 32-column chunks; only the
-// generic vector-store epilogue: token GEMMs with wide bf16 outputs, whose per-chunk latency is what bounds them)
-// PAIR: the CTA-pair instantiation (clusters of two, tcgen05 cta_group::2). The two CTAs take neighbouring pixel tiles of the
-// same N tile; each loads its own A tile and HALF of the filter rows, the leader (cluster rank 0) issues one M = 256 MMA per
-// k-step over both CTAs' shared memory and tensor memory. Per SM and instruction the tensor pipe then reads 128 + BN / 2
-// operand rows instead of 128 + BN (the MMA rate is bound by that read, profiles/r01_mma_probe.txt) and half the weight
-// bytes come through L2. 3x3 halo mode only.
-template <int EPI, bool PAIR>
-__global__ void __launch_bounds__(64 + 32 * EPI, 1)
-conv_gemm_tf32_kernel(const __grid_constant__ ConvGemmParams p) {
-  constexpr int kEpiWarps = EPI;
-  constexpr int kMma2Warp = -1;
+// BN_T = N tile (wgmma N), MT_T = 128-pixel sub-tiles per CTA tile, BF16 = operand type; the host launches the
+// instantiation equal to (p.BN, p.MT, p.in_bf16). Between the wgmma instructions of a group there is no control flow
+// (ptxas would otherwise serialise them): every k-block issues 4 k-steps, the channel tail of a 128-byte k-block is
+// zero-filled by TMA, and the 3 unused k-steps of a 32-byte tail group read the zero page.
+template <int BN_T, int MT_T, bool BF16>
+__global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t s_bars[4 * kMaxSlots + 6];
-  __shared__ uint32_t s_tmem_base;
+  __shared__ __align__(8) uint64_t s_bars[4 * kMaxSlots];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t smem_a = smem_base;
   const uint32_t smem_b = smem_base + p.a_slots * p.a_slot_bytes;
-  const uint32_t smem_stg = smem_base + static_cast<uint32_t>(p.ring_bytes);
+  const uint32_t smem_zero = smem_base + kRingBytes;
   const uint32_t bar_base = smem_u32(s_bars);
-  // barriers: a_full[8], a_empty[8], b_full[8], b_empty[8], tmem_full[2], tmem_empty[2].
-  // Generic mode uses one ring (A and B tile of a k-block share slot and barriers: the "a" set);
-  // halo mode uses both rings.
+  // barriers: a_full[8], a_empty[8], b_full[8], b_empty[8]. Generic mode uses one ring (A and B tile of a k-block share
+  // slot and barriers: the "a" set); halo mode uses both rings. An empty barrier completes when every MMA warp released it.
   auto a_full = [&](int s) { return bar_base + 8u * s; };
   auto a_empty = [&](int s) { return bar_base + 8u * (kMaxSlots + s); };
   auto b_full = [&](int s) { return bar_base + 8u * (2 * kMaxSlots + s); };
   auto b_empty = [&](int s) { return bar_base + 8u * (3 * kMaxSlots + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (4 * kMaxSlots + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (4 * kMaxSlots + 2 + a); };
-  auto tstart_bar = [&](int a) { return bar_base + 8u * (4 * kMaxSlots + 4 + a); };   // "the tile's first MMA is in the pipe"
 
-  const int warp = threadIdx.x >> 5;
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);   // warp-uniform role
   const int lane = threadIdx.x & 31;
-  const bool dbg_on = p.dbg != nullptr && blockIdx.x == 0;
-  long long w_a = 0, w_b = 0, w_t = 0, w_c = 0;   // debug (w_c: the MMA issuer's commit sections): cycles waited for A slots / B slots / accumulator hand-over by this warp's role
-  const long long t_role0 = dbg_on ? clock64() : 0;
-  if (threadIdx.x == 0) MFR_STAMP(0);
 
-  if (warp == 0 && lane == 0) {
+  for (int i = threadIdx.x; i < kZeroBytes / 16; i += blockDim.x)
+    asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(smem_zero + 16u * i), "r"(0u) : "memory");
+  fence_proxy_async_smem();   // the zero page is read by wgmma (async proxy)
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmB);
-    for (int s = 0; s < 4 * kMaxSlots; ++s) mbar_init(bar_base + 8u * s, 1);
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), kDualIssue ? 2 : 1);   // every MMA issuer commits the accumulator
-      mbar_init(tempty_bar(a), PAIR ? 2 * kEpiWarps : kEpiWarps);   // pair: the epilogue warps of both CTAs report to the leader
-      mbar_init(tstart_bar(a), 1);
+    for (int s = 0; s < kMaxSlots; ++s) {
+      mbar_init(a_full(s), 1);
+      mbar_init(a_empty(s), kMmaWarps);
+      mbar_init(b_full(s), 1);
+      mbar_init(b_empty(s), kMmaWarps);
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    if constexpr (PAIR) {
-      tmem_alloc2(smem_u32(&s_tmem_base), kTmemCols);
-      tmem_relinquish2();
-    } else {
-      tmem_alloc(smem_u32(&s_tmem_base), kTmemCols);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  if constexpr (PAIR) cluster_sync_all();   // the peer's barriers are initialised before anything arrives on them
-  const uint32_t tmem_base = s_tmem_base;
-  if (threadIdx.x == 0) MFR_STAMP(1);
 
   int w_lim = p.Wo, tiles_x = p.tiles_x;
   if (p.dyn_w != nullptr) {
@@ -494,21 +170,9 @@ conv_gemm_tf32_kernel(const __grid_constant__ ConvGemmParams p) {
   }
   const int m_tiles = p.N * p.tiles_y * tiles_x;
   const int total_tiles = m_tiles * p.n_tiles;
-  const int tile_rows = p.MT * p.TH;          // output rows of one CTA tile
-  // work items: tiles (item -> tile), or in multicast mode PAIRS of neighbouring pixel tiles of one N tile
-  // (item -> pair; this CTA takes tile 2*pm + rank of the pair, the last odd one is computed twice)
-  const int crank = PAIR ? static_cast<int>(cluster_ctarank()) : 0;
-  const int pairs_per_nt = (m_tiles + 1) >> 1;
-  const int item_first = PAIR ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int item_step = PAIR ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-  const int item_count = PAIR ? pairs_per_nt * p.n_tiles : total_tiles;
-  // the leader's barriers as seen from either CTA of the pair (shared::cluster addresses)
-  const uint32_t lead_off = PAIR ? mapa_shared(bar_base, 0u) - bar_base : 0u;
+  const int tile_rows = MT_T * p.TH;          // output rows of one CTA tile
   auto item_tile = [&](int item, int& mt, int& nt) {
-    if (PAIR) {
-      nt = item / pairs_per_nt;
-      mt = min(2 * (item - nt * pairs_per_nt) + crank, m_tiles - 1);
-    } else if (p.nt_fast) {   // the N tiles of a pixel tile run at the same time on neighbouring SMs: its A tiles are read from DRAM once
+    if (p.nt_fast) {   // the N tiles of a pixel tile run at the same time on neighbouring SMs: its A tiles are read from DRAM once
       mt = item / p.n_tiles;
       nt = item - mt * p.n_tiles;
     } else {
@@ -516,18 +180,15 @@ conv_gemm_tf32_kernel(const __grid_constant__ ConvGemmParams p) {
       mt = item - nt * m_tiles;
     }
   };
-  // The two issue loops below are executed by whole (converged) warps with elect.sync around the
-  // TMA / MMA instructions, and keep their per-k-block instruction count minimal: with one thread
-  // issuing, instruction latency is what bounds them.
   const int kb_per_tap = p.kb_per_tap, kblk = p.kblk, R = p.R, S = p.S;
-  const int a_slots = p.a_slots, b_slots = p.b_slots, cbatch = p.cbatch;
+  const int a_slots = p.a_slots, b_slots = p.b_slots;
   const uint32_t a_slot_bytes = p.a_slot_bytes, a_bytes = p.a_bytes, b_bytes = p.b_bytes;
 
   if (warp == 0) {
     // ------------------------------------------------------------------ TMA producer
     int sa = 0, sb = 0;
     uint32_t pa = 0, pb = 0;
-    for (int item = item_first; item < item_count; item += item_step) {
+    for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
       int mt, nt;
       item_tile(item, mt, nt);
       const int tx = mt % tiles_x;
@@ -544,33 +205,23 @@ conv_gemm_tf32_kernel(const __grid_constant__ ConvGemmParams p) {
           const CUtensorMap* tmB = tail ? &p.tmB2 : &p.tmB;
           const uint32_t ab = tail ? p.a_bytes2 : a_bytes, bb = tail ? p.b_bytes2 : b_bytes;
           for (int kx = 0; kx < 3; ++kx) {
-            MFR_TIMED_WAIT(w_a, a_empty(sa), pa ^ 1u, 1);
+            mbar_wait_inl(a_empty(sa), pa ^ 1u, 1);
             if (elect_one_sync()) {
-              if constexpr (PAIR) {   // both CTAs' boxes are counted on the leader's barrier
-                if (crank == 0) mbar_arrive_expect_tx(a_full(sa), 2 * ab);
-                tma_load_4d_2sm(smem_a + sa * a_slot_bytes, tmA, a_full(sa) + lead_off, c0, x_in0 + kx, y_in0, img);
-              } else {
-                mbar_arrive_expect_tx(a_full(sa), ab);
-                tma_load_4d(smem_a + sa * a_slot_bytes, tmA, a_full(sa), c0, x_in0 + kx, y_in0, img);
-              }
+              mbar_arrive_expect_tx(a_full(sa), ab);
+              tma_load_4d(smem_a + sa * a_slot_bytes, tmA, a_full(sa), c0, x_in0 + kx, y_in0, img);
             }
             if (++sa == a_slots) { sa = 0; pa ^= 1u; }
             for (int ky = 0; ky < 3; ++ky) {
-              MFR_TIMED_WAIT(w_b, b_empty(sb), pb ^ 1u, 5);
+              mbar_wait_inl(b_empty(sb), pb ^ 1u, 5);
               if (elect_one_sync()) {
-                if constexpr (PAIR) {   // my half of the filter rows (b_bytes = bytes of one half)
-                  if (crank == 0) mbar_arrive_expect_tx(b_full(sb), 2 * bb);
-                  tma_load_3d_2sm(smem_b + sb * b_bytes, tmB, b_full(sb) + lead_off, c0, ky * 3 + kx, n0 + crank * (p.BN >> 1));
-                } else {
-                  mbar_arrive_expect_tx(b_full(sb), bb);
-                  tma_load_3d(smem_b + sb * b_bytes, tmB, b_full(sb), c0, ky * 3 + kx, n0);
-                }
+                mbar_arrive_expect_tx(b_full(sb), bb);
+                tma_load_3d(smem_b + sb * b_bytes, tmB, b_full(sb), c0, ky * 3 + kx, n0);
               }
               if (++sb == b_slots) { sb = 0; pb ^= 1u; }
             }
           }
         }
-      } else if constexpr (!PAIR) {
+      } else {
         const int bz = p.b_batched ? img : -1;
         for (int cb = 0; cb < kb_per_tap; ++cb) {
           const int c0 = cb * kblk;
@@ -581,7 +232,7 @@ conv_gemm_tf32_kernel(const __grid_constant__ ConvGemmParams p) {
           int tap = 0;
           for (int ky = 0; ky < R; ++ky) {
             for (int kx = 0; kx < S; ++kx, ++tap) {
-              MFR_TIMED_WAIT(w_a, a_empty(sa), pa ^ 1u, 1);
+              mbar_wait_inl(a_empty(sa), pa ^ 1u, 1);
               if (elect_one_sync()) {
                 mbar_arrive_expect_tx(a_full(sa), ab);
                 if (p.a_yx) tma_load_4d(smem_a + sa * a_slot_bytes, tmA, a_full(sa), c0, y_in0 + ky, x_in0 + kx, img);
@@ -598,319 +249,123 @@ conv_gemm_tf32_kernel(const __grid_constant__ ConvGemmParams p) {
         }
       }
     }
-  } else if (PAIR && warp == 1 && crank != 0) {
-    // the leader issues the pair's MMAs
-  } else if (warp == 1 || warp == kMma2Warp) {
-    // ------------------------------------------------------------------ MMA issuers
-    // Two warps issue alternate commit groups into the same accumulator: a tcgen05.commit stalls its issuing thread
-    // until the MMAs before it have drained (~215 ns); with a second instruction stream the pipe keeps running
-    // (measured: 12 MMAs per commit cost 96 ns each from one thread, 75 ns from two; profiles/r01_mma_probe2.txt).
-    // Only the very first MMA of a tile overwrites the accumulator, so the issuer that owns the tile's first group
-    // tells the other one (tstart barrier) once that group is in the pipe.
-    const int role = warp == 1 ? 0 : 1;
-    int gcount = 0;                           // commit groups issued so far by both issuers together (parity = owner)
-    const uint32_t idesc = umma_idesc(p.in_bf16 ? 1u : 2u, PAIR ? 2 * kTileM : kTileM, static_cast<uint32_t>(p.BN));
-    const uint32_t idesc_swap = umma_idesc(p.in_bf16 ? 1u : 2u, kTileM, 2u * kTileM);
-    const bool bf16_in = p.in_bf16 != 0;
-    const int MT = p.MT, ksteps_last = p.ksteps_last;
+  } else if (warp >= 4) {
+    // ------------------------------------------------------------------ MMA + epilogue warpgroups
+    const int wg = (warp - 4) >> 2;                   // rows 64 wg .. 64 wg + 63 of each sub-tile
+    const int row0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);
     const uint32_t sub_bytes = static_cast<uint32_t>(p.TH * p.TW * 128);   // A bytes of one 128-row sub-tile
     const uint32_t ky_bytes = static_cast<uint32_t>(p.TW * 128);           // one halo row
+    const bool obf = p.out_bf16 != 0;
+    // two neighbouring channels per store: every element offset even and the base pointers aligned accordingly
+    const bool vec2 = ((p.Cout | p.ldo | p.out_y_stride | p.out_img_stride) & 1) == 0 &&
+                      (reinterpret_cast<uintptr_t>(p.out) & (obf ? 3 : 7)) == 0 &&
+                      (p.residual == nullptr ||
+                       (((p.ldr | p.res_img_stride) & 1) == 0 && (reinterpret_cast<uintptr_t>(p.residual) & (obf ? 3 : 7)) == 0));
+    float acc[MT_T][BN_T / 2];
     int sa = 0, sb = 0;
     uint32_t pa = 0, pb = 0;
-    int it = 0;
-    for (int item = item_first; item < item_count; item += item_step, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1u;
-      MFR_TIMED_WAIT(w_t, tempty_bar(acc), acc_phase ^ 1u, 2);
-      tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + static_cast<uint32_t>(acc * kMaxBN);
-      const bool first_owner = !kDualIssue || (gcount & 1) == role;   // this issuer has the tile's first group
-      uint32_t accum = first_owner ? 0u : 1u;          // first MMA of the tile overwrites the accumulator
-      bool started = first_owner;
-      int g = 0;                                       // group index inside the tile
+    // slots of the wgmma group still in flight: released once the next group is issued and this one has completed
+    int rel_a = -1, rel_b = 0, rel_nb = 0;
+    auto release = [&]() {
+      if (rel_a < 0) return;
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(a_empty(rel_a));
+        int s2 = rel_b;
+        for (int j = 0; j < rel_nb; ++j) {
+          mbar_arrive(b_empty(s2));
+          if (++s2 == b_slots) s2 = 0;
+        }
+      }
+      rel_a = -1;
+    };
+    auto mma = [&](float (&d)[BN_T / 2], uint64_t adesc, uint64_t bdesc) {
+      if constexpr (BF16) wgmma_bf16<BN_T>(d, adesc, bdesc);
+      else wgmma_tf32<BN_T>(d, adesc, bdesc);
+    };
+    const uint64_t zdesc = kDescHi32 | ((smem_zero >> 4) & 0x3fffu);
+    // k-step k of a group whose step 0 is (adesc, bdesc): +32 B of K = +2 in the address field; a tail group has one step
+    auto kdesc = [&](uint64_t d, int k, bool tail) { return (tail && k > 0) ? zdesc : d + 2 * k; };
+    for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
+      int mt, nt;
+      item_tile(item, mt, nt);
+#pragma unroll
+      for (int m = 0; m < MT_T; ++m)
+#pragma unroll
+        for (int i = 0; i < BN_T / 2; ++i) acc[m][i] = 0.f;
       if (p.halo) {
         for (int cb = 0; cb < kb_per_tap; ++cb) {
-          const int nk = cb == kb_per_tap - 1 ? ksteps_last : kBlockK / kUmmaK;
           const bool tail = p.tail32 && cb == kb_per_tap - 1;   // 32-byte rows: one k-step, 32B-swizzle descriptors
           const uint64_t dhi = tail ? kDescHi32 : kDescHi;
+          const uint32_t row_b = tail ? 32u : 128u;
           const uint32_t subb = tail ? sub_bytes >> 2 : sub_bytes, kyb = tail ? ky_bytes >> 2 : ky_bytes;
-          for (int kx = 0; kx < 3; ++kx, ++g) {
-            if (kDualIssue && ((gcount + g) & 1) != role) {   // the other issuer's group: just step over its slots
-              if (++sa == a_slots) { sa = 0; pa ^= 1u; }
-              for (int j = 0; j < 3; ++j)
-                if (++sb == b_slots) { sb = 0; pb ^= 1u; }
-              continue;
-            }
-            if (!started) {
-              mbar_wait(tstart_bar(acc), acc_phase, 9);
-              started = true;
-            }
-            MFR_TIMED_WAIT(w_a, a_full(sa), pa, 3);
-            const uint32_t a_slot = smem_a + sa * a_slot_bytes;
+          for (int kx = 0; kx < 3; ++kx) {
+            mbar_wait_inl(a_full(sa), pa, 3);
+            const uint32_t a_slot = smem_a + sa * a_slot_bytes + static_cast<uint32_t>(64 * wg) * row_b;
             const int sb0 = sb;
+            // all three B tiles of the group are waited for before its first wgmma: no barrier wait between them
+            uint32_t b_addr[3];
             for (int ky = 0; ky < 3; ++ky) {
-              MFR_TIMED_WAIT(w_b, b_full(sb), pb, 6);
-              tc_fence_after();
-              if (!PAIR && p.swap) {
-                if (elect_one_sync()) {   // filters are the M operand, the tile's 256 pixels the N operand
-                  const uint64_t wdesc = dhi | (((smem_b + sb * b_bytes) >> 4) & 0x3fffu);
-                  const uint64_t xdesc = dhi | (((a_slot + ky * kyb) >> 4) & 0x3fffu);
-                  uint32_t acc_m = accum;
-                  for (int k = 0; k < nk; ++k) {
-                    if (bf16_in) tc_mma_bf16(tmem_acc, wdesc + 2 * k, xdesc + 2 * k, idesc_swap, acc_m);
-                    else tc_mma_tf32(tmem_acc, wdesc + 2 * k, xdesc + 2 * k, idesc_swap, acc_m);
-                    acc_m = 1u;
-                  }
-                }
-              } else if (elect_one_sync()) {
-                const uint64_t bdesc = dhi | (((smem_b + sb * b_bytes) >> 4) & 0x3fffu);
-                for (int m = 0; m < MT; ++m) {
-                  const uint64_t adesc = dhi | (((a_slot + m * subb + ky * kyb) >> 4) & 0x3fffu);
-                  const uint32_t d_addr = tmem_acc + static_cast<uint32_t>(m * 128);
-                  uint32_t acc_m = accum;
-                  for (int k = 0; k < nk; ++k) {   // +32 B of K per step = +2 in the descriptor address field
-                    if constexpr (PAIR) {          // the same descriptors address both CTAs' shared memory
-                      if (bf16_in) tc_mma_bf16_2(d_addr, adesc + 2 * k, bdesc + 2 * k, idesc, acc_m);
-                      else tc_mma_tf32_2(d_addr, adesc + 2 * k, bdesc + 2 * k, idesc, acc_m);
-                    } else {
-                      if (bf16_in) tc_mma_bf16(d_addr, adesc + 2 * k, bdesc + 2 * k, idesc, acc_m);
-                      else tc_mma_tf32(d_addr, adesc + 2 * k, bdesc + 2 * k, idesc, acc_m);
-                    }
-                    acc_m = 1u;
-                  }
-                }
-              }
-              accum = 1u;
+              mbar_wait_inl(b_full(sb), pb, 6);
+              b_addr[ky] = smem_b + sb * b_bytes;
               if (++sb == b_slots) { sb = 0; pb ^= 1u; }
             }
-            // one pipeline drain per group: release the three B slots and the A slot together
-            const long long tc0 = dbg_on ? clock64() : 0;
-            if (elect_one_sync()) {
-              int s2 = sb0;
-              if constexpr (PAIR) {   // the slots of both CTAs were read: tell both producers
-                tc_commit2_mcast(b_empty(s2), 3);
-                if (++s2 == b_slots) s2 = 0;
-                tc_commit2_mcast(b_empty(s2), 3);
-                if (++s2 == b_slots) s2 = 0;
-                tc_commit2_mcast(b_empty(s2), 3);
-                tc_commit2_mcast(a_empty(sa), 3);
-              } else {
-                tc_commit(b_empty(s2));
-                if (++s2 == b_slots) s2 = 0;
-                tc_commit(b_empty(s2));
-                if (++s2 == b_slots) s2 = 0;
-                tc_commit(b_empty(s2));
-                tc_commit(a_empty(sa));
+            wgmma_fence();
+#pragma unroll
+            for (int ky = 0; ky < 3; ++ky) {
+              const uint64_t bdesc = dhi | ((b_addr[ky] >> 4) & 0x3fffu);
+#pragma unroll
+              for (int m = 0; m < MT_T; ++m) {
+                const uint64_t adesc = dhi | (((a_slot + m * subb + ky * kyb) >> 4) & 0x3fffu);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) mma(acc[m], kdesc(adesc, k, tail), kdesc(bdesc, k, tail));
               }
             }
-            if (dbg_on) { __syncwarp(); w_c += clock64() - tc0; }
-            if (kDualIssue && g == 0) {                // (first_owner) the tile's first MMAs are queued
-              __syncwarp();
-              if (lane == 0) mbar_arrive(tstart_bar(acc));
-            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            release();
+            rel_a = sa; rel_b = sb0; rel_nb = 3;
             if (++sa == a_slots) { sa = 0; pa ^= 1u; }
           }
         }
-      } else if constexpr (!PAIR) {
+      } else {
         const int num_kb = R * S * kb_per_tap, taps = R * S;
-        int in_batch = 0, batch_first = sa, tap = 0, cb = 0;
+        int tap = 0, cb = 0;
         for (int i = 0; i < num_kb; ++i) {
-          const int nk = cb == kb_per_tap - 1 ? ksteps_last : kBlockK / kUmmaK;
-          ++in_batch;
-          const bool close = in_batch == cbatch || i == num_kb - 1;
-          if (kDualIssue && ((gcount + g) & 1) != role) {     // the other issuer's batch
-            if (++sa == a_slots) { sa = 0; pa ^= 1u; }
-            if (close) { in_batch = 0; batch_first = sa; ++g; }
-            if (++tap == taps) { tap = 0; ++cb; }
-            continue;
+          mbar_wait_inl(a_full(sa), pa, 3);
+          const bool tail = p.tail32 && cb == kb_per_tap - 1;
+          const uint64_t dhi = tail ? kDescHi32 : kDescHi;
+          const uint64_t bdesc = dhi | (((smem_b + sa * b_bytes) >> 4) & 0x3fffu);
+          const uint32_t a_slot = smem_a + sa * a_slot_bytes + static_cast<uint32_t>(64 * wg) * (tail ? 32u : 128u);
+          wgmma_fence();
+#pragma unroll
+          for (int m = 0; m < MT_T; ++m) {
+            const uint64_t adesc = dhi | (((a_slot + m * (tail ? sub_bytes >> 2 : sub_bytes)) >> 4) & 0x3fffu);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) mma(acc[m], kdesc(adesc, k, tail), kdesc(bdesc, k, tail));
           }
-          if (!started) {
-            mbar_wait(tstart_bar(acc), acc_phase, 9);
-            started = true;
-          }
-          MFR_TIMED_WAIT(w_a, a_full(sa), pa, 3);
-          tc_fence_after();
-          if (elect_one_sync()) {
-            const bool tail = p.tail32 && cb == kb_per_tap - 1;
-            const uint64_t dhi = tail ? kDescHi32 : kDescHi;
-            const uint64_t bdesc = dhi | (((smem_b + sa * b_bytes) >> 4) & 0x3fffu);
-            const uint32_t a_slot = smem_a + sa * a_slot_bytes;
-            for (int m = 0; m < MT; ++m) {
-              const uint64_t adesc = dhi | (((a_slot + m * (tail ? sub_bytes >> 2 : sub_bytes)) >> 4) & 0x3fffu);
-              const uint32_t d_addr = tmem_acc + static_cast<uint32_t>(m * 128);
-              uint32_t acc_m = accum;
-              for (int k = 0; k < nk; ++k) {
-                if (bf16_in) tc_mma_bf16(d_addr, adesc + 2 * k, bdesc + 2 * k, idesc, acc_m);
-                else tc_mma_tf32(d_addr, adesc + 2 * k, bdesc + 2 * k, idesc, acc_m);
-                acc_m = 1u;
-              }
-            }
-            if (close) {   // one pipeline drain per batch of k-blocks
-              int s2 = batch_first;
-              for (int j = 0; j < in_batch; ++j) {
-                tc_commit(a_empty(s2));
-                if (++s2 == a_slots) s2 = 0;
-              }
-            }
-          }
-          accum = 1u;
+          wgmma_commit();
+          wgmma_wait<1>();
+          release();
+          rel_a = sa; rel_b = 0; rel_nb = 0;
           if (++sa == a_slots) { sa = 0; pa ^= 1u; }
-          if (close) {
-            if (kDualIssue && g == 0) {                // (first_owner) the tile's first batch is queued
-              __syncwarp();
-              if (lane == 0) mbar_arrive(tstart_bar(acc));
-            }
-            in_batch = 0; batch_first = sa; ++g;
-          }
           if (++tap == taps) { tap = 0; ++cb; }
         }
       }
-      gcount += g;
-      if (elect_one_sync()) {
-        if constexpr (PAIR) tc_commit2_mcast(tfull_bar(acc), 3);   // the accumulator halves of both CTAs are complete
-        else tc_commit(tfull_bar(acc));
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (kEpiWarps warps)
-    const int q = warp & 3;  // TMEM lane quadrant this warp is allowed to read
-    const int c_begin = kEpiWarps == 4 ? 0 : ((warp - 2) >> 2) * 32;   // 8 warps: the two warps of a quadrant alternate chunks
-    const int row = q * 32 + lane;
-    const int ly0 = row / p.TW, lx = row - ly0 * p.TW;
-    const int obf = p.out_bf16;
-    const bool vec_ok = ((p.Cout & 3) == 0) && ((p.ldo & 3) == 0) &&
-                        ((reinterpret_cast<uintptr_t>(p.out) & (obf ? 7 : 15)) == 0) &&
-                        (p.bias == nullptr || (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0) &&
-                        (p.residual == nullptr ||
-                         (((p.ldr & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & (obf ? 7 : 15)) == 0)));
-    float* stg = reinterpret_cast<float*>(smem_raw + (smem_stg - smem_u32(smem_raw))) + (warp - 2) * (32 * kStgStride);
-    const int sub_r = lane >> 3;
-    int it = 0;
-    for (int item = item_first; item < item_count; item += item_step, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1u;
-      int mt, nt;
-      item_tile(item, mt, nt);
+      wgmma_wait<0>();
+#pragma unroll
+      for (int m = 0; m < MT_T; ++m) wgmma_fence_regs(acc[m]);
+      release();
       const int tx = mt % tiles_x;
       const int ty = (mt / tiles_x) % p.tiles_y;
       const int img = mt / (tiles_x * p.tiles_y);
-      const int n0 = nt * p.BN;
-      if (dbg_on) MFR_TIMED_WAIT(w_t, tfull_bar(acc), acc_phase, 4);   // (the epilogue's own wait then falls through)
-      if (p.swap) {
-        const uint32_t taddr_s = tmem_base + static_cast<uint32_t>(acc * kMaxBN) + (static_cast<uint32_t>(q * 32) << 16);
-#define MFR_EPS(ACTV)                                                                                              \
-  do {                                                                                                             \
-    if (p.residual != nullptr) {                                                                                   \
-      if (obf) epilogue_tile_swap<ACTV, true, true>(p, taddr_s, stg, lane, q, tx, ty, img, tile_rows, w_lim, tfull_bar(acc), acc_phase);      \
-      else epilogue_tile_swap<ACTV, true, false>(p, taddr_s, stg, lane, q, tx, ty, img, tile_rows, w_lim, tfull_bar(acc), acc_phase);         \
-    } else {                                                                                                       \
-      if (obf) epilogue_tile_swap<ACTV, false, true>(p, taddr_s, stg, lane, q, tx, ty, img, tile_rows, w_lim, tfull_bar(acc), acc_phase);     \
-      else epilogue_tile_swap<ACTV, false, false>(p, taddr_s, stg, lane, q, tx, ty, img, tile_rows, w_lim, tfull_bar(acc), acc_phase);        \
-    }                                                                                                              \
-  } while (0)
-        switch (p.act) {
-          case ACT_RELU: MFR_EPS(ACT_RELU); break;
-          case ACT_LEAKY: MFR_EPS(ACT_LEAKY); break;
-          case ACT_ELU1: MFR_EPS(ACT_ELU1); break;
-          default: MFR_EPS(ACT_NONE); break;
-        }
-#undef MFR_EPS
-      } else
-      for (int m = 0; m < p.MT; ++m) {
-        const int y = ty * tile_rows + m * p.TH + ly0, x = tx * p.TW + lx;
-        const bool row_ok = (row < p.TW * p.TH) && (y < p.Ho) && (x < w_lim);
-        const long long pix = static_cast<long long>(y) * p.Wo + x;   // pixel inside the image
-        const long long opix = static_cast<long long>(y) * p.out_y_stride + static_cast<long long>(x) * p.ldo;   // its output offset
-        const uint32_t taddr = tmem_base + static_cast<uint32_t>(acc * kMaxBN + m * 128) +
-                               (static_cast<uint32_t>(q * 32) << 16);
-        const bool do_wait = m == 0;
-        if (p.tma_store) {
-          // this warp's 32 pixels: rows q*32 .. q*32+31 of the sub-tile = a (min(TW,32) x 32/min(TW,32)) pixel box
-          const int r0 = q * 32;
-          const int bx = tx * p.TW + (r0 % p.TW);
-          const int by = ty * tile_rows + m * p.TH + r0 / p.TW;
-          const uint32_t stg_t = smem_stg + static_cast<uint32_t>(warp - 2) * 4096u;
-          if (p.tma_store == 2) {
-            const int cb64 = 2 * c_begin;   // 8 warps: the second warp of a quadrant starts at the second 64-channel group
-            switch (p.act) {
-              case ACT_RELU: epilogue_subtile_tma_bf16<ACT_RELU, EPI>(p, taddr, stg_t, lane, n0, bx, by, img, tfull_bar(acc), acc_phase, do_wait, cb64); break;
-              case ACT_LEAKY: epilogue_subtile_tma_bf16<ACT_LEAKY, EPI>(p, taddr, stg_t, lane, n0, bx, by, img, tfull_bar(acc), acc_phase, do_wait, cb64); break;
-              case ACT_ELU1: epilogue_subtile_tma_bf16<ACT_ELU1, EPI>(p, taddr, stg_t, lane, n0, bx, by, img, tfull_bar(acc), acc_phase, do_wait, cb64); break;
-              default: epilogue_subtile_tma_bf16<ACT_NONE, EPI>(p, taddr, stg_t, lane, n0, bx, by, img, tfull_bar(acc), acc_phase, do_wait, cb64); break;
-            }
-          } else
-          switch (p.act) {
-            case ACT_RELU: epilogue_subtile_tma<ACT_RELU>(p, taddr, stg_t, lane, n0, bx, by, img, tfull_bar(acc), acc_phase, do_wait); break;
-            case ACT_LEAKY: epilogue_subtile_tma<ACT_LEAKY>(p, taddr, stg_t, lane, n0, bx, by, img, tfull_bar(acc), acc_phase, do_wait); break;
-            case ACT_ELU1: epilogue_subtile_tma<ACT_ELU1>(p, taddr, stg_t, lane, n0, bx, by, img, tfull_bar(acc), acc_phase, do_wait); break;
-            default: epilogue_subtile_tma<ACT_NONE>(p, taddr, stg_t, lane, n0, bx, by, img, tfull_bar(acc), acc_phase, do_wait); break;
-          }
-        } else if (vec_ok) {
-          // rows this lane stores in the coalesced phase: staged row k*4+sub_r of this warp's 32 pixels
-          long long off_o[8], off_r[8];
-          uint32_t okmask = 0;
 #pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const int rr = k * 4 + sub_r;
-            const long long pr = __shfl_sync(0xffffffffu, pix, rr);
-            okmask |= (__shfl_sync(0xffffffffu, row_ok ? 1 : 0, rr) != 0 ? 1u : 0u) << k;
-            off_o[k] = img * p.out_img_stride + __shfl_sync(0xffffffffu, opix, rr);
-            off_r[k] = img * p.res_img_stride + pr * p.ldr;
-          }
-#define MFR_EPI(ACTV)                                                                                               \
-  do {                                                                                                              \
-    if (p.residual != nullptr) {                                                                                    \
-      if (obf) epilogue_subtile<ACTV, true, true, EPI>(p, taddr, stg, lane, n0, off_o, off_r, okmask, tfull_bar(acc), acc_phase, do_wait, c_begin);   \
-      else epilogue_subtile<ACTV, true, false, EPI>(p, taddr, stg, lane, n0, off_o, off_r, okmask, tfull_bar(acc), acc_phase, do_wait, c_begin);      \
-    } else {                                                                                                        \
-      if (obf) epilogue_subtile<ACTV, false, true, EPI>(p, taddr, stg, lane, n0, off_o, off_r, okmask, tfull_bar(acc), acc_phase, do_wait, c_begin);  \
-      else epilogue_subtile<ACTV, false, false, EPI>(p, taddr, stg, lane, n0, off_o, off_r, okmask, tfull_bar(acc), acc_phase, do_wait, c_begin);     \
-    }                                                                                                               \
-  } while (0)
-          switch (p.act) {
-            case ACT_RELU: MFR_EPI(ACT_RELU); break;
-            case ACT_LEAKY: MFR_EPI(ACT_LEAKY); break;
-            case ACT_ELU1: MFR_EPI(ACT_ELU1); break;
-            default: MFR_EPI(ACT_NONE); break;
-          }
-#undef MFR_EPI
-        } else {
-          if (do_wait) {
-            mbar_wait(tfull_bar(acc), acc_phase, 4);
-            tc_fence_after();
-          }
-          epilogue_subtile_scalar<EPI>(p, taddr, n0, row_ok, img * p.out_img_stride + opix,
-                                  img * p.res_img_stride + pix * p.ldr, c_begin);
-        }
-        if (it == 0 && m == 0 && threadIdx.x == 64) MFR_STAMP(6);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (PAIR) mbar_arrive_cluster(tempty_bar(acc) + lead_off);
-        else mbar_arrive(tempty_bar(acc));
-      }
-      if (it == 0 && threadIdx.x == 64) MFR_STAMP(7);
-    }
-    if (p.tma_store) {   // bulk stores are tracked per issuing thread: every lane may have been elected
-      tma_store_wait<0>();
+      for (int m = 0; m < MT_T; ++m)
+        epilogue_subtile<BN_T>(p, acc[m], row0, lane, nt * p.BN, tx, ty, img, m, tile_rows, w_lim, vec2);
     }
   }
-
-  if (dbg_on && lane == 0 && warp < 3) {   // roles: 0 producer, 1 MMA issuer, 2 first epilogue warp
-    p.dbg[16 + 4 * warp] = w_a; p.dbg[17 + 4 * warp] = w_b; p.dbg[18 + 4 * warp] = w_t; p.dbg[19 + 4 * warp] = clock64() - t_role0;
-    if (warp == 1) p.dbg[28] = w_c;
-  }
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (PAIR) cluster_sync_all();   // no CTA leaves while its peer may still arrive on its barriers / use its tensor memory
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (PAIR) tmem_dealloc2(tmem_base, kTmemCols);
-    else tmem_dealloc(tmem_base, kTmemCols);
-  }
-  if (threadIdx.x == 0) MFR_STAMP(8);
 }
+
 
 // ------------------------------------------------------------------------------------------------
 // host side
@@ -937,21 +392,27 @@ EncodeTiledFn get_encode_fn() {
 
 // Tiling of one op: output tile = MT sub-tiles of TW x TH (<= 128) pixels, BN output channels.
 struct TileCfg {
-  int TW, TH, MT, BN, n_tiles, halo, swap, pair;
+  int TW, TH, MT, BN, n_tiles, halo;
   double cost;
 };
 
-// Cost model used to pick the tiling (ns per CTA tile; constants measured with mfr_debug_mma_probe on B200):
-//   MMA      : one 128 x BN x (32 B of K) tcgen05.mma takes 30.5 + 0.2415 * BN ns when issued back to back;
-//              every tcgen05.commit that releases operand slots drains the pipe, ~215 ns
-//   feed     : operand bytes through L2 -> shared memory at ~100 GB/s per SM when all SMs pull at once
-//   epilogue : ~500 ns per 32-channel chunk of a 128-pixel sub-tile (4 epilogue warps)
+// N tiles the kernel is instantiated for (the wgmma N of one instruction)
+int bn_for(int cols) {
+  for (int bn : {32, 64, 128}) if (cols <= bn) return bn;
+  return 256;
+}
+
+// Relative cost model used to pick the tiling (units ~ ns per CTA tile). The constants are estimates, not measured on
+// an H100; only the ranking of the candidate tilings matters:
+//   MMA      : one 128 x BN x (32 B of K) step, issued as two m64 wgmma, ~ 30 + 0.25 * BN; every wgmma group waits for
+//              its predecessor, ~ 200 per group; a k-block always issues 4 steps
+//   feed     : operand bytes through L2 -> shared memory at ~ 100 bytes per unit per SM when all SMs pull at once
+//   epilogue : ~ 500 per 32-channel chunk of a 128-pixel sub-tile
 // times the number of waves of tiles over the SMs.
-struct RingCfg { int a_slots, b_slots, cbatch, a_slot_bytes; };
-RingCfg ring_cfg(int halo, int MT, int TW, int TH, int BN, int ring_bytes = kRingBytes, int pair = 0) {
-  const int kRingBytes = ring_bytes;      // shadows the constant: the 8-epilogue-warp launches have an 18 KB smaller ring
+struct RingCfg { int a_slots, b_slots, a_slot_bytes; };
+RingCfg ring_cfg(int halo, int MT, int TW, int TH, int BN) {
   RingCfg r{};
-  const int b_bytes = (pair ? BN / 2 : BN) * 128;   // CTA pairs: each CTA holds half of the filter rows
+  const int b_bytes = BN * 128;
   if (halo) {
     r.a_slot_bytes = TW * (MT * TH + 2) * 128;   // multiple of 1 KB (TW % 8 == 0)
     r.a_slots = 3;
@@ -960,35 +421,32 @@ RingCfg ring_cfg(int halo, int MT, int TW, int TH, int BN, int ring_bytes = kRin
       r.a_slots = 2;
       r.b_slots = std::min(kMaxSlots, (kRingBytes - r.a_slots * r.a_slot_bytes) / b_bytes);
     }
-    r.cbatch = 3;
   } else {
     // generic mode pads the A slot to whole 128-row sub-tiles (the MMA reads 128 rows regardless)
     r.a_slot_bytes = std::max((TW * TH * MT * 128 + 1023) / 1024 * 1024, MT * kAStage);
     r.a_slots = r.b_slots = std::min(kMaxSlots, kRingBytes / (r.a_slot_bytes + b_bytes));
-    r.cbatch = std::max(1, std::min(4, r.a_slots / 2));
-    if (const char* e = getenv("MFR_CONV_CBATCH")) r.cbatch = std::max(1, std::min(r.a_slots - 1, atoi(e)));
   }
   return r;
 }
 
 TileCfg choose_cfg(int N, int Ho, int Wo, int Cout, int R, int S, int stride, int pad, int kb_per_tap,
-                   int ksteps_last, bool allow_mt2, int tma_store_cw, bool epi8, bool allow_swap, bool allow_pair,
-                   bool single_row_tiles = false, int ring_bytes = kRingBytes) {
+                   int ksteps_last, bool allow_mt2, bool single_row_tiles = false) {
   const int sms = conv_gemm_num_sms();
   const int c16 = (Cout + 15) / 16 * 16;
   const int taps = R * S;
-  const int ksteps_tap = (kb_per_tap - 1) * 4 + ksteps_last;
+  const int ksteps_tap = kb_per_tap * 4;
+  (void)ksteps_last;
   const bool can_halo = R == 3 && S == 3 && stride == 1 && pad == 1;
   TileCfg best{};
   best.cost = 1e300;
   // test hook: MFR_CONV_FORCE="halo,MT,TW" restricts the search (-1 = free); unusable values fall back to free
-  int f_halo = -1, f_mt = -1, f_tw = -1, f_swap = -1, f_mc = -1;
-  if (const char* e = getenv("MFR_CONV_FORCE")) sscanf(e, "%d,%d,%d,%d,%d", &f_halo, &f_mt, &f_tw, &f_swap, &f_mc);
+  int f_halo = -1, f_mt = -1, f_tw = -1;
+  if (const char* e = getenv("MFR_CONV_FORCE")) sscanf(e, "%d,%d,%d", &f_halo, &f_mt, &f_tw);
   for (int pass = 0; pass < 2 && best.cost > 1e299; ++pass) {
-  if (pass == 1) f_halo = f_mt = f_tw = f_swap = f_mc = -1;
+  if (pass == 1) f_halo = f_mt = f_tw = -1;
   const int nt0 = (c16 + kMaxBN - 1) / kMaxBN;
   for (int nt = nt0; nt <= nt0 * 4; nt *= 2) {
-    const int BN = ((c16 / 16 + nt - 1) / nt) * 16;
+    const int BN = bn_for((c16 + nt - 1) / nt);
     if (nt > nt0 && BN < 64) break;
     for (int halo = 0; halo <= (can_halo ? 1 : 0); ++halo) {
       for (int MT = 1; MT <= 2; ++MT) {
@@ -1005,56 +463,21 @@ TileCfg choose_cfg(int N, int Ho, int Wo, int Cout, int R, int S, int stride, in
           const int box_rows = halo ? MT * th + 2 : MT * th * stride;
           if (box_rows > 256) continue;
           const long long tiles = static_cast<long long>(N) * ((Wo + tw - 1) / tw) * ((Ho + MT * th - 1) / (MT * th)) * nt;
-          const RingCfg rc = ring_cfg(halo, MT, tw, th, BN, ring_bytes);
-          if (rc.a_slots < 2 || rc.b_slots < (halo ? 4 : 2)) continue;
-          const double commits = halo ? 3.0 * kb_per_tap : std::ceil(static_cast<double>(taps) * kb_per_tap / rc.cbatch);
-          const double mma = static_cast<double>(MT) * taps * ksteps_tap * (30.5 + 0.2415 * BN) + commits * 215.0;
+          const RingCfg rc = ring_cfg(halo, MT, tw, th, BN);
+          // the MMA warps hold the slots of one wgmma group while they wait for the next group's: halo groups take 3 B slots
+          if (rc.a_slots < 2 || rc.b_slots < (halo ? 6 : 2)) continue;
+          const double groups = halo ? 3.0 * kb_per_tap : static_cast<double>(taps) * kb_per_tap;
+          const double mma = static_cast<double>(MT) * taps * ksteps_tap * (30.0 + 0.25 * BN) + groups * 200.0;
           const double a_bytes = halo ? static_cast<double>(tw) * (MT * th + 2) * 128.0 * 3 * kb_per_tap
                                       : static_cast<double>(tw) * th * MT * 128.0 * taps * kb_per_tap;
           const double b_bytes = static_cast<double>(BN) * 128.0 * taps * kb_per_tap;
           const double l2 = (a_bytes + b_bytes) / 100.0;
-          // the TMA-store epilogue (fp32 out, power-of-two TW) costs roughly half of the STG one per chunk
-          const bool tma_epi = tma_store_cw > 0 && (tw & (tw - 1)) == 0 && tw >= 8 && tw * th == 128 && (BN % tma_store_cw == 0 || nt == 1);
-          // epilogue per tile (relative costs): per-thread stores ~500 ns per 32-channel chunk, TMA stores half of that per
-          // channel (fp32: 32-channel chunks, bf16: 64-channel groups); with 8 epilogue warps the two warps of a lane
-          // quadrant alternate chunks / groups
-          double epi;
-          if (tma_epi && tma_store_cw == 64) {
-            const int groups = (BN + 63) / 64;
-            epi = MT * (epi8 ? (groups + 1) / 2 : groups) * 500.0;
-          } else {
-            const int chunks = (BN + 31) / 32;
-            epi = MT * (epi8 && !tma_epi ? (chunks + 1) / 2 : chunks) * (tma_epi ? 250.0 : 500.0);
-          }
-          const double t = std::max(mma, std::max(l2, epi)) + 800.0;
+          const double epi = MT * ((BN + 31) / 32) * 500.0;
+          // the epilogue does not overlap the main loop of the same warps: the two add up
+          const double t = std::max(mma, l2) + epi + 800.0;
           const double cost = static_cast<double>((tiles + sms - 1) / sms) * t;
-          if (f_swap != 1 && f_mc != 1 && (cost < best.cost * (1.0 - 1e-9) || (cost < best.cost * (1.0 + 1e-9) && tw > best.TW))) {
-            best = TileCfg{tw, th, MT, BN, nt, halo, 0, 0, cost};
-          }
-          // CTA pairs (cta_group::2): per SM an MMA reads 128 + BN / 2 operand rows (133 B/ns) but cannot beat the math rate
-          // (~0.27 ns per accumulator column); half the weight bytes per CTA through L2
-          // Measured (scripts/pair_check.py, profiles/r02_pair_check.txt): 12-20 % faster than single CTAs on every 3x3 layer
-          // that cannot use the swapped-operand mode, slower than that mode where it applies (Cout <= 128, no residual).
-          const bool swap_applies = c16 <= 128 && allow_swap;
-          if (halo && allow_pair && f_mc != 0 && f_swap != 1 && BN % 16 == 0 && (!swap_applies || f_mc == 1)) {
-            const RingCfg rp = ring_cfg(1, MT, tw, th, BN, ring_bytes, 1);
-            const long long m_tiles_c = tiles / nt;
-            const long long pairs = ((m_tiles_c + 1) / 2) * nt;
-            const double mma_p = static_cast<double>(MT) * taps * ksteps_tap * std::max(30.5 + 0.12075 * BN, 0.27 * BN) + commits * 215.0;
-            const double l2_m = (a_bytes + 0.5 * b_bytes) / 100.0;
-            const double t_m = std::max(mma_p, std::max(l2_m, epi)) + 800.0;
-            const int clusters = sms / 2;
-            const double cost_m = static_cast<double>((pairs + clusters - 1) / clusters) * t_m;
-            if (rp.a_slots >= 2 && rp.b_slots >= 4 && (f_mc == 1 || cost_m < best.cost * (1.0 - 0.03)) && (f_mc != 1 || !best.pair || cost_m < best.cost))
-              best = TileCfg{tw, th, MT, BN, nt, 1, 0, 1, cost_m};
-          }
-          // swapped operands: the MT = 2 halo geometry with the filters as the M operand (Cout <= 128, one N tile)
-          if (halo && MT == 2 && nt == nt0 && c16 <= 128 && allow_swap && f_swap != 0 && (tw & (tw - 1)) == 0) {
-            const double mma_s = static_cast<double>(taps) * ksteps_tap * (30.5 + 0.2415 * 256) + commits * 215.0;
-            const double b_s = 128.0 * 128.0 * taps * kb_per_tap;
-            const double t_s = std::max(mma_s, std::max((a_bytes + b_s) / 100.0, 8 * 500.0)) + 800.0;
-            const double cost_s = static_cast<double>((tiles + sms - 1) / sms) * t_s;
-            if (cost_s < best.cost * (1.0 - 1e-9)) best = TileCfg{tw, th, 2, 128, 1, 1, 1, 0, cost_s};
+          if (cost < best.cost * (1.0 - 1e-9) || (cost < best.cost * (1.0 + 1e-9) && tw > best.TW)) {
+            best = TileCfg{tw, th, MT, BN, nt, halo, cost};
           }
         }
       }
@@ -1062,27 +485,14 @@ TileCfg choose_cfg(int N, int Ho, int Wo, int Cout, int R, int S, int stride, in
   }
   }
   if (getenv("MFR_CONV_DEBUG"))
-    fprintf(stderr, "[conv_gemm cfg] N%d %dx%d Cout%d R%d s%d kb%d -> TW%d TH%d MT%d BN%d nt%d halo%d swap%d pair%d cost %.0f\n", N, Ho, Wo,
-            Cout, R, stride, kb_per_tap, best.TW, best.TH, best.MT, best.BN, best.n_tiles, best.halo, best.swap, best.pair, best.cost);
+    fprintf(stderr, "[conv_gemm cfg] N%d %dx%d Cout%d R%d s%d kb%d -> TW%d TH%d MT%d BN%d nt%d halo%d cost %.0f\n", N, Ho, Wo,
+            Cout, R, stride, kb_per_tap, best.TW, best.TH, best.MT, best.BN, best.n_tiles, best.halo, best.cost);
   return best;
 }
 
 }  // namespace
 
-int conv_gemm_num_sms() {
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 148;
-  }
-  return sms;
-}
-
-static bool pair_allowed() {
-  const char* e = getenv("MFR_CONV_PAIR");
-  return e == nullptr || atoi(e) != 0;
-}
+int conv_gemm_num_sms() { return sm_count(); }
 
 int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
   EncodeTiledFn enc = get_encode_fn();
@@ -1118,23 +528,9 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
     p->tail32 = (p->ksteps_last == 1 && tail * es <= 32 && p->kb_per_tap > 1 && d.b_batched != 2 &&
                  getenv("MFR_CONV_NO_TAIL32") == nullptr) ? 1 : 0;
   }
-  // 8 epilogue warps for token GEMMs with wide bf16 outputs (q|k|v: K = 128 / 256, 384 / 768 output columns, elu+1 on two
-  // thirds of them): their tiles are epilogue-latency bound, two warps per TMEM quadrant halve that. Vector-store path only.
-  const bool epi8 = d.out_bf16 && d.in_bf16 && d.R == 1 && d.S == 1 && d.stride == 1 && d.H == 1 && d.residual == nullptr && !d.b_batched &&
-                    d.Cout >= 256 && (d.Cout % 4 == 0) && (d.ldo % 4 == 0) && getenv("MFR_CONV_EPI4") == nullptr;
-  p->epi_warps = epi8 ? 8 : 4;
-  p->ring_bytes = epi8 ? kRingBytes8 : kRingBytes;
   const TileCfg cfg = choose_cfg(d.N, p->Ho, p->Wo, d.Cout, d.R, d.S, d.stride, d.pad, p->kb_per_tap, p->ksteps_last,
-                                 d.dyn_w == nullptr && d.b_batched != 2,
-                                 d.residual != nullptr ? 0 : (d.out_bf16 ? 64 : 32),   // channels per chunk of the TMA-store epilogue
-                                 epi8,
-                                 // swapped operands: not with a residual (measured: its transposed epilogue then becomes the bottleneck)
-                                 (d.Cout % 4 == 0) && (d.ldo % 4 == 0) && !d.b_batched &&
-                                     (d.residual == nullptr || (getenv("MFR_CONV_FORCE") != nullptr && d.ldr % 4 == 0)),
-                                 // CTA pairs (cta_group::2) for the 3x3 halo mode; MFR_CONV_PAIR=0 switches them off
-                                 !d.b_batched && d.dyn_w == nullptr && pair_allowed(),
-                                 d.b_batched == 2, p->ring_bytes);
-  p->TW = cfg.TW; p->TH = cfg.TH; p->MT = cfg.MT; p->halo = cfg.halo; p->swap = cfg.swap; p->pair = cfg.pair;
+                                 d.dyn_w == nullptr && d.b_batched != 2, d.b_batched == 2);
+  p->TW = cfg.TW; p->TH = cfg.TH; p->MT = cfg.MT; p->halo = cfg.halo;
   p->BN = cfg.BN; p->n_tiles = cfg.n_tiles;
   p->nt_fast = (!p->halo && p->n_tiles > 1 && getenv("MFR_CONV_NT_SLOW") == nullptr) ? 1 : 0;
   p->tiles_x = (p->Wo + p->TW - 1) / p->TW;
@@ -1144,12 +540,12 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
   p->b_batched = d.b_batched;
   const int a_rows = p->halo ? p->MT * p->TH + 2 : p->MT * p->TH;   // pixel rows of the A box
   p->a_bytes = p->TW * a_rows * 128;
-  p->b_bytes = (p->pair ? p->BN / 2 : p->BN) * 128;                // multiple of 1 KB (BN % 16 == 0); CTA pairs: one CTA's half
+  p->b_bytes = p->BN * 128;                                           // multiple of 1 KB (BN % 8 == 0)
   {
-    const RingCfg rc = ring_cfg(p->halo, p->MT, p->TW, p->TH, p->BN, p->ring_bytes, p->pair);
-    p->a_slot_bytes = rc.a_slot_bytes; p->a_slots = rc.a_slots; p->b_slots = rc.b_slots; p->cbatch = rc.cbatch;
+    const RingCfg rc = ring_cfg(p->halo, p->MT, p->TW, p->TH, p->BN);
+    p->a_slot_bytes = rc.a_slot_bytes; p->a_slots = rc.a_slots; p->b_slots = rc.b_slots;
   }
-  if (p->a_slots < 2 || p->b_slots < 2) return MFR_ERR_ARG;
+  if (p->a_slots < 2 || p->b_slots < (p->halo ? 6 : 2)) return MFR_ERR_ARG;
   p->act = d.act;
   p->act_cols = d.act_cols > 0 ? d.act_cols : d.Cout;
   p->dyn_w = d.dyn_w;
@@ -1164,7 +560,6 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
   p->out_img_stride = d.out_img_stride > 0 ? d.out_img_stride : static_cast<long long>(p->Ho) * p->Wo * d.ldo;
   p->b_xor = d.b_xor;
   p->res_img_stride = static_cast<long long>(p->Ho) * p->Wo * d.ldr;
-  p->dbg = nullptr;
 
   {  // activations: {C, W, H, N}
     cuuint64_t dims[4] = {(cuuint64_t)d.Cin, (cuuint64_t)d.W, (cuuint64_t)d.H, (cuuint64_t)d.N};
@@ -1195,36 +590,6 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       if (r != CUDA_SUCCESS) p->tail32 = 0;
     }
-  }
-  {  // TMA-store epilogue: output without residual, power-of-two TW, whole 32-channel (fp32) / 64-channel (bf16) chunks per N tile
-    const bool pow2 = (p->TW & (p->TW - 1)) == 0;
-    const int oes = d.out_bf16 ? 2 : 4, cw = d.out_bf16 ? 64 : 32;   // output element size, channels per stored chunk
-    const bool ok = !p->swap && d.residual == nullptr && pow2 && p->TW >= 8 && p->TW * p->TH == 128 &&
-                    (p->BN % cw == 0 || p->n_tiles == 1) && (p->act_cols % 32 == 0 || p->act_cols >= d.Cout) &&
-                    (d.ldo * oes % 16 == 0) && (reinterpret_cast<uintptr_t>(d.out) & 15) == 0 && (d.Cout % 4 == 0) &&
-                    // the store engine writes whole 16-byte units: with bf16 outputs and Cout % 8 != 0 the (zero) values of up to 7
-                    // channels past Cout land in the row — allowed only when those are the row's own padding (ldo = Cout rounded up to 8)
-                    (!d.out_bf16 || d.Cout % 8 == 0 || d.ldo == (d.Cout + 7) / 8 * 8) &&
-                    (p->out_img_stride * oes % 16 == 0) && (p->out_y_stride * oes % 16 == 0) &&
-                    (d.bias == nullptr || (reinterpret_cast<uintptr_t>(d.bias) & 15) == 0) &&
-                    !(d.out_bf16 && p->epi_warps == 8 && getenv("MFR_CONV_EPI8") != nullptr) &&
-                    !(d.out_bf16 && getenv("MFR_CONV_NO_TMA_STORE_BF16") != nullptr) && getenv("MFR_CONV_NO_TMA_STORE") == nullptr;
-    p->tma_store = ok ? (d.out_bf16 ? 2 : 1) : 0;
-    if (ok) {
-      const int bw = std::min(p->TW, 32);
-      cuuint64_t dims[4] = {(cuuint64_t)d.Cout, (cuuint64_t)p->Wo, (cuuint64_t)p->Ho, (cuuint64_t)d.N};
-      cuuint64_t strides[3] = {(cuuint64_t)d.ldo * oes, (cuuint64_t)p->out_y_stride * oes, (cuuint64_t)p->out_img_stride * oes};
-      cuuint32_t box[4] = {(cuuint32_t)cw, (cuuint32_t)bw, (cuuint32_t)(32 / bw), 1};
-      cuuint32_t estr[4] = {1, 1, 1, 1};
-      CUresult r = enc(&p->tmC, d.out_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, d.out, dims, strides, box,
-                       estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) p->tma_store = 0;   // e.g. strides the tensor map cannot express: keep the STG epilogue
-      if (getenv("MFR_CONV_DEBUG") && r != CUDA_SUCCESS) fprintf(stderr, "[conv_gemm cfg] store tensor map rejected (%d)\n", (int)r);
-    }
-    if (getenv("MFR_CONV_DEBUG"))
-      fprintf(stderr, "[conv_gemm cfg] Cout%d ldo%lld out_bf16 %d res %d TW%d TH%d BN%d nt%d act_cols %d epi %d -> tma_store %d\n", d.Cout, d.ldo,
-              d.out_bf16, d.residual != nullptr, p->TW, p->TH, p->BN, p->n_tiles, p->act_cols, p->epi_warps, p->tma_store);
   }
   {  // weights: {Cin, Z, Cout}; Z = tap (shared weights) or image (batched B operand)
     const int taps = d.R * d.S;
@@ -1260,7 +625,7 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
       strides[0] = (cuuint64_t)ldw_e * es;
       strides[1] = (cuuint64_t)ldw_e * es * taps;
     }
-    cuuint32_t box[3] = {(cuuint32_t)kblk, 1, (cuuint32_t)(p->pair ? p->BN / 2 : p->BN)};   // CTA pairs: each CTA loads half of the filter rows
+    cuuint32_t box[3] = {(cuuint32_t)kblk, 1, (cuuint32_t)p->BN};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = enc(&p->tmB, d.in_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3,
                      const_cast<float*>(d.w), dims,
@@ -1285,270 +650,48 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
   return MFR_OK;
 }
 
-int conv_gemm_launch(const ConvGemmParams& p, cudaStream_t stream) {
+namespace {
+template <int BN_T, int MT_T, bool BF16>
+int launch_one(const ConvGemmParams& p, int grid, cudaStream_t stream) {
   static bool attr_seen[64] = {};
-  if (first_call_on_device(attr_seen)) {
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_tf32_kernel<4, false>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_tf32_kernel<8, false>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_tf32_kernel<4, true>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-  }
-  const int total = p.N * p.tiles_y * p.tiles_x * p.n_tiles;
-  if (total <= 0) return MFR_OK;
-  if (p.pair) {   // clusters of two CTAs, one pair of pixel tiles per cluster iteration
-    const int m_tiles = p.N * p.tiles_y * p.tiles_x;
-    const int pairs = ((m_tiles + 1) / 2) * p.n_tiles;
-    const int clusters = std::min(pairs, (p.grid_limit > 0 ? std::min(p.grid_limit, conv_gemm_num_sms()) : conv_gemm_num_sms()) / 2);
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(2 * clusters));
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = kSmemBytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr{};
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = 1;
-    MFR_CUDA_CHECK(cudaLaunchKernelEx(&cfg, conv_gemm_tf32_kernel<4, true>, p));
-    return MFR_OK;
-  }
-  const int grid = std::min(total, p.grid_limit > 0 ? std::min(p.grid_limit, conv_gemm_num_sms()) : conv_gemm_num_sms());
-  if (p.epi_warps == 8 && !p.swap && p.tma_store != 1) conv_gemm_tf32_kernel<8, false><<<grid, 64 + 32 * 8, kSmemBytes, stream>>>(p);
-  else conv_gemm_tf32_kernel<4, false><<<grid, kThreads, kSmemBytes, stream>>>(p);
+  if (first_call_on_device(attr_seen))
+    MFR_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_kernel<BN_T, MT_T, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+  conv_gemm_kernel<BN_T, MT_T, BF16><<<grid, kThreads, kSmemBytes, stream>>>(p);
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
 }
-
-// ------------------------------------------------------------------------------------------------
-// launch-overhead probes (debug): same launch shape as the GEMM kernel, progressively more set-up
-// ------------------------------------------------------------------------------------------------
-namespace {
-__global__ void __launch_bounds__(kThreads, 1) overhead_probe_kernel(int mode, int* sink) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t s_bars[4 * kMaxSlots + 4];
-  __shared__ uint32_t s_tmem_base;
-  if (mode == 0) return;
-  const int warp = threadIdx.x >> 5;
-  if (mode >= 2 && threadIdx.x == 0) {
-    for (int s = 0; s < 4 * kMaxSlots + 4; ++s) mbar_init(smem_u32(s_bars) + 8u * s, 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(smem_u32(&s_tmem_base), kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (mode >= 3 && threadIdx.x == 0 && sink != nullptr) smem_raw[0] = static_cast<uint8_t>(*sink);
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(s_tmem_base, kTmemCols);
+template <int BN_T, int MT_T>
+int launch_inst(const ConvGemmParams& p, int grid, cudaStream_t stream) {
+  return p.in_bf16 ? launch_one<BN_T, MT_T, true>(p, grid, stream) : launch_one<BN_T, MT_T, false>(p, grid, stream);
 }
 }  // namespace
 
-namespace {
-// Tensor-pipe probe: operands static in shared memory (no TMA), one thread issues `n_per_commit`
-// 128 x BN x (32 B of K) MMAs followed by one tcgen05.commit, `iters` times; optionally waits for
-// every commit before issuing the next group (the dependency a 1-slot ring would impose).
-__global__ void __launch_bounds__(kThreads, 1) mma_probe_kernel(int n_per_commit, int BN, int bf16, int wait_each,
-                                                                 int iters, int two_commits) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t mfr_probe_bars_s[6];
-  uint64_t* mfr_probe_bars = mfr_probe_bars_s;
-  __shared__ uint32_t s_tmem_base;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  if (threadIdx.x == 0) {
-    for (int k = 0; k < 6; ++k) mbar_init(smem_u32(&mfr_probe_bars[k]), 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(smem_u32(&s_tmem_base), kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem_base;
-  // two_commits == 2 / 3: TWO issuing threads (warps 1 and 2) run the same loop concurrently, into the same (2) or into
-  // different (3) accumulators — does a second instruction stream keep the pipe busy while the first sits at its commit?
-  const bool second = two_commits >= 2 && warp == 2 && lane == 0;
-  if ((warp == 1 && lane == 0) || second) {
-    const uint32_t idesc = umma_idesc(bf16 ? 1u : 2u, kTileM, static_cast<uint32_t>(BN));
-    const uint32_t a_addr = smem_base + (second ? 96 * 1024 : 0), b_addr = smem_base + 64 * 1024;
-    const uint32_t tmem_base = s_tmem_base + ((second && two_commits == 3) ? 256u : 0u);
-    uint64_t* s_bar = mfr_probe_bars + (second ? 3 : 0);
-    uint32_t phase = 0;
-    for (int it = 0; it < iters; ++it) {
-      for (int k = 0; k < n_per_commit; ++k) {
-        const uint32_t off = static_cast<uint32_t>((k & 3) * 32 + (k >> 2) * 16384) & 0xffffu;
-        const uint64_t adesc = umma_desc_sw128_kmajor(a_addr + off);
-        const uint64_t bdesc = umma_desc_sw128_kmajor(b_addr + ((k & 3) * 32));
-        if (bf16) tc_mma_bf16(tmem_base, adesc, bdesc, idesc, 1u);
-        else tc_mma_tf32(tmem_base, adesc, bdesc, idesc, 1u);
-      }
-      tc_commit(smem_u32(&s_bar[0]));
-      if (two_commits == 1) tc_commit(smem_u32(&s_bar[2]));
-      if (wait_each) {
-        mbar_wait(smem_u32(&s_bar[0]), phase, 7);
-        phase ^= 1u;
-      }
+int conv_gemm_launch(const ConvGemmParams& p, cudaStream_t stream) {
+  const int total = p.N * p.tiles_y * p.tiles_x * p.n_tiles;
+  if (total <= 0) return MFR_OK;
+  const int grid = std::min(total, p.grid_limit > 0 ? std::min(p.grid_limit, conv_gemm_num_sms()) : conv_gemm_num_sms());
+  if (p.MT == 2) {
+    switch (p.BN) {
+      case 32: return launch_inst<32, 2>(p, grid, stream);
+      case 64: return launch_inst<64, 2>(p, grid, stream);
+      case 128: return launch_inst<128, 2>(p, grid, stream);
     }
-    tc_commit(smem_u32(&s_bar[1]));
-    mbar_wait(smem_u32(&s_bar[1]), 0u, 8);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
-}
-}  // namespace
-
-// ns per MMA instruction of the probe above (CUDA events around one launch of `grid` CTAs).
-// CTA-pair version of the probe: clusters of two, the leader issues M = 256 cta_group::2 MMAs over both CTAs' (uninitialised,
-// resident) shared memory; ns per MMA as above.
-__global__ void __launch_bounds__(kThreads, 1) mma_probe_pair_kernel(int n_per_commit, int BN, int bf16, int iters) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bars[2];
-  __shared__ uint32_t s_tmem_base;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  if (threadIdx.x == 0) {
-    mbar_init(smem_u32(&bars[0]), 1); mbar_init(smem_u32(&bars[1]), 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc2(smem_u32(&s_tmem_base), kTmemCols);
-    tmem_relinquish2();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  cluster_sync_all();
-  const uint32_t tmem_base = s_tmem_base;
-  if (warp == 1 && lane == 0 && cluster_ctarank() == 0) {
-    const uint32_t idesc = umma_idesc(bf16 ? 1u : 2u, 2 * kTileM, static_cast<uint32_t>(BN));
-    const uint32_t a_addr = smem_base, b_addr = smem_base + 64 * 1024;
-    for (int it = 0; it < iters; ++it) {
-      for (int k = 0; k < n_per_commit; ++k) {
-        const uint32_t off = static_cast<uint32_t>((k & 3) * 32 + (k >> 2) * 16384) & 0xffffu;
-        const uint64_t adesc = umma_desc_sw128_kmajor(a_addr + off);
-        const uint64_t bdesc = umma_desc_sw128_kmajor(b_addr + ((k & 3) * 32));
-        if (bf16) tc_mma_bf16_2(tmem_base, adesc, bdesc, idesc, 1u);
-        else tc_mma_tf32_2(tmem_base, adesc, bdesc, idesc, 1u);
-      }
-      tc_commit2_mcast(smem_u32(&bars[0]), 1);
+  } else if (p.MT == 1) {
+    switch (p.BN) {
+      case 32: return launch_inst<32, 1>(p, grid, stream);
+      case 64: return launch_inst<64, 1>(p, grid, stream);
+      case 128: return launch_inst<128, 1>(p, grid, stream);
+      case 256: return launch_inst<256, 1>(p, grid, stream);
     }
-    tc_commit2_mcast(smem_u32(&bars[1]), 1);
-    mbar_wait(smem_u32(&bars[1]), 0u, 8);
   }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, kTmemCols);
-  }
-}
-
-static void launch_probe_pair(int grid, int n_per_commit, int BN, int bf16, int iters) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(grid & ~1));
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = kSmemBytes;
-  cudaLaunchAttribute attr{};
-  attr.id = cudaLaunchAttributeClusterDimension;
-  attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-  cfg.attrs = &attr;
-  cfg.numAttrs = 1;
-  cudaLaunchKernelEx(&cfg, mma_probe_pair_kernel, n_per_commit, BN, bf16, iters);
-}
-
-float conv_gemm_mma_probe(int n_per_commit, int BN, int bf16, int wait_each, int iters, int grid, int two_commits) {
-  if (two_commits == 4) {   // CTA pairs
-    cudaFuncSetAttribute(mma_probe_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-    if (grid < 2) grid = 2;
-    cudaEvent_t e0, e1;
-    cudaEventCreate(&e0);
-    cudaEventCreate(&e1);
-    launch_probe_pair(grid, n_per_commit, BN, bf16, 10);
-    cudaEventRecord(e0);
-    launch_probe_pair(grid, n_per_commit, BN, bf16, iters);
-    cudaEventRecord(e1);
-    cudaEventSynchronize(e1);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    if (cudaGetLastError() != cudaSuccess) return -1.f;
-    return ms * 1e6f / (static_cast<float>(iters) * n_per_commit);
-  }
-  cudaFuncSetAttribute(mma_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0);
-  cudaEventCreate(&e1);
-  mma_probe_kernel<<<grid, kThreads, kSmemBytes>>>(n_per_commit, BN, bf16, wait_each, 10, two_commits);
-  cudaEventRecord(e0);
-  mma_probe_kernel<<<grid, kThreads, kSmemBytes>>>(n_per_commit, BN, bf16, wait_each, iters, two_commits);
-  cudaEventRecord(e1);
-  cudaEventSynchronize(e1);
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, e0, e1);
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  if (cudaGetLastError() != cudaSuccess) return -1.f;
-  return ms * 1e6f / (static_cast<float>(iters) * n_per_commit);
-}
-
-float conv_gemm_probe_overhead(int mode, int smem_bytes, int grid, int iters, cudaStream_t st) {
-  cudaFuncSetAttribute(overhead_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0);
-  cudaEventCreate(&e1);
-  for (int i = 0; i < 5; ++i) overhead_probe_kernel<<<grid, kThreads, smem_bytes, st>>>(mode, nullptr);
-  cudaEventRecord(e0, st);
-  for (int i = 0; i < iters; ++i) overhead_probe_kernel<<<grid, kThreads, smem_bytes, st>>>(mode, nullptr);
-  cudaEventRecord(e1, st);
-  cudaEventSynchronize(e1);
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, e0, e1);
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  return ms * 1000.f / iters;
+  fprintf(stderr, "[mfr_b200] conv_gemm: no kernel for BN %d MT %d\n", p.BN, p.MT);
+  return MFR_ERR_UNSUPPORTED;
 }
 
 float conv_gemm_time_prebuilt(const ConvGemmParams& p, int iters, cudaStream_t st) {
-  {  // one instrumented launch: milestone stamps of block 0
-    long long* d = nullptr;
-    cudaMalloc(&d, 32 * sizeof(long long));
-    cudaMemset(d, 0, 32 * sizeof(long long));
-    ConvGemmParams q = p;
-    q.dbg = d;
-    conv_gemm_launch(q, st);
-    cudaStreamSynchronize(st);
-    cudaMemset(d, 0, 32 * sizeof(long long));
-    conv_gemm_launch(q, st);
-    cudaStreamSynchronize(st);
-    long long h[32];
-    cudaMemcpy(h, d, sizeof(h), cudaMemcpyDeviceToHost);
-    cudaFree(d);
-    const char* names[13] = {"start", "setup done", "first TMA issued", "last TMA issued", "first stage landed",
-                             "last stage landed", "accumulator ready", "epilogue done", "exit", "c0 begin",
-                             "c0 tmem loaded", "c0 staged", "c0 stored"};
-    fprintf(stderr, "[conv_gemm stamps, block 0, ns since start]");
-    for (int i = 0; i < 13; ++i) fprintf(stderr, " %s=%lld", names[i], h[i] ? h[i] - h[0] : -1);
-    fprintf(stderr, "\n[conv_gemm cfg] TW%d TH%d MT%d BN%d nt%d halo%d swap%d pair%d slots %d/%d cbatch %d\n", p.TW, p.TH, p.MT, p.BN,
-            p.n_tiles, p.halo, p.swap, p.pair, p.a_slots, p.b_slots, p.cbatch);
-    const char* roles[3] = {"producer", "mma", "epilogue warp 2"};
-    for (int r = 0; r < 3; ++r)
-      fprintf(stderr, "[conv_gemm waits, block 0, %s] cycles total %lld: A-slot wait %lld, B-slot wait %lld, accumulator wait %lld\n", roles[r],
-              h[19 + 4 * r], h[16 + 4 * r], h[17 + 4 * r], h[18 + 4 * r]);
-    fprintf(stderr, "[conv_gemm waits, block 0, mma] cycles in commit sections %lld\n", h[28]);
-  }
+  if (getenv("MFR_CONV_DEBUG"))
+    fprintf(stderr, "[conv_gemm cfg] TW%d TH%d MT%d BN%d nt%d halo%d slots %d/%d\n", p.TW, p.TH, p.MT, p.BN, p.n_tiles, p.halo,
+            p.a_slots, p.b_slots);
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0);
   cudaEventCreate(&e1);

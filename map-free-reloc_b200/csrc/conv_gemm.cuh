@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution / GEMM on the 5th-gen tensor cores (tcgen05, TF32 in, fp32 accumulate).
+// Implicit-GEMM convolution / GEMM on the Hopper tensor cores (wgmma, TF32 or BF16 in, fp32 accumulate).
 //
 // One kernel serves every GEMM-shaped op of the matcher networks:
 //   * 3x3 / 1x1 convolutions over NHWC activations (stride 1 or 2, zero padding),
@@ -18,34 +18,23 @@ struct alignas(64) ConvGemmParams {
   CUtensorMap tmB;  // rank 3 {Cin, Z, Cout} box {32, 1, BN}          (Z = filter tap or image)
   CUtensorMap tmA2; // channel tail (tail32): same tensors, 32-byte-wide boxes, 32B swizzle — the last k-block of a tap then moves
   CUtensorMap tmB2; //   a quarter of the bytes (Cin = 196 leaves 4 channels for it) and issues one MMA per tap
-  CUtensorMap tmC;  // rank 4 {Cout, Wo, Ho, N} fp32, box {32, min(TW,32), 32/min(TW,32), 1}, 128B swizzle (TMA-store epilogue)
   int N, Ho, Wo, Cout, Cin;
   int R, S, stride, pad;
   int TW, TH, tiles_x, tiles_y;
-  int BN, n_tiles, kb_per_tap, b_batched;
+  int BN, n_tiles, kb_per_tap, b_batched;   // BN: 32, 64, 128 or 256 (the wgmma N)
   int a_bytes, b_bytes;   // TMA transaction bytes of one A / B load
-  int MT;                 // 128-pixel sub-tiles per CTA tile (2 only when BN <= 128: 2 x 2 x 128 TMEM columns)
+  int MT;                 // 128-pixel sub-tiles per CTA tile (2 only when BN <= 128: the accumulators of a tile are registers)
   int halo;               // 3x3 stride-1 conv: A is loaded as a (MT*TH+2)-row box per (k-block, kx) and the three
                           // ky taps read it at row offsets 0, TW, 2*TW (TW % 8 == 0 keeps the swizzle phase)
-  int swap;               // halo mode with swapped operands (Cout <= 128): M = 128 filters, N = the 256 pixels of the tile —
-                          // one N = 256 MMA per k-step instead of two N = 128 ones (92 ns vs 2 x 61 ns); TMEM lane = filter
-  int pair;               // halo mode in clusters of two CTAs (cta_group::2): the pair works on neighbouring pixel tiles of the same N tile
-                          // and the leader issues M = 256 MMAs over both CTAs' shared / tensor memory; each CTA loads its own A
-                          // tile and HALF of the filter rows (b_bytes = that half): the tensor pipe reads 128 + BN / 2 operand
-                          // rows per SM and MMA instead of 128 + BN, half the weight bytes come through L2
   int a_slots, b_slots;   // depth of the A ring / B ring (two rings: one A slot serves 3 B tiles in halo mode)
   int a_slot_bytes;
-  int epi_warps;          // 4, or 8 for token GEMMs with wide bf16 outputs (two warps per TMEM lane quadrant)
-  int ring_bytes;         // operand ring size (the 8-warp epilogue takes its second staging area out of the ring)
   int grid_limit;         // > 0: at most this many CTAs (the engine leaves SMs to the pose back end of the previous batch during the first layers)
   int nt_fast;            // work-item order: N tile index fastest (generic mode with several N tiles: the A tiles of a pixel tile stay in L2)
-  int tma_store;          // epilogue writes 32 px x 32 ch fp32 chunks with cp.async.bulk.tensor stores (see conv_gemm.cu)
-  int cbatch;             // generic mode: k-blocks whose slots are released by one tcgen05.commit batch (pipe drain)
   int ksteps_last;        // MMAs issued for the last k-block of a tap (channel tail)
   int tail32;             // the tail fits one 32-byte k-step: it is loaded through tmA2 / tmB2 (a_bytes2 / b_bytes2 per load)
   int a_bytes2, b_bytes2;
   int act, act_cols;    // activation applies to output channels < act_cols
-  int in_bf16, out_bf16;  // operands bf16 (kind::f16) instead of fp32 (kind::tf32); out/residual bf16
+  int in_bf16, out_bf16;  // operands bf16 instead of fp32 (tf32 MMA); out/residual bf16
   int kblk;             // K elements per 128-byte k-block: 32 (fp32) or 64 (bf16)
   const int* dyn_w;     // optional device int: effective W (rows of a token GEMM), H must be 1
   float alpha;
@@ -58,7 +47,6 @@ struct alignas(64) ConvGemmParams {
   int b_xor;
   int a_yx, b_yx;                            // tensor map dims 1 and 2 swapped (row stride smaller than the pixel / filter-row stride:
                                              // attention heads interleaved inside a token row) -> coordinate order (c, y, x|n, img)
-  long long* dbg;       // optional: block 0 writes globaltimer stamps (ns) at pipeline milestones
 };
 
 // Describes one op; build once (tensor maps are encoded on the host), launch many times.
@@ -89,8 +77,6 @@ struct ConvGemmDesc {
 int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p);
 int conv_gemm_launch(const ConvGemmParams& p, cudaStream_t stream);
 int conv_gemm_num_sms();
-float conv_gemm_probe_overhead(int mode, int smem_bytes, int grid, int iters, cudaStream_t st);
-float conv_gemm_mma_probe(int n_per_commit, int BN, int bf16, int wait_each, int iters, int grid, int two_commits);
 float conv_gemm_time_prebuilt(const ConvGemmParams& p, int iters, cudaStream_t st);
 
 }  // namespace mfr

@@ -1,444 +1,276 @@
-// Fused tail of a LoFTREncoderLayer on the 5th-gen tensor cores (sm_100a, bf16 engine mode).
+// Fused LoFTREncoderLayer tail (bf16 engine mode) on wgmma. See encoder_tail.cuh for the op.
 //
-// Reference (LoFTR/src/loftr/loftr_module/transformer.py:52-58), per token row:
-//     m  = LayerNorm1(message @ Wm^T)                       merge + norm1
-//     h  = relu([x | m] @ W0^T)                             mlp.0 on the concatenation (2C -> 2C)
-//     x += LayerNorm2(h @ W2^T)                             mlp.2 (2C -> C) + norm2 + residual
-// Unfused this is 3 GEMM launches + 2 LayerNorm launches whose intermediates (merge output, norm1 output, the 2C-wide
-// hidden tensor, the mlp.2 output) each make a round trip through HBM: ~7 KB of the ~14 KB a token row moves per layer.
-// Rows are independent, so one persistent CTA per SM takes 128-row tiles through the whole chain with every
-// intermediate kept on chip:
-//
-//   TMEM   D3  [128 x C]  fp32   accumulator of GEMM3 (mlp.2), columns [0, C)
-//          scratch, 256 columns  D1 = accumulator of GEMM1 (merge); once LayerNorm1 has consumed it, the two D2 buffers
-//                                [128 x 128] = double-buffered accumulator of GEMM2 (mlp.0), one 128-column chunk q of the hidden layer
-//   SMEM   L   [128 x C]  bf16   LayerNorm1 output = k-blocks C/64 .. 2C/64-1 of GEMM2's A operand (K-major, 128B swizzle)
-//          M   64 KB             two [128 x 128] bf16 buffers H1[q & 1]: relu(D2_q), the A operand of GEMM3
-//          ring of 16 KB slots   every streamed tile [128 rows x 64 bf16]: message / x k-blocks of this row tile and 128
-//                                filter rows of a weight k-block, by TMA from L2 (6-8 slots in flight: the per-tile traffic
-//                                of ~1.1 MB needs depth, not width, to hide the L2 latency)
-//
-//   warp 0     TMA producer: the ring items in exactly the order the MMA warp consumes them
-//   warp 1     MMA issuer  : GEMM1; then GEMM2 chunk q+1 is issued BEFORE GEMM3 chunk q, so the tensor pipe runs the
-//                            next chunk while the epilogue warps turn chunk q into the bf16 A operand of GEMM3
-//   warps 2-5  front epilogue, thread = row: LayerNorm1 (TMEM -> registers -> swizzled smem), relu + bf16 (TMEM -> smem)
-//   warps 6-9  back epilogue, thread = row: LayerNorm2 + residual of the PREVIOUS tile (TMEM -> staging -> coalesced fp32
-//              store of x and its bf16 shadow; the residual rows are prefetched a chunk ahead) while the front group and
-//              the tensor pipe already work on the next tile
-//
-// The hidden layer is produced and consumed in 128-column chunks because GEMM3 accumulates over exactly those
-// columns: D3 += relu(D2_q) @ W2[:, q]^T can start as soon as chunk q exists, and 2C-wide rows never exist anywhere.
+// One warpgroup per CTA, persistent over 64-row tiles of token rows. Per tile:
+//   * TMA brings the x half of the bf16 token shadow and the message (64 rows x C each, 128B-swizzled k-blocks of 64
+//     columns) into the operand buffer A2 = [x | message].
+//   * merge: D1 [64 x C] = message * Wm^T in registers (C / 128 accumulators of m64n128); LayerNorm1 on the fragments
+//     (row statistics across the four lanes of a quad), written as bf16 over the message half of A2: A2 is now the
+//     mlp.0 operand [x | norm1(merge(message))].
+//   * the 2C-wide hidden layer in chunks (64 columns at C = 256, 128 at C = 128): D2 = A2 * W0[chunk]^T (registers), relu, bf16 into the swizzled
+//     operand buffer H, then D3 [64 x C] += H * W2[:, chunk]^T (registers). 2C-wide rows never exist anywhere.
+//   * LayerNorm2 on D3, x += it (fp32), the bf16 shadow rewritten from the new x.
+// Weights stream through a 3-slot ring of [<= 128 output rows x 64 input columns] tiles (TMA, one mbarrier per slot): the
+// tile two ahead is requested as soon as the previous wgmma group has completed, so L2 latency overlaps the MMAs. The
+// next row tile's A2 is requested as soon as the last mlp.0 chunk has read the current one. HBM traffic per row: the
+// message and x shadow read, x read and written, the shadow written; every intermediate stays on the SM.
 #include "encoder_tail.cuh"
+#include "wgmma.cuh"
 
 #include <algorithm>
 #include <cstdio>
 #include <cstring>
 #include <mutex>
 
-#include "conv_gemm.cuh"
-
 namespace mfr {
+
+int conv_gemm_num_sms();
 
 namespace {
 
-constexpr int kEpiWarps = 8;          // front group (warps 2-5) and back group (warps 6-9), one warp per TMEM lane quadrant each
-constexpr int kThreads = 64 + 32 * kEpiWarps;
-constexpr int kRelBatch = 3;        // ring slots handed back per tcgen05.commit batch
-constexpr int kKbBytes = 16384;     // one k-block of an A operand: [128 rows x 64 bf16], 128B-swizzled
-constexpr int kTmemCols = 512;
-constexpr uint64_t kDescHi = (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-__device__ __forceinline__ uint64_t desc_at(uint32_t addr) { return kDescHi | ((addr >> 4) & 0x3fffu); }
+constexpr int kRows = 64;                 // token rows per tile: the M of one warpgroup's wgmma
+constexpr int kThreads = 128;             // one warpgroup
+constexpr int kWSlots = 3;
+constexpr uint32_t kKb = kRows * 128;     // one 64-row x 64-column bf16 operand k-block (8 KB)
+constexpr uint32_t kWTile = 128 * 128;    // one weight tile: 128 output rows x 64 input columns (16 KB)
+constexpr uint64_t kDescHi = (1ull << 16) | (64ull << 32) | (1ull << 62);   // K-major, 128B swizzle, 1024 B atoms
+__device__ __forceinline__ uint64_t desc(uint32_t a) { return kDescHi | ((a >> 4) & 0x3fffu); }
 
 template <int C>
 struct Cfg {
-  static constexpr int KB = C / 64;            // k-blocks of a C-wide operand
-  static constexpr int NQ = 2 * C / 128;       // 128-column chunks of the hidden layer
-  static constexpr int L_BYTES = KB * kKbBytes;
-  static constexpr int M_BYTES = 4 * kKbBytes; // message tile (KB k-blocks) / two H1 buffers of two k-blocks
-  static constexpr int NH = C / 128;           // 128-column halves of a C-wide output (every MMA is N = 128)
-  static constexpr int NS = (C == 256) ? 5 : 7;  // ring slots of 16 KB
-  static constexpr int STG_BYTES = 4 * 4096;     // staging tiles of the LayerNorm2 warps (32 rows x 32 fp32 each)
-  static constexpr int SMEM = L_BYTES + M_BYTES + NS * kKbBytes + STG_BYTES + 1024;
-  // TMEM: D3 (mlp.2 accumulator) in columns [0, C); a 256-column scratch at [256, 512) holds D1 (merge accumulator, read by
-  // LayerNorm1) and, once that is consumed, the two 128-column D2 buffers of the hidden-layer chunks.
-  static constexpr int SCRATCH = 256;
+  static constexpr int KB1 = C / 64;                 // k-blocks of C columns
+  static constexpr int NH = C / 128;                 // 128-column accumulators of a C-wide result
+  // hidden-layer chunk width: 64 columns at C = 256 (the merge / mlp.2 accumulators already take 128 registers),
+  // 128 at C = 128
+  static constexpr int QW = C == 256 ? 64 : 128;
+  static constexpr int QK = QW / 64;                 // k-blocks of one hidden chunk
+  static constexpr int NQ = 2 * C / QW;              // chunks of the hidden layer
+  static constexpr int T_MERGE = NH * KB1;           // weight tiles of the merge GEMM
+  static constexpr int T_CHUNK = 2 * KB1 + NH * QK;  // weight tiles of one hidden chunk: mlp.0 (K = 2C), mlp.2 (K = QW)
+  static constexpr int T_ROW = T_MERGE + NQ * T_CHUNK;
+  static constexpr uint32_t A2 = 2 * KB1 * kKb;
+  static constexpr uint32_t H = QK * kKb;
+  static constexpr int SMEM = static_cast<int>(A2 + H + kWSlots * kWTile) + 1024;
 };
 
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+// weight tile t (0 <= t < T_ROW) of a row tile's sequence: tensor map, (input column, output row) coordinates, bytes
+template <int C>
+__device__ __forceinline__ uint32_t wtile(const EncoderTailParams& p, int t, const CUtensorMap*& tm, int& k0, int& n0) {
+  using G = Cfg<C>;
+  if (t < G::T_MERGE) {
+    tm = &p.tmWm; n0 = (t / G::KB1) * 128; k0 = (t % G::KB1) * 64;
+    return kWTile;
+  }
+  t -= G::T_MERGE;
+  const int q = t / G::T_CHUNK;
+  int u = t - q * G::T_CHUNK;
+  if (u < 2 * G::KB1) {
+    tm = &p.tmW0; n0 = q * G::QW; k0 = u * 64;
+    return G::QW * 128;
+  }
+  u -= 2 * G::KB1;
+  tm = &p.tmW2; n0 = (u / G::QK) * 128; k0 = q * G::QW + (u % G::QK) * 64;
+  return kWTile;
+}
+
+// byte address of element (row, col) in a 128B-swizzled stack of 64-column k-blocks (the TMA / wgmma layout)
+__device__ __forceinline__ uint32_t sw_addr(uint32_t base, int row, int col) {
+  const int c64 = col & 63;
+  return base + static_cast<uint32_t>((col >> 6) * kKb + row * 128 + (((c64 >> 3) ^ (row & 7)) << 4) + (c64 & 7) * 2);
+}
+
+__device__ __forceinline__ uint32_t bf16x2(float lo, float hi) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }
 
-template <int C>
-__global__ void __launch_bounds__(kThreads, 1) encoder_tail_kernel(const __grid_constant__ EncoderTailParams p) {
-  using G = Cfg<C>;
-  constexpr int KB = G::KB, NQ = G::NQ, NS = G::NS, NH = G::NH;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t s_bars[2 * NS + 12];
-  __shared__ uint32_t s_tmem_base;
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sL = base, sM = base + G::L_BYTES, sRing = sM + G::M_BYTES, sStg = sRing + NS * kKbBytes;
-  const uint32_t bb = smem_u32(s_bars);
-  auto full = [&](int s) { return bb + 8u * s; };
-  auto empty = [&](int s) { return bb + 8u * (NS + s); };
-  const uint32_t m_full = bb + 8u * (2 * NS), d1_full = m_full + 8, ln1_ready = m_full + 16, d3_full = m_full + 24;
-  auto d2_full = [&](int b) { return m_full + 32 + 8u * b; };
-  auto h1_full = [&](int b) { return m_full + 48 + 8u * b; };
-  auto h1_empty = [&](int b) { return m_full + 64 + 8u * b; };
-  auto d13_empty = [&](int b) { return m_full + 80 + 8u * b; };
+// mean and 1 / std (LayerNorm, eps 1e-5) of fragment row h: the row's C values sit in the four lanes of a quad
+template <int NH>
+__device__ __forceinline__ void row_stats(const float (&a)[NH][64], int h, float& mean, float& rstd) {
+  constexpr float kInvC = 1.f / (NH * 128);
+  float s = 0.f;
+#pragma unroll
+  for (int nh = 0; nh < NH; ++nh)
+#pragma unroll
+    for (int j = 0; j < 16; ++j) s += a[nh][4 * j + 2 * h] + a[nh][4 * j + 2 * h + 1];
+  s += __shfl_xor_sync(0xffffffffu, s, 1);
+  s += __shfl_xor_sync(0xffffffffu, s, 2);
+  mean = s * kInvC;
+  float q = 0.f;
+#pragma unroll
+  for (int nh = 0; nh < NH; ++nh)
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const float d0 = a[nh][4 * j + 2 * h] - mean, d1 = a[nh][4 * j + 2 * h + 1] - mean;
+      q += d0 * d0 + d1 * d1;
+    }
+  q += __shfl_xor_sync(0xffffffffu, q, 1);
+  q += __shfl_xor_sync(0xffffffffu, q, 2);
+  rstd = 1.f / sqrtf(q * kInvC + 1e-5f);
+}
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int dbg_n = 0;
-  auto stamp = [&](int role, int id) {           // debug timeline of block 0 (first 32 events per role)
-    if (p.dbg != nullptr && blockIdx.x == 0 && lane == 0 && dbg_n < 32) {
-      long long t;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      p.dbg[role * 64 + 2 * dbg_n] = id;
-      p.dbg[role * 64 + 2 * dbg_n + 1] = t;
-      ++dbg_n;
-    }
-  };
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&p.tmMsg); tma_prefetch_desc(&p.tmX); tma_prefetch_desc(&p.tmWm); tma_prefetch_desc(&p.tmW0); tma_prefetch_desc(&p.tmW2);
-    for (int s = 0; s < 2 * NS; ++s) mbar_init(bb + 8u * s, 1);
-    mbar_init(m_full, 1); mbar_init(d1_full, 1); mbar_init(ln1_ready, 4); mbar_init(d3_full, 1);
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(d2_full(b), 1); mbar_init(h1_full(b), 4); mbar_init(h1_empty(b), 1); mbar_init(d13_empty(b), 4);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(smem_u32(&s_tmem_base), kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem_base;
+template <int C>
+__global__ void __launch_bounds__(kThreads) encoder_tail_kernel(const __grid_constant__ EncoderTailParams p) {
+  using G = Cfg<C>;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t s_bar[1 + kWSlots];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t sA = base, sH = base + G::A2, sW = sH + G::H;
+  const uint32_t a_bar = smem_u32(&s_bar[0]);
+  auto w_full = [&](int s) { return smem_u32(&s_bar[1 + s]); };
+  const int tid = threadIdx.x;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
 
   long long live = p.rows_cap;
-  if (p.dyn_rows != nullptr) live = min(live, static_cast<long long>(*p.dyn_rows));
-  const int tpi = static_cast<int>((live + 127) / 128);        // tiles per row block
-  const int total = p.n_img * tpi;
-  auto tile_row0 = [&](int tile, int& r_in_img) -> long long {
-    const int img = tile / tpi;
-    r_in_img = (tile - img * tpi) * 128;
-    return static_cast<long long>(img) * p.rows_cap + r_in_img;
+  if (p.dyn_rows != nullptr) live = max(0LL, min(live, static_cast<long long>(*p.dyn_rows)));
+  const int tiles_img = static_cast<int>((live + kRows - 1) / kRows);
+  const int n_tiles = tiles_img * p.n_img;
+  const int my_tiles = static_cast<int>(blockIdx.x) < n_tiles ? (n_tiles - 1 - static_cast<int>(blockIdx.x)) / gridDim.x + 1 : 0;
+  const long long n_w = static_cast<long long>(my_tiles) * G::T_ROW;   // weight tiles this CTA streams
+  if (my_tiles == 0) return;
+
+  auto issue_w = [&](long long g) {   // thread 0: weight tile g of this CTA's sequence into slot g % kWSlots
+    const CUtensorMap* tm;
+    int k0, n0;
+    const uint32_t bytes = wtile<C>(p, static_cast<int>(g % G::T_ROW), tm, k0, n0);
+    const int s = static_cast<int>(g % kWSlots);
+    mbar_arrive_expect_tx(w_full(s), bytes);
+    tma_load_2d(sW + s * kWTile, tm, w_full(s), k0, n0);
+  };
+  auto issue_a = [&](int item) {      // thread 0: x and message k-blocks of row tile `item` into A2
+    const int img = item / tiles_img, tt = item - img * tiles_img;
+    const int r0 = static_cast<int>(img * p.rows_cap) + tt * kRows;
+    mbar_arrive_expect_tx(a_bar, 2 * G::KB1 * kKb);
+    for (int kb = 0; kb < G::KB1; ++kb) {
+      tma_load_2d(sA + kb * kKb, &p.tmX, a_bar, kb * 64, r0);
+      tma_load_2d(sA + (G::KB1 + kb) * kKb, &p.tmMsg, a_bar, kb * 64, r0);
+    }
+  };
+  if (tid == 0) {
+    tma_prefetch_desc(&p.tmMsg); tma_prefetch_desc(&p.tmX);
+    tma_prefetch_desc(&p.tmWm); tma_prefetch_desc(&p.tmW0); tma_prefetch_desc(&p.tmW2);
+    mbar_init(a_bar, 1);
+    for (int s = 0; s < kWSlots; ++s) mbar_init(w_full(s), 1);
+    fence_barrier_init();
+    issue_a(blockIdx.x);
+    issue_w(0);
+    if (n_w > 1) issue_w(1);
+  }
+  __syncthreads();
+
+  long long g = 0;   // weight tiles consumed
+  // one weight tile: 4 k-steps of (A k-block at a_addr) x (tile)^T into d; once the previous tile's group has completed,
+  // its slot is refilled with the tile two ahead
+  auto step = [&](auto& d, uint32_t a_addr) {
+    constexpr int N = 2 * static_cast<int>(sizeof(d) / sizeof(float));
+    const int s = static_cast<int>(g % kWSlots);
+    mbar_wait_inl(w_full(s), static_cast<uint32_t>((g / kWSlots) & 1), 1);
+    const uint32_t b_addr = sW + s * kWTile;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_bf16<N>(d, desc(a_addr) + 2 * k, desc(b_addr) + 2 * k);
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (tid == 0 && g + 2 < n_w) issue_w(g + 2);
+    ++g;
   };
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------------------------------ TMA producer
-    // Every ring item is one 16 KB tile [128 rows x 64 bf16]: an A k-block (message or x rows of this tile) or 128 filter
-    // rows of a weight k-block. Items are produced in exactly the order the MMA warp consumes them.
-    int s = 0;
-    uint32_t ph = 0;
-    auto put = [&](const CUtensorMap* tm, int c0, int c1) {
-      mbar_wait(empty(s), ph ^ 1u, 12);
-      if (elect_one_sync()) {
-        mbar_arrive_expect_tx(full(s), kKbBytes);
-        tma_load_2d(sRing + s * kKbBytes, tm, full(s), c0, c1);
-      }
-      if (++s == NS) { s = 0; ph ^= 1u; }
-    };
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-      int rin;
-      const int row0 = static_cast<int>(tile_row0(tile, rin));
-      stamp(2, tile);
-      for (int kb = 0; kb < KB; ++kb) {                         // GEMM1: message k-block + merge weights
-        put(&p.tmMsg, kb * 64, row0);
-        for (int h = 0; h < NH; ++h) put(&p.tmWm, kb * 64, h * 128);
-      }
-      auto g2 = [&](int q) {                                    // GEMM2 chunk q: W0 rows [128 q, 128 q + 128), all 2C input channels
-        for (int kb = 0; kb < 2 * KB; ++kb) {
-          if (kb < KB) put(&p.tmX, kb * 64, row0);              // x half of the A operand (the other half is region L)
-          put(&p.tmW0, kb * 64, q * 128);
-        }
-      };
-      auto g3 = [&](int q) {                                    // GEMM3 chunk q: W2 input channels [128 q, 128 q + 128)
-        for (int j = 0; j < 2; ++j)
-          for (int h = 0; h < NH; ++h) put(&p.tmW2, (2 * q + j) * 64, h * 128);
-      };
-      g2(0);
-      for (int q = 1; q < NQ; ++q) { g2(q); g3(q - 1); }
-      g3(NQ - 1);
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------------------------------ MMA issuer
-    const uint32_t idesc = umma_idesc(1u, 128u, 128u);          // every MMA is 128 x 128 x 16 (bf16)
-    int s = 0;
-    uint32_t ph = 0;
-    int rel_from = 0, n_unrel = 0;                              // consumed ring slots not yet handed back
-    // take the next ring item: wait for its bytes, return its shared-memory address
-    auto take = [&]() -> uint32_t {
-      mbar_wait(full(s), ph, 23);
-      const uint32_t a = sRing + s * kKbBytes;
-      if (++s == NS) { s = 0; ph ^= 1u; }
-      ++n_unrel;
-      return a;
-    };
-    // hand consumed slots back in batches: a tcgen05.commit costs the issuing thread a pipe drain however many barriers it
-    // signals, so several slots (and, where one is due, an accumulator barrier) go out together
-    auto flush = [&](uint32_t extra_bar) {
-      if (elect_one_sync()) {
-        int r = rel_from;
-        for (int i = 0; i < n_unrel; ++i) {
-          tc_commit(empty(r));
-          if (++r == NS) r = 0;
-        }
-        if (extra_bar) tc_commit(extra_bar);
-      }
-      rel_from += n_unrel;
-      if (rel_from >= NS) rel_from -= NS;
-      n_unrel = 0;
-    };
-    auto mma4 = [&](uint32_t d, uint32_t a_addr, uint32_t b_addr, bool first) {
-      if (elect_one_sync()) {
-        const uint64_t ad = desc_at(a_addr), bd = desc_at(b_addr);
-        for (int k = 0; k < 4; ++k) tc_mma_bf16(d, ad + 2 * k, bd + 2 * k, idesc, (first && k == 0) ? 0u : 1u);
-      }
-    };
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++it) {
-      const uint32_t d3 = tmem_base;                                       // mlp.2 accumulator
-      const uint32_t d1 = tmem_base + G::SCRATCH, d2b = tmem_base + G::SCRATCH;   // merge accumulator, then the two D2 buffers
-      stamp(0, 100 * it);
-      // ---- GEMM1: D1 = message @ Wm^T  (the scratch is free: every D2 chunk of the previous tile was consumed before its last GEMM3)
-      for (int kb = 0; kb < KB; ++kb) {
-        const uint32_t a = take();
-        tc_fence_after();
-        for (int h = 0; h < NH; ++h) {
-          const uint32_t b = take();
-          tc_fence_after();
-          mma4(d1 + 128u * h, a, b, kb == 0);
-        }
-        if (n_unrel >= kRelBatch) flush(0);
-      }
-      flush(d1_full);
-      stamp(0, 100 * it + 1);
-      mbar_wait(ln1_ready, it & 1, 26);          // LayerNorm1 has read D1 (the D2 buffers overwrite it) and written region L
-      bool d3_ok = it == 0;
-      auto g2 = [&](int q) {
-        const uint32_t d2 = d2b + static_cast<uint32_t>((q & 1) * 128);
-        for (int kb = 0; kb < 2 * KB; ++kb) {
-          uint32_t a;
-          if (kb < KB) {
-            a = take();
-          } else {
-            a = sL + (kb - KB) * kKbBytes;
-          }
-          const uint32_t b = take();
-          tc_fence_after();
-          mma4(d2, a, b, kb == 0);
-          if (n_unrel >= kRelBatch && kb != 2 * KB - 1) flush(0);
-        }
-        flush(d2_full(q & 1));
-        stamp(0, 100 * it + 10 + q);
-      };
-      auto g3 = [&](int q) {
-        const int u = it * (NQ / 2) + (q >> 1);                  // use index of H1 buffer q & 1
-        mbar_wait(h1_full(q & 1), u & 1, 27);
-        if (!d3_ok) { mbar_wait(d13_empty(0), (it - 1) & 1, 21); d3_ok = true; }   // LayerNorm2 of the previous tile has read D3
-        tc_fence_after();
-        for (int j = 0; j < 2; ++j)
-          for (int h = 0; h < NH; ++h) {
-            const uint32_t b = take();
-            tc_fence_after();
-            mma4(d3 + 128u * h, sM + (q & 1) * 2 * kKbBytes + j * kKbBytes, b, q == 0 && j == 0);
-          }
-        flush(q == NQ - 1 ? 0u : h1_empty(q & 1));
-        if (q == NQ - 1 && elect_one_sync()) { tc_commit(h1_empty(q & 1)); tc_commit(d3_full); }
-        stamp(0, 100 * it + 20 + q);
-      };
-      g2(0);
-      for (int q = 1; q < NQ; ++q) { g2(q); g3(q - 1); }
-      g3(NQ - 1);
-    }
-  } else {
-    // ------------------------------------------------------------------------------------------ epilogue (thread = row)
-    // Two groups of four warps (one warp per TMEM lane quadrant each) that work on DIFFERENT tiles at the same time:
-    //   front (warps 2-5): LayerNorm1 of the merge output -> region L, then relu + bf16 of every hidden chunk -> H1 buffers
-    //   back  (warps 6-9): LayerNorm2 of the mlp.2 output + residual -> fp32 x and its bf16 shadow in global memory
-    // While the back group streams tile i to HBM (the long, bandwidth-bound phase), the front group and the tensor pipe are
-    // already in tile i+1; the MMA issuer only waits for the back group before the first GEMM3 of tile i+1 overwrites D3.
-    const int q4 = warp & 3;                                    // TMEM lane quadrant of this warp
-    const bool back = warp >= 6;
-    const int r = q4 * 32 + lane;                               // row of the tile
-    const uint32_t lane_off = static_cast<uint32_t>(q4 * 32) << 16;
-    const uint32_t sw = static_cast<uint32_t>(r & 7);
-    const float inv_c = 1.f / static_cast<float>(C);
-    // row statistics of a [128 x C] accumulator in one pass: sums of (v - v0), v0 = the row's first element
-    auto row_stats = [&](uint32_t acc, float& mean, float& rstd) {
-      float v0 = 0.f, s1 = 0.f, s2 = 0.f;
-      for (int c0 = 0; c0 < C; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(acc + static_cast<uint32_t>(c0), v);
-        tmem_ld_wait();
-        if (c0 == 0) v0 = __uint_as_float(v[0]);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float d = __uint_as_float(v[j]) - v0;
-          s1 += d;
-          s2 = fmaf(d, d, s2);
-        }
-      }
-      const float md = s1 * inv_c;
-      mean = v0 + md;
-      rstd = rsqrtf(fmaxf(fmaf(-md, md, s2 * inv_c), 0.f) + 1e-5f);
-    };
-    if (!back) {
-      const uint32_t d1 = tmem_base + G::SCRATCH + lane_off, d2b = d1;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++it) {
-        // ---- E1: LayerNorm1 of the merge output -> bf16 A operand (region L)
-        mbar_wait(d1_full, it & 1, 31);
-        tc_fence_after();
-        if (warp == 2) stamp(1, 100 * it + 1);
-        {
-          float mean, rstd;
-          row_stats(d1, mean, rstd);
-          for (int c0 = 0; c0 < C; c0 += 32) {
-            uint32_t v[32];
-            tmem_ld_32x32b_x32(d1 + static_cast<uint32_t>(c0), v);
-            tmem_ld_wait();
-            uint32_t o[16];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {                         // the same 4 gammas / betas for every lane: broadcast 16-byte loads
-              const float4 g = __ldg(reinterpret_cast<const float4*>(p.g1 + c0) + j);
-              const float4 bt = __ldg(reinterpret_cast<const float4*>(p.b1 + c0) + j);
-              o[2 * j] = pack_bf16x2(fmaf((__uint_as_float(v[4 * j]) - mean) * rstd, g.x, bt.x),
-                                     fmaf((__uint_as_float(v[4 * j + 1]) - mean) * rstd, g.y, bt.y));
-              o[2 * j + 1] = pack_bf16x2(fmaf((__uint_as_float(v[4 * j + 2]) - mean) * rstd, g.z, bt.z),
-                                         fmaf((__uint_as_float(v[4 * j + 3]) - mean) * rstd, g.w, bt.w));
-            }
-            const uint32_t rowa = sL + (c0 >> 6) * kKbBytes + r * 128;
-            const uint32_t cc0 = static_cast<uint32_t>((c0 & 63) >> 3);
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(rowa + (((cc0 + i) ^ sw) << 4)), "r"(o[4 * i]),
-                           "r"(o[4 * i + 1]), "r"(o[4 * i + 2]), "r"(o[4 * i + 3]) : "memory");
-          }
-          fence_proxy_async_smem();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(ln1_ready);
-          if (warp == 2) stamp(1, 100 * it + 2);
-        }
-        // ---- E2: relu + bf16 of hidden chunk q -> H1 buffer q & 1 (A operand of GEMM3)
-        for (int q = 0; q < NQ; ++q) {
-          const int b = q & 1;
-          const int u = it * (NQ / 2) + (q >> 1);
-          mbar_wait(d2_full(b), u & 1, 32);
-          tc_fence_after();
-          if (u >= 1) mbar_wait(h1_empty(b), (u - 1) & 1, 33);   // GEMM3 of the previous use of this buffer has read it
-          if (warp == 2) stamp(1, 100 * it + 10 + q);
-          const uint32_t acc = d2b + static_cast<uint32_t>(b * 128);
-          for (int c0 = 0; c0 < 128; c0 += 32) {
-            uint32_t v[32];
-            tmem_ld_32x32b_x32(acc + static_cast<uint32_t>(c0), v);
-            tmem_ld_wait();
-            uint32_t o[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              o[j] = pack_bf16x2(fmaxf(__uint_as_float(v[2 * j]), 0.f), fmaxf(__uint_as_float(v[2 * j + 1]), 0.f));
-            const uint32_t rowa = sM + b * 2 * kKbBytes + (c0 >> 6) * kKbBytes + r * 128;
-            const uint32_t cc0 = static_cast<uint32_t>((c0 & 63) >> 3);
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(rowa + (((cc0 + i) ^ sw) << 4)), "r"(o[4 * i]),
-                           "r"(o[4 * i + 1]), "r"(o[4 * i + 2]), "r"(o[4 * i + 3]) : "memory");
-          }
-          fence_proxy_async_smem();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(h1_full(b));
-          if (warp == 2) stamp(1, 100 * it + 20 + q);
-        }
-      }
-    } else {
-      // ---- E3: x += LayerNorm2(mlp.2 output); fp32 x and its bf16 shadow, coalesced through this warp's private staging tile
-      // (32 rows x 32 floats, 16-byte chunk j of row i at chunk position j ^ (i & 7): conflict-free both ways)
-      const uint32_t d3 = tmem_base + lane_off;
-      float* stg = reinterpret_cast<float*>(smem_raw + (sStg - smem_u32(smem_raw))) + q4 * 1024;
-      const int sub_r = lane >> 3, sub_c = (lane & 7) * 4;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++it) {
-        int rin;
-        const long long row0 = tile_row0(tile, rin);
-        // the residual rows of a chunk are requested one chunk ahead of their use (the first before the accumulator is ready):
-        // 8 independent 16-byte loads in flight per lane instead of one DRAM round trip per store
-        const long long grow0 = row0 + q4 * 32;                  // first row of this warp
-        const bool ok = rin + r < live;
-        uint32_t okm = 0;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) okm |= (__shfl_sync(0xffffffffu, ok ? 1 : 0, k * 4 + sub_r) ? 1u : 0u) << k;
-        float4 xn[8];
-        auto load_res = [&](int c0) {
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            xn[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if ((okm >> k) & 1u) xn[k] = *reinterpret_cast<const float4*>(p.x + (grow0 + k * 4 + sub_r) * p.ldx + c0 + sub_c);
-          }
-        };
-        load_res(0);
-        mbar_wait(d3_full, it & 1, 34);
-        tc_fence_after();
-        if (warp == 6) stamp(3, 100 * it + 30);
-        float mean, rstd;
-        row_stats(d3, mean, rstd);
-        float mk[8], rk[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const int rr = k * 4 + sub_r;
-          mk[k] = __shfl_sync(0xffffffffu, mean, rr);
-          rk[k] = __shfl_sync(0xffffffffu, rstd, rr);
-        }
-        for (int c0 = 0; c0 < C; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(d3 + static_cast<uint32_t>(c0), v);
-          tmem_ld_wait();
-          if (c0 + 32 >= C) {                                    // last read of D3: the tensor pipe may overwrite it
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(d13_empty(0));
-          }
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<uint4*>(stg + lane * 32 + ((j ^ (lane & 7)) << 2)) = make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-          __syncwarp();
-          const float4 g = __ldg(reinterpret_cast<const float4*>(p.g2 + c0 + sub_c));
-          const float4 bt = __ldg(reinterpret_cast<const float4*>(p.b2 + c0 + sub_c));
-          float4 xc[8];
-#pragma unroll
-          for (int k = 0; k < 8; ++k) xc[k] = xn[k];
-          if (c0 + 32 < C) load_res(c0 + 32);
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            if (!((okm >> k) & 1u)) continue;
-            const int rr = k * 4 + sub_r;
-            const float4 a = *reinterpret_cast<const float4*>(stg + rr * 32 + (((sub_c >> 2) ^ (rr & 7)) << 2));
-            float* xr = p.x + (grow0 + rr) * p.ldx + c0 + sub_c;
-            const float4 xo = xc[k];
-            float4 o;
-            o.x = xo.x + fmaf((a.x - mk[k]) * rk[k], g.x, bt.x);
-            o.y = xo.y + fmaf((a.y - mk[k]) * rk[k], g.y, bt.y);
-            o.z = xo.z + fmaf((a.z - mk[k]) * rk[k], g.z, bt.z);
-            o.w = xo.w + fmaf((a.w - mk[k]) * rk[k], g.w, bt.w);
-            *reinterpret_cast<float4*>(xr) = o;
-            *reinterpret_cast<uint2*>(p.xb + (grow0 + rr) * p.ld_xb + c0 + sub_c) = make_uint2(pack_bf16x2(o.x, o.y), pack_bf16x2(o.z, o.w));
-          }
-          __syncwarp();
-        }
-        if (warp == 6) stamp(3, 100 * it + 31);
-      }
-    }
-  }
+  const int rq = 16 * warp + (lane >> 2);   // fragment rows rq and rq + 8
+  const int cq = 2 * (lane & 3);            // fragment columns 8j + cq, 8j + cq + 1
+  uint32_t a_phase = 0;
+  for (int it = 0; it < my_tiles; ++it) {
+    const int item = static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x);
+    const int img = item / tiles_img, tt = item - img * tiles_img;
+    mbar_wait_inl(a_bar, a_phase, 0);
+    a_phase ^= 1u;
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
+    // ---- merge + LayerNorm1 -> message half of A2 (bf16)
+    float acc[G::NH][64];
+#pragma unroll
+    for (int nh = 0; nh < G::NH; ++nh)
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[nh][i] = 0.f;
+#pragma unroll
+    for (int nh = 0; nh < G::NH; ++nh)
+      for (int kb = 0; kb < G::KB1; ++kb) step(acc[nh], sA + (G::KB1 + kb) * kKb);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int nh = 0; nh < G::NH; ++nh) wgmma_fence_regs(acc[nh]);
+    __syncthreads();   // every warp's merge MMAs have read the message before it is overwritten
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mean, rstd;
+      row_stats<G::NH>(acc, h, mean, rstd);
+#pragma unroll
+      for (int nh = 0; nh < G::NH; ++nh)
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int col = nh * 128 + 8 * j + cq;
+          const float y0 = (acc[nh][4 * j + 2 * h] - mean) * rstd * __ldg(p.g1 + col) + __ldg(p.b1 + col);
+          const float y1 = (acc[nh][4 * j + 2 * h + 1] - mean) * rstd * __ldg(p.g1 + col + 1) + __ldg(p.b1 + col + 1);
+          asm volatile("st.shared.u32 [%0], %1;" ::"r"(sw_addr(sA, rq + 8 * h, C + col)), "r"(bf16x2(y0, y1)) : "memory");
+        }
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+
+    // ---- hidden layer in 128-column chunks: mlp.0 + relu -> H (bf16), mlp.2 accumulates into acc3
+    float acc3[G::NH][64];
+#pragma unroll
+    for (int nh = 0; nh < G::NH; ++nh)
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc3[nh][i] = 0.f;
+    for (int q = 0; q < G::NQ; ++q) {
+      float acc2[G::QW / 2];
+#pragma unroll
+      for (int i = 0; i < G::QW / 2; ++i) acc2[i] = 0.f;
+      for (int kb = 0; kb < 2 * G::KB1; ++kb) step(acc2, sA + kb * kKb);
+      wgmma_wait<0>();   // this chunk's mlp.0 and the previous chunk's mlp.2 (reads of H) have completed
+      wgmma_fence_regs(acc2);
+      __syncthreads();
+      if (q == G::NQ - 1 && tid == 0 && it + 1 < my_tiles) issue_a(item + static_cast<int>(gridDim.x));   // A2 is free
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < G::QW / 8; ++j) {
+          const float y0 = fmaxf(acc2[4 * j + 2 * h], 0.f), y1 = fmaxf(acc2[4 * j + 2 * h + 1], 0.f);
+          asm volatile("st.shared.u32 [%0], %1;" ::"r"(sw_addr(sH, rq + 8 * h, 8 * j + cq)), "r"(bf16x2(y0, y1)) : "memory");
+        }
+      fence_proxy_async_smem();
+      __syncthreads();
+#pragma unroll
+      for (int nh = 0; nh < G::NH; ++nh)
+        for (int kb = 0; kb < G::QK; ++kb) step(acc3[nh], sH + kb * kKb);
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int nh = 0; nh < G::NH; ++nh) wgmma_fence_regs(acc3[nh]);
+
+    // ---- LayerNorm2 + residual: x (fp32) and its bf16 shadow, live rows only
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mean, rstd;
+      row_stats<G::NH>(acc3, h, mean, rstd);
+      const int r = tt * kRows + rq + 8 * h;
+      if (r < live) {
+        const long long grow = img * p.rows_cap + r;
+        float* xr = p.x + grow * p.ldx;
+        unsigned short* xbr = p.xb + grow * p.ld_xb;
+#pragma unroll
+        for (int nh = 0; nh < G::NH; ++nh)
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            const int col = nh * 128 + 8 * j + cq;
+            const float y0 = (acc3[nh][4 * j + 2 * h] - mean) * rstd * __ldg(p.g2 + col) + __ldg(p.b2 + col);
+            const float y1 = (acc3[nh][4 * j + 2 * h + 1] - mean) * rstd * __ldg(p.g2 + col + 1) + __ldg(p.b2 + col + 1);
+            float2 xo = *reinterpret_cast<const float2*>(xr + col);
+            xo.x += y0;
+            xo.y += y1;
+            *reinterpret_cast<float2*>(xr + col) = xo;
+            *reinterpret_cast<uint32_t*>(xbr + col) = bf16x2(xo.x, xo.y);
+          }
+      }
+    }
   }
 }
 
@@ -480,20 +312,20 @@ int map2d(CUtensorMap* tm, const void* ptr, long long rows, int cols, long long 
 
 int encoder_tail_build(const EncoderTailDesc& d, EncoderTailParams* p) {
   if ((d.C != 128 && d.C != 256) || d.n_img < 1 || d.rows_cap < 1) return MFR_ERR_ARG;
-  if ((d.ldx & 3) || (d.ld_xb & 3) || (reinterpret_cast<uintptr_t>(d.x) & 15) || (reinterpret_cast<uintptr_t>(d.xb_in) & 7)) return MFR_ERR_ARG;
+  if ((d.ldx & 1) || (d.ld_xb & 1) || (reinterpret_cast<uintptr_t>(d.x) & 7) || (reinterpret_cast<uintptr_t>(d.xb_in) & 15))
+    return MFR_ERR_ARG;
   memset(p, 0, sizeof(*p));
   const long long rows = d.rows_cap * d.n_img;
   int rc;
-  if ((rc = map2d(&p->tmMsg, d.msg, rows, d.C, d.ld_msg, 128)) != MFR_OK) return rc;
-  if ((rc = map2d(&p->tmX, d.xb_in, rows, d.C, d.ld_xb, 128)) != MFR_OK) return rc;
+  if ((rc = map2d(&p->tmMsg, d.msg, rows, d.C, d.ld_msg, kRows)) != MFR_OK) return rc;
+  if ((rc = map2d(&p->tmX, d.xb_in, rows, d.C, d.ld_xb, kRows)) != MFR_OK) return rc;
   if ((rc = map2d(&p->tmWm, d.w_merge, d.C, d.C, d.C, 128)) != MFR_OK) return rc;
-  if ((rc = map2d(&p->tmW0, d.w_mlp0, 2 * d.C, 2 * d.C, 2 * d.C, 128)) != MFR_OK) return rc;
+  if ((rc = map2d(&p->tmW0, d.w_mlp0, 2 * d.C, 2 * d.C, 2 * d.C, d.C == 256 ? Cfg<256>::QW : Cfg<128>::QW)) != MFR_OK) return rc;
   if ((rc = map2d(&p->tmW2, d.w_mlp2, d.C, 2 * d.C, 2 * d.C, 128)) != MFR_OK) return rc;
   p->g1 = d.g1; p->b1 = d.b1; p->g2 = d.g2; p->b2 = d.b2;
   p->x = d.x; p->xb = static_cast<unsigned short*>(const_cast<void*>(d.xb_in));
   p->ldx = d.ldx; p->ld_xb = d.ld_xb;
   p->C = d.C; p->n_img = d.n_img; p->rows_cap = d.rows_cap; p->dyn_rows = d.dyn_rows;
-  p->dbg = nullptr;
   return MFR_OK;
 }
 
@@ -503,8 +335,10 @@ int encoder_tail_launch(const EncoderTailParams& p, cudaStream_t st) {
     MFR_CUDA_CHECK(cudaFuncSetAttribute(encoder_tail_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<256>::SMEM));
     MFR_CUDA_CHECK(cudaFuncSetAttribute(encoder_tail_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::SMEM));
   }
-  const long long tiles = static_cast<long long>(p.n_img) * ((p.rows_cap + 127) / 128);
-  const int grid = static_cast<int>(std::min<long long>(tiles, conv_gemm_num_sms()));
+  const long long tiles = static_cast<long long>(p.n_img) * ((p.rows_cap + kRows - 1) / kRows);
+  // C = 256: one 129 KB CTA per SM; C = 128: two 97 KB CTAs per SM
+  const int per_sm = p.C == 256 ? 1 : 2;
+  const int grid = static_cast<int>(std::min<long long>(tiles, static_cast<long long>(conv_gemm_num_sms()) * per_sm));
   if (grid <= 0) return MFR_OK;
   if (p.C == 256) encoder_tail_kernel<256><<<grid, kThreads, Cfg<256>::SMEM, st>>>(p);
   else encoder_tail_kernel<128><<<grid, kThreads, Cfg<128>::SMEM, st>>>(p);

@@ -1531,7 +1531,7 @@ int emat_ransac(PoseSolver* s, const float* kpts0, const float* kpts1, const int
   // hypotheses per block: 128 when that already gives >= 2 blocks per SM, else down to one warp per block
   // (enough pairs: full 128-thread blocks, one per SM beside the matcher's GEMM CTAs — see emat_hyp_kernel)
   int hpb = kHypPerBlock;
-  while (hpb > 32 && static_cast<long long>(P) * ((num_hyp + hpb - 1) / hpb) < 148 / 2) hpb /= 2;
+  while (hpb > 32 && static_cast<long long>(P) * ((num_hyp + hpb - 1) / hpb) < sm_count() / 2) hpb /= 2;
   const int blocks = (num_hyp + hpb - 1) / hpb;
   const size_t smem = static_cast<size_t>(s->max_pts) * 16;
   emat_normalise_kernel<<<dim3((s->max_pts + 255) / 256, P), 256, 0, st>>>(kpts0, kpts1, offsets, K0, K1, s->max_pts,
@@ -1616,7 +1616,7 @@ int icp_refine(PoseSolver* s, const float* depth0, const float* depth1, int H, i
   f32_to_f64_kernel<<<(9 * P + 255) / 256, 256, 0, st>>>(R_in, Rd, 9 * P);
   f32_to_f64_kernel<<<(3 * P + 255) / 256, 256, 0, st>>>(t_in, td, 3 * P);
   icp_count_kernel<<<dim3(64, P), 256, 0, st>>>(depth0, depth1, H * W, Rd, td, state);
-  const int blocks = std::max(1, std::min((H * W + 255) / 256, 4 * 148 / P + 1));
+  const int blocks = std::max(1, std::min((H * W + 255) / 256, 4 * sm_count() / P + 1));
   for (int it = 0; it <= max_iter; ++it) {
     // association under the current transform; the update kernel evaluates it (fitness, rmse), tests convergence against the
     // previous association and applies the Kabsch step. The last pass (it == max_iter) only evaluates.

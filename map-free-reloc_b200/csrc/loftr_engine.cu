@@ -1,5 +1,5 @@
 // LoFTR matcher engine: the whole coarse-to-fine network as a static launch list of hand-written
-// sm_100a kernels (tcgen05 implicit-GEMM convs / linears + SIMT glue), replayed through a CUDA graph.
+// sm_90a kernels (wgmma implicit-GEMM convs / linears + SIMT glue), replayed through a CUDA graph.
 // Mirrors etc/feature_matching_baselines/LoFTR/src/loftr/loftr.py:29-75 of the reference
 // (backbone -> pos-enc -> coarse transformer -> dual-softmax mutual-NN -> fine windows -> fine
 // transformer -> expectation), for B image pairs per call, channel-last fp32 activations.
@@ -31,7 +31,7 @@ struct DebugTensor {
 
 struct StepInfo {
   std::string name;
-  int kind;             // 1 = tcgen05 conv/GEMM launch, 0 = SIMT kernel(s)
+  int kind;             // 1 = tensor-core conv/GEMM launch, 0 = SIMT kernel(s)
   double flops;         // algorithmic FLOPs (static part); for dyn steps: FLOPs per live row
   const int* dyn_rows;  // device row count (per image) or null
   int dyn_images;
@@ -420,7 +420,7 @@ struct LoftrEngine {
     if (bf) tokb = reinterpret_cast<float*>(alloc<unsigned short>(px8 * 512, "tok_bf16"));
     qkv = alloc<float>(px8 * 768, "qkv"); msg = alloc<float>(px8 * 256, "msg"); mrg = alloc<float>(px8 * 256, "mrg");
     h1 = alloc<float>(px8 * 512, "h1"); h2 = alloc<float>(px8 * 256, "h2");
-    splits_kv = std::max(1, std::min(L / 16, (2 * 148 + NI - 1) / NI));   // ~2 blocks per SM when all images run
+    splits_kv = std::max(1, std::min(L / 16, (2 * sm_count() + NI - 1) / NI));   // ~2 blocks per SM when all images run
     kvp = alloc<float>(static_cast<size_t>(NI) * 8 * splits_kv * 1056, "kvp");
     kv = alloc<float>(static_cast<size_t>(NI) * 8 * 1056, "kv");
     S = alloc<float>(static_cast<size_t>(B) * L * L, "sim");

@@ -987,203 +987,6 @@ __global__ void __launch_bounds__(256, 1) fine_attn_fused_kernel(const unsigned 
   }
 }
 
-// The same fusion with the projection on tcgen05 (the mma.sync projection above is bound by the legacy tensor path, ~1/8
-// of the tcgen05 rate on B200). One persistent block per SM, 8 warps, no warp specialisation:
-//   W [384][128] bf16 stays in shared memory as the K-major, 128B-swizzled B operand (2 k-blocks x 384 rows);
-//   per tile of WIN windows (WIN x 25 token rows as the M = 128 rows of the MMA; the spare rows stay zero) the token rows
-//   arrive by cp.async straight into the swizzled A layout; one thread issues the 16 tcgen05.mma (N = 256 + 128 per k-step;
-//   cross attention: Q from the query rows, K | V from the source rows) into 384 TMEM columns and commits to an mbarrier;
-//   all 8 warps read the accumulator (warp = lane quadrant x column half), apply elu + 1 to q and k and write the bf16
-//   Q', K', V of each window into the shared layout the mma.sync attention part expects (25 rows per window, ldmatrix rows
-//   25..31 come from a zero page); then warp = head runs the window attention of the WIN windows as above.
-// The next tile's rows are prefetched (cp.async) as soon as the MMAs have read this tile's. Self attention: WIN = 5 (one
-// token tile); cross: WIN = 3 (query and source tiles both resident).
-constexpr uint64_t kFtDescHi = (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-__device__ __forceinline__ uint64_t ft_desc(uint32_t addr) { return kFtDescHi | ((addr >> 4) & 0x3fffu); }
-template <int WIN, bool CROSS>
-constexpr int fine_tc_smem() { return 98304 + (CROSS ? 2 : 1) * 32768 + WIN * 3 * 25 * 256 + 256 + 1024; }
-
-template <int WIN, bool CROSS>
-__global__ void __launch_bounds__(256, 1) fine_attn_tc_kernel(const unsigned short* __restrict__ xq, long long ldq,
-                                                              const unsigned short* __restrict__ xs, long long lds,
-                                                              const unsigned short* __restrict__ W,   // [384][128]: Wq, Wk, Wv
-                                                              unsigned short* __restrict__ msg, long long ldm,
-                                                              const int* __restrict__ n_items_dev, float eps) {
-  constexpr int T = 25, ROWS = WIN * T;
-  extern __shared__ __align__(1024) uint8_t ft_smem[];
-  __shared__ __align__(8) uint64_t s_bar;
-  __shared__ uint32_t s_tmem;
-  const uint32_t base = (smem_u32(ft_smem) + 1023u) & ~1023u;
-  uint8_t* gen = ft_smem + (base - smem_u32(ft_smem));
-  uint8_t* gW = gen;                                 // [2 k-blocks][384 rows][128 B]
-  uint8_t* gXq = gen + 98304;                        // [2 k-blocks][128 rows][128 B]
-  uint8_t* gXs = CROSS ? gXq + 32768 : gXq;
-  uint8_t* gP = gXq + (CROSS ? 2 : 1) * 32768;       // [WIN][3][25 rows][256 B]: Q', K', V of each window
-  uint8_t* gZ = gP + WIN * 3 * T * 256;              // 256 zero bytes: token rows 25..31 of a window
-  const uint32_t sW = base, sXq = base + 98304, sXs = CROSS ? sXq + 32768 : sXq;
-  const uint32_t bar = smem_u32(&s_bar);
-  const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
-  const int n_items = *n_items_dev;
-  const int tiles = (n_items + WIN - 1) / WIN;
-  if (t == 0) {
-    mbar_init(bar, 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) {
-    tmem_alloc(smem_u32(&s_tmem), 512);
-    tmem_relinquish();
-  }
-  for (int idx = t; idx < 384 * 16; idx += 256) {    // B operand: row n = output channel, 16-byte chunk c = input channels 8 c .. 8 c + 7
-    const int n = idx >> 4, c = idx & 15;
-    const uint4 v = *reinterpret_cast<const uint4*>(W + static_cast<size_t>(n) * 128 + c * 8);
-    *reinterpret_cast<uint4*>(gW + (c >> 3) * 49152 + n * 128 + (((c & 7) ^ (n & 7)) << 4)) = v;
-  }
-  for (int idx = t; idx < (CROSS ? 2 : 1) * 2 * (128 - ROWS) * 8; idx += 256) {   // spare A rows: zero, never written again
-    const int blk = idx / ((128 - ROWS) * 8), rc = idx % ((128 - ROWS) * 8);
-    *reinterpret_cast<uint4*>(gXq + blk * 16384 + (ROWS + (rc >> 3)) * 128 + ((rc & 7) << 4)) = make_uint4(0, 0, 0, 0);
-  }
-  if (t < 16) *reinterpret_cast<uint4*>(gZ + t * 16) = make_uint4(0, 0, 0, 0);
-  fence_proxy_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = s_tmem;
-  // token rows of a tile -> swizzled A layout (rows of items past n_items: zero fill)
-  auto load_tile = [&](int tile) {
-    const int item0 = tile * WIN;
-    const int valid_rows = min(WIN, n_items - item0) * T;
-    const size_t row0 = static_cast<size_t>(item0) * T;
-    for (int c = t; c < (CROSS ? 2 : 1) * ROWS * 16; c += 256) {
-      const int which = c / (ROWS * 16), rc = c % (ROWS * 16), r = rc >> 4, ch = rc & 15;
-      const bool ok = r < valid_rows;
-      const unsigned short* src = which == 0 ? xq + (row0 + (ok ? r : 0)) * ldq : xs + (row0 + (ok ? r : 0)) * lds;
-      cp_async16((which == 0 ? gXq : gXs) + (ch >> 3) * 16384 + r * 128 + (((ch & 7) ^ (r & 7)) << 4), src + ch * 8, ok);
-    }
-    cp_async_commit();
-  };
-  const int h = warp, j = lane >> 3, r8 = lane & 7, g = lane >> 2, tq = lane & 3;
-  const uint32_t idesc256 = umma_idesc(1u, 128u, 256u), idesc128 = umma_idesc(1u, 128u, 128u);
-  int it = 0;
-  if (static_cast<int>(blockIdx.x) < tiles) load_tile(blockIdx.x);
-  for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++it) {
-    cp_async_wait<0>();
-    fence_proxy_async_smem();                        // the cp.async writes become visible to the tensor pipe
-    __syncthreads();                                 // ... of every thread; everyone is done with the previous tile's Q'/K'/V
-    if (t == 0) {
-      tc_fence_after();
-#pragma unroll
-      for (int kb = 0; kb < 2; ++kb) {
-        const uint64_t aq = ft_desc(sXq + kb * 16384), as = ft_desc(sXs + kb * 16384);
-        const uint64_t b0 = ft_desc(sW + kb * 49152);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint32_t acc = (kb | k) ? 1u : 0u;
-          if constexpr (CROSS) {                     // columns [0, 128) = q of the query rows, [128, 384) = k | v of the source rows
-            tc_mma_bf16(tmem, aq + 2 * k, b0 + 2 * k, idesc128, acc);
-            tc_mma_bf16(tmem + 128, as + 2 * k, ft_desc(sW + kb * 49152 + 128 * 128) + 2 * k, idesc256, acc);
-          } else {
-            tc_mma_bf16(tmem, aq + 2 * k, b0 + 2 * k, idesc256, acc);
-            tc_mma_bf16(tmem + 256, aq + 2 * k, ft_desc(sW + kb * 49152 + 256 * 128) + 2 * k, idesc128, acc);
-          }
-        }
-      }
-      tc_commit(bar);
-    }
-    mbar_wait(bar, it & 1, 45);
-    tc_fence_after();
-    if (tile + static_cast<int>(gridDim.x) < tiles) load_tile(tile + gridDim.x);   // the MMAs have read this tile's rows
-    // ---- accumulator -> Q', K', V tiles: warp = (lane quadrant, column half); thread = token row of the tile
-    {
-      const int q = warp & 3, hh = warp >> 2, r = q * 32 + lane;
-      const int win = r / T, lr = r - win * T;
-      const uint32_t taddr = tmem + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(192 * hh);
-#pragma unroll 1
-      for (int c0 = 0; c0 < 192; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>(c0), v);
-        tmem_ld_wait();
-        const int col = 192 * hh + c0, which = col >> 7, ch0 = (col & 127) >> 3;
-        if (r < ROWS) {
-          uint8_t* dst = gP + ((win * 3 + which) * T + lr) * 256;
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            uint32_t o[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              float a = __uint_as_float(v[8 * i + 2 * e]), b = __uint_as_float(v[8 * i + 2 * e + 1]);
-              if (which < 2) { a = elu1_fast(a); b = elu1_fast(b); }
-              o[e] = pack_bf16(a, b);
-            }
-            *reinterpret_cast<uint4*>(dst + (((ch0 + i) ^ (lr & 7)) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
-          }
-        }
-      }
-    }
-    tc_fence_before();
-    __syncthreads();                                 // Q', K', V complete; the accumulator may be overwritten by the next tile
-    // ---- window attention, warp = head (see attn_windows_mma_kernel)
-    const int item0 = tile * WIN;
-    for (int wi = 0; wi < WIN && item0 + wi < n_items; ++wi) {
-      const uint8_t* pw = gP + wi * 3 * T * 256;
-      auto addr = [&](int which, int row, int chunk) -> const uint8_t* {
-        return row < T ? pw + (which * T + row) * 256 + ((chunk ^ (row & 7)) << 4) : gZ + (chunk << 4);
-      };
-      float ckv[2][4], cks[2][4];
-#pragma unroll
-      for (int a = 0; a < 2; ++a) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) { ckv[a][e] = 0.f; cks[a][e] = 0.f; }
-      }
-      const unsigned one = (g == 0) ? 0x3F803F80u : 0u;
-      const unsigned aones[4] = {one, 0u, one, 0u};
-#pragma unroll
-      for (int ks = 0; ks < 2; ++ks) {
-        unsigned a[4], b[4];
-        ldsm_x4_t(a, addr(2, 16 * ks + r8 + 8 * (j >> 1), 2 * h + (j & 1)));     // A = V^T: m = v, k = token
-        ldsm_x4_t(b, addr(1, 16 * ks + r8 + 8 * (j & 1), 2 * h + (j >> 1)));     // B = K': k = token, n = d
-#pragma unroll
-        for (int nt = 0; nt < 2; ++nt) {
-          mma_bf16(ckv[nt], a, b[2 * nt], b[2 * nt + 1]);
-          mma_bf16(cks[nt], aones, b[2 * nt], b[2 * nt + 1]);
-        }
-      }
-      const unsigned bv0[2] = {pack_bf16(ckv[0][0], ckv[0][1]), pack_bf16(ckv[1][0], ckv[1][1])};
-      const unsigned bv1[2] = {pack_bf16(ckv[0][2], ckv[0][3]), pack_bf16(ckv[1][2], ckv[1][3])};
-      const unsigned bd[2] = {pack_bf16(cks[0][0], cks[0][1]), pack_bf16(cks[1][0], cks[1][1])};
-      const size_t row0 = static_cast<size_t>(item0 + wi) * T;
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt) {
-        unsigned a[4];
-        ldsm_x4(a, addr(0, 16 * mt + r8 + 8 * (j & 1), 2 * h + (j >> 1)));       // A = Q': m = token, k = d
-        float c0[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f}, cd[4] = {0.f, 0.f, 0.f, 0.f};
-        mma_bf16(c0, a, bv0[0], bv0[1]);
-        mma_bf16(c1, a, bv1[0], bv1[1]);
-        mma_bf16(cd, a, bd[0], bd[1]);
-        const float den_lo = __shfl_sync(0xffffffffu, cd[0], lane & ~3), den_hi = __shfl_sync(0xffffffffu, cd[2], lane & ~3);
-        const float z_lo = 1.f / (den_lo + eps), z_hi = 1.f / (den_hi + eps);
-        const int l0 = 16 * mt + g;
-        if (l0 < T) {
-          unsigned short* o = msg + (row0 + l0) * ldm + 16 * h + 2 * tq;
-          *reinterpret_cast<unsigned*>(o) = pack_bf16(c0[0] * z_lo, c0[1] * z_lo);
-          *reinterpret_cast<unsigned*>(o + 8) = pack_bf16(c1[0] * z_lo, c1[1] * z_lo);
-        }
-        if (l0 + 8 < T) {
-          unsigned short* o = msg + (row0 + l0 + 8) * ldm + 16 * h + 2 * tq;
-          *reinterpret_cast<unsigned*>(o) = pack_bf16(c0[2] * z_hi, c0[3] * z_hi);
-          *reinterpret_cast<unsigned*>(o + 8) = pack_bf16(c1[2] * z_hi, c1[3] * z_hi);
-        }
-      }
-    }
-  }
-  cp_async_wait<0>();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
-  }
-}
-
 // ------------------------------------------------------------------------------------------ layernorm
 template <int C>
 __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ in, long long ldi,
@@ -2012,8 +1815,6 @@ __global__ void __launch_bounds__(128) stem_mma_kernel(const float* __restrict__
 int stem_conv7x7(const float* img, const float* w, const float* bias, float* out, int NI, int H, int W,
                  cudaStream_t st, int out_bf16, int exact_fp32, int grid_limit) {
   const int Ho = (H + 6 - 7) / 2 + 1, Wo = (W + 6 - 7) / 2 + 1;
-  if (out_bf16 && !exact_fp32 && (getenv("MFR_STEM_TC") == nullptr || atoi(getenv("MFR_STEM_TC")) != 0))
-    return stem_conv7x7_tc(img, w, bias, out, NI, H, W, st, grid_limit);   // tcgen05 version (stem_tc.cu)
   if (kUseMmaStem && !exact_fp32) {
     const int PW = 32 * ((Wo + 15) / 16) + 8;                 // patch columns: 2 px + kx for every pixel of the padded row
     const int smem = 2 * 8 * PW * 2;
@@ -2088,10 +1889,10 @@ int linear_attention_long(const void* Q, long long ldq, const void* K, long long
     MFR_CUDA_CHECK(cudaFuncSetAttribute(kv_partial_mma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kMStages * kMSlabBytes));
     MFR_CUDA_CHECK(cudaFuncSetAttribute(attn_apply_mma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMStages * kMSlabBytes));
   }
-  const int asplits = std::max(1, std::min((L + kSlab - 1) / kSlab, (4 * 148 + n - 1) / n));
+  const int asplits = std::max(1, std::min((L + kSlab - 1) / kSlab, (4 * sm_count() + n - 1) / n));
   if (bf16) {
     if (kUseMmaAttention) {
-      const int msplits = std::max(1, std::min((L + kMS - 1) / kMS, (4 * 148 + n - 1) / n));
+      const int msplits = std::max(1, std::min((L + kMS - 1) / kMS, (4 * sm_count() + n - 1) / n));
       if (bf16 == 2) kv_partial_mma_kernel<true><<<dim3(splits, n), 256, 2 * kMStages * kMSlabBytes, st>>>(K, ldk, V, ldv, kv_part, S, splits);
       else kv_partial_mma_kernel<false><<<dim3(splits, n), 256, 2 * kMStages * kMSlabBytes, st>>>(K, ldk, V, ldv, kv_part, S, splits);
       kv_reduce_kernel<<<dim3((8 * 1056 + 255) / 256, n), 256, 0, st>>>(kv_part, kv, splits);
@@ -2144,23 +1945,8 @@ int fine_attention_fused(const void* xq, long long ldq, const void* xs, long lon
   static bool attr_seen[64] = {};
   if (first_call_on_device(attr_seen)) {
     MFR_CUDA_CHECK(cudaFuncSetAttribute(fine_attn_fused_kernel<25>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(fine_attn_tc_kernel<5, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, fine_tc_smem<5, false>()));
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(fine_attn_tc_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, fine_tc_smem<3, true>()));
   }
-  if (getenv("MFR_FINE_ATTN_MMA_SYNC") == nullptr) {   // projection on tcgen05 (default); the mma.sync version below otherwise
-    int sms = 148, dev = 0;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const unsigned short *q16 = static_cast<const unsigned short*>(xq), *s16 = static_cast<const unsigned short*>(xs);
-    if (xq == xs)
-      fine_attn_tc_kernel<5, false><<<std::min((max_items + 4) / 5, sms), 256, fine_tc_smem<5, false>(), st>>>(
-          q16, ldq, s16, lds, static_cast<const unsigned short*>(w_qkv), static_cast<unsigned short*>(msg), ldm, n_items_dev, 1e-6f);
-    else
-      fine_attn_tc_kernel<3, true><<<std::min((max_items + 2) / 3, sms), 256, fine_tc_smem<3, true>(), st>>>(
-          q16, ldq, s16, lds, static_cast<const unsigned short*>(w_qkv), static_cast<unsigned short*>(msg), ldm, n_items_dev, 1e-6f);
-    MFR_CUDA_CHECK(cudaGetLastError());
-    return MFR_OK;
-  }
-  const int grid = std::min(max_items, 2 * 148);
+  const int grid = std::min(max_items, 2 * sm_count());
   fine_attn_fused_kernel<25><<<grid, 256, kSmem, st>>>(static_cast<const unsigned short*>(xq), ldq, static_cast<const unsigned short*>(xs), lds,
                                                        static_cast<const unsigned short*>(w_qkv), static_cast<unsigned short*>(msg), ldm,
                                                        n_items_dev, 1e-6f);
@@ -2171,7 +1957,7 @@ int fine_attention_fused(const void* xq, long long ldq, const void* xs, long lon
 int layernorm_rows(const float* in, long long ldi, const float* gamma, const float* beta,
                    const float* res, long long ldr, float* out, long long ldo, long long rows, int C,
                    const int* dyn_rows, cudaStream_t st, void* out16, long long ldo16) {
-  unsigned grid = static_cast<unsigned>(std::min<long long>((rows + 7) / 8, 148LL * 16));
+  unsigned grid = static_cast<unsigned>(std::min<long long>((rows + 7) / 8, static_cast<long long>(sm_count()) * 16));
   if (grid == 0) return MFR_OK;
   if (out == nullptr && out16 == nullptr) return MFR_ERR_ARG;
   if (out16 != nullptr && ((ldo16 & 3) || (reinterpret_cast<uintptr_t>(out16) & 7))) return MFR_ERR_ARG;
@@ -2190,7 +1976,7 @@ int rows_to_bf16(const float* src, long long lds, void* dst, long long ldd, long
                  cudaStream_t st) {
   if ((C & 3) || (lds & 3) || (ldd & 3) || rows <= 0) return MFR_ERR_ARG;
   const long long total = rows * (C / 4);
-  const unsigned grid = static_cast<unsigned>(std::min<long long>((total + 255) / 256, 148LL * 16));
+  const unsigned grid = static_cast<unsigned>(std::min<long long>((total + 255) / 256, static_cast<long long>(sm_count()) * 16));
   rows_to_bf16_kernel<<<grid, 256, 0, st>>>(src, lds, static_cast<unsigned short*>(dst), ldd, rows, C / 4, dyn_rows);
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
@@ -2200,7 +1986,7 @@ int rows_split3(const float* src, long long lds, long long src_img_stride, float
                 int images, int C, int pattern, const int* dyn_rows, cudaStream_t st) {
   if ((C & 3) || (lds & 3) || (src_img_stride & 3) || rows_per_img <= 0 || images <= 0 || images > 65535) return MFR_ERR_ARG;
   const long long total = rows_per_img * (C / 4);
-  const unsigned gx = static_cast<unsigned>(std::min<long long>((total + 255) / 256, std::max(1LL, 148LL * 16 / images)));
+  const unsigned gx = static_cast<unsigned>(std::min<long long>((total + 255) / 256, std::max(1LL, static_cast<long long>(sm_count()) * 16 / images)));
   rows_split3_kernel<<<dim3(gx, static_cast<unsigned>(images)), 256, 0, st>>>(src, lds, src_img_stride, dst, rows_per_img,
                                                                              C / 4, pattern, dyn_rows);
   MFR_CUDA_CHECK(cudaGetLastError());
@@ -2250,8 +2036,8 @@ int coarse_match(const float* S, CoarseMatchBuffers f, int B, int L, int h_c, in
 }
 
 // row slabs per pair: the fused kernels run one block per SM (their cp.async ring fills the shared memory), so B * splits
-// is kept at or just under two full waves of the 148 SMs (rounding up would add a nearly empty third wave)
-int coarse_match_splits(int B, int L) { return std::max(1, std::min((L + 3) / 4, (2 * 148) / B)); }
+// is kept at or just under two full waves of the SMs (rounding up would add a nearly empty third wave)
+int coarse_match_splits(int B, int L) { return std::max(1, std::min((L + 3) / 4, (2 * sm_count()) / B)); }
 
 int coarse_match_alloc(int B, int L, int splits, CoarseMatchBuffers* o) {
   const size_t BL = static_cast<size_t>(B) * L;

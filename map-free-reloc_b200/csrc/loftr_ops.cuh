@@ -10,10 +10,6 @@ namespace mfr {
 int stem_conv7x7(const float* img, const float* w /*[128][49]*/, const float* bias, float* out,
                  int NI, int H, int W, cudaStream_t st, int out_bf16 = 0, int exact_fp32 = 0, int grid_limit = 0);
 
-// the same op on tcgen05 (stem_tc.cu): bf16 output only, same hi/lo split arithmetic
-int stem_conv7x7_tc(const float* img, const float* w, const float* bias, void* out_bf16, int NI, int H, int W, cudaStream_t st,
-                    int grid_limit = 0);
-
 // dst[n,y,x,:] += bilinear_x2_align_corners(src)[n,y,x,:]   (resnet_fpn.py:110,114)
 // pixel strides lds / ldd in elements; src / dst fp32 or bf16
 int upsample2x_add(const void* src, void* dst, int N, int Hs, int Ws, int C, int lds, int ldd, int src_bf16,

@@ -1,4 +1,4 @@
-// SuperPoint + SuperGlue matcher engine (B image pairs per call): static launch list of tcgen05
+// SuperPoint + SuperGlue matcher engine (B image pairs per call): static launch list of wgmma
 // conv/GEMM launches + SIMT kernels, replayed through a CUDA graph. Mirrors the reference's
 // SuperGlue/models/matching.py:56-84 (SuperPoint x2 -> SuperGlue) with the settings hard-wired in
 // etc/feature_matching_baselines/matchers.py:65-71 (nms 4, threshold 0.005, <= 1024 keypoints,
@@ -203,7 +203,7 @@ struct SpsgEngine {
       const std::string p = "gnn." + std::to_string(i);
       gemm(p + ".qkv", X, NI, 1, K, 256, 512, 768, 1, ACT_NONE, nullptr, qkv, 768);
       {
-        // multi-head softmax attention (superglue.py:85-89) as two tcgen05 GEMMs with the heads as the H dimension:
+        // multi-head softmax attention (superglue.py:85-89) as two tensor-core GEMMs with the heads as the H dimension:
         //   S[img][h][q][k] = Q_h K_h^T / 8   (B operand = keys of image img ^ cross, head h)
         //   P = softmax_k(S) in place, masked to the source image's keypoint count
         //   msg[img][q][64 h + d] = sum_k P[img][h][q][k] V[img ^ cross][k][64 h + d]   (B operand = V^T of that image / head)

@@ -421,7 +421,7 @@ __global__ void __launch_bounds__(128) sg_attention_kernel(const float* __restri
 }
 
 // ------------------------------------------------------------------------------------------ softmax attention on the tensor cores
-// The scores Q_h K_h^T / 8 and the product P V_h are tcgen05 GEMMs (conv_gemm, per-(image, head) B operand); in between:
+// The scores Q_h K_h^T / 8 and the product P V_h are tensor-core GEMMs (conv_gemm, per-(image, head) B operand); in between:
 //   sg_softmax_rows : P[img][h][q][:] = softmax over the source image's nk keys (0 beyond them), in place
 //   sg_transpose_v  : Vt[img][h][d][k] = qkv[img][k][512 + 64 h + d]  (the P V GEMM needs V K-major along the keys)
 __global__ void __launch_bounds__(256) sg_softmax_rows_kernel(float* __restrict__ S, const int* __restrict__ counts,

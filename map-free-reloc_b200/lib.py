@@ -87,8 +87,6 @@ SIGNATURES = {
     "mfr_resize_linear": (c_int, [c_vp, c_int, c_int, c_int, c_ll, c_int, c_vp, c_int, c_int, c_int, c_float, c_int, c_vp]),
     "mfr_pose_metrics": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
     "mfr_encoder_tail": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_ll, c_vp, c_int, c_vp]),
-    "mfr_debug_probe_overhead": (c_float, [c_int, c_int, c_int, c_int]),
-    "mfr_debug_mma_probe": (c_float, [c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
     "mfr_debug_time_conv": (c_float, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),
     "mfr_procrustes_ransac": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int,
                                       c_float, ctypes.c_ulonglong, c_vp, c_vp, c_vp, c_vp]),

@@ -2,7 +2,7 @@
 with the reference's interface (``LoFTR_matcher(resize, outdoor).match((path0, path1)) -> [N,4]``,
 etc/feature_matching_baselines/matchers.py:12-59 of the reference).
 
-All network arithmetic runs in libmfr_b200.so (hand-written sm_100a kernels); torch is used for
+All network arithmetic runs in libmfr_b200.so (hand-written sm_90a kernels); torch is used for
 device memory and streams only. There is no CPU fallback.
 """
 import ctypes

@@ -1,4 +1,4 @@
-"""Times the tcgen05 conv kernel at LoFTR layer shapes (CUDA events) and cuDNN beside it."""
+"""Times the wgmma conv kernel at LoFTR layer shapes (CUDA events) and cuDNN beside it."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

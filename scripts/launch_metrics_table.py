@@ -55,7 +55,7 @@ groups = collections.OrderedDict()
 for r in recs:
     if r["label"] in BACKBONE: g = "= backbone (21 conv launches)"
     elif r["label"].startswith("correlation"): continue
-    elif r["kernel"].startswith("conv_gemm"): g = "= other tcgen05 GEMMs (q|k|v, fine level)"
+    elif r["kernel"].startswith("conv_gemm"): g = "= other tensor-core GEMMs (q|k|v, fine level)"
     else: g = r["kernel"]
     groups.setdefault(g, []).append(r)
 print("-- by kernel family")

@@ -195,9 +195,57 @@ def make_spsg_real_golden():
     np.savez_compressed(os.path.join(HERE, "spsg_real_reference.npz"), **out)
 
 
+def make_oracle_ref_golden():
+    """What tests/test_oracle_vs_reference.py compares the oracle restatements against: the UNMODIFIED reference
+    FeatureMatchingModel (both solvers) on pose_case(1), and the reference LoFTR (its parameter names and its outputs)
+    on a small random pair with the oracle's seeded state dict."""
+    from helpers import pose_case as test_pose_case
+    import tempfile
+    model = ref_import.load_model_module()
+    c = test_pose_case(1)
+    corr = np.concatenate([c["kpts0"], c["kpts1"]], 1)[None].astype(np.float64)
+    out = {"pose_checksum": checksum(c["kpts0"], c["kpts1"], c["depth0"], c["depth1"])}
+    with tempfile.TemporaryDirectory() as td:
+        path = os.path.join(td, "corr.npz")
+        np.savez_compressed(path, correspondences=corr)
+        for solver in ("EssentialMatrixMetric", "PNP"):
+            cfg = ref_import.Cfg.wrap(dict(FEATURE_MATCHING="Precomputed", DEBUG=False, POSE_SOLVER=solver, MATCHES_FILE_PATH=path,
+                                           EMAT_RANSAC=dict(PIX_THRESHOLD=2.0, SCALE_THRESHOLD=0.1, CONFIDENCE=0.9999),
+                                           PNP=dict(RANSAC_ITER=1000, REPROJECTION_INLIER_THRESHOLD=3, CONFIDENCE=0.9999),
+                                           DATASET=dict(PAIRS_TXT=dict(TEST=None))))
+            m = model.FeatureMatchingModel(cfg)
+            data = {"depth0": torch.from_numpy(c["depth0"])[None], "depth1": torch.from_numpy(c["depth1"])[None],
+                    "K_color0": torch.from_numpy(c["K_color0"])[None], "K_color1": torch.from_numpy(c["K_color1"])[None],
+                    "pair_id": torch.tensor([0])}
+            R, t = m(data)
+            out[f"{solver}_R"], out[f"{solver}_t"], out[f"{solver}_inliers"] = R[0].numpy(), t[0, 0].numpy(), np.int64(data["inliers"])
+    LoFTR, default_cfg = ref_import.load_loftr()
+    lm = LoFTR(config=default_cfg).eval()
+    out["loftr_param_names"] = np.array(sorted(k for k in lm.state_dict() if "num_batches_tracked" not in k))
+    sd = loftr_oracle.make_state_dict(3)
+    lm.load_state_dict({k: v.clone() for k, v in sd.items()}, strict=False)
+    g = torch.Generator().manual_seed(5)
+    i0 = torch.rand(1, 1, 96, 64, generator=g)
+    i1 = torch.roll(i0, (8, 8), (2, 3))
+    lm.coarse_matching.thr = 0.0
+    with torch.no_grad():
+        b = {"image0": i0, "image1": i1}
+        lm(b)
+    out["loftr_checksum"] = checksum(i0.numpy())
+    for k in ("i_ids", "j_ids", "conf_matrix", "mkpts1_f"):
+        out["loftr_" + k] = b[k].numpy()
+    np.savez_compressed(os.path.join(HERE, "oracle_vs_reference.npz"), **out)
+
+
+def make_metrics_golden():
+    """The reference's MetricManager / precision_recall on the seeded cases of tests/test_metrics_oracle.py."""
+    from test_metrics_oracle import reference_outputs
+    np.savez_compressed(os.path.join(HERE, "metrics_reference.npz"), **reference_outputs())
+
+
 if __name__ == "__main__":
     assert ref_import.available(), "needs /root/reference"
-    which = sys.argv[1:] or ["pose", "loftr", "fullres", "spsg", "spsg_real"]
+    which = sys.argv[1:] or ["pose", "loftr", "fullres", "spsg", "spsg_real", "oracle_ref", "metrics"]
     if "pose" in which:
         make_pose_golden()
     if "loftr" in which:
@@ -208,3 +256,7 @@ if __name__ == "__main__":
         make_spsg_golden()
     if "spsg_real" in which:
         make_spsg_real_golden()
+    if "oracle_ref" in which:
+        make_oracle_ref_golden()
+    if "metrics" in which:
+        make_metrics_golden()

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 implicit-GEMM conv kernel against plain PyTorch fp32 (cuDNN/cuBLAS
+"""GPU parity of the wgmma implicit-GEMM conv kernel against plain PyTorch fp32 (cuDNN/cuBLAS
 with TF32 disabled). TF32 inputs => tolerance 3e-3 of the output range (stated here)."""
 import pytest
 import torch
@@ -87,9 +87,8 @@ def test_conv_matches_torch(mfr, N, H, W, Cin, Cout, R, stride, act, use_bias, u
 ])
 def test_conv3x3_tilings_agree(mfr, monkeypatch, force, N, H, W, Cin, Cout, use_res):
     """Every tiling of the 3x3 stride-1 path (per-tap A loads vs halo A box shared by the three ky taps,
-    one or two 128-pixel sub-tiles per CTA, swapped operands = filters as M / 256 pixels as N) against the
-    fp64 reference. Force string: halo,MT,TW[,swap[,pair]] (pair = clusters of two CTAs issuing M = 256 tcgen05 cta_group::2 MMAs);
-    shapes a mode cannot take fall back to the free search."""
+    one or two 128-pixel sub-tiles per CTA, tile widths) against the fp64 reference. Force string: halo,MT,TW
+    (fields after the third are ignored); shapes a mode cannot take fall back to the free search."""
     monkeypatch.setenv("MFR_CONV_FORCE", force)
     g = torch.Generator(device="cpu").manual_seed(4321)
     x = torch.randn(N, H, W, Cin, generator=g).cuda()
@@ -144,7 +143,7 @@ def test_batched_xyt(mfr):
 
 @pytest.mark.parametrize("force", ["-1,-1,-1,0", "1,2,16,1", "1,2,16,0,1", "1,1,-1,0,1"])
 def test_bf16_conv_swapped_operands(mfr, monkeypatch, force):
-    """bf16 residual block conv (layer1 shape class) with and without the swapped-operand mode, and as CTA pairs."""
+    """bf16 residual block conv (layer1 shape class) under several forced tilings (halo,MT,TW; further fields ignored)."""
     monkeypatch.setenv("MFR_CONV_FORCE", force)
     _bf16_conv_case(mfr, 2, 72, 48, 128, 128, 3, 1, True, True)
     _bf16_conv_case(mfr, 2, 40, 36, 196, 128, 3, 1, False, False)
@@ -189,16 +188,16 @@ def _bf16_conv_case(mfr, N, H, W, Cin, Cout, R, stride, out_bf16, use_res):
 
 
 @pytest.mark.parametrize("N,H,W,Cin,Cout,R,stride,act", [
-    (2, 40, 36, 196, 196, 3, 1, 2),      # CTA pairs, BN = 208: the last 64-channel chunk is clipped by the tensor map
+    (2, 40, 36, 196, 196, 3, 1, 2),      # BN = 256 for 196 channels: the columns past Cout are not stored
     (2, 37, 50, 128, 196, 1, 1, 0),      # 1x1, ragged tiles
     (2, 40, 36, 128, 196, 3, 2, 1),      # stride 2
     (1, 1, 777, 256, 768, 1, 1, 3),      # token GEMM (q|k|v shape): three N tiles, elu+1
     (1, 1, 300, 128, 384, 1, 1, 3),
 ])
-def test_bf16_tma_store_epilogue(mfr, monkeypatch, N, H, W, Cin, Cout, R, stride, act):
-    """bf16 outputs without a residual leave through the TMA-store epilogue (64-channel swizzled chunks); the same launch with
-    the per-thread store epilogue (MFR_CONV_NO_TMA_STORE_BF16) must give identical bits; the channel padding of the
-    output rows (stride 200 for 196 channels) is untouched or zero."""
+def test_bf16_tma_store_epilogue(mfr, N, H, W, Cin, Cout, R, stride, act):
+    """bf16 outputs without a residual (the register epilogue's packed bf16x2 stores): two launches of the same op give
+    identical bits, the channel padding of the output rows (stride 200 for 196 channels) stays untouched, and the
+    result matches an fp64 reference."""
     lib = mfr.load()
     g = torch.Generator(device="cpu").manual_seed(123)
     Cp, Co = (Cin + 7) // 8 * 8, (Cout + 7) // 8 * 8
@@ -209,19 +208,15 @@ def test_bf16_tma_store_epilogue(mfr, monkeypatch, N, H, W, Cin, Cout, R, stride
     Ho = (H + 2 * pad - R) // stride + 1; Wo = (W + 2 * pad - R) // stride + 1
     bias = torch.randn(Cout, generator=g).cuda()
     outs = []
-    for no_tma in (False, True):
-        if no_tma:
-            monkeypatch.setenv("MFR_CONV_NO_TMA_STORE_BF16", "1")
+    for _ in range(2):
         out = torch.full((N, Ho, Wo, Co), -7.0, device="cuda", dtype=torch.bfloat16)
         mfr.check(lib.mfr_conv2d_nhwc_bf16(mfr.ptr(xb), N, H, W, Cin, Cp, mfr.ptr(wb), Cp, Cout, R, R, stride, pad,
                                            mfr.ptr(bias), None, Co, act, 1.0, mfr.ptr(out), Co, 1, mfr.cur_stream()))
         torch.cuda.synchronize()
         outs.append(out)
     assert torch.equal(outs[0][..., :Cout], outs[1][..., :Cout])
-    if Co != Cout:   # the row's own channel padding: untouched, or zero-filled by the 16-byte units of the store engine (mfr_b200.h)
-        assert (outs[1][..., Cout:] == -7.0).all()
-        pad_vals = outs[0][..., Cout:]
-        assert ((pad_vals == -7.0) | (pad_vals == 0.0)).all()
+    if Co != Cout:   # the row's own channel padding
+        assert (outs[0][..., Cout:] == -7.0).all() and (outs[1][..., Cout:] == -7.0).all()
     xr = xb[..., :Cin].double().permute(0, 3, 1, 2)
     wr = wb[..., :Cin].double().reshape(Cout, R, R, Cin).permute(0, 3, 1, 2)
     ref = F.conv2d(xr, wr, None, stride=stride, padding=pad).permute(0, 2, 3, 1) + bias.double()

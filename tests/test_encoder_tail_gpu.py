@@ -1,4 +1,4 @@
-"""Stage test of the fused encoder-layer tail kernel (csrc/encoder_tail.cu) against a torch restatement of
+"""Stage test of the fused wgmma encoder-layer tail kernel (csrc/encoder_tail.cu) against a torch restatement of
 LoFTREncoderLayer.forward's second half (loftr_module/transformer.py:52-58) with the same roundings the kernel applies
 (bf16 operands, fp32 accumulation, fp32 LayerNorm, bf16 hidden tensors): merge -> norm1 -> mlp on [x | message] ->
 norm2 -> residual. Ragged row counts, several row blocks with a device-side live-row count, both channel widths."""

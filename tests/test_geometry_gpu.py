@@ -71,7 +71,7 @@ def test_emat_vs_oracle_and_ground_truth(solvers, seed, n, ratio, noise):
     R, t, ninl = solvers[0].estimate_pose(c["kpts0"], c["kpts1"], _data(c))
     assert t.shape == (3,) and abs(np.linalg.norm(t) - 1) < 1e-5
     m = solvers[0].mask.ravel().astype(bool); mo = mo.ravel().astype(bool)
-    # leg (a) of the protocol, SURVEY target 0.98 (measured 0.996-0.998, profiles/r02_emat_protocol.txt). Seed 44 (40 %
+    # leg (a) of the protocol, SURVEY target 0.98. Seed 44 (40 %
     # inliers): OpenCV stops at 1172 of the ~1210 inliers its own threshold admits, so there the bar is on its recall
     if seed == 44:
         assert (m & mo).sum() / mo.sum() >= 0.98 and m.sum() >= mo.sum()
@@ -101,8 +101,8 @@ def test_emat_polished_oracle_leg(solvers, seed, n, ratio, noise):
     cost = po.msac_cost(R, t, c["kpts0"], c["kpts1"], c["K_color0"], c["K_color1"], 2.0)
     cost_f = po.msac_cost(Rf, tf, c["kpts0"], c["kpts1"], c["K_color0"], c["K_color1"], 2.0)
     same_point = rot_angle(R, Rf) < 1e-3 and vec_angle(t, tf) < 1e-3
-    # measured (profiles/r02_emat_protocol.txt): 3 of 7 cases sit on the polished reference's fixed point (< 3e-5 rad), 3 on
-    # a lower local minimum, and seed 43 on one whose cost is 0.45 % higher (while 10x closer to ground truth)
+    # the truncated least-squares cost is not convex: the solver may sit on the polished reference's fixed point or on
+    # another local minimum whose cost is at most 1 % higher
     assert same_point or cost < cost_f * 1.01, (rot_angle(R, Rf), vec_angle(t, tf), cost, cost_f)
     assert cost < po.msac_cost(Ro, to, c["kpts0"], c["kpts1"], c["K_color0"], c["K_color1"], 2.0)   # always better than raw OpenCV
 

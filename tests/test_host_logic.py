@@ -113,13 +113,21 @@ def test_linear_attention_stage_reference_matches_oracle():
     assert torch.allclose(got.float(), want, rtol=1e-4, atol=1e-5)
 
 
-def test_launch_summary_of_committed_profile():
-    """profiles/ tooling: the committed launch list of one bench step summarises to the table quoted in profiles/README.md."""
+def test_launch_summary_of_committed_profile(tmp_path):
+    """profiles tooling: an ncu launch list (warm-up pass, then one step starting at its stem launch) summarises to the
+    per-kernel totals of the last step."""
     import os, subprocess, sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = subprocess.run([sys.executable, os.path.join(root, "scripts", "summarize_launches.py"),
-                          os.path.join(root, "profiles", "r01_launches_bf16_B16.csv")], capture_output=True, text=True, check=True).stdout
+    rows = ['"ID","Kernel Name","Metric Name","Metric Unit","Metric Value"']
+    step = [("stem_mma_kernel", "usecond", "10.5")] + [("conv_gemm_kernel<128, 1>", "nsecond", "2,000")] * 94 + \
+           [("layernorm_kernel", "usecond", "1")] * 91
+    for i, (k, u, v) in enumerate(step[:40] + step):              # a partial warm-up pass before the step
+        rows.append(f'"{i}","{k}(params)","gpu__time_duration.sum","{u}","{v}"')
+    csv_path = tmp_path / "launches.csv"
+    csv_path.write_text("\n".join(rows) + "\n")
+    out = subprocess.run([sys.executable, os.path.join(root, "scripts", "summarize_launches.py"), str(csv_path)],
+                         capture_output=True, text=True, check=True).stdout
     first = out.splitlines()[0]
-    assert first.startswith("186 launches"), first
-    conv = next(l for l in out.splitlines() if l.startswith("conv_gemm_tf32_kernel"))
+    assert first.startswith("186 launches, 289.5 us total"), first
+    conv = next(l for l in out.splitlines() if l.startswith("conv_gemm_kernel"))
     assert int(conv.split("x")[1].split()[0]) == 94

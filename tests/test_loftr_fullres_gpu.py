@@ -5,7 +5,7 @@ the three engine precisions and three weight sets:
                     set itself is tiny: a random network has almost no mutual nearest neighbours)
   functional        the hand-constructed matcher weights of the benchmark's accuracy block, reference threshold 0.2
   functional_dense  the same + dense Gaussian perturbation = the weights of the throughput benchmark
-Bars are the measured values of profiles/r02_fullres_parity.txt with margin (see DESIGN.md §4)."""
+Bars per precision: DESIGN.md §4."""
 import pytest
 
 from helpers import FULLRES_CASES, fullres_compare
@@ -14,8 +14,6 @@ pytestmark = pytest.mark.gpu
 
 # precision -> (min match-set IoU on the functional weights, max |mkpts1_f| difference in px on common matches,
 #               max relative error of the coarse tokens, max abs error of the sampled confidence matrix)
-# measured: fp32x3 IoU 1.0 / 1.0 / 1.0 / 0.9982 (2 of 1135 matches), 1.4e-3 px, tokens 1.1e-4; tf32 IoU 0.958-0.993, 0.2 px,
-# tokens 1.4e-2; bf16 IoU 0.79-0.96, 1.3 px (one match of 1135; the rest < 0.5 px), tokens 8.4e-2
 BARS = {"fp32x3": (0.995, 0.02, 5e-4, 1e-4), "tf32": (0.93, 0.3, 3e-2, 0.5), "bf16": (0.75, 2.0, 0.12, 1.0)}
 
 

@@ -1,8 +1,7 @@
 """The metrics oracle (oracle/metrics_oracle.py) against the reference's OWN tests for this code
 (benchmark/test_metrics.py: properties of trans_err / rot_err / reproj_err and the known-answer vectors of
-test_projection, replayed here with seeded randomness), and — when /root/reference is mounted — against the reference
-module itself on random poses (transforms3d, which the reference imports and this image lacks, is stood in for by the
-oracle's restatement of its four quaternion helpers)."""
+test_projection, replayed here with seeded randomness), and against the outputs of the reference module itself on seeded random poses,
+stored in tests/golden/metrics_reference.npz."""
 import sys
 import types
 
@@ -55,8 +54,26 @@ def test_precision_recall_small_case():
     assert np.isclose(ap, 0.2 * 0.75 + 0.4 * 2 / 3 + 0.2 * 1.0)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="needs /root/reference")
-def test_oracle_equals_reference_module():
+def _cases():
+    """40 seeded (q_gt, t_gt, q_est, t_est, confidence) cases around a ground-truth pose."""
+    rng = np.random.default_rng(1)
+    out = []
+    for _ in range(40):
+        qg = _rq(rng)
+        qe = mo.qmult(qg, mo.axangle2quat(rng.uniform(-1, 1, 3), rng.uniform(0, 0.3)))
+        tg = rng.normal(0, 1, 3); te_ = tg + rng.normal(0, 0.2, 3)
+        out.append((qg, tg, qe, te_, float(rng.integers(0, 50))))
+    return out
+
+
+def _tp(trans_err, rot_err):
+    return (np.array(trans_err) < 0.25) * (np.array(rot_err) < 5)
+
+
+def reference_outputs():
+    """The reference's MetricManager and precision_recall (benchmark/metrics.py, benchmark/utils.py) on _cases(), imported
+    from the unmodified reference tree (tests/golden/make_golden.py stores the result in metrics_reference.npz);
+    transforms3d, which the reference imports, is stood in for by the oracle's restatement of its quaternion helpers."""
     t3d = types.ModuleType("transforms3d"); tq = types.ModuleType("transforms3d.quaternions"); te = types.ModuleType("transforms3d.euler")
     for n in ("quat2mat", "qmult", "qinverse", "rotate_vector", "axangle2quat"):
         setattr(tq, n, getattr(mo, n))
@@ -68,25 +85,15 @@ def test_oracle_equals_reference_module():
     try:
         from benchmark.metrics import Inputs, MetricManager
         from benchmark.utils import precision_recall
-        rng = np.random.default_rng(1)
         res = {"trans_err": [], "rot_err": [], "reproj_err": [], "confidence": []}
         mm = MetricManager()
-        ours = {k: [] for k in res}
-        for _ in range(40):
-            qg = _rq(rng)
-            qe = mo.qmult(qg, mo.axangle2quat(rng.uniform(-1, 1, 3), rng.uniform(0, 0.3)))
-            tg = rng.normal(0, 1, 3); te_ = tg + rng.normal(0, 0.2, 3)
-            conf = float(rng.integers(0, 50))
+        for qg, tg, qe, te_, conf in _cases():
             mm(Inputs(q_gt=qg, t_gt=tg, q_est=qe, t_est=te_, confidence=conf, K=K0, W=540, H=720), res)
-            m = mo.pose_metrics(qg, tg, qe, te_, K0, 540, 720)
-            for k in ("trans_err", "rot_err", "reproj_err"):
-                ours[k].append(m[k])
-            ours["confidence"].append(conf)
-        for k in res:
-            assert np.allclose(res[k], ours[k], rtol=1e-10, atol=1e-10), k
-        tp = (np.array(ours["trans_err"]) < 0.25) * (np.array(ours["rot_err"]) < 5)
-        a, b = precision_recall(ours["confidence"], tp, 3), mo.precision_recall(ours["confidence"], tp, 3)
-        assert np.allclose(a[0], b[0]) and np.allclose(a[1], b[1]) and np.isclose(a[2], b[2])
+        prec, rec, ap = precision_recall(res["confidence"], _tp(res["trans_err"], res["rot_err"]), 3)
+        out = {k: np.asarray(v, dtype=np.float64) for k, v in res.items()}
+        out.update(pr_precision=np.asarray(prec, dtype=np.float64), pr_recall=np.asarray(rec, dtype=np.float64),
+                   pr_ap=np.float64(ap))
+        return out
     finally:
         sys.path.remove(ref_import.REF)
         for k, v in saved.items():
@@ -96,3 +103,19 @@ def test_oracle_equals_reference_module():
                 sys.modules[k] = v
         for k in [k for k in sys.modules if k == "benchmark" or k.startswith("benchmark.")]:
             sys.modules.pop(k)
+
+
+def test_oracle_equals_reference_module():
+    """The oracle against the reference module's outputs on the same 40 cases (tests/golden/metrics_reference.npz)."""
+    import os
+    G = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "metrics_reference.npz"))
+    ours = {k: [] for k in ("trans_err", "rot_err", "reproj_err", "confidence")}
+    for qg, tg, qe, te_, conf in _cases():
+        m = mo.pose_metrics(qg, tg, qe, te_, K0, 540, 720)
+        for k in ("trans_err", "rot_err", "reproj_err"):
+            ours[k].append(m[k])
+        ours["confidence"].append(conf)
+    for k in ours:
+        assert np.allclose(G[k], ours[k], rtol=1e-10, atol=1e-10), k
+    prec, rec, ap = mo.precision_recall(ours["confidence"], _tp(ours["trans_err"], ours["rot_err"]), 3)
+    assert np.allclose(G["pr_precision"], prec) and np.allclose(G["pr_recall"], rec) and np.isclose(G["pr_ap"], ap)

@@ -78,7 +78,7 @@ def test_tf32_close_to_reference(real_weights, cases, name):
     for side in ("0", "1"):
         got = {tuple(x) for x in r["k" + side].astype(int).tolist()}
         exp = {tuple(x) for x in G[f"{name}_keypoints{side}"].astype(int).tolist()}
-        assert len(got & exp) >= 0.9 * len(got | exp)          # measured 0.93 - 0.96 (profiles/r02_spsg_real_parity.txt)
+        assert len(got & exp) >= 0.9 * len(got | exp)          # keypoint-set IoU
     got_m = _match_pairs(r["k0"], r["k1"], r["m0"])
     exp_m = _match_pairs(G[name + "_keypoints0"], G[name + "_keypoints1"], G[name + "_matches0"])
-    assert len(got_m & exp_m) >= 0.8 * len(got_m | exp_m)      # measured 0.86 - 0.89
+    assert len(got_m & exp_m) >= 0.8 * len(got_m | exp_m)      # match-set IoU

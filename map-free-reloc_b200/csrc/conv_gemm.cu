@@ -65,6 +65,21 @@ constexpr uint64_t kDescHi = (1ull << 16) | (64ull << 32) | (1ull << 62);
 // same for 32-byte rows with the 32B swizzle (8-row groups 256 B apart, layout type 3): the narrow channel-tail tiles
 constexpr uint64_t kDescHi32 = (1ull << 16) | (16ull << 32) | (3ull << 62);
 
+// Epilogue kinds (ConvGemmParams::epi): bit 3 = bf16 output, bit 2 = residual, bits 0-1 = Act; kEpiAny = decided at
+// run time per element (token GEMMs with a dyn_w row count or act_cols, odd strides, the tf32 engine)
+constexpr int kEpiAny = -1, kEpiOutBf16 = 8, kEpiResidual = 4;
+constexpr int epi_kind(bool out_bf16, bool residual, int act) {
+  return (out_bf16 ? kEpiOutBf16 : 0) | (residual ? kEpiResidual : 0) | act;
+}
+
+// two neighbouring channels per store: every element offset even and the base pointers aligned accordingly
+__host__ __device__ __forceinline__ bool epilogue_vec2(const ConvGemmParams& p) {
+  const uintptr_t align = p.out_bf16 ? 3 : 7;
+  return ((p.Cout | p.ldo | p.out_y_stride | p.out_img_stride) & 1) == 0 && (reinterpret_cast<uintptr_t>(p.out) & align) == 0 &&
+         (p.residual == nullptr ||
+          (((p.ldr | p.res_img_stride) & 1) == 0 && (reinterpret_cast<uintptr_t>(p.residual) & align) == 0));
+}
+
 // Epilogue of one accumulator fragment: rows (pixels) r0 and r0 + 8 of sub-tile m, columns 8j + 2(lane % 4) + {0, 1}.
 template <int BN_T>
 __device__ __forceinline__ void epilogue_subtile(const ConvGemmParams& p, const float (&acc)[BN_T / 2], int row0, int lane, int n0,
@@ -124,11 +139,55 @@ __device__ __forceinline__ void epilogue_subtile(const ConvGemmParams& p, const 
   }
 }
 
-// BN_T = N tile (wgmma N), MT_T = 128-pixel sub-tiles per CTA tile, BF16 = operand type; the host launches the
-// instantiation equal to (p.BN, p.MT, p.in_bf16). Between the wgmma instructions of a group there is no control flow
-// (ptxas would otherwise serialise them): every k-block issues 4 k-steps, the channel tail of a 128-byte k-block is
-// zero-filled by TMA, and the 3 unused k-steps of a 32-byte tail group read the zero page.
-template <int BN_T, int MT_T, bool BF16>
+// Epilogue with the output type, residual and activation fixed at compile time (EPI = epi_kind(...)): the kinds the
+// ResNet-FPN convs of the bf16 engine use. Every column pair is stored as one 4- or 8-byte vector (p.epi is set only
+// when Cout, the strides and the pointers allow that), all columns get the activation, and there is no dyn_w row limit.
+template <int BN_T, int EPI>
+__device__ __forceinline__ void epilogue_fixed(const ConvGemmParams& p, const float (&acc)[BN_T / 2], int row0, int lane,
+                                               int n0, int tx, int ty, int img, int m, int tile_rows) {
+  constexpr bool kOutBf16 = (EPI & kEpiOutBf16) != 0, kRes = (EPI & kEpiResidual) != 0;
+  constexpr int kAct = EPI & 3;
+  const float alpha = p.alpha;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + 8 * h;
+    const int ly = row / p.TW, lx = row - ly * p.TW;
+    const int y = ty * tile_rows + m * p.TH + ly, x = tx * p.TW + lx;
+    if (row >= p.TW * p.TH || y >= p.Ho || x >= p.Wo) continue;
+    const long long o_off = img * p.out_img_stride + static_cast<long long>(y) * p.out_y_stride + static_cast<long long>(x) * p.ldo;
+    const long long r_off = img * p.res_img_stride + (static_cast<long long>(y) * p.Wo + x) * p.ldr;
+#pragma unroll
+    for (int j = 0; j < BN_T / 8; ++j) {
+      const int n = n0 + 8 * j + 2 * (lane & 3);
+      if (n >= p.Cout) continue;   // Cout is even: n + 1 is a column too
+      float2 b = make_float2(0.f, 0.f);
+      if (p.bias != nullptr) b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+      float v0 = fmaf(acc[4 * j + 2 * h], alpha, b.x), v1 = fmaf(acc[4 * j + 2 * h + 1], alpha, b.y);
+      if constexpr (kRes) {
+        if constexpr (kOutBf16) {
+          const uint32_t r = __ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.residual) + r_off + n));
+          v0 += __uint_as_float(r << 16);
+          v1 += __uint_as_float(r & 0xffff0000u);
+        } else {
+          const float2 r = __ldg(reinterpret_cast<const float2*>(p.residual + r_off + n));
+          v0 += r.x;
+          v1 += r.y;
+        }
+      }
+      v0 = act_fn(v0, kAct, kOutBf16);
+      v1 = act_fn(v1, kAct, kOutBf16);
+      if constexpr (kOutBf16) *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out) + o_off + n) = pack_bf16x2(v0, v1);
+      else *reinterpret_cast<float2*>(p.out + o_off + n) = make_float2(v0, v1);
+    }
+  }
+}
+
+// BN_T = N tile (wgmma N), MT_T = 128-pixel sub-tiles per CTA tile, BF16 = operand type, EPI = epilogue kind (kEpiAny:
+// the run-time generic epilogue); the host launches the instantiation equal to (p.BN, p.MT, p.in_bf16, p.epi) and
+// falls back to kEpiAny for an epilogue kind without its own instantiation. Between the wgmma instructions of a group
+// there is no control flow (ptxas would otherwise serialise them): every k-block issues 4 k-steps, the channel tail of
+// a 128-byte k-block is zero-filled by TMA, and the 3 unused k-steps of a 32-byte tail group read the zero page.
+template <int BN_T, int MT_T, bool BF16, int EPI>
 __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t s_bars[4 * kMaxSlots];
@@ -204,21 +263,23 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
           const CUtensorMap* tmA = tail ? &p.tmA2 : &p.tmA;
           const CUtensorMap* tmB = tail ? &p.tmB2 : &p.tmB;
           const uint32_t ab = tail ? p.a_bytes2 : a_bytes, bb = tail ? p.b_bytes2 : b_bytes;
-          for (int kx = 0; kx < 3; ++kx) {
-            mbar_wait_inl(a_empty(sa), pa ^ 1u, 1);
-            if (elect_one_sync()) {
-              mbar_arrive_expect_tx(a_full(sa), ab);
-              tma_load_4d(smem_a + sa * a_slot_bytes, tmA, a_full(sa), c0, x_in0 + kx, y_in0, img);
-            }
-            if (++sa == a_slots) { sa = 0; pa ^= 1u; }
-            for (int ky = 0; ky < 3; ++ky) {
-              mbar_wait_inl(b_empty(sb), pb ^ 1u, 5);
+          // B tiles in the order the taps are summed; the A box of column kx goes ahead of its first tap (ky = 0)
+          for (int g = 0; g < 9; ++g) {
+            const int kx = p.kx_major ? g / 3 : g % 3, ky = p.kx_major ? g % 3 : g / 3;
+            if (ky == 0) {
+              mbar_wait_inl(a_empty(sa), pa ^ 1u, 1);
               if (elect_one_sync()) {
-                mbar_arrive_expect_tx(b_full(sb), bb);
-                tma_load_3d(smem_b + sb * b_bytes, tmB, b_full(sb), c0, ky * 3 + kx, n0);
+                mbar_arrive_expect_tx(a_full(sa), ab);
+                tma_load_4d(smem_a + sa * a_slot_bytes, tmA, a_full(sa), c0, x_in0 + kx, y_in0, img);
               }
-              if (++sb == b_slots) { sb = 0; pb ^= 1u; }
+              if (++sa == a_slots) { sa = 0; pa ^= 1u; }
             }
+            mbar_wait_inl(b_empty(sb), pb ^ 1u, 5);
+            if (elect_one_sync()) {
+              mbar_arrive_expect_tx(b_full(sb), bb);
+              tma_load_3d(smem_b + sb * b_bytes, tmB, b_full(sb), c0, ky * 3 + kx, n0);
+            }
+            if (++sb == b_slots) { sb = 0; pb ^= 1u; }
           }
         }
       } else {
@@ -229,22 +290,21 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
           const CUtensorMap* tmA = tail ? &p.tmA2 : &p.tmA;
           const CUtensorMap* tmB = tail ? &p.tmB2 : &p.tmB;
           const uint32_t ab = tail ? p.a_bytes2 + p.b_bytes2 : a_bytes + b_bytes;
-          int tap = 0;
-          for (int ky = 0; ky < R; ++ky) {
-            for (int kx = 0; kx < S; ++kx, ++tap) {
-              mbar_wait_inl(a_empty(sa), pa ^ 1u, 1);
-              if (elect_one_sync()) {
-                mbar_arrive_expect_tx(a_full(sa), ab);
-                if (p.a_yx) tma_load_4d(smem_a + sa * a_slot_bytes, tmA, a_full(sa), c0, y_in0 + ky, x_in0 + kx, img);
-                else tma_load_4d(smem_a + sa * a_slot_bytes, tmA, a_full(sa), c0, x_in0 + kx, y_in0 + ky, img);
-                if (p.b_batched == 2) {
-                  if (p.b_yx) tma_load_4d(smem_b + sa * b_bytes, tmB, a_full(sa), c0, ty, n0, img ^ p.b_xor);
-                  else tma_load_4d(smem_b + sa * b_bytes, tmB, a_full(sa), c0, n0, ty, img ^ p.b_xor);
-                }
-                else tma_load_3d(smem_b + sa * b_bytes, tmB, a_full(sa), c0, bz >= 0 ? bz : tap, n0);
+          // taps in the order they are summed (p.kx_major)
+          for (int t = 0; t < R * S; ++t) {
+            const int ky = p.kx_major ? t % R : t / S, kx = p.kx_major ? t / R : t % S, tap = ky * S + kx;
+            mbar_wait_inl(a_empty(sa), pa ^ 1u, 1);
+            if (elect_one_sync()) {
+              mbar_arrive_expect_tx(a_full(sa), ab);
+              if (p.a_yx) tma_load_4d(smem_a + sa * a_slot_bytes, tmA, a_full(sa), c0, y_in0 + ky, x_in0 + kx, img);
+              else tma_load_4d(smem_a + sa * a_slot_bytes, tmA, a_full(sa), c0, x_in0 + kx, y_in0 + ky, img);
+              if (p.b_batched == 2) {
+                if (p.b_yx) tma_load_4d(smem_b + sa * b_bytes, tmB, a_full(sa), c0, ty, n0, img ^ p.b_xor);
+                else tma_load_4d(smem_b + sa * b_bytes, tmB, a_full(sa), c0, n0, ty, img ^ p.b_xor);
               }
-              if (++sa == a_slots) { sa = 0; pa ^= 1u; }
+              else tma_load_3d(smem_b + sa * b_bytes, tmB, a_full(sa), c0, bz >= 0 ? bz : tap, n0);
             }
+            if (++sa == a_slots) { sa = 0; pa ^= 1u; }
           }
         }
       }
@@ -255,29 +315,21 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     const int row0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);
     const uint32_t sub_bytes = static_cast<uint32_t>(p.TH * p.TW * 128);   // A bytes of one 128-row sub-tile
     const uint32_t ky_bytes = static_cast<uint32_t>(p.TW * 128);           // one halo row
-    const bool obf = p.out_bf16 != 0;
-    // two neighbouring channels per store: every element offset even and the base pointers aligned accordingly
-    const bool vec2 = ((p.Cout | p.ldo | p.out_y_stride | p.out_img_stride) & 1) == 0 &&
-                      (reinterpret_cast<uintptr_t>(p.out) & (obf ? 3 : 7)) == 0 &&
-                      (p.residual == nullptr ||
-                       (((p.ldr | p.res_img_stride) & 1) == 0 && (reinterpret_cast<uintptr_t>(p.residual) & (obf ? 3 : 7)) == 0));
+    const bool vec2 = epilogue_vec2(p);
     float acc[MT_T][BN_T / 2];
     int sa = 0, sb = 0;
     uint32_t pa = 0, pb = 0;
-    // slots of the wgmma group still in flight: released once the next group is issued and this one has completed
-    int rel_a = -1, rel_b = 0, rel_nb = 0;
+    // slots of the wgmma group still in flight (-1: none): released once the next group is issued and this one has
+    // completed
+    int rel_a = -1, rel_b = -1;
     auto release = [&]() {
-      if (rel_a < 0) return;
+      if (rel_a < 0 && rel_b < 0) return;
       __syncwarp();
       if (lane == 0) {
-        mbar_arrive(a_empty(rel_a));
-        int s2 = rel_b;
-        for (int j = 0; j < rel_nb; ++j) {
-          mbar_arrive(b_empty(s2));
-          if (++s2 == b_slots) s2 = 0;
-        }
+        if (rel_a >= 0) mbar_arrive(a_empty(rel_a));
+        if (rel_b >= 0) mbar_arrive(b_empty(rel_b));
       }
-      rel_a = -1;
+      rel_a = rel_b = -1;
     };
     auto mma = [&](float (&d)[BN_T / 2], uint64_t adesc, uint64_t bdesc) {
       if constexpr (BF16) wgmma_bf16<BN_T>(d, adesc, bdesc);
@@ -299,34 +351,34 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
           const uint64_t dhi = tail ? kDescHi32 : kDescHi;
           const uint32_t row_b = tail ? 32u : 128u;
           const uint32_t subb = tail ? sub_bytes >> 2 : sub_bytes, kyb = tail ? ky_bytes >> 2 : ky_bytes;
-          for (int kx = 0; kx < 3; ++kx) {
-            mbar_wait_inl(a_full(sa), pa, 3);
-            const uint32_t a_slot = smem_a + sa * a_slot_bytes + static_cast<uint32_t>(64 * wg) * row_b;
-            const int sb0 = sb;
-            // all three B tiles of the group are waited for before its first wgmma: no barrier wait between them
-            uint32_t b_addr[3];
-            for (int ky = 0; ky < 3; ++ky) {
-              mbar_wait_inl(b_full(sb), pb, 6);
-              b_addr[ky] = smem_b + sb * b_bytes;
-              if (++sb == b_slots) { sb = 0; pb ^= 1u; }
-            }
+          // one wgmma group per tap, in the tap order of p.kx_major: its B slot goes back as soon as the group has
+          // completed (4 B slots keep the producer ahead at BN = 256); the A slot of column kx (slot sa + kx of the
+          // ring) goes back with its third tap
+#pragma unroll 1
+          for (int g = 0; g < 9; ++g) {
+            const int kx = p.kx_major ? g / 3 : g % 3, ky = p.kx_major ? g % 3 : g / 3;
+            int sx = sa + kx;
+            uint32_t px = pa;
+            if (sx >= a_slots) { sx -= a_slots; px ^= 1u; }
+            if (ky == 0) mbar_wait_inl(a_full(sx), px, 3);
+            mbar_wait_inl(b_full(sb), pb, 6);
+            const uint32_t a_slot = smem_a + sx * a_slot_bytes + static_cast<uint32_t>(64 * wg) * row_b;
+            const uint64_t bdesc = dhi | (((smem_b + sb * b_bytes) >> 4) & 0x3fffu);
             wgmma_fence();
 #pragma unroll
-            for (int ky = 0; ky < 3; ++ky) {
-              const uint64_t bdesc = dhi | ((b_addr[ky] >> 4) & 0x3fffu);
+            for (int m = 0; m < MT_T; ++m) {
+              const uint64_t adesc = dhi | (((a_slot + m * subb + ky * kyb) >> 4) & 0x3fffu);
 #pragma unroll
-              for (int m = 0; m < MT_T; ++m) {
-                const uint64_t adesc = dhi | (((a_slot + m * subb + ky * kyb) >> 4) & 0x3fffu);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) mma(acc[m], kdesc(adesc, k, tail), kdesc(bdesc, k, tail));
-              }
+              for (int k = 0; k < 4; ++k) mma(acc[m], kdesc(adesc, k, tail), kdesc(bdesc, k, tail));
             }
             wgmma_commit();
             wgmma_wait<1>();
             release();
-            rel_a = sa; rel_b = sb0; rel_nb = 3;
-            if (++sa == a_slots) { sa = 0; pa ^= 1u; }
+            rel_a = ky == 2 ? sx : -1; rel_b = sb;
+            if (++sb == b_slots) { sb = 0; pb ^= 1u; }
           }
+          sa += 3;
+          while (sa >= a_slots) { sa -= a_slots; pa ^= 1u; }
         }
       } else {
         const int num_kb = R * S * kb_per_tap, taps = R * S;
@@ -347,7 +399,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
           wgmma_commit();
           wgmma_wait<1>();
           release();
-          rel_a = sa; rel_b = 0; rel_nb = 0;
+          rel_a = sa;
           if (++sa == a_slots) { sa = 0; pa ^= 1u; }
           if (++tap == taps) { tap = 0; ++cb; }
         }
@@ -360,8 +412,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
       const int ty = (mt / tiles_x) % p.tiles_y;
       const int img = mt / (tiles_x * p.tiles_y);
 #pragma unroll
-      for (int m = 0; m < MT_T; ++m)
-        epilogue_subtile<BN_T>(p, acc[m], row0, lane, nt * p.BN, tx, ty, img, m, tile_rows, w_lim, vec2);
+      for (int m = 0; m < MT_T; ++m) {
+        if constexpr (EPI == kEpiAny) epilogue_subtile<BN_T>(p, acc[m], row0, lane, nt * p.BN, tx, ty, img, m, tile_rows, w_lim, vec2);
+        else epilogue_fixed<BN_T, EPI>(p, acc[m], row0, lane, nt * p.BN, tx, ty, img, m, tile_rows);
+      }
     }
   }
 }
@@ -398,7 +452,7 @@ struct TileCfg {
 
 // N tiles the kernel is instantiated for (the wgmma N of one instruction)
 int bn_for(int cols) {
-  for (int bn : {32, 64, 128}) if (cols <= bn) return bn;
+  for (int bn : {32, 64, 128, 200}) if (cols <= bn) return bn;
   return 256;
 }
 
@@ -410,16 +464,20 @@ int bn_for(int cols) {
 //   epilogue : ~ 500 per 32-channel chunk of a 128-pixel sub-tile
 // times the number of waves of tiles over the SMs.
 struct RingCfg { int a_slots, b_slots, a_slot_bytes; };
-RingCfg ring_cfg(int halo, int MT, int TW, int TH, int BN) {
+RingCfg ring_cfg(int halo, bool kx_major, int MT, int TW, int TH, int BN) {
   RingCfg r{};
   const int b_bytes = BN * 128;
   if (halo) {
+    // 3 A slots and >= 6 B slots (two kx groups of B tiles in flight) where they fit, else 2 A slots, else the
+    // least that keeps one group in flight while the next one loads: 4 B slots (BN > 128). Summed ky-major, a k-block
+    // holds the A boxes of all three columns at once: 3 A slots at least.
     r.a_slot_bytes = TW * (MT * TH + 2) * 128;   // multiple of 1 KB (TW % 8 == 0)
-    r.a_slots = 3;
-    r.b_slots = std::min(kMaxSlots, (kRingBytes - r.a_slots * r.a_slot_bytes) / b_bytes);
-    if (r.b_slots < 6) {
-      r.a_slots = 2;
-      r.b_slots = std::min(kMaxSlots, (kRingBytes - r.a_slots * r.a_slot_bytes) / b_bytes);
+    for (int min_b : {6, 4}) {
+      for (int a = 3; a >= (kx_major ? 2 : 3); --a) {
+        r.a_slots = a;
+        r.b_slots = std::min(kMaxSlots, (kRingBytes - a * r.a_slot_bytes) / b_bytes);
+        if (r.b_slots >= min_b) return r;
+      }
     }
   } else {
     // generic mode pads the A slot to whole 128-row sub-tiles (the MMA reads 128 rows regardless)
@@ -430,12 +488,11 @@ RingCfg ring_cfg(int halo, int MT, int TW, int TH, int BN) {
 }
 
 TileCfg choose_cfg(int N, int Ho, int Wo, int Cout, int R, int S, int stride, int pad, int kb_per_tap,
-                   int ksteps_last, bool allow_mt2, bool single_row_tiles = false) {
+                   bool tail32, bool kx_major, bool allow_mt2, bool single_row_tiles = false) {
   const int sms = conv_gemm_num_sms();
-  const int c16 = (Cout + 15) / 16 * 16;
+  const int c8 = (Cout + 7) / 8 * 8;
   const int taps = R * S;
   const int ksteps_tap = kb_per_tap * 4;
-  (void)ksteps_last;
   const bool can_halo = R == 3 && S == 3 && stride == 1 && pad == 1;
   TileCfg best{};
   best.cost = 1e300;
@@ -444,9 +501,9 @@ TileCfg choose_cfg(int N, int Ho, int Wo, int Cout, int R, int S, int stride, in
   if (const char* e = getenv("MFR_CONV_FORCE")) sscanf(e, "%d,%d,%d", &f_halo, &f_mt, &f_tw);
   for (int pass = 0; pass < 2 && best.cost > 1e299; ++pass) {
   if (pass == 1) f_halo = f_mt = f_tw = -1;
-  const int nt0 = (c16 + kMaxBN - 1) / kMaxBN;
+  const int nt0 = (c8 + kMaxBN - 1) / kMaxBN;
   for (int nt = nt0; nt <= nt0 * 4; nt *= 2) {
-    const int BN = bn_for((c16 + nt - 1) / nt);
+    const int BN = bn_for((c8 + nt - 1) / nt);
     if (nt > nt0 && BN < 64) break;
     for (int halo = 0; halo <= (can_halo ? 1 : 0); ++halo) {
       for (int MT = 1; MT <= 2; ++MT) {
@@ -463,10 +520,10 @@ TileCfg choose_cfg(int N, int Ho, int Wo, int Cout, int R, int S, int stride, in
           const int box_rows = halo ? MT * th + 2 : MT * th * stride;
           if (box_rows > 256) continue;
           const long long tiles = static_cast<long long>(N) * ((Wo + tw - 1) / tw) * ((Ho + MT * th - 1) / (MT * th)) * nt;
-          const RingCfg rc = ring_cfg(halo, MT, tw, th, BN);
-          // the MMA warps hold the slots of one wgmma group while they wait for the next group's: halo groups take 3 B slots
-          if (rc.a_slots < 2 || rc.b_slots < (halo ? 6 : 2)) continue;
-          const double groups = halo ? 3.0 * kb_per_tap : static_cast<double>(taps) * kb_per_tap;
+          const RingCfg rc = ring_cfg(halo, kx_major, MT, tw, th, BN);
+          // the MMA warps hold the slots of one wgmma group while they wait for the next group's
+          if (rc.a_slots < (halo && !kx_major ? 3 : 2) || rc.b_slots < (halo ? 4 : 2)) continue;
+          const double groups = static_cast<double>(taps) * kb_per_tap;   // one wgmma group per (tap, k-block)
           const double mma = static_cast<double>(MT) * taps * ksteps_tap * (30.0 + 0.25 * BN) + groups * 200.0;
           const double a_bytes = halo ? static_cast<double>(tw) * (MT * th + 2) * 128.0 * 3 * kb_per_tap
                                       : static_cast<double>(tw) * th * MT * 128.0 * taps * kb_per_tap;
@@ -475,7 +532,12 @@ TileCfg choose_cfg(int N, int Ho, int Wo, int Cout, int R, int S, int stride, in
           const double epi = MT * ((BN + 31) / 32) * 500.0;
           // the epilogue does not overlap the main loop of the same warps: the two add up
           const double t = std::max(mma, l2) + epi + 800.0;
-          const double cost = static_cast<double>((tiles + sms - 1) / sms) * t;
+          double cost = static_cast<double>((tiles + sms - 1) / sms) * t;
+          // 3x3 stride-1 convs, bf16, 32 images (scripts/conv_decompose.py, H100 SXM 700 W): halo mode is 7-38 % faster
+          // than per-tap A loads when the channels end in a 32-byte tail group (Cin 196) or BN = 200; at Cin 128 / BN 128
+          // and Cin 256 / BN 256 the two are within 4 % of each other. The model ranks them within a few percent either
+          // way, so halo mode is preferred where it measurably wins.
+          if (can_halo && f_halo < 0 && halo != ((tail32 || BN == 200) ? 1 : 0)) cost *= 1.25;
           if (cost < best.cost * (1.0 - 1e-9) || (cost < best.cost * (1.0 + 1e-9) && tw > best.TW)) {
             best = TileCfg{tw, th, MT, BN, nt, halo, cost};
           }
@@ -528,8 +590,12 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
     p->tail32 = (p->ksteps_last == 1 && tail * es <= 32 && p->kb_per_tap > 1 && d.b_batched != 2 &&
                  getenv("MFR_CONV_NO_TAIL32") == nullptr) ? 1 : 0;
   }
-  const TileCfg cfg = choose_cfg(d.N, p->Ho, p->Wo, d.Cout, d.R, d.S, d.stride, d.pad, p->kb_per_tap, p->ksteps_last,
-                                 d.dyn_w == nullptr && d.b_batched != 2, d.b_batched == 2);
+  // Order of the fp32 sums over the taps, fixed per shape and the same in halo and per-tap mode, so that the tiling
+  // never changes the result bits: kx-major for 3x3 stride-1 convs with at most 128 output channels, ky-major
+  // otherwise (the orders the engine's convs have been summed in since halo mode exists)
+  p->kx_major = (d.R == 3 && d.S == 3 && d.stride == 1 && d.pad == 1 && d.Cout <= 128) ? 1 : 0;
+  const TileCfg cfg = choose_cfg(d.N, p->Ho, p->Wo, d.Cout, d.R, d.S, d.stride, d.pad, p->kb_per_tap, p->tail32 != 0,
+                                 p->kx_major != 0, d.dyn_w == nullptr && d.b_batched != 2, d.b_batched == 2);
   p->TW = cfg.TW; p->TH = cfg.TH; p->MT = cfg.MT; p->halo = cfg.halo;
   p->BN = cfg.BN; p->n_tiles = cfg.n_tiles;
   p->nt_fast = (!p->halo && p->n_tiles > 1 && getenv("MFR_CONV_NT_SLOW") == nullptr) ? 1 : 0;
@@ -542,10 +608,10 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
   p->a_bytes = p->TW * a_rows * 128;
   p->b_bytes = p->BN * 128;                                           // multiple of 1 KB (BN % 8 == 0)
   {
-    const RingCfg rc = ring_cfg(p->halo, p->MT, p->TW, p->TH, p->BN);
+    const RingCfg rc = ring_cfg(p->halo, p->kx_major != 0, p->MT, p->TW, p->TH, p->BN);
     p->a_slot_bytes = rc.a_slot_bytes; p->a_slots = rc.a_slots; p->b_slots = rc.b_slots;
   }
-  if (p->a_slots < 2 || p->b_slots < (p->halo ? 6 : 2)) return MFR_ERR_ARG;
+  if (p->a_slots < (p->halo && !p->kx_major ? 3 : 2) || p->b_slots < (p->halo ? 4 : 2)) return MFR_ERR_ARG;
   p->act = d.act;
   p->act_cols = d.act_cols > 0 ? d.act_cols : d.Cout;
   p->dyn_w = d.dyn_w;
@@ -560,6 +626,10 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
   p->out_img_stride = d.out_img_stride > 0 ? d.out_img_stride : static_cast<long long>(p->Ho) * p->Wo * d.ldo;
   p->b_xor = d.b_xor;
   p->res_img_stride = static_cast<long long>(p->Ho) * p->Wo * d.ldr;
+  p->epi = kEpiAny;
+  if (d.in_bf16 && d.dyn_w == nullptr && p->act_cols >= p->Cout && epilogue_vec2(*p) &&
+      (reinterpret_cast<uintptr_t>(d.bias) & 7) == 0)
+    p->epi = epi_kind(d.out_bf16 != 0, d.residual != nullptr, d.act);
 
   {  // activations: {C, W, H, N}
     cuuint64_t dims[4] = {(cuuint64_t)d.Cin, (cuuint64_t)d.W, (cuuint64_t)d.H, (cuuint64_t)d.N};
@@ -651,18 +721,31 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
 }
 
 namespace {
-template <int BN_T, int MT_T, bool BF16>
+template <int BN_T, int MT_T, bool BF16, int EPI>
 int launch_one(const ConvGemmParams& p, int grid, cudaStream_t stream) {
   static bool attr_seen[64] = {};
   if (first_call_on_device(attr_seen))
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_kernel<BN_T, MT_T, BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-  conv_gemm_kernel<BN_T, MT_T, BF16><<<grid, kThreads, kSmemBytes, stream>>>(p);
+    MFR_CUDA_CHECK(cudaFuncSetAttribute(conv_gemm_kernel<BN_T, MT_T, BF16, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+  conv_gemm_kernel<BN_T, MT_T, BF16, EPI><<<grid, kThreads, kSmemBytes, stream>>>(p);
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
 }
 template <int BN_T, int MT_T>
 int launch_inst(const ConvGemmParams& p, int grid, cudaStream_t stream) {
-  return p.in_bf16 ? launch_one<BN_T, MT_T, true>(p, grid, stream) : launch_one<BN_T, MT_T, false>(p, grid, stream);
+  if (!p.in_bf16) return launch_one<BN_T, MT_T, false, kEpiAny>(p, grid, stream);
+  if constexpr (BN_T >= 128) {   // the N tiles of the ResNet-FPN convs: their epilogue kinds have their own instantiations
+    constexpr int kBf = epi_kind(true, false, ACT_NONE), kBfRelu = epi_kind(true, false, ACT_RELU),
+                  kBfLeaky = epi_kind(true, false, ACT_LEAKY), kBfResRelu = epi_kind(true, true, ACT_RELU),
+                  kF32 = epi_kind(false, false, ACT_NONE);
+    switch (p.epi) {
+      case kBf: return launch_one<BN_T, MT_T, true, kBf>(p, grid, stream);
+      case kBfRelu: return launch_one<BN_T, MT_T, true, kBfRelu>(p, grid, stream);
+      case kBfLeaky: return launch_one<BN_T, MT_T, true, kBfLeaky>(p, grid, stream);
+      case kBfResRelu: return launch_one<BN_T, MT_T, true, kBfResRelu>(p, grid, stream);
+      case kF32: return launch_one<BN_T, MT_T, true, kF32>(p, grid, stream);
+    }
+  }
+  return launch_one<BN_T, MT_T, true, kEpiAny>(p, grid, stream);
 }
 }  // namespace
 
@@ -681,6 +764,7 @@ int conv_gemm_launch(const ConvGemmParams& p, cudaStream_t stream) {
       case 32: return launch_inst<32, 1>(p, grid, stream);
       case 64: return launch_inst<64, 1>(p, grid, stream);
       case 128: return launch_inst<128, 1>(p, grid, stream);
+      case 200: return launch_inst<200, 1>(p, grid, stream);
       case 256: return launch_inst<256, 1>(p, grid, stream);
     }
   }

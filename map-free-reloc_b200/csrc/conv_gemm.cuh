@@ -21,12 +21,14 @@ struct alignas(64) ConvGemmParams {
   int N, Ho, Wo, Cout, Cin;
   int R, S, stride, pad;
   int TW, TH, tiles_x, tiles_y;
-  int BN, n_tiles, kb_per_tap, b_batched;   // BN: 32, 64, 128 or 256 (the wgmma N)
+  int BN, n_tiles, kb_per_tap, b_batched;   // BN: 32, 64, 128, 200 or 256 (the wgmma N)
   int a_bytes, b_bytes;   // TMA transaction bytes of one A / B load
   int MT;                 // 128-pixel sub-tiles per CTA tile (2 only when BN <= 128: the accumulators of a tile are registers)
   int halo;               // 3x3 stride-1 conv: A is loaded as a (MT*TH+2)-row box per (k-block, kx) and the three
                           // ky taps read it at row offsets 0, TW, 2*TW (TW % 8 == 0 keeps the swizzle phase)
-  int a_slots, b_slots;   // depth of the A ring / B ring (two rings: one A slot serves 3 B tiles in halo mode)
+  int kx_major;           // 3x3: the taps are summed column by column (kx outer, ky inner) instead of row by row
+  int a_slots, b_slots;   // depth of the A ring / B ring (two rings: one A slot serves 3 B tiles in halo mode, each
+                          // B tile is one wgmma group)
   int a_slot_bytes;
   int grid_limit;         // > 0: at most this many CTAs (the engine leaves SMs to the pose back end of the previous batch during the first layers)
   int nt_fast;            // work-item order: N tile index fastest (generic mode with several N tiles: the A tiles of a pixel tile stay in L2)
@@ -34,6 +36,7 @@ struct alignas(64) ConvGemmParams {
   int tail32;             // the tail fits one 32-byte k-step: it is loaded through tmA2 / tmB2 (a_bytes2 / b_bytes2 per load)
   int a_bytes2, b_bytes2;
   int act, act_cols;    // activation applies to output channels < act_cols
+  int epi;              // epilogue kind with a compile-time body (conv_gemm.cu: epi_kind), -1: run-time generic epilogue
   int in_bf16, out_bf16;  // operands bf16 instead of fp32 (tf32 MMA); out/residual bf16
   int kblk;             // K elements per 128-byte k-block: 32 (fp32) or 64 (bf16)
   const int* dyn_w;     // optional device int: effective W (rows of a token GEMM), H must be 1

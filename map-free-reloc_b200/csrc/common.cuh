@@ -167,4 +167,51 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm,
       : "memory");
 }
 
+// ---------------------------------------------------------------------------------------------
+// TMA (tiled mode) : shared -> global, bulk async-group completion
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* tm, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(tm)),
+               "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the shared-memory sources of every committed store have been read (the buffer may be refilled)
+__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// every committed store has completed
+__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+// named barrier over `count` threads (a multiple of 32); id 0 is __syncthreads
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
+// byte address of the 2-byte element (row, col) in a 128B-swizzled stack of 64-column k-blocks, kb_bytes apart (the
+// TMA / wgmma layout: 128-byte rows whose 16-byte chunks are permuted by row % 8; base 1 KB aligned)
+__device__ __forceinline__ uint32_t sw_addr(uint32_t base, int row, int col, uint32_t kb_bytes) {
+  const int c64 = col & 63;
+  return base + static_cast<uint32_t>((col >> 6) * kb_bytes + row * 128 + (((c64 >> 3) ^ (row & 7)) << 4) + (c64 & 7) * 2);
+}
+
+// 8x8 b16 matrices between registers and shared memory in the mma fragment layout (lane l: row l / 4, columns
+// 2 (l % 4) + {0, 1} of matrix i in register i); lanes 8i .. 8i + 7 give the row addresses of matrix i
+__device__ __forceinline__ void stsm_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3)
+               : "memory");
+}
+__device__ __forceinline__ void stsm_x2(uint32_t addr, uint32_t r0, uint32_t r1) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x2.shared.b16 [%0], {%1, %2};" ::"r"(addr), "r"(r0), "r"(r1) : "memory");
+}
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(addr)
+               : "memory");
+}
+__device__ __forceinline__ void ldsm_x2(uint32_t addr, uint32_t& r0, uint32_t& r1) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0, %1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(addr) : "memory");
+}
+
 }  // namespace mfr

@@ -5,12 +5,15 @@
 //                     box (rank-4 tensor map over NHWC; halo / padding comes back as zeros through the TMA
 //                     out-of-bounds fill, stride-2 through the map's traversal stride) and a [BN filters] x [same
 //                     channels] weight box, both 128B-swizzled, into the operand rings.
-//   warps 1..3      : idle (they complete the producer's warpgroup, so that the MMA warpgroups start on a warpgroup
+//   warp 1          : TMA store warp of the compile-time epilogue kinds (epilogue_staged / store_warp).
+//   warps 2..3      : idle (they complete the first warpgroup, so that the MMA warpgroups start on a warpgroup
 //                     boundary as wgmma requires).
 //   warpgroups 1, 2 : MMA + epilogue. Warpgroup g owns rows 64g..64g+63 of every 128-pixel sub-tile: per k-step it
 //                     issues one m64nBNk(32 B) wgmma per sub-tile, accumulating in registers; one wgmma group stays in
 //                     flight while the slots of the previous one are handed back to the producer. The epilogue
-//                     applies alpha / bias / residual / activation straight from the accumulator registers.
+//                     applies alpha / bias / residual / activation to the accumulator registers and either stores
+//                     straight to global memory (run-time generic epilogue) or writes a shared-memory staging buffer
+//                     that the store warp copies out with TMA stores while the MMA warps go on to the next tile.
 // The producer runs ahead by the depth of the rings, so the loads of tile i+1 overlap the epilogue of tile i.
 #include "conv_gemm.cuh"
 #include "wgmma.cuh"
@@ -30,10 +33,11 @@ constexpr int kBlockK = 32;                     // fp32 elements per k-block = 1
 constexpr int kTileM = 128;
 constexpr int kMaxBN = 256;
 constexpr int kAStage = kTileM * kBlockK * 4;   // 16 KB
-constexpr int kRingBytes = 212 * 1024;          // operand rings (A slots + B slots)
+constexpr int kOperandBytes = 216 * 1024;       // operand rings (A slots + B slots) + the epilogue's staging buffer
 constexpr int kZeroBytes = kMaxBN * 32;         // zero page: operand of the unused k-steps of a 32-byte channel-tail group
-constexpr int kSmemBytes = kRingBytes + kZeroBytes + 1024 /*align slack*/;
+constexpr int kSmemBytes = kZeroBytes + kOperandBytes + 1024 /*align slack*/;
 constexpr int kMmaWarps = 8;                    // two MMA warpgroups
+constexpr double kEpiStagedUnit = 250.0;       // cost-model epilogue term of the TMA-store epilogue (choose_cfg)
 constexpr int kThreads = 128 + 32 * kMmaWarps;
 
 __device__ __forceinline__ float act_fn(float v, int act, bool fast) {
@@ -71,6 +75,11 @@ constexpr int kEpiAny = -1, kEpiOutBf16 = 8, kEpiResidual = 4;
 constexpr int epi_kind(bool out_bf16, bool residual, int act) {
   return (out_bf16 ? kEpiOutBf16 : 0) | (residual ? kEpiResidual : 0) | act;
 }
+// the kinds with their own (TMA-store) instantiations, at BN >= 128
+constexpr int kBf = epi_kind(true, false, ACT_NONE), kBfRelu = epi_kind(true, false, ACT_RELU),
+              kBfLeaky = epi_kind(true, false, ACT_LEAKY), kBfResRelu = epi_kind(true, true, ACT_RELU),
+              kF32 = epi_kind(false, false, ACT_NONE);
+constexpr bool staged_kind(int k) { return k == kBf || k == kBfRelu || k == kBfLeaky || k == kBfResRelu || k == kF32; }
 
 // two neighbouring channels per store: every element offset even and the base pointers aligned accordingly
 __host__ __device__ __forceinline__ bool epilogue_vec2(const ConvGemmParams& p) {
@@ -139,47 +148,220 @@ __device__ __forceinline__ void epilogue_subtile(const ConvGemmParams& p, const 
   }
 }
 
-// Epilogue with the output type, residual and activation fixed at compile time (EPI = epi_kind(...)): the kinds the
-// ResNet-FPN convs of the bf16 engine use. Every column pair is stored as one 4- or 8-byte vector (p.epi is set only
-// when Cout, the strides and the pointers allow that), all columns get the activation, and there is no dyn_w row limit.
-template <int BN_T, int EPI>
-__device__ __forceinline__ void epilogue_fixed(const ConvGemmParams& p, const float (&acc)[BN_T / 2], int row0, int lane,
-                                               int n0, int tx, int ty, int img, int m, int tile_rows) {
+// Staging layout of the TMA-store epilogue. A CTA tile leaves shared memory as boxes {kCW channels, TW, TH, 1}: box
+// b = m * nbox + c holds channel chunk c of sub-tile m, 128 rows (pixel ly * TW + lx) of 128 bytes, 128B-swizzled; a
+// BN that is not a multiple of kCW (200) ends in a narrow box of BN % kCW channels, unswizzled rows (tmO2 / tmR2). The
+// boxes are placed in order into passes of at most kStageMax bytes: one pass for every bf16 tile, two for the larger fp32
+// tiles. stage_place packs (pass << 16) | byte offset in the staging buffer.
+constexpr int kStageMax = 64 * 1024;
+constexpr int kBox = kTileM * 128;   // one full box
+__host__ __device__ constexpr int stage_cw(bool bf16) { return bf16 ? 64 : 32; }
+__host__ __device__ constexpr int stage_nbox(int BN, bool bf16) { return (BN + stage_cw(bf16) - 1) / stage_cw(bf16); }
+__host__ __device__ constexpr int stage_narrow_row(int BN, bool bf16) { return (BN % stage_cw(bf16)) * (bf16 ? 2 : 4); }
+__host__ __device__ constexpr int stage_box_bytes(int BN, bool bf16, int c) {
+  return (c + 1) * stage_cw(bf16) <= BN ? kBox : kTileM * stage_narrow_row(BN, bf16);
+}
+__host__ __device__ constexpr int stage_place(int BN, bool bf16, int b) {
+  int pass = 0, off = 0;
+  for (int i = 0;; ++i) {
+    const int sz = stage_box_bytes(BN, bf16, i % stage_nbox(BN, bf16));
+    if (off + sz > kStageMax) { ++pass; off = 0; }
+    if (i == b) return (pass << 16) | off;
+    off += sz;
+  }
+}
+// staging bytes of a tile (its first and largest pass)
+__host__ __device__ constexpr int stage_bytes(int BN, bool bf16, int MT) {
+  int bytes = 0;
+  for (int b = 0; b < MT * stage_nbox(BN, bf16); ++b)
+    if ((stage_place(BN, bf16, b) >> 16) == 0) bytes = (stage_place(BN, bf16, b) & 0xffff) + stage_box_bytes(BN, bf16, b % stage_nbox(BN, bf16));
+  return bytes;
+}
+
+// Epilogue with the output type, residual and activation fixed at compile time (EPI = epi_kind(...)): the kinds of the
+// ResNet-FPN convs, the coarse q|k|v projections and the correlation. The MMA warps apply alpha / bias / residual /
+// activation to the accumulators and write the result into the staging buffer (bf16 through stmatrix, fp32 as 8-byte
+// vectors); the store warp copies it out with TMA stores, whose tensor map clips ragged tiles and the channels >= Cout.
+// A residual has been loaded into the staging buffer by the store warp (zero outside the tensor) and is read from the
+// positions the result then overwrites. Per pass: wait for the buffer (st_empty), fill it, fence + barrier over the 256
+// MMA threads, hand it to the store warp (st_full).
+template <int BN_T, int MT_T, int EPI>
+__device__ __forceinline__ void epilogue_staged(const ConvGemmParams& p, const float (&acc)[MT_T][BN_T / 2], uint32_t stage,
+                                                uint32_t st_empty, uint32_t st_full, int tile_index, int row_base,
+                                                int lane, int n0) {
   constexpr bool kOutBf16 = (EPI & kEpiOutBf16) != 0, kRes = (EPI & kEpiResidual) != 0;
   constexpr int kAct = EPI & 3;
+  constexpr int kNBox = stage_nbox(BN_T, kOutBf16), kCW = stage_cw(kOutBf16);
+  constexpr int kPasses = (stage_place(BN_T, kOutBf16, MT_T * kNBox - 1) >> 16) + 1;
+  static_assert(!kRes || (kOutBf16 && kPasses == 1), "a residual is staged in one pass");
   const float alpha = p.alpha;
+  const int q = lane & 3;
+  auto bias2 = [&](int n) {   // columns n, n + 1 (Cout is even); the columns of a tile beyond Cout are clipped by the store
+    return (p.bias != nullptr && n < p.Cout) ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.f, 0.f);
+  };
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int row = row0 + 8 * h;
-    const int ly = row / p.TW, lx = row - ly * p.TW;
-    const int y = ty * tile_rows + m * p.TH + ly, x = tx * p.TW + lx;
-    if (row >= p.TW * p.TH || y >= p.Ho || x >= p.Wo) continue;
-    const long long o_off = img * p.out_img_stride + static_cast<long long>(y) * p.out_y_stride + static_cast<long long>(x) * p.ldo;
-    const long long r_off = img * p.res_img_stride + (static_cast<long long>(y) * p.Wo + x) * p.ldr;
+  for (int pass = 0; pass < kPasses; ++pass) {
+    mbar_wait_inl(st_empty, static_cast<uint32_t>(tile_index * kPasses + pass) & 1u, 7);
+    if constexpr (kOutBf16) {
+      // stmatrix / ldmatrix x4 over columns 8j .. 8j + 15: matrix i = (column group j + i / 2, row half i % 2), whose
+      // row addresses come from lanes 8i .. 8i + 7; x2 for a last odd column group
+      const int mi = lane >> 3;
+      const int arow = row_base + (lane & 7) + 8 * (mi & 1);
 #pragma unroll
-    for (int j = 0; j < BN_T / 8; ++j) {
-      const int n = n0 + 8 * j + 2 * (lane & 3);
-      if (n >= p.Cout) continue;   // Cout is even: n + 1 is a column too
-      float2 b = make_float2(0.f, 0.f);
-      if (p.bias != nullptr) b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
-      float v0 = fmaf(acc[4 * j + 2 * h], alpha, b.x), v1 = fmaf(acc[4 * j + 2 * h + 1], alpha, b.y);
-      if constexpr (kRes) {
-        if constexpr (kOutBf16) {
-          const uint32_t r = __ldg(reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint16_t*>(p.residual) + r_off + n));
-          v0 += __uint_as_float(r << 16);
-          v1 += __uint_as_float(r & 0xffff0000u);
-        } else {
-          const float2 r = __ldg(reinterpret_cast<const float2*>(p.residual + r_off + n));
-          v0 += r.x;
-          v1 += r.y;
+      for (int j = 0; j < BN_T / 8; j += 2) {
+        const bool two = j + 1 < BN_T / 8;
+        float2 bb[2];
+#pragma unroll
+        for (int t = 0; t < 2; ++t) bb[t] = (j + t < BN_T / 8) ? bias2(n0 + 8 * (j + t) + 2 * q) : make_float2(0.f, 0.f);
+#pragma unroll
+        for (int m = 0; m < MT_T; ++m) {
+          const int c = (8 * j) / kCW, b = m * kNBox + c;
+          const uint32_t box = stage + (stage_place(BN_T, true, b) & 0xffff);
+          const int acol = 8 * j + (two ? 8 * (mi >> 1) : 0) - c * kCW;
+          const uint32_t addr = (c + 1) * kCW <= BN_T ? sw_addr(box, arow, acol, 0)
+                                                      : box + static_cast<uint32_t>(arow * stage_narrow_row(BN_T, true));
+          uint32_t r[4] = {0u, 0u, 0u, 0u};
+          if constexpr (kRes) {
+            if (two) ldsm_x4(addr, r[0], r[1], r[2], r[3]);
+            else ldsm_x2(addr, r[0], r[1]);
+          }
+          uint32_t o[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int jj = j + (i >> 1), h = i & 1;
+            if (jj >= BN_T / 8) { o[i] = 0u; continue; }
+            float v0 = fmaf(acc[m][4 * jj + 2 * h], alpha, bb[i >> 1].x), v1 = fmaf(acc[m][4 * jj + 2 * h + 1], alpha, bb[i >> 1].y);
+            if constexpr (kRes) {
+              v0 += __uint_as_float(r[i] << 16);
+              v1 += __uint_as_float(r[i] & 0xffff0000u);
+            }
+            o[i] = pack_bf16x2(act_fn(v0, kAct, true), act_fn(v1, kAct, true));
+          }
+          if (two) stsm_x4(addr, o[0], o[1], o[2], o[3]);
+          else stsm_x2(addr, o[0], o[1]);
         }
       }
-      v0 = act_fn(v0, kAct, kOutBf16);
-      v1 = act_fn(v1, kAct, kOutBf16);
-      if constexpr (kOutBf16) *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out) + o_off + n) = pack_bf16x2(v0, v1);
-      else *reinterpret_cast<float2*>(p.out + o_off + n) = make_float2(v0, v1);
+    } else {
+      const int row0 = row_base + (lane >> 2);
+#pragma unroll
+      for (int j = 0; j < BN_T / 8; ++j) {
+        const float2 bb = bias2(n0 + 8 * j + 2 * q);
+#pragma unroll
+        for (int m = 0; m < MT_T; ++m) {
+          const int c = (8 * j) / kCW, b = m * kNBox + c;
+          if ((stage_place(BN_T, false, b) >> 16) != pass) continue;
+          const uint32_t box = stage + (stage_place(BN_T, false, b) & 0xffff);
+          const int col = 8 * j + 2 * q - c * kCW;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = row0 + 8 * h;
+            const uint32_t addr = (c + 1) * kCW <= BN_T ? sw_addr(box, row, 2 * col, 0)
+                                                        : box + static_cast<uint32_t>(row * stage_narrow_row(BN_T, false) + 4 * col);
+            const float v0 = act_fn(fmaf(acc[m][4 * j + 2 * h], alpha, bb.x), kAct, false);
+            const float v1 = act_fn(fmaf(acc[m][4 * j + 2 * h + 1], alpha, bb.y), kAct, false);
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v0), "f"(v1) : "memory");
+          }
+        }
+      }
+    }
+    fence_proxy_async_smem();   // the staging buffer is read by the TMA store (async proxy)
+    named_bar_sync(1, 32 * kMmaWarps);
+    if (threadIdx.x == 128) mbar_arrive(st_full);
+  }
+}
+
+// Store warp of the TMA-store epilogue: per pass of every tile it waits for the staging buffer, stores its boxes, and
+// once the stores have read it hands it back -- for the residual kind after loading the next tile's residual into it.
+template <int BN_T, int MT_T, int EPI>
+__device__ __forceinline__ void store_warp(const ConvGemmParams& p, uint32_t stage, uint32_t st_empty, uint32_t st_full,
+                                           int total_tiles, int tiles_x, int tile_rows) {
+  constexpr bool kOutBf16 = (EPI & kEpiOutBf16) != 0, kRes = (EPI & kEpiResidual) != 0;
+  constexpr int kNBox = stage_nbox(BN_T, kOutBf16), kCW = stage_cw(kOutBf16);
+  constexpr int kPasses = (stage_place(BN_T, kOutBf16, MT_T * kNBox - 1) >> 16) + 1;
+  struct Tile { int n0, x0, y0, img; };
+  auto tile_of = [&](int item) {
+    int mt, nt;
+    if (p.nt_fast) { mt = item / p.n_tiles; nt = item - mt * p.n_tiles; }
+    else { nt = item / (p.N * p.tiles_y * tiles_x); mt = item - nt * (p.N * p.tiles_y * tiles_x); }
+    const int tx = mt % tiles_x, ty = (mt / tiles_x) % p.tiles_y;
+    return Tile{nt * p.BN, tx * p.TW, ty * tile_rows, mt / (tiles_x * p.tiles_y)};
+  };
+  // the staging buffer is free for the next pass; with a residual: load the residual boxes of tile t into it
+  auto hand_back = [&](const Tile& t) {
+    if constexpr (kRes) {
+      if (elect_one_sync()) {
+        uint32_t bytes = 0;
+#pragma unroll
+        for (int b = 0; b < MT_T * kNBox; ++b)
+          if (t.y0 + (b / kNBox) * p.TH < p.Ho) bytes += static_cast<uint32_t>(p.TW * p.TH * ((b % kNBox + 1) * kCW <= BN_T ? 128 : stage_narrow_row(BN_T, true)));
+        mbar_arrive_expect_tx(st_empty, bytes);
+#pragma unroll
+        for (int b = 0; b < MT_T * kNBox; ++b) {
+          const int m = b / kNBox, c = b % kNBox;
+          if (t.y0 + m * p.TH >= p.Ho) continue;
+          tma_load_4d(stage + (stage_place(BN_T, true, b) & 0xffff), (c + 1) * kCW <= BN_T ? &p.tmR : &p.tmR2, st_empty,
+                      t.n0 + c * kCW, t.x0, t.y0 + m * p.TH, t.img);
+        }
+      }
+    } else {
+      if (elect_one_sync()) mbar_arrive(st_empty);
+    }
+    __syncwarp();
+  };
+  if (static_cast<int>(blockIdx.x) < total_tiles) hand_back(tile_of(blockIdx.x));
+  uint32_t parity = 0;
+  for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
+    const Tile t = tile_of(item);
+#pragma unroll
+    for (int pass = 0; pass < kPasses; ++pass) {
+      mbar_wait_inl(st_full, parity, 8);
+      parity ^= 1u;
+      if (elect_one_sync()) {
+#pragma unroll
+        for (int b = 0; b < MT_T * kNBox; ++b) {
+          const int m = b / kNBox, c = b % kNBox;
+          if ((stage_place(BN_T, kOutBf16, b) >> 16) != pass || t.y0 + m * p.TH >= p.Ho) continue;
+          tma_store_4d((c + 1) * kCW <= BN_T ? &p.tmO : &p.tmO2, stage + (stage_place(BN_T, kOutBf16, b) & 0xffff),
+                       t.n0 + c * kCW, t.x0, t.y0 + m * p.TH, t.img);
+        }
+        tma_store_commit();
+      }
+      // TMA stores write whole 16-byte groups of channels: the output map ends at p.cout_tma (Cout rounded down to 16
+      // bytes), and the warp copies the channels from there to Cout (196 = 192 + 4) with plain stores
+      if (p.cout_tma < p.Cout) {
+        const int c_lo = max(p.cout_tma - t.n0, 0), c_hi = min(p.Cout - t.n0, BN_T);
+        for (int m = 0; m < MT_T; ++m)
+          for (int row = static_cast<int>(threadIdx.x & 31); row < p.TW * p.TH; row += 32) {
+            const int ly = row / p.TW, y = t.y0 + m * p.TH + ly, x = t.x0 + row - ly * p.TW;
+            if (y >= p.Ho || x >= p.Wo) continue;
+            const long long o = t.img * p.out_img_stride + static_cast<long long>(y) * p.out_y_stride + static_cast<long long>(x) * p.ldo + t.n0;
+            for (int cl = c_lo; cl < c_hi; cl += 2) {
+              const int c = cl / kCW, b = m * kNBox + c;
+              if ((stage_place(BN_T, kOutBf16, b) >> 16) != pass) continue;
+              const uint32_t box = stage + (stage_place(BN_T, kOutBf16, b) & 0xffff);
+              const int cc = cl - c * kCW;
+              const uint32_t addr = (c + 1) * kCW <= BN_T ? sw_addr(box, row, kOutBf16 ? cc : 2 * cc, 0)
+                                                          : box + static_cast<uint32_t>(row * stage_narrow_row(BN_T, kOutBf16) + cc * (kOutBf16 ? 2 : 4));
+              if constexpr (kOutBf16) {
+                uint32_t v;
+                asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+                *reinterpret_cast<uint32_t*>(reinterpret_cast<uint16_t*>(p.out) + o + cl) = v;
+              } else {
+                float2 v;
+                asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+                *reinterpret_cast<float2*>(p.out + o + cl) = v;
+              }
+            }
+          }
+      }
+      if (elect_one_sync()) tma_store_wait_read();
+      __syncwarp();
+      if (pass + 1 < kPasses) hand_back(t);
+      else if (item + static_cast<int>(gridDim.x) < total_tiles) hand_back(tile_of(item + gridDim.x));
     }
   }
+  if (elect_one_sync()) tma_store_wait_all();
+  __syncwarp();
 }
 
 // BN_T = N tile (wgmma N), MT_T = 128-pixel sub-tiles per CTA tile, BF16 = operand type, EPI = epilogue kind (kEpiAny:
@@ -190,11 +372,12 @@ __device__ __forceinline__ void epilogue_fixed(const ConvGemmParams& p, const fl
 template <int BN_T, int MT_T, bool BF16, int EPI>
 __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t s_bars[4 * kMaxSlots];
+  __shared__ __align__(8) uint64_t s_bars[4 * kMaxSlots + 2];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t smem_a = smem_base;
-  const uint32_t smem_b = smem_base + p.a_slots * p.a_slot_bytes;
-  const uint32_t smem_zero = smem_base + kRingBytes;
+  const uint32_t smem_zero = smem_base;
+  const uint32_t smem_a = smem_base + kZeroBytes;
+  const uint32_t smem_b = smem_a + p.a_slots * p.a_slot_bytes;
+  const uint32_t stage = smem_a + kOperandBytes - p.stage_bytes;   // TMA-store epilogue: the top of the operand space
   const uint32_t bar_base = smem_u32(s_bars);
   // barriers: a_full[8], a_empty[8], b_full[8], b_empty[8]. Generic mode uses one ring (A and B tile of a k-block share
   // slot and barriers: the "a" set); halo mode uses both rings. An empty barrier completes when every MMA warp released it.
@@ -202,6 +385,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
   auto a_empty = [&](int s) { return bar_base + 8u * (kMaxSlots + s); };
   auto b_full = [&](int s) { return bar_base + 8u * (2 * kMaxSlots + s); };
   auto b_empty = [&](int s) { return bar_base + 8u * (3 * kMaxSlots + s); };
+  const uint32_t st_empty = bar_base + 8u * (4 * kMaxSlots), st_full = st_empty + 8u;   // staging buffer free / filled
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);   // warp-uniform role
   const int lane = threadIdx.x & 31;
@@ -212,6 +396,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmB);
+    if constexpr (EPI != kEpiAny) {
+      mbar_init(st_empty, 1);
+      mbar_init(st_full, 1);
+    }
     for (int s = 0; s < kMaxSlots; ++s) {
       mbar_init(a_full(s), 1);
       mbar_init(a_empty(s), kMmaWarps);
@@ -309,6 +497,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
         }
       }
     }
+  } else if (warp == 1) {
+    // ------------------------------------------------------------------ TMA store warp
+    if constexpr (EPI != kEpiAny) store_warp<BN_T, MT_T, EPI>(p, stage, st_empty, st_full, total_tiles, tiles_x, tile_rows);
   } else if (warp >= 4) {
     // ------------------------------------------------------------------ MMA + epilogue warpgroups
     const int wg = (warp - 4) >> 2;                   // rows 64 wg .. 64 wg + 63 of each sub-tile
@@ -408,13 +599,19 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
 #pragma unroll
       for (int m = 0; m < MT_T; ++m) wgmma_fence_regs(acc[m]);
       release();
-      const int tx = mt % tiles_x;
-      const int ty = (mt / tiles_x) % p.tiles_y;
-      const int img = mt / (tiles_x * p.tiles_y);
+      if constexpr (EPI == kEpiAny) {
+        const int tx = mt % tiles_x;
+        const int ty = (mt / tiles_x) % p.tiles_y;
+        const int img = mt / (tiles_x * p.tiles_y);
 #pragma unroll
-      for (int m = 0; m < MT_T; ++m) {
-        if constexpr (EPI == kEpiAny) epilogue_subtile<BN_T>(p, acc[m], row0, lane, nt * p.BN, tx, ty, img, m, tile_rows, w_lim, vec2);
-        else epilogue_fixed<BN_T, EPI>(p, acc[m], row0, lane, nt * p.BN, tx, ty, img, m, tile_rows);
+        for (int m = 0; m < MT_T; ++m)
+          epilogue_subtile<BN_T>(p, acc[m], row0, lane, nt * p.BN, tx, ty, img, m, tile_rows, w_lim, vec2);
+      } else {
+        // staging address and barriers recomputed here: nothing extra stays live across the main loop
+        const uint32_t stage_ = ((smem_u32(smem_raw) + 1023u) & ~1023u) + kZeroBytes + kOperandBytes - p.stage_bytes;
+        const uint32_t bars = smem_u32(s_bars) + 8u * (4 * kMaxSlots);
+        epilogue_staged<BN_T, MT_T, EPI>(p, acc, stage_, bars, bars + 8u, (item - static_cast<int>(blockIdx.x)) / static_cast<int>(gridDim.x),
+                                         row0 - (lane >> 2), lane, nt * p.BN);
       }
     }
   }
@@ -461,10 +658,12 @@ int bn_for(int cols) {
 //   MMA      : one 128 x BN x (32 B of K) step, issued as two m64 wgmma, ~ 30 + 0.25 * BN; every wgmma group waits for
 //              its predecessor, ~ 200 per group; a k-block always issues 4 steps
 //   feed     : operand bytes through L2 -> shared memory at ~ 100 bytes per unit per SM when all SMs pull at once
-//   epilogue : ~ 500 per 32-channel chunk of a 128-pixel sub-tile
+//   epilogue : ~ 500 per 32-channel chunk of a 128-pixel sub-tile (run-time generic epilogue), kEpiStagedUnit with the
+//              TMA-store epilogue
 // times the number of waves of tiles over the SMs.
 struct RingCfg { int a_slots, b_slots, a_slot_bytes; };
-RingCfg ring_cfg(int halo, bool kx_major, int MT, int TW, int TH, int BN) {
+// ring_bytes: what the staging buffer of the TMA-store epilogue leaves of kOperandBytes
+RingCfg ring_cfg(int halo, bool kx_major, int MT, int TW, int TH, int BN, int ring_bytes) {
   RingCfg r{};
   const int b_bytes = BN * 128;
   if (halo) {
@@ -475,20 +674,23 @@ RingCfg ring_cfg(int halo, bool kx_major, int MT, int TW, int TH, int BN) {
     for (int min_b : {6, 4}) {
       for (int a = 3; a >= (kx_major ? 2 : 3); --a) {
         r.a_slots = a;
-        r.b_slots = std::min(kMaxSlots, (kRingBytes - a * r.a_slot_bytes) / b_bytes);
+        r.b_slots = std::min(kMaxSlots, (ring_bytes - a * r.a_slot_bytes) / b_bytes);
         if (r.b_slots >= min_b) return r;
       }
     }
   } else {
     // generic mode pads the A slot to whole 128-row sub-tiles (the MMA reads 128 rows regardless)
     r.a_slot_bytes = std::max((TW * TH * MT * 128 + 1023) / 1024 * 1024, MT * kAStage);
-    r.a_slots = r.b_slots = std::min(kMaxSlots, kRingBytes / (r.a_slot_bytes + b_bytes));
+    r.a_slots = r.b_slots = std::min(kMaxSlots, ring_bytes / (r.a_slot_bytes + b_bytes));
   }
   return r;
 }
 
+// staging bytes of the TMA-store epilogue (staged: -1 none, 0 fp32, 1 bf16 output; only the BN >= 128 tiles have it)
+int staging_for(int staged, int MT, int BN) { return (staged >= 0 && BN >= 128) ? stage_bytes(BN, staged != 0, MT) : 0; }
+
 TileCfg choose_cfg(int N, int Ho, int Wo, int Cout, int R, int S, int stride, int pad, int kb_per_tap,
-                   bool tail32, bool kx_major, bool allow_mt2, bool single_row_tiles = false) {
+                   bool tail32, bool kx_major, bool allow_mt2, bool single_row_tiles, int staged) {
   const int sms = conv_gemm_num_sms();
   const int c8 = (Cout + 7) / 8 * 8;
   const int taps = R * S;
@@ -520,7 +722,8 @@ TileCfg choose_cfg(int N, int Ho, int Wo, int Cout, int R, int S, int stride, in
           const int box_rows = halo ? MT * th + 2 : MT * th * stride;
           if (box_rows > 256) continue;
           const long long tiles = static_cast<long long>(N) * ((Wo + tw - 1) / tw) * ((Ho + MT * th - 1) / (MT * th)) * nt;
-          const RingCfg rc = ring_cfg(halo, kx_major, MT, tw, th, BN);
+          const int st_bytes = staging_for(staged, MT, BN);
+          const RingCfg rc = ring_cfg(halo, kx_major, MT, tw, th, BN, kOperandBytes - st_bytes);
           // the MMA warps hold the slots of one wgmma group while they wait for the next group's
           if (rc.a_slots < (halo && !kx_major ? 3 : 2) || rc.b_slots < (halo ? 4 : 2)) continue;
           const double groups = static_cast<double>(taps) * kb_per_tap;   // one wgmma group per (tap, k-block)
@@ -529,7 +732,7 @@ TileCfg choose_cfg(int N, int Ho, int Wo, int Cout, int R, int S, int stride, in
                                       : static_cast<double>(tw) * th * MT * 128.0 * taps * kb_per_tap;
           const double b_bytes = static_cast<double>(BN) * 128.0 * taps * kb_per_tap;
           const double l2 = (a_bytes + b_bytes) / 100.0;
-          const double epi = MT * ((BN + 31) / 32) * 500.0;
+          const double epi = MT * ((BN + 31) / 32) * (st_bytes > 0 ? kEpiStagedUnit : 500.0);
           // the epilogue does not overlap the main loop of the same warps: the two add up
           const double t = std::max(mma, l2) + epi + 800.0;
           double cost = static_cast<double>((tiles + sms - 1) / sms) * t;
@@ -594,26 +797,8 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
   // never changes the result bits: kx-major for 3x3 stride-1 convs with at most 128 output channels, ky-major
   // otherwise (the orders the engine's convs have been summed in since halo mode exists)
   p->kx_major = (d.R == 3 && d.S == 3 && d.stride == 1 && d.pad == 1 && d.Cout <= 128) ? 1 : 0;
-  const TileCfg cfg = choose_cfg(d.N, p->Ho, p->Wo, d.Cout, d.R, d.S, d.stride, d.pad, p->kb_per_tap, p->tail32 != 0,
-                                 p->kx_major != 0, d.dyn_w == nullptr && d.b_batched != 2, d.b_batched == 2);
-  p->TW = cfg.TW; p->TH = cfg.TH; p->MT = cfg.MT; p->halo = cfg.halo;
-  p->BN = cfg.BN; p->n_tiles = cfg.n_tiles;
-  p->nt_fast = (!p->halo && p->n_tiles > 1 && getenv("MFR_CONV_NT_SLOW") == nullptr) ? 1 : 0;
-  p->tiles_x = (p->Wo + p->TW - 1) / p->TW;
-  p->tiles_y = (p->Ho + p->MT * p->TH - 1) / (p->MT * p->TH);
-  p->in_bf16 = d.in_bf16;
-  p->out_bf16 = d.out_bf16;
-  p->b_batched = d.b_batched;
-  const int a_rows = p->halo ? p->MT * p->TH + 2 : p->MT * p->TH;   // pixel rows of the A box
-  p->a_bytes = p->TW * a_rows * 128;
-  p->b_bytes = p->BN * 128;                                           // multiple of 1 KB (BN % 8 == 0)
-  {
-    const RingCfg rc = ring_cfg(p->halo, p->kx_major != 0, p->MT, p->TW, p->TH, p->BN);
-    p->a_slot_bytes = rc.a_slot_bytes; p->a_slots = rc.a_slots; p->b_slots = rc.b_slots;
-  }
-  if (p->a_slots < (p->halo && !p->kx_major ? 3 : 2) || p->b_slots < (p->halo ? 4 : 2)) return MFR_ERR_ARG;
   p->act = d.act;
-  p->act_cols = d.act_cols > 0 ? d.act_cols : d.Cout;
+  p->act_cols = (d.act_cols > 0 && d.act != ACT_NONE) ? d.act_cols : d.Cout;   // without an activation act_cols is moot
   p->dyn_w = d.dyn_w;
   if (d.dyn_w != nullptr && (d.H != 1 || d.R != 1 || d.S != 1 || d.stride != 1)) return MFR_ERR_ARG;
   p->alpha = d.alpha;
@@ -626,10 +811,64 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
   p->out_img_stride = d.out_img_stride > 0 ? d.out_img_stride : static_cast<long long>(p->Ho) * p->Wo * d.ldo;
   p->b_xor = d.b_xor;
   p->res_img_stride = static_cast<long long>(p->Ho) * p->Wo * d.ldr;
+  // compile-time epilogue kind with TMA stores: bf16 operands, every column activated, no device row count, one B
+  // operand per image at most, and output / residual rows that tensor maps can address (16-byte strides and pointers)
   p->epi = kEpiAny;
-  if (d.in_bf16 && d.dyn_w == nullptr && p->act_cols >= p->Cout && epilogue_vec2(*p) &&
-      (reinterpret_cast<uintptr_t>(d.bias) & 7) == 0)
-    p->epi = epi_kind(d.out_bf16 != 0, d.residual != nullptr, d.act);
+  {
+    const int osz = d.out_bf16 ? 2 : 4;
+    auto a16 = [](long long bytes) { return bytes % 16 == 0; };
+    const int kind = epi_kind(d.out_bf16 != 0, d.residual != nullptr, d.act);
+    if (d.in_bf16 && d.dyn_w == nullptr && d.b_batched != 2 && p->act_cols >= p->Cout && staged_kind(kind) &&
+        epilogue_vec2(*p) && (reinterpret_cast<uintptr_t>(d.bias) & 7) == 0 && (reinterpret_cast<uintptr_t>(d.out) & 15) == 0 &&
+        a16(p->ldo * osz) && a16(p->out_y_stride * osz) && a16(p->out_img_stride * osz) &&
+        (d.residual == nullptr || ((reinterpret_cast<uintptr_t>(d.residual) & 15) == 0 && a16(p->ldr * osz))))
+      p->epi = kind;
+  }
+  const TileCfg cfg = choose_cfg(d.N, p->Ho, p->Wo, d.Cout, d.R, d.S, d.stride, d.pad, p->kb_per_tap, p->tail32 != 0,
+                                 p->kx_major != 0, d.dyn_w == nullptr && d.b_batched != 2, d.b_batched == 2,
+                                 p->epi == kEpiAny ? -1 : (d.out_bf16 ? 1 : 0));
+  p->TW = cfg.TW; p->TH = cfg.TH; p->MT = cfg.MT; p->halo = cfg.halo;
+  p->BN = cfg.BN; p->n_tiles = cfg.n_tiles;
+  p->nt_fast = (!p->halo && p->n_tiles > 1 && getenv("MFR_CONV_NT_SLOW") == nullptr) ? 1 : 0;
+  p->tiles_x = (p->Wo + p->TW - 1) / p->TW;
+  p->tiles_y = (p->Ho + p->MT * p->TH - 1) / (p->MT * p->TH);
+  p->in_bf16 = d.in_bf16;
+  p->out_bf16 = d.out_bf16;
+  p->b_batched = d.b_batched;
+  const int a_rows = p->halo ? p->MT * p->TH + 2 : p->MT * p->TH;   // pixel rows of the A box
+  p->a_bytes = p->TW * a_rows * 128;
+  p->b_bytes = p->BN * 128;                                           // multiple of 1 KB (BN % 8 == 0)
+  if (p->BN < 128) p->epi = kEpiAny;   // the narrow N tiles run the run-time generic epilogue
+  p->stage_bytes = staging_for(p->epi == kEpiAny ? -1 : (d.out_bf16 ? 1 : 0), p->MT, p->BN);
+  {
+    const RingCfg rc = ring_cfg(p->halo, p->kx_major != 0, p->MT, p->TW, p->TH, p->BN, kOperandBytes - p->stage_bytes);
+    p->a_slot_bytes = rc.a_slot_bytes; p->a_slots = rc.a_slots; p->b_slots = rc.b_slots;
+  }
+  if (p->a_slots < (p->halo && !p->kx_major ? 3 : 2) || p->b_slots < (p->halo ? 4 : 2)) return MFR_ERR_ARG;
+  if (p->epi != kEpiAny) {   // output / residual: {Cout, Wo, Ho, N}; the bounds clip ragged tiles and channels >= Cout
+    const int osz = d.out_bf16 ? 2 : 4, cw = stage_cw(d.out_bf16 != 0);
+    const CUtensorMapDataType dt = d.out_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    // TMA stores write whole 16-byte groups: the output map ends at the last full group, the rest goes from registers
+    p->cout_tma = d.Cout / (16 / osz) * (16 / osz);
+    cuuint64_t dims[4] = {(cuuint64_t)p->cout_tma, (cuuint64_t)p->Wo, (cuuint64_t)p->Ho, (cuuint64_t)d.N};
+    cuuint32_t box[4] = {(cuuint32_t)cw, (cuuint32_t)p->TW, (cuuint32_t)p->TH, 1};
+    cuuint32_t box2[4] = {(cuuint32_t)(p->BN % cw), (cuuint32_t)p->TW, (cuuint32_t)p->TH, 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    auto encode = [&](CUtensorMap* tm, CUtensorMap* tm2, const float* ptr, long long ld, long long y_stride, long long img_stride) {
+      cuuint64_t strides[3] = {(cuuint64_t)(ld * osz), (cuuint64_t)(y_stride * osz), (cuuint64_t)(img_stride * osz)};
+      CUresult r = enc(tm, dt, 4, const_cast<float*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (r == CUDA_SUCCESS && box2[0] > 0)
+        r = enc(tm2, dt, 4, const_cast<float*>(ptr), dims, strides, box2, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      return r == CUDA_SUCCESS;
+    };
+    bool ok = encode(&p->tmO, &p->tmO2, d.out, p->ldo, p->out_y_stride, p->out_img_stride);
+    dims[0] = d.Cout;   // the residual is read up to Cout (channels beyond come back as zeros)
+    if (ok && d.residual != nullptr)
+      ok = encode(&p->tmR, &p->tmR2, d.residual, p->ldr, static_cast<long long>(p->Wo) * p->ldr, p->res_img_stride);
+    if (!ok) p->epi = kEpiAny;   // strides a tensor map cannot take: the run-time generic epilogue (the ring stays valid)
+  }
 
   {  // activations: {C, W, H, N}
     cuuint64_t dims[4] = {(cuuint64_t)d.Cin, (cuuint64_t)d.W, (cuuint64_t)d.H, (cuuint64_t)d.N};
@@ -733,10 +972,7 @@ int launch_one(const ConvGemmParams& p, int grid, cudaStream_t stream) {
 template <int BN_T, int MT_T>
 int launch_inst(const ConvGemmParams& p, int grid, cudaStream_t stream) {
   if (!p.in_bf16) return launch_one<BN_T, MT_T, false, kEpiAny>(p, grid, stream);
-  if constexpr (BN_T >= 128) {   // the N tiles of the ResNet-FPN convs: their epilogue kinds have their own instantiations
-    constexpr int kBf = epi_kind(true, false, ACT_NONE), kBfRelu = epi_kind(true, false, ACT_RELU),
-                  kBfLeaky = epi_kind(true, false, ACT_LEAKY), kBfResRelu = epi_kind(true, true, ACT_RELU),
-                  kF32 = epi_kind(false, false, ACT_NONE);
+  if constexpr (BN_T >= 128) {   // the compile-time epilogue kinds (TMA stores) have their own instantiations
     switch (p.epi) {
       case kBf: return launch_one<BN_T, MT_T, true, kBf>(p, grid, stream);
       case kBfRelu: return launch_one<BN_T, MT_T, true, kBfRelu>(p, grid, stream);

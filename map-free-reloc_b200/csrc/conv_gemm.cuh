@@ -18,6 +18,10 @@ struct alignas(64) ConvGemmParams {
   CUtensorMap tmB;  // rank 3 {Cin, Z, Cout} box {32, 1, BN}          (Z = filter tap or image)
   CUtensorMap tmA2; // channel tail (tail32): same tensors, 32-byte-wide boxes, 32B swizzle — the last k-block of a tap then moves
   CUtensorMap tmB2; //   a quarter of the bytes (Cin = 196 leaves 4 channels for it) and issues one MMA per tap
+  CUtensorMap tmO;  // TMA-store epilogue (epi >= 0): output rank 4 {Cout, Wo, Ho, N}, box {64 bf16 | 32 fp32, TW, TH, 1}, 128B swizzle
+  CUtensorMap tmO2; //   the narrow last box of a BN = 200 tile: {BN % 64 | BN % 32 channels, TW, TH, 1}, no swizzle
+  CUtensorMap tmR;  //   residual, same boxes as tmO / tmO2 (loaded into the staging buffer)
+  CUtensorMap tmR2;
   int N, Ho, Wo, Cout, Cin;
   int R, S, stride, pad;
   int TW, TH, tiles_x, tiles_y;
@@ -36,7 +40,10 @@ struct alignas(64) ConvGemmParams {
   int tail32;             // the tail fits one 32-byte k-step: it is loaded through tmA2 / tmB2 (a_bytes2 / b_bytes2 per load)
   int a_bytes2, b_bytes2;
   int act, act_cols;    // activation applies to output channels < act_cols
-  int epi;              // epilogue kind with a compile-time body (conv_gemm.cu: epi_kind), -1: run-time generic epilogue
+  int epi;              // epilogue kind with a compile-time body and TMA stores (conv_gemm.cu: epi_kind), -1: run-time
+                        // generic epilogue
+  int stage_bytes;      // shared-memory staging buffer of the TMA-store epilogue (0: none)
+  int cout_tma;         // channels written by the TMA stores (Cout rounded down to 16 bytes; the rest from registers)
   int in_bf16, out_bf16;  // operands bf16 instead of fp32 (tf32 MMA); out/residual bf16
   int kblk;             // K elements per 128-byte k-block: 32 (fp32) or 64 (bf16)
   const int* dyn_w;     // optional device int: effective W (rows of a token GEMM), H must be 1

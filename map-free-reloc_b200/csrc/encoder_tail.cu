@@ -72,12 +72,6 @@ __device__ __forceinline__ uint32_t wtile(const EncoderTailParams& p, int t, con
   return kWTile;
 }
 
-// byte address of element (row, col) in a 128B-swizzled stack of 64-column k-blocks (the TMA / wgmma layout)
-__device__ __forceinline__ uint32_t sw_addr(uint32_t base, int row, int col) {
-  const int c64 = col & 63;
-  return base + static_cast<uint32_t>((col >> 6) * kKb + row * 128 + (((c64 >> 3) ^ (row & 7)) << 4) + (c64 & 7) * 2);
-}
-
 __device__ __forceinline__ uint32_t bf16x2(float lo, float hi) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
@@ -208,7 +202,7 @@ __global__ void __launch_bounds__(kThreads) encoder_tail_kernel(const __grid_con
           const int col = nh * 128 + 8 * j + cq;
           const float y0 = (acc[nh][4 * j + 2 * h] - mean) * rstd * __ldg(p.g1 + col) + __ldg(p.b1 + col);
           const float y1 = (acc[nh][4 * j + 2 * h + 1] - mean) * rstd * __ldg(p.g1 + col + 1) + __ldg(p.b1 + col + 1);
-          asm volatile("st.shared.u32 [%0], %1;" ::"r"(sw_addr(sA, rq + 8 * h, C + col)), "r"(bf16x2(y0, y1)) : "memory");
+          asm volatile("st.shared.u32 [%0], %1;" ::"r"(sw_addr(sA, rq + 8 * h, C + col, kKb)), "r"(bf16x2(y0, y1)) : "memory");
         }
     }
     fence_proxy_async_smem();
@@ -234,7 +228,7 @@ __global__ void __launch_bounds__(kThreads) encoder_tail_kernel(const __grid_con
 #pragma unroll
         for (int j = 0; j < G::QW / 8; ++j) {
           const float y0 = fmaxf(acc2[4 * j + 2 * h], 0.f), y1 = fmaxf(acc2[4 * j + 2 * h + 1], 0.f);
-          asm volatile("st.shared.u32 [%0], %1;" ::"r"(sw_addr(sH, rq + 8 * h, 8 * j + cq)), "r"(bf16x2(y0, y1)) : "memory");
+          asm volatile("st.shared.u32 [%0], %1;" ::"r"(sw_addr(sH, rq + 8 * h, 8 * j + cq, kKb)), "r"(bf16x2(y0, y1)) : "memory");
         }
       fence_proxy_async_smem();
       __syncthreads();

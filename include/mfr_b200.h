@@ -173,6 +173,47 @@ int mfr_knn2_l2(const float* query, int nq, const float* train, int nt, int dim,
                 float* dist1, int* idx2, float* dist2, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * SIFT detector + descriptor engine. Replaces cv2.SIFT_create(nfeatures).detectAndCompute of the reference's SIFT
+ * plugins (lib/models/matching/feature_matching.py:58,88-89, etc/feature_matching_baselines/matchers.py:158-161) at
+ * OpenCV's default settings (3 layers per octave, contrast threshold 0.04, edge threshold 10, sigma 1.6, doubled
+ * first octave, CV_32F descriptors), for B uint8 gray images [B][H][W] of one size per call (device memory).
+ * nfeatures = 0: no cap; else retainBest(nfeatures): every keypoint whose response is >= the N-th largest (the
+ * orientations of one point share a response, so an image may return more than N). max_candidates caps the refined
+ * extrema and the oriented keypoints of an image; the true counts are reported, so the caller can detect an
+ * overflow (results are then incomplete). root_sift != 0: descriptors are RootSIFT rows (L1 normalisation with
+ * eps 1e-7, square root: feature_matching.py:67-73). Keypoints of an image are ordered by response descending, then
+ * x, y, size, angle ascending. Deterministic: the same images give bit-identical outputs, whatever the batch. */
+typedef struct mfr_sift mfr_sift;
+typedef struct {
+  const int* counts;          /* device int[B] keypoints per image */
+  const int* raw_counts;      /* device int[B] oriented keypoints before duplicate removal / retainBest */
+  const int* extrema_counts;  /* device int[B] refined extrema before orientation assignment */
+  const float* keypoints;     /* device float[B][capacity][5]: x, y, size, angle, response (cv2.KeyPoint fields) */
+  const int* octaves;         /* device int[B][capacity]: cv2.KeyPoint.octave (packed octave | layer << 8 | ...) */
+  const float* descriptors;   /* device float[B][capacity][128] */
+  int capacity;               /* = max_candidates */
+} mfr_sift_outputs;
+int mfr_sift_create(int B, int H, int W, int nfeatures, int max_candidates, int root_sift, mfr_sift** out);
+void mfr_sift_destroy(mfr_sift* h);
+/* imgs: device uint8 [B][H][W]. One static launch list (replayed as a CUDA graph unless disabled). */
+int mfr_sift_detect(mfr_sift* h, const unsigned char* imgs, void* stream);
+void mfr_sift_set_graph(mfr_sift* h, int enabled);
+int mfr_sift_get_outputs(mfr_sift* h, mfr_sift_outputs* out);
+/* Lowe ratio matching of the last detect for P = B / 2 pairs (images 2p, 2p + 1), the matcher of the SIFT plugins
+ * (feature_matching.py:91-99, matchers.py:163-175) with an exact 2-NN (mfr_knn2_l2's search): query p's keypoint i
+ * matches its nearest neighbour j in image 2p + 1 when d1 < ratio * d2 (and image 2p + 1 has >= 2 keypoints).
+ * Matches are written in query order into caller-owned device buffers in the pose back end's layout:
+ * kpts0 / kpts1 float[P * capacity][2] (x, y of keypoint i of image 2p / j of image 2p + 1), offsets int[P + 1]. */
+int mfr_sift_match_pairs(mfr_sift* h, float ratio, float* kpts0, float* kpts1, int* offsets, void* stream);
+/* named intermediate buffers for stage tests: "gauss_<o>" float[B][6][h_o][w_o], "dog_<o>" float[B][5][h_o][w_o]
+ * (o = 0 is the doubled image), "kp_pre" float[B][capacity][5] / "kp_pre_octave" int[B][capacity] (oriented keypoints
+ * before selection, internal octave coordinates, unordered), "counters" int[3][B] (extrema, oriented, selected) */
+int mfr_sift_debug_tensor(mfr_sift* h, const char* name, float** ptr, long long* numel);
+/* Eager detect with CUDA events between the stages: ms (host float[5]) = pyramid, extrema + refinement, orientation,
+ * selection, descriptors. */
+int mfr_sift_profile(mfr_sift* h, const unsigned char* imgs, float* ms, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Pose back end (batched-hypothesis RANSAC). Replaces lib/models/matching/pose_solver.py.
  * Correspondences of P pairs are concatenated: kpts0/kpts1 device float[total][2] in pixels (x,y),
  * offsets device int[P+1]; K0/K1 device float[P][9] row-major intrinsics; depth maps device

@@ -15,6 +15,8 @@ FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xptxas", "-v",
 ]
+# sift.cu restates OpenCV's float arithmetic operation by operation: no contraction into FMAs
+FILE_FLAGS = {"sift.cu": ["-fmad=false"]}
 
 
 def sources():
@@ -41,7 +43,7 @@ def build(force=False, verbose=True):
     for src in sources():
         obj = os.path.join(build_dir, os.path.basename(src)[:-3] + ".o")
         objs.append(obj)
-        cmd = [NVCC, *FLAGS, "-c", src, "-o", obj]
+        cmd = [NVCC, *FLAGS, *FILE_FLAGS.get(os.path.basename(src), []), "-c", src, "-o", obj]
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
     ok = True
     for src, p in procs:

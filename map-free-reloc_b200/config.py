@@ -6,7 +6,8 @@ pre-declared keys may be set. The reference's yaml files load unchanged.
 
 Additive keys (not in the reference): FEATURE_MATCHING may also be 'LoFTR' (fused on-GPU matcher),
 LOFTR.{WEIGHTS, THR, BORDER_RM, TEMPERATURE, BATCH}, GPU_RANSAC.{NUM_HYPOTHESES, MAX_HYPOTHESES, SEED,
-LOCAL_OPTIMISATION, FINAL_REFIT}.
+LOCAL_OPTIMISATION, FINAL_REFIT}, SIFT.GPU_DETECTOR (False: OpenCV's host SIFT as in the reference; True: the CUDA
+SIFT engine detects, describes and ratio-matches on the device).
 """
 import copy
 
@@ -57,7 +58,7 @@ def get_default_cfg():
     return _node({
         "MODEL": None, "DEBUG": False,
         "FEATURE_MATCHING": None, "POSE_SOLVER": None,
-        "SIFT": {"NUM_FEATURES": None, "RATIO_THRESHOLD": None},
+        "SIFT": {"NUM_FEATURES": None, "RATIO_THRESHOLD": None, "GPU_DETECTOR": False},
         "MATCHES_FILE_PATH": None,
         "EMAT_RANSAC": {"PIX_THRESHOLD": None, "SCALE_THRESHOLD": None, "CONFIDENCE": None},
         "PROCRUSTES": {"MAX_CORR_DIST": None, "REFINE": False},

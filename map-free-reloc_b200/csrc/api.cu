@@ -12,6 +12,7 @@
 #include "geometry_solvers.cuh"
 #include "geometry.cuh"
 #include "descriptor_match.cuh"
+#include "sift.cuh"
 
 namespace mfr {   // image_io.cu
 int resize_linear(const void* src, int src_is_u8, int sw, int sh, long long src_stride, int channels, float* dst, int dw, int dh,
@@ -184,6 +185,42 @@ int mfr_coarse_match(const float* sim, int B, int h_c, int w_c, float thr, int b
 int mfr_knn2_l2(const float* query, int nq, const float* train, int nt, int dim, int* idx1, float* dist1,
                 int* idx2, float* dist2, void* stream) {
   return mfr::knn2_l2(query, nq, train, nt, dim, idx1, dist1, idx2, dist2, static_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------------------------------ SIFT
+struct mfr_sift { mfr::SiftEngine* e; };
+int mfr_sift_create(int B, int H, int W, int nfeatures, int max_candidates, int root_sift, mfr_sift** out) {
+  if (!out) return MFR_ERR_ARG;
+  mfr::SiftEngine* e = nullptr;
+  int rc = mfr::sift_create(B, H, W, nfeatures, max_candidates, root_sift, &e);
+  if (rc != MFR_OK) return rc;
+  *out = new mfr_sift{e};
+  return MFR_OK;
+}
+void mfr_sift_destroy(mfr_sift* h) { if (h) { mfr::sift_destroy(h->e); delete h; } }
+int mfr_sift_detect(mfr_sift* h, const unsigned char* imgs, void* stream) {
+  if (!h) return MFR_ERR_ARG;
+  return mfr::sift_detect(h->e, imgs, static_cast<cudaStream_t>(stream));
+}
+void mfr_sift_set_graph(mfr_sift* h, int enabled) { if (h) mfr::sift_set_graph(h->e, enabled); }
+int mfr_sift_get_outputs(mfr_sift* h, mfr_sift_outputs* out) {
+  if (!h || !out) return MFR_ERR_ARG;
+  mfr::SiftOutputs o = mfr::sift_outputs(h->e);
+  out->counts = o.counts; out->raw_counts = o.raw_counts; out->extrema_counts = o.extrema_counts;
+  out->keypoints = o.keypoints; out->octaves = o.octaves; out->descriptors = o.descriptors; out->capacity = o.capacity;
+  return MFR_OK;
+}
+int mfr_sift_match_pairs(mfr_sift* h, float ratio, float* kpts0, float* kpts1, int* offsets, void* stream) {
+  if (!h) return MFR_ERR_ARG;
+  return mfr::sift_match_pairs(h->e, ratio, kpts0, kpts1, offsets, static_cast<cudaStream_t>(stream));
+}
+int mfr_sift_debug_tensor(mfr_sift* h, const char* name, float** ptr, long long* numel) {
+  if (!h || !name || !ptr || !numel) return MFR_ERR_ARG;
+  return mfr::sift_debug_tensor(h->e, name, ptr, numel);
+}
+int mfr_sift_profile(mfr_sift* h, const unsigned char* imgs, float* ms, void* stream) {
+  if (!h) return MFR_ERR_ARG;
+  return mfr::sift_profile(h->e, imgs, ms, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------ pose back end

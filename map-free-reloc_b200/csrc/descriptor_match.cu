@@ -5,6 +5,8 @@
 // (= cv2.BFMatcher(NORM_L2).knnMatch), so integer match indices are reproducible bit for bit.
 #include "descriptor_match.cuh"
 
+#include <algorithm>
+
 namespace mfr {
 
 namespace {
@@ -23,14 +25,23 @@ __device__ __forceinline__ void push(Best2& b, float d, int j) {
   }
 }
 
-// one block (128 threads) per query descriptor; dim <= 256 and a multiple of 4
-__global__ void __launch_bounds__(128) knn2_kernel(const float* __restrict__ q, int nq,
+// one block (128 threads) per query descriptor (grid-stride over queries); dim <= 256 and a multiple of 4.
+// blockIdx.y = pair p: its queries / train rows / outputs start p * q_stride / t_stride / o_stride rows in, and
+// with `counts` non-null the row counts are counts[2p] (queries) and counts[2p + 1] (train), read on the device.
+__global__ void __launch_bounds__(128, 8) knn2_kernel(const float* __restrict__ q, int nq,
                                                    const float* __restrict__ t, int nt, int dim,
                                                    int* __restrict__ idx1, float* __restrict__ dist1,
-                                                   int* __restrict__ idx2, float* __restrict__ dist2) {
+                                                   int* __restrict__ idx2, float* __restrict__ dist2,
+                                                   long long q_stride, long long t_stride, long long o_stride,
+                                                   const int* __restrict__ counts) {
   __shared__ __align__(16) float sq[256];
   __shared__ Best2 sb[4];
-  const int qi = blockIdx.x;
+  const int p = blockIdx.y;
+  if (counts) { nq = counts[2 * p]; nt = counts[2 * p + 1]; }
+  q += p * q_stride * dim; t += p * t_stride * dim;
+  idx1 += p * o_stride; dist1 += p * o_stride; idx2 += p * o_stride; dist2 += p * o_stride;
+  for (int qi = blockIdx.x; qi < nq; qi += gridDim.x) {
+  __syncthreads();
   for (int k = threadIdx.x; k < dim; k += blockDim.x) sq[k] = q[static_cast<size_t>(qi) * dim + k];
   __syncthreads();
   Best2 b{3.0e38f, 3.0e38f, 0x7fffffff, 0x7fffffff};
@@ -67,6 +78,7 @@ __global__ void __launch_bounds__(128) knn2_kernel(const float* __restrict__ q, 
     dist1[qi] = sqrtf(r.d1);
     dist2[qi] = sqrtf(r.d2);
   }
+  }
 }
 
 }  // namespace
@@ -75,7 +87,18 @@ int knn2_l2(const float* q, int nq, const float* t, int nt, int dim, int* idx1, 
             float* dist2, cudaStream_t st) {
   if (nq <= 0) return MFR_OK;
   if (dim > 256 || (dim & 3) || nt < 0) return MFR_ERR_ARG;
-  knn2_kernel<<<nq, 128, 0, st>>>(q, nq, t, nt, dim, idx1, dist1, idx2, dist2);
+  knn2_kernel<<<nq, 128, 0, st>>>(q, nq, t, nt, dim, idx1, dist1, idx2, dist2, 0, 0, 0, nullptr);
+  MFR_CUDA_CHECK(cudaGetLastError());
+  return MFR_OK;
+}
+
+int knn2_l2_pairs(const float* desc, const int* counts, int P, int cap, int dim, int* idx1, float* dist1, int* idx2,
+                  float* dist2, cudaStream_t st) {
+  if (P <= 0 || cap <= 0) return MFR_OK;
+  if (dim > 256 || (dim & 3)) return MFR_ERR_ARG;
+  const dim3 grid(std::min(cap, 1024), P);
+  knn2_kernel<<<grid, 128, 0, st>>>(desc, cap, desc + static_cast<size_t>(cap) * dim, cap, dim, idx1, dist1, idx2, dist2,
+                                    2LL * cap, 2LL * cap, cap, counts);
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
 }

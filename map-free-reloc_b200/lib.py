@@ -29,6 +29,12 @@ class SpsgOutputs(ctypes.Structure):
                 ("mkpts0", c_vp), ("mkpts1", c_vp), ("max_keypoints", c_int)]
 
 
+class SiftOutputs(ctypes.Structure):
+    """mfr_sift_outputs of include/mfr_b200.h."""
+    _fields_ = [("counts", c_vp), ("raw_counts", c_vp), ("extrema_counts", c_vp), ("keypoints", c_vp),
+                ("octaves", c_vp), ("descriptors", c_vp), ("capacity", c_int)]
+
+
 c_pp = ctypes.POINTER(ctypes.c_void_p)
 
 # name -> (restype, argtypes); mirrors include/mfr_b200.h one to one
@@ -69,6 +75,14 @@ SIGNATURES = {
     "mfr_coarse_match": (c_int, [c_vp, c_int, c_int, c_int, c_float, c_int, c_float, c_int, c_vp, c_vp,
                                  c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "mfr_knn2_l2": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "mfr_sift_create": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_pp]),
+    "mfr_sift_destroy": (None, [c_vp]),
+    "mfr_sift_detect": (c_int, [c_vp, c_vp, c_vp]),
+    "mfr_sift_set_graph": (None, [c_vp, c_int]),
+    "mfr_sift_get_outputs": (c_int, [c_vp, ctypes.POINTER(SiftOutputs)]),
+    "mfr_sift_match_pairs": (c_int, [c_vp, c_float, c_vp, c_vp, c_vp, c_vp]),
+    "mfr_sift_debug_tensor": (c_int, [c_vp, ctypes.c_char_p, c_pp, ctypes.POINTER(c_ll)]),
+    "mfr_sift_profile": (c_int, [c_vp, c_vp, c_vp, c_vp]),
     "mfr_pose_solver_create": (c_int, [c_int, c_int, c_int, c_pp]),
     "mfr_pose_solver_destroy": (None, [c_vp]),
     "mfr_emat_ransac": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_float, c_int,

@@ -11,17 +11,35 @@ from .spsg import SuperGlue_matcher
 
 
 class SIFT_matcher:
-    """matchers.py:123-188: 2048 SIFT features, RootSIFT, 2-NN + ratio 0.8 (exact NN on the GPU)."""
+    """matchers.py:123-188: 2048 SIFT features, RootSIFT, 2-NN + ratio 0.8 (exact NN on the GPU).
+    gpu_detector=True: detection, description and matching run on the CUDA SIFT engine (mfr_b200.sift)."""
 
-    def __init__(self, resize, outdoor=False):
+    def __init__(self, resize, outdoor=False, gpu_detector=False):
         self.resize = resize
+        self.gpu_detector = gpu_detector
+        self.engines = {}
 
     def match(self, pair_path):
         import cv2
-        sift = cv2.SIFT_create(2048)
         img0 = cv2.resize(cv2.imread(pair_path[0], 0), self.resize)
         img1 = cv2.resize(cv2.imread(pair_path[1], 0), self.resize)
+        if self.gpu_detector and img0.shape == img1.shape:
+            return self.match_arrays_gpu(img0, img1)
+        sift = cv2.SIFT_create(2048)
         return self.match_arrays(sift, img0, img1)
+
+    def match_arrays_gpu(self, img0, img1, ratio=0.8):
+        import torch
+        from . import sift
+        key = img0.shape
+        if key not in self.engines:
+            self.engines[key] = sift.SIFT(2, key[0], key[1], nfeatures=2048, root_sift=True)
+        eng = self.engines[key]
+        eng.detect(torch.from_numpy(np.stack([img0, img1])).to(eng.device))
+        k0, k1, _ = eng.match_pairs(ratio)
+        if k0.shape[0] == 0:
+            return np.full((1, 4), np.nan)
+        return torch.cat([k0, k1], 1).cpu().numpy()
 
     @staticmethod
     def match_arrays(sift, img0, img1, ratio=0.8):

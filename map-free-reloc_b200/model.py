@@ -66,25 +66,41 @@ def knn2_gpu(des0, des1):
 
 
 class SIFTMatching:
-    """SIFT + RootSIFT + 2-NN ratio test (feature_matching.py:53-118). Detection/description stays on
-    OpenCV's CPU SIFT exactly as in the reference (SURVEY §8 a14 lists a GPU SIFT as not yet built);
-    the descriptor search runs on the GPU as an EXACT brute-force 2-NN instead of the reference's
+    """SIFT + RootSIFT + 2-NN ratio test (feature_matching.py:53-118). By default detection/description
+    stays on OpenCV's CPU SIFT exactly as in the reference; with SIFT.GPU_DETECTOR the CUDA SIFT engine
+    (mfr_b200.sift, one engine per frame size) detects, describes and matches on the device. The
+    descriptor search runs on the GPU as an EXACT brute-force 2-NN instead of the reference's
     approximate, non-deterministic FLANN kd-tree."""
 
     def __init__(self, cfg):
         import cv2 as cv
         self.cv = cv
         self.ratio_threshold = cfg.SIFT.RATIO_THRESHOLD
+        self.num_features = cfg.SIFT.NUM_FEATURES
         self.sift = cv.SIFT_create(cfg.SIFT.NUM_FEATURES)
+        self.gpu_detector = bool(cfg.SIFT.get("GPU_DETECTOR", False))
+        self.engines = {}
         self.debug = cfg.DEBUG
 
     def transform_grayscale(self, img):
         img = torch.as_tensor(img).permute(1, 2, 0).numpy()
         return self.cv.cvtColor((255 * img).astype(np.uint8), self.cv.COLOR_RGB2GRAY)
 
+    def _gpu_correspondences(self, img0, img1):
+        from . import sift
+        key = img0.shape
+        if key not in self.engines:
+            self.engines[key] = sift.SIFT(2, key[0], key[1], nfeatures=self.num_features, root_sift=True)
+        eng = self.engines[key]
+        eng.detect(torch.from_numpy(np.stack([img0, img1])).to(eng.device))
+        k0, k1, _ = eng.match_pairs(self.ratio_threshold)
+        return k0.cpu().numpy().reshape(-1, 2), k1.cpu().numpy().reshape(-1, 2)
+
     def get_correspondences(self, data):
         img0 = self.transform_grayscale(torch.as_tensor(data["image0"]).squeeze(0))
         img1 = self.transform_grayscale(torch.as_tensor(data["image1"]).squeeze(0))
+        if self.gpu_detector and img0.shape == img1.shape:
+            return self._gpu_correspondences(img0, img1)
         kp0, des0 = self.sift.detectAndCompute(img0, None)
         kp1, des1 = self.sift.detectAndCompute(img1, None)
         if des0 is None or des1 is None or len(des1) < 2:

@@ -1,0 +1,108 @@
+"""Host side of the CUDA SIFT engine: ``SIFT(batch, height, width)`` detects, describes and ratio-matches keypoints
+of uint8 gray images on the device, as cv2.SIFT_create(nfeatures).detectAndCompute + exact 2-NN + Lowe's ratio test
+do on the host in the reference's SIFT plugins (lib/models/matching/feature_matching.py:53-118,
+etc/feature_matching_baselines/matchers.py:123-188). All arithmetic runs in libmfr_b200.so; torch is used for
+device memory and streams only. No CPU fallback."""
+import ctypes
+
+import numpy as np
+import torch
+
+from . import lib as _lib
+
+
+class SIFT:
+    """Engine for ``batch`` images of ``height`` x ``width``. ``nfeatures`` = 0 keeps every keypoint; otherwise
+    OpenCV's retainBest (all keypoints whose response is >= the N-th largest). ``root_sift`` makes the descriptors
+    RootSIFT rows. ``max_candidates`` bounds the refined extrema and the oriented keypoints per image; ``detect``
+    raises when an image has more."""
+
+    def __init__(self, batch, height, width, nfeatures=2048, root_sift=False, max_candidates=32768, graph=True):
+        if not torch.cuda.is_available():
+            raise _lib.MfrError("SIFT engine needs a CUDA device (there is no CPU fallback)")
+        self.l = _lib.load()
+        self.B, self.H, self.W = int(batch), int(height), int(width)
+        self.device = torch.device("cuda", torch.cuda.current_device())
+        h = ctypes.c_void_p()
+        _lib.check(self.l.mfr_sift_create(self.B, self.H, self.W, int(nfeatures), int(max_candidates), int(bool(root_sift)),
+                                          ctypes.byref(h)), "mfr_sift_create")
+        self.h = h
+        self.l.mfr_sift_set_graph(self.h, int(bool(graph)))
+        o = _lib.SiftOutputs()
+        _lib.check(self.l.mfr_sift_get_outputs(self.h, ctypes.byref(o)), "mfr_sift_get_outputs")
+        self.cap = o.capacity
+        B, cap = self.B, self.cap
+        self._counts = self._wrap(o.extrema_counts, (3, B), torch.int32)   # rows: extrema, oriented, selected
+        self._kp = self._wrap(o.keypoints, (B, cap, 5), torch.float32)
+        self._oct = self._wrap(o.octaves, (B, cap), torch.int32)
+        self._desc = self._wrap(o.descriptors, (B, cap, 128), torch.float32)
+
+    def _wrap(self, addr, shape, dtype):
+        """Zero-copy torch view of an engine-owned device buffer (valid while the engine lives)."""
+        class _A:
+            pass
+        a = _A()
+        a.__cuda_array_interface__ = {"shape": (int(np.prod(shape)),), "typestr": "<f4" if dtype == torch.float32 else "<i4",
+                                      "data": (int(addr), False), "version": 2}
+        return torch.as_tensor(a, device=self.device).view(*shape)
+
+    def debug_tensor(self, name, shape, dtype=torch.float32):
+        """Named intermediate buffer (see mfr_sift_debug_tensor): "gauss_<o>", "dog_<o>", "kp_pre", "kp_pre_octave"."""
+        p, n = ctypes.c_void_p(), ctypes.c_longlong()
+        _lib.check(self.l.mfr_sift_debug_tensor(self.h, name.encode(), ctypes.byref(p), ctypes.byref(n)), name)
+        assert int(np.prod(shape)) <= n.value, (name, shape, n.value)
+        return self._wrap(p.value, shape, dtype)
+
+    def octave_shapes(self):
+        """(h, w) of every octave's levels, octave 0 = the doubled image."""
+        shapes, h, w = [], 2 * self.H, 2 * self.W
+        n = int(np.rint(np.log(min(h, w)) / np.log(2.0) - 2)) + 1
+        for _ in range(n):
+            shapes.append((h, w)); h //= 2; w //= 2
+        return shapes
+
+    def detect(self, imgs):
+        """imgs: uint8 [B, H, W] CUDA tensor -> dict of device tensors: counts int32 [B], keypoints float32
+        [B, cap, 5] (x, y, size, angle, response), octaves int32 [B, cap], descriptors float32 [B, cap, 128]; rows past
+        counts[b] are unused. Also raw_counts / extrema_counts (before selection / orientation)."""
+        if imgs.dtype != torch.uint8 or tuple(imgs.shape) != (self.B, self.H, self.W) or not imgs.is_cuda:
+            raise ValueError(f"expected a uint8 CUDA tensor of shape {(self.B, self.H, self.W)}")
+        imgs = imgs.contiguous()
+        _lib.check(self.l.mfr_sift_detect(self.h, _lib.ptr(imgs), _lib.cur_stream()), "mfr_sift_detect")
+        c = self._counts.cpu()
+        if int(c[:2].max()) > self.cap:
+            raise _lib.MfrError(f"SIFT candidates exceed max_candidates={self.cap}: extrema {c[0].tolist()}, "
+                                f"oriented {c[1].tolist()}")
+        return {"counts": self._counts[2], "raw_counts": self._counts[1], "extrema_counts": self._counts[0],
+                "keypoints": self._kp, "octaves": self._oct, "descriptors": self._desc}
+
+    def match_pairs(self, ratio):
+        """Ratio-test matches of the last detect for pairs (2p, 2p + 1) -> (kpts0, kpts1 float32 [total, 2], offsets
+        int32 [P + 1]) on the device, in query order: the pose back end's layout."""
+        P = self.B // 2
+        if P < 1 or self.B % 2:
+            raise ValueError("match_pairs needs an even batch (pairs of images 2p, 2p + 1)")
+        k0 = torch.empty(P * self.cap, 2, device=self.device); k1 = torch.empty_like(k0)
+        off = torch.empty(P + 1, dtype=torch.int32, device=self.device)
+        _lib.check(self.l.mfr_sift_match_pairs(self.h, float(ratio), _lib.ptr(k0), _lib.ptr(k1), _lib.ptr(off),
+                                               _lib.cur_stream()), "mfr_sift_match_pairs")
+        n = int(off[-1])
+        return k0[:n], k1[:n], off
+
+    def profile(self, imgs):
+        """Eager detect with events between the stages -> dict of milliseconds."""
+        ms = (ctypes.c_float * 5)()
+        _lib.check(self.l.mfr_sift_profile(self.h, _lib.ptr(imgs.contiguous()), ms, _lib.cur_stream()), "mfr_sift_profile")
+        return dict(zip(("pyramid", "extrema", "orientation", "selection", "descriptors"), list(ms)))
+
+    def close(self):
+        if getattr(self, "h", None):
+            torch.cuda.synchronize()
+            self.l.mfr_sift_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

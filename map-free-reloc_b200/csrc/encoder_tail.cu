@@ -1,18 +1,25 @@
 // Fused LoFTREncoderLayer tail (bf16 engine mode) on wgmma. See encoder_tail.cuh for the op.
 //
-// One warpgroup per CTA, persistent over 64-row tiles of token rows. Per tile:
-//   * TMA brings the x half of the bf16 token shadow and the message (64 rows x C each, 128B-swizzled k-blocks of 64
-//     columns) into the operand buffer A2 = [x | message].
-//   * merge: D1 [64 x C] = message * Wm^T in registers (C / 128 accumulators of m64n128); LayerNorm1 on the fragments
-//     (row statistics across the four lanes of a quad), written as bf16 over the message half of A2: A2 is now the
-//     mlp.0 operand [x | norm1(merge(message))].
-//   * the 2C-wide hidden layer in chunks (64 columns at C = 256, 128 at C = 128): D2 = A2 * W0[chunk]^T (registers), relu, bf16 into the swizzled
-//     operand buffer H, then D3 [64 x C] += H * W2[:, chunk]^T (registers). 2C-wide rows never exist anywhere.
-//   * LayerNorm2 on D3, x += it (fp32), the bf16 shadow rewritten from the new x.
-// Weights stream through a 3-slot ring of [<= 128 output rows x 64 input columns] tiles (TMA, one mbarrier per slot): the
-// tile two ahead is requested as soon as the previous wgmma group has completed, so L2 latency overlaps the MMAs. The
-// next row tile's A2 is requested as soon as the last mlp.0 chunk has read the current one. HBM traffic per row: the
-// message and x shadow read, x read and written, the shadow written; every intermediate stays on the SM.
+// Persistent, one CTA per SM, 128-row tiles of token rows, three warpgroups:
+//   * warpgroup 0: the TMA producer (warp 0; the warpgroup hands its registers to the consumers with setmaxnreg). Per
+//     row tile, in the order the consumers use them, it loads A2 = [x | message] (the x half of the bf16 token shadow
+//     and the message, 128 rows, 128B-swizzled k-blocks of 64 columns), prefetches the tile's fp32 x rows into L2 for
+//     the LayerNorm2 epilogue, then loads every weight tile of the chain ([<= 128 output rows x 64 input columns]) into
+//     a ring of slots, as deep as shared memory allows, with a full and an empty mbarrier per slot.
+//   * warpgroups 1 and 2: the consumers, rows 0-63 and 64-127 of the tile. Both read every weight tile from the same
+//     slot, so the weights cross L2 once per 128 rows. Per tile and warpgroup:
+//       - merge: D1 [64 x C] = message * Wm^T in registers (C / 128 accumulators of m64n128); LayerNorm1 on the fragments
+//         (row statistics across the four lanes of a quad), written as bf16 over the message half of A2: A2 is now the
+//         mlp.0 operand [x | norm1(merge(message))].
+//       - the 2C-wide hidden layer in chunks (64 columns at C = 256, 128 at C = 128): D2 = A2 * W0[chunk]^T (registers),
+//         relu, bf16 into the warpgroup's rows of the swizzled operand buffer H, then D3 [64 x C] += H * W2[:, chunk]^T
+//         (registers). 2C-wide rows never exist anywhere.
+//       - LayerNorm2 on D3, x += it (fp32), the bf16 shadow rewritten from the new x.
+//     A consumer never issues a load. Each warp hands a weight slot back (an arrive on its empty barrier) once the wgmma
+//     group that read it has completed, and A2 once the last mlp.0 chunk has read it, so the next tile's A2 arrives
+//     while the last mlp.2 tiles and the LayerNorm2 epilogue run.
+// HBM traffic per row: the message and x shadow read, x read and written, the shadow written; every intermediate stays
+// on the SM.
 #include "encoder_tail.cuh"
 #include "wgmma.cuh"
 
@@ -27,11 +34,12 @@ int conv_gemm_num_sms();
 
 namespace {
 
-constexpr int kRows = 64;                 // token rows per tile: the M of one warpgroup's wgmma
-constexpr int kThreads = 128;             // one warpgroup
-constexpr int kWSlots = 3;
-constexpr uint32_t kKb = kRows * 128;     // one 64-row x 64-column bf16 operand k-block (8 KB)
-constexpr uint32_t kWTile = 128 * 128;    // one weight tile: 128 output rows x 64 input columns (16 KB)
+constexpr int kRows = 128;                // token rows per tile: 64 per warpgroup (the M of its wgmma)
+constexpr int kThreads = 384;             // producer warpgroup + two consumer warpgroups
+constexpr int kConsumerWarps = 8;
+constexpr uint32_t kKb = kRows * 128;     // one 128-row x 64-column bf16 operand k-block (16 KB)
+constexpr uint32_t kWgKb = 64 * 128;      // warpgroup w's 64 rows of a k-block start at w * kWgKb
+constexpr uint32_t kWTile = 128 * 128;    // one weight slot: 128 output rows x 64 input columns (16 KB)
 constexpr uint64_t kDescHi = (1ull << 16) | (64ull << 32) | (1ull << 62);   // K-major, 128B swizzle, 1024 B atoms
 __device__ __forceinline__ uint64_t desc(uint32_t a) { return kDescHi | ((a >> 4) & 0x3fffu); }
 
@@ -49,7 +57,10 @@ struct Cfg {
   static constexpr int T_ROW = T_MERGE + NQ * T_CHUNK;
   static constexpr uint32_t A2 = 2 * KB1 * kKb;
   static constexpr uint32_t H = QK * kKb;
-  static constexpr int SMEM = static_cast<int>(A2 + H + kWSlots * kWTile) + 1024;
+  // weight slots: what shared memory holds next to A2 and H (224 KB in all at both widths). The per-tile traffic needs
+  // depth to hide the L2 latency.
+  static constexpr int WS = C == 256 ? 5 : 8;
+  static constexpr int SMEM = static_cast<int>(A2 + H + WS * kWTile) + 1024;
 };
 
 // weight tile t (0 <= t < T_ROW) of a row tile's sequence: tensor map, (input column, output row) coordinates, bytes
@@ -103,15 +114,41 @@ __device__ __forceinline__ void row_stats(const float (&a)[NH][64], int h, float
   rstd = 1.f / sqrtf(q * kInvC + 1e-5f);
 }
 
+// v, hidden from the optimiser: values derived from it are recomputed where it is taken instead of hoisted out of loops
+__device__ __forceinline__ int opaque(int v) {
+  asm volatile("mov.b32 %0, %0;" : "+r"(v));
+  return v;
+}
+__device__ __forceinline__ const float* opaque(const float* v) {
+  asm volatile("mov.b64 %0, %0;" : "+l"(v));
+  return v;
+}
+
+// mbar_wait_inl with the trap after the spin loop rather than inside it: a trap inside the loop makes ptxas allocate the
+// whole kernel at the launch-bounds register count (168 at 384 threads), ignoring the consumers' setmaxnreg.inc
+__device__ __forceinline__ void wait_bounded(uint32_t bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  bool ok;
+  while (!(ok = mbar_try_wait(bar, parity)) && clock64() - t0 <= MFR_SPIN_TIMEOUT_CYCLES) {
+  }
+  if (!ok) __trap();
+}
+
+__device__ __forceinline__ void prefetch_l2(const void* ptr, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(ptr), "r"(bytes) : "memory");
+}
+
 template <int C>
-__global__ void __launch_bounds__(kThreads) encoder_tail_kernel(const __grid_constant__ EncoderTailParams p) {
+__global__ void __launch_bounds__(kThreads, 1) encoder_tail_kernel(const __grid_constant__ EncoderTailParams p) {
   using G = Cfg<C>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t s_bar[1 + kWSlots];
+  __shared__ __align__(8) uint64_t s_bar[2 + 2 * G::WS];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sA = base, sH = base + G::A2, sW = sH + G::H;
-  const uint32_t a_bar = smem_u32(&s_bar[0]);
-  auto w_full = [&](int s) { return smem_u32(&s_bar[1 + s]); };
+  const uint32_t a_full = smem_u32(&s_bar[0]), a_empty = smem_u32(&s_bar[1]);
+  auto w_full = [&](int s) { return smem_u32(&s_bar[2 + s]); };
+  auto w_empty = [&](int s) { return smem_u32(&s_bar[2 + G::WS + s]); };
   const int tid = threadIdx.x;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
 
@@ -120,63 +157,106 @@ __global__ void __launch_bounds__(kThreads) encoder_tail_kernel(const __grid_con
   const int tiles_img = static_cast<int>((live + kRows - 1) / kRows);
   const int n_tiles = tiles_img * p.n_img;
   const int my_tiles = static_cast<int>(blockIdx.x) < n_tiles ? (n_tiles - 1 - static_cast<int>(blockIdx.x)) / gridDim.x + 1 : 0;
-  const long long n_w = static_cast<long long>(my_tiles) * G::T_ROW;   // weight tiles this CTA streams
   if (my_tiles == 0) return;
 
-  auto issue_w = [&](long long g) {   // thread 0: weight tile g of this CTA's sequence into slot g % kWSlots
-    const CUtensorMap* tm;
-    int k0, n0;
-    const uint32_t bytes = wtile<C>(p, static_cast<int>(g % G::T_ROW), tm, k0, n0);
-    const int s = static_cast<int>(g % kWSlots);
-    mbar_arrive_expect_tx(w_full(s), bytes);
-    tma_load_2d(sW + s * kWTile, tm, w_full(s), k0, n0);
-  };
-  auto issue_a = [&](int item) {      // thread 0: x and message k-blocks of row tile `item` into A2
-    const int img = item / tiles_img, tt = item - img * tiles_img;
-    const int r0 = static_cast<int>(img * p.rows_cap) + tt * kRows;
-    mbar_arrive_expect_tx(a_bar, 2 * G::KB1 * kKb);
-    for (int kb = 0; kb < G::KB1; ++kb) {
-      tma_load_2d(sA + kb * kKb, &p.tmX, a_bar, kb * 64, r0);
-      tma_load_2d(sA + (G::KB1 + kb) * kKb, &p.tmMsg, a_bar, kb * 64, r0);
-    }
-  };
   if (tid == 0) {
     tma_prefetch_desc(&p.tmMsg); tma_prefetch_desc(&p.tmX);
     tma_prefetch_desc(&p.tmWm); tma_prefetch_desc(&p.tmW0); tma_prefetch_desc(&p.tmW2);
-    mbar_init(a_bar, 1);
-    for (int s = 0; s < kWSlots; ++s) mbar_init(w_full(s), 1);
+    mbar_init(a_full, 1);
+    mbar_init(a_empty, kConsumerWarps);
+    for (int s = 0; s < G::WS; ++s) {
+      mbar_init(w_full(s), 1);
+      mbar_init(w_empty(s), kConsumerWarps);
+    }
     fence_barrier_init();
-    issue_a(blockIdx.x);
-    issue_w(0);
-    if (n_w > 1) issue_w(1);
   }
   __syncthreads();
 
-  long long g = 0;   // weight tiles consumed
-  // one weight tile: 4 k-steps of (A k-block at a_addr) x (tile)^T into d; once the previous tile's group has completed,
-  // its slot is refilled with the tile two ahead
+  if (warp < 4) {
+    // ------------------------------------------------------------------ TMA producer (warp 0)
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 0) {
+      long long gi = 0;   // weight tiles issued
+      uint32_t a_ph = 1;  // a fresh barrier's preceding phase counts as complete
+      for (int it = 0; it < my_tiles; ++it) {
+        const int item = static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x);
+        const int img = item / tiles_img, tt = item - img * tiles_img;
+        const int r0 = static_cast<int>(img * p.rows_cap) + tt * kRows;
+        wait_bounded(a_empty, a_ph);
+        a_ph ^= 1u;
+        if (elect_one_sync()) {
+          mbar_arrive_expect_tx(a_full, G::A2);
+          for (int kb = 0; kb < G::KB1; ++kb) {
+            tma_load_2d(sA + kb * kKb, &p.tmX, a_full, kb * 64, r0);
+            tma_load_2d(sA + (G::KB1 + kb) * kKb, &p.tmMsg, a_full, kb * 64, r0);
+          }
+        }
+        // the tile's live fp32 x rows into L2 for the LayerNorm2 epilogue, widened to 16-byte bounds (bulk prefetch
+        // granularity)
+        const int n_live = static_cast<int>(min(static_cast<long long>(kRows), live - static_cast<long long>(tt) * kRows));
+        for (int r = lane; r < n_live; r += 32) {
+          const uintptr_t a = reinterpret_cast<uintptr_t>(p.x + (r0 + r) * p.ldx);
+          const uintptr_t a0 = a & ~uintptr_t(15), a1 = (a + C * sizeof(float) + 15) & ~uintptr_t(15);
+          prefetch_l2(reinterpret_cast<const void*>(a0), static_cast<uint32_t>(a1 - a0));
+        }
+        for (int t = 0; t < G::T_ROW; ++t, ++gi) {
+          const int s = static_cast<int>(gi % G::WS);
+          wait_bounded(w_empty(s), static_cast<uint32_t>(((gi / G::WS) & 1) ^ 1));
+          if (elect_one_sync()) {
+            const CUtensorMap* tm;
+            int k0, n0;
+            const uint32_t bytes = wtile<C>(p, t, tm, k0, n0);
+            mbar_arrive_expect_tx(w_full(s), bytes);
+            tma_load_2d(sW + s * kWTile, tm, w_full(s), k0, n0);
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers (warpgroups 1 and 2)
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  const int wg = (warp >> 2) - 1;                           // rows 64 wg .. 64 wg + 63 of each tile
+  const uint32_t sAw = sA + wg * kWgKb, sHw = sH + wg * kWgKb;
+  auto wg_sync = [&]() { named_bar_sync(1 + wg, 128); };
+  auto arrive = [&](uint32_t bar) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar);
+  };
+  long long g = 0, held = -1;   // weight tiles consumed; the tile read by the wgmma group still in flight (-1: none)
+  auto release = [&]() {        // the group in flight has completed: its slot goes back to the producer
+    if (held >= 0) arrive(w_empty(static_cast<int>(held % G::WS)));
+    held = -1;
+  };
+  // one weight tile: 4 k-steps of (A k-block at a_addr) x (tile)^T into d; then the previous tile's group has completed
   auto step = [&](auto& d, uint32_t a_addr) {
     constexpr int N = 2 * static_cast<int>(sizeof(d) / sizeof(float));
-    const int s = static_cast<int>(g % kWSlots);
-    mbar_wait_inl(w_full(s), static_cast<uint32_t>((g / kWSlots) & 1), 1);
+    const int s = static_cast<int>(g % G::WS);
+    wait_bounded(w_full(s), static_cast<uint32_t>((g / G::WS) & 1));
     const uint32_t b_addr = sW + s * kWTile;
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < 4; ++k) wgmma_bf16<N>(d, desc(a_addr) + 2 * k, desc(b_addr) + 2 * k);
     wgmma_commit();
     wgmma_wait<1>();
-    if (tid == 0 && g + 2 < n_w) issue_w(g + 2);
-    ++g;
+    release();
+    held = g++;
   };
 
-  const int rq = 16 * warp + (lane >> 2);   // fragment rows rq and rq + 8
-  const int cq = 2 * (lane & 3);            // fragment columns 8j + cq, 8j + cq + 1
-  uint32_t a_phase = 0;
+  const int rq0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+  const int cq0 = 2 * (lane & 3);
+  uint32_t a_ph = 0;
   for (int it = 0; it < my_tiles; ++it) {
     const int item = static_cast<int>(blockIdx.x) + it * static_cast<int>(gridDim.x);
     const int img = item / tiles_img, tt = item - img * tiles_img;
-    mbar_wait_inl(a_bar, a_phase, 0);
-    a_phase ^= 1u;
+    // tile rows rq and rq + 8 of the fragments, fragment columns 8j + cq, 8j + cq + 1, and the LayerNorm parameters.
+    // Taken per tile: the shared memory addresses and parameter loads derived from them are tile-invariant, and hoisted
+    // out of the loop they hold ~100 (addresses) and C (parameters) registers for the kernel's lifetime.
+    const int rq = opaque(rq0), cq = opaque(cq0);
+    const float *g1 = opaque(p.g1), *b1 = opaque(p.b1), *g2 = opaque(p.g2), *b2 = opaque(p.b2);
+    wait_bounded(a_full, a_ph);
+    a_ph ^= 1u;
 
     // ---- merge + LayerNorm1 -> message half of A2 (bf16)
     float acc[G::NH][64];
@@ -186,11 +266,12 @@ __global__ void __launch_bounds__(kThreads) encoder_tail_kernel(const __grid_con
       for (int i = 0; i < 64; ++i) acc[nh][i] = 0.f;
 #pragma unroll
     for (int nh = 0; nh < G::NH; ++nh)
-      for (int kb = 0; kb < G::KB1; ++kb) step(acc[nh], sA + (G::KB1 + kb) * kKb);
+      for (int kb = 0; kb < G::KB1; ++kb) step(acc[nh], sAw + (G::KB1 + kb) * kKb);
     wgmma_wait<0>();
+    release();
 #pragma unroll
     for (int nh = 0; nh < G::NH; ++nh) wgmma_fence_regs(acc[nh]);
-    __syncthreads();   // every warp's merge MMAs have read the message before it is overwritten
+    wg_sync();   // every warp's merge MMAs have read the message before it is overwritten
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       float mean, rstd;
@@ -200,15 +281,15 @@ __global__ void __launch_bounds__(kThreads) encoder_tail_kernel(const __grid_con
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const int col = nh * 128 + 8 * j + cq;
-          const float y0 = (acc[nh][4 * j + 2 * h] - mean) * rstd * __ldg(p.g1 + col) + __ldg(p.b1 + col);
-          const float y1 = (acc[nh][4 * j + 2 * h + 1] - mean) * rstd * __ldg(p.g1 + col + 1) + __ldg(p.b1 + col + 1);
+          const float y0 = (acc[nh][4 * j + 2 * h] - mean) * rstd * __ldg(g1 + col) + __ldg(b1 + col);
+          const float y1 = (acc[nh][4 * j + 2 * h + 1] - mean) * rstd * __ldg(g1 + col + 1) + __ldg(b1 + col + 1);
           asm volatile("st.shared.u32 [%0], %1;" ::"r"(sw_addr(sA, rq + 8 * h, C + col, kKb)), "r"(bf16x2(y0, y1)) : "memory");
         }
     }
     fence_proxy_async_smem();
-    __syncthreads();
+    wg_sync();
 
-    // ---- hidden layer in 128-column chunks: mlp.0 + relu -> H (bf16), mlp.2 accumulates into acc3
+    // ---- hidden layer in chunks: mlp.0 + relu -> H (bf16), mlp.2 accumulates into acc3
     float acc3[G::NH][64];
 #pragma unroll
     for (int nh = 0; nh < G::NH; ++nh)
@@ -218,11 +299,12 @@ __global__ void __launch_bounds__(kThreads) encoder_tail_kernel(const __grid_con
       float acc2[G::QW / 2];
 #pragma unroll
       for (int i = 0; i < G::QW / 2; ++i) acc2[i] = 0.f;
-      for (int kb = 0; kb < 2 * G::KB1; ++kb) step(acc2, sA + kb * kKb);
+      for (int kb = 0; kb < 2 * G::KB1; ++kb) step(acc2, sAw + kb * kKb);
       wgmma_wait<0>();   // this chunk's mlp.0 and the previous chunk's mlp.2 (reads of H) have completed
+      release();
       wgmma_fence_regs(acc2);
-      __syncthreads();
-      if (q == G::NQ - 1 && tid == 0 && it + 1 < my_tiles) issue_a(item + static_cast<int>(gridDim.x));   // A2 is free
+      if (q == G::NQ - 1) arrive(a_empty);   // A2 is free for the next row tile
+      wg_sync();
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -231,12 +313,13 @@ __global__ void __launch_bounds__(kThreads) encoder_tail_kernel(const __grid_con
           asm volatile("st.shared.u32 [%0], %1;" ::"r"(sw_addr(sH, rq + 8 * h, 8 * j + cq, kKb)), "r"(bf16x2(y0, y1)) : "memory");
         }
       fence_proxy_async_smem();
-      __syncthreads();
+      wg_sync();
 #pragma unroll
       for (int nh = 0; nh < G::NH; ++nh)
-        for (int kb = 0; kb < G::QK; ++kb) step(acc3[nh], sH + kb * kKb);
+        for (int kb = 0; kb < G::QK; ++kb) step(acc3[nh], sHw + kb * kKb);
     }
     wgmma_wait<0>();
+    release();
 #pragma unroll
     for (int nh = 0; nh < G::NH; ++nh) wgmma_fence_regs(acc3[nh]);
 
@@ -251,18 +334,22 @@ __global__ void __launch_bounds__(kThreads) encoder_tail_kernel(const __grid_con
         float* xr = p.x + grow * p.ldx;
         unsigned short* xbr = p.xb + grow * p.ld_xb;
 #pragma unroll
-        for (int nh = 0; nh < G::NH; ++nh)
+        for (int nh = 0; nh < G::NH; ++nh) {
+          // the 16 x loads of a 128-column block go out together, so their L2 latency is paid once rather than per store
+          float2 xo[16];
+#pragma unroll
+          for (int j = 0; j < 16; ++j) xo[j] = *reinterpret_cast<const float2*>(xr + nh * 128 + 8 * j + cq);
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
             const int col = nh * 128 + 8 * j + cq;
-            const float y0 = (acc3[nh][4 * j + 2 * h] - mean) * rstd * __ldg(p.g2 + col) + __ldg(p.b2 + col);
-            const float y1 = (acc3[nh][4 * j + 2 * h + 1] - mean) * rstd * __ldg(p.g2 + col + 1) + __ldg(p.b2 + col + 1);
-            float2 xo = *reinterpret_cast<const float2*>(xr + col);
-            xo.x += y0;
-            xo.y += y1;
-            *reinterpret_cast<float2*>(xr + col) = xo;
-            *reinterpret_cast<uint32_t*>(xbr + col) = bf16x2(xo.x, xo.y);
+            const float y0 = (acc3[nh][4 * j + 2 * h] - mean) * rstd * __ldg(g2 + col) + __ldg(b2 + col);
+            const float y1 = (acc3[nh][4 * j + 2 * h + 1] - mean) * rstd * __ldg(g2 + col + 1) + __ldg(b2 + col + 1);
+            xo[j].x += y0;
+            xo[j].y += y1;
+            *reinterpret_cast<float2*>(xr + col) = xo[j];
+            *reinterpret_cast<uint32_t*>(xbr + col) = bf16x2(xo[j].x, xo[j].y);
           }
+        }
       }
     }
   }
@@ -330,9 +417,8 @@ int encoder_tail_launch(const EncoderTailParams& p, cudaStream_t st) {
     MFR_CUDA_CHECK(cudaFuncSetAttribute(encoder_tail_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::SMEM));
   }
   const long long tiles = static_cast<long long>(p.n_img) * ((p.rows_cap + kRows - 1) / kRows);
-  // C = 256: one 129 KB CTA per SM; C = 128: two 97 KB CTAs per SM
-  const int per_sm = p.C == 256 ? 1 : 2;
-  const int grid = static_cast<int>(std::min<long long>(tiles, static_cast<long long>(conv_gemm_num_sms()) * per_sm));
+  // one 225 KB CTA per SM at both widths
+  const int grid = static_cast<int>(std::min<long long>(tiles, static_cast<long long>(conv_gemm_num_sms())));
   if (grid <= 0) return MFR_OK;
   if (p.C == 256) encoder_tail_kernel<256><<<grid, kThreads, Cfg<256>::SMEM, st>>>(p);
   else encoder_tail_kernel<128><<<grid, kThreads, Cfg<128>::SMEM, st>>>(p);

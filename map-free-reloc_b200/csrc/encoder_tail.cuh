@@ -7,10 +7,10 @@
 namespace mfr {
 
 struct alignas(64) EncoderTailParams {
-  CUtensorMap tmMsg;  // bf16 [rows][C]  attention message (row stride ld_msg)      box {64, 64}
-  CUtensorMap tmX;    // bf16 [rows][C]  x half of the token shadow (row stride ld_xb) box {64, 64}
+  CUtensorMap tmMsg;  // bf16 [rows][C]  attention message (row stride ld_msg)      box {64, 128}
+  CUtensorMap tmX;    // bf16 [rows][C]  x half of the token shadow (row stride ld_xb) box {64, 128}
   CUtensorMap tmWm;   // bf16 [C][C]     merge.weight                                 box {64, 128}
-  CUtensorMap tmW0;   // bf16 [2C][2C]   mlp.0.weight                                 box {64, 128}
+  CUtensorMap tmW0;   // bf16 [2C][2C]   mlp.0.weight                                 box {64, 64 (C = 256) | 128}
   CUtensorMap tmW2;   // bf16 [C][2C]    mlp.2.weight                                 box {64, 128}
   const float *g1, *b1, *g2, *b2;   // norm1 / norm2 affine parameters [C]
   float* x;            // fp32 residual stream, in/out, row stride ldx (elements)

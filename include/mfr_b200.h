@@ -87,7 +87,10 @@ typedef struct {
 #define MFR_PRECISION_TF32 0
 #define MFR_PRECISION_BF16 1
 #define MFR_PRECISION_FP32X3 2
-int mfr_loftr_create(int B, int H, int W, float thr, int border_rm, float temperature, int precision,
+/* reserved_sms: the first four conv launches of every forward use at most (SM count - reserved_sms) SMs, so that
+ * other work on the device, such as the pose solver of the previous batch on another stream, is not held up behind
+ * them. 0 uses every SM; 0 <= reserved_sms < SM count, else MFR_ERR_ARG. The results do not depend on it. */
+int mfr_loftr_create(int B, int H, int W, float thr, int border_rm, float temperature, int precision, int reserved_sms,
                      mfr_loftr** out);
 void mfr_loftr_destroy(mfr_loftr* h);
 int mfr_loftr_num_weights(const mfr_loftr* h);
@@ -290,8 +293,9 @@ float mfr_debug_time_conv(const float* x, int N, int H, int W, int Cin, const fl
 /* Stage entry for tests: LoFTR's linear attention (LoFTR/src/loftr/loftr_module/linear_attention.py:31-45) on
  * already feature-mapped q' = elu(q)+1, k' and values. windows = 0: q [n][L][256], k / v [n][S][256], 8 heads of 32
  * (coarse level); windows = 1: q, k, v [n][25][128], 8 heads of 16, n items (fine level, L and S ignored).
- * bf16 = 1: all four tensors are bf16 (the tensor-core kernels), else fp32. bf16 = 2: bf16 tensors with RAW q and k (the
- * projections as the GEMM leaves them): the kernels apply elu(x) + 1 themselves. Device pointers, dense rows. */
+ * bf16 = 0: fp32 tensors, q and k already feature-mapped. bf16 = 2: bf16 tensors (the tensor-core kernels) with RAW q and k
+ * (the projections as the GEMM leaves them): the kernels apply elu(x) + 1 themselves. bf16 = 1 (bf16 tensors with
+ * pre-mapped q, k) returns MFR_ERR_UNSUPPORTED. Device pointers, dense rows. */
 int mfr_linear_attention(const void* q, const void* k, const void* v, void* msg, int n, int L, int S, int windows,
                          int bf16, void* stream);
 
@@ -300,13 +304,6 @@ int mfr_linear_attention(const void* q, const void* k, const void* v, void* msg,
  * out_bf16 != 0, else fp32 (both on mma.sync); exact_fp32: plain FMA kernel. */
 int mfr_stem_conv7x7(const float* img, const float* w, const float* bias, void* out, int NI, int H, int W, int out_bf16,
                      int exact_fp32, void* stream);
-
-/* Stage entry for tests: the fine level's q|k|v projection + window attention as ONE kernel (bf16 mode; the projection is
- * LoFTREncoderLayer's q_proj / k_proj / v_proj, transformer.py:21-23,41-46, the attention linear_attention.py:31-45 on 5x5
- * windows). xq / xs: bf16 token rows [n_items * 25][>= 128] of the query / source side with element strides ldq / lds (the same
- * pointer = self attention); w_qkv: bf16 [384][128] = rows of Wq, Wk, Wv; msg: bf16 [n_items * 25][ldm]. Device pointers. */
-int mfr_fine_attention_fused(const void* xq, long long ldq, const void* xs, long long lds, const void* w_qkv, void* msg,
-                             long long ldm, int n_items, void* stream);
 
 /* ProcrustesSolver's ICP refinement (PROCRUSTES.REFINE, pose_solver.py:289-315: Open3D registration_icp, point-to-point,
  * correspondence radius max_corr_dist, criteria relative_fitness / relative_rmse / max_iterations = 1e-4 / 1e-4 / 30 in the

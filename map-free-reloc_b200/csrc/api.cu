@@ -27,7 +27,7 @@ int pose_metrics(const double* q_gt, const double* t_gt, const double* q_est, co
 
 extern "C" {
 
-int mfr_version(void) { return 100; }
+int mfr_version(void) { return 101; }
 
 int mfr_device_sm_count(void) {
   int n = 0;
@@ -67,11 +67,11 @@ int mfr_conv2d_nhwc_bf16(const void* x, int N, int H, int W, int Cin, long long 
 // ------------------------------------------------------------------------------------------ LoFTR
 struct mfr_loftr { mfr::LoftrEngine* e; };
 
-int mfr_loftr_create(int B, int H, int W, float thr, int border_rm, float temperature, int precision,
+int mfr_loftr_create(int B, int H, int W, float thr, int border_rm, float temperature, int precision, int reserved_sms,
                      mfr_loftr** out) {
   if (!out) return MFR_ERR_ARG;
   mfr::LoftrEngine* e = nullptr;
-  int rc = mfr::loftr_create(B, H, W, thr, border_rm, temperature, precision, &e);
+  int rc = mfr::loftr_create(B, H, W, thr, border_rm, temperature, precision, reserved_sms, &e);
   if (rc != MFR_OK) return rc;
   *out = new mfr_loftr{e};
   return MFR_OK;
@@ -309,22 +309,10 @@ int mfr_stem_conv7x7(const float* img, const float* w, const float* bias, void* 
   return mfr::stem_conv7x7(img, w, bias, static_cast<float*>(out), NI, H, W, static_cast<cudaStream_t>(stream), out_bf16, exact_fp32);
 }
 
-int mfr_fine_attention_fused(const void* xq, long long ldq, const void* xs, long long lds, const void* w_qkv, void* msg,
-                             long long ldm, int n_items, void* stream) {
-  if (!xq || !xs || !w_qkv || !msg || n_items <= 0) return MFR_ERR_ARG;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int* cnt = nullptr;
-  if (cudaMalloc(&cnt, sizeof(int)) != cudaSuccess) return MFR_ERR_CUDA;
-  cudaMemcpyAsync(cnt, &n_items, sizeof(int), cudaMemcpyHostToDevice, st);
-  const int r = mfr::fine_attention_fused(xq, ldq, xs, lds, w_qkv, msg, ldm, cnt, n_items, 25, st);
-  cudaStreamSynchronize(st);
-  cudaFree(cnt);
-  return r;
-}
-
 int mfr_linear_attention(const void* q, const void* k, const void* v, void* msg, int n, int L, int S, int windows,
                          int bf16, void* stream) {
   if (!q || !k || !v || !msg || n <= 0) return MFR_ERR_ARG;
+  if (bf16 != 0 && bf16 != 2) return MFR_ERR_UNSUPPORTED;   // bf16 takes raw q, k: pre-mapped ones would be mapped twice
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (windows) {
     int* cnt = nullptr;

@@ -790,8 +790,7 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
     p->ksteps_last = (tail + ummak - 1) / ummak;
     // a tail of one k-step (<= 32 bytes of channels) is moved as 32-byte-wide tiles (32B swizzle) instead of zero-filled
     // 128-byte ones: Cin = 196 otherwise spends a quarter of its operand traffic on 4 channels
-    p->tail32 = (p->ksteps_last == 1 && tail * es <= 32 && p->kb_per_tap > 1 && d.b_batched != 2 &&
-                 getenv("MFR_CONV_NO_TAIL32") == nullptr) ? 1 : 0;
+    p->tail32 = (p->ksteps_last == 1 && tail * es <= 32 && p->kb_per_tap > 1 && d.b_batched != 2) ? 1 : 0;
   }
   // Order of the fp32 sums over the taps, fixed per shape and the same in halo and per-tap mode, so that the tiling
   // never changes the result bits: kx-major for 3x3 stride-1 convs with at most 128 output channels, ky-major
@@ -829,7 +828,7 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
                                  p->epi == kEpiAny ? -1 : (d.out_bf16 ? 1 : 0));
   p->TW = cfg.TW; p->TH = cfg.TH; p->MT = cfg.MT; p->halo = cfg.halo;
   p->BN = cfg.BN; p->n_tiles = cfg.n_tiles;
-  p->nt_fast = (!p->halo && p->n_tiles > 1 && getenv("MFR_CONV_NT_SLOW") == nullptr) ? 1 : 0;
+  p->nt_fast = (!p->halo && p->n_tiles > 1) ? 1 : 0;
   p->tiles_x = (p->Wo + p->TW - 1) / p->TW;
   p->tiles_y = (p->Ho + p->MT * p->TH - 1) / (p->MT * p->TH);
   p->in_bf16 = d.in_bf16;

@@ -5,7 +5,6 @@
 // transformer -> expectation), for B image pairs per call, channel-last fp32 activations.
 #include "loftr_engine.cuh"
 
-#include <cstdlib>
 #include <cstring>
 #include <functional>
 #include <map>
@@ -38,9 +37,8 @@ struct StepInfo {
   int launches = 1;     // kernels this step launches
 };
 
-// bf16 mode: the coarse correlation reads the bf16 shadow of the final tokens (kind::f16, half the operand bytes)
-constexpr bool kCorrelationBf16 = true;
 constexpr size_t kW16Capacity = static_cast<size_t>(16) * 1024 * 1024;   // bf16 weight copies (elements): ~11.5 M used
+constexpr int kReservedLayers = 4;   // conv launches at the start of the list that leave LoftrEngine::reserved_sms SMs free
 
 struct LoftrEngine {
   int B, H, W, NI;
@@ -49,17 +47,12 @@ struct LoftrEngine {
   int border;
   int splits_kv = 96, splits_col = 32;   // splits_kv is set from the image count in build()
   int precision = 0;   // MFR_PRECISION_* (include/mfr_b200.h)
-  bool fused_tail = getenv("MFR_FUSED_TAIL") == nullptr || atoi(getenv("MFR_FUSED_TAIL")) != 0;   // bf16 mode: encoder_tail.cu
-  bool fused_fine_attn = getenv("MFR_FUSED_FINE_ATTN") != nullptr && atoi(getenv("MFR_FUSED_FINE_ATTN")) != 0;   // bf16 mode, fine level (opt-in)
-  // bf16 mode: the q|k|v GEMMs store raw projections and the attention kernels apply elu + 1 to their mma fragments
   // The pose back end of the previous batch runs on its own stream under the first layers of this batch's matcher. Its blocks
   // do not fit next to the persistent GEMM CTAs, and a persistent kernel with a static tile assignment whose CTA has to wait
-  // for an SM is late by that CTA's whole share: the first `reserve_layers` conv launches (and the stem) therefore leave
-  // `reserve_sms` SMs free (MFR_RESERVE_SMS / MFR_RESERVE_LAYERS; 0 = use every SM).
-  int reserve_sms = getenv("MFR_RESERVE_SMS") ? atoi(getenv("MFR_RESERVE_SMS")) : 0;
-  int reserve_layers = getenv("MFR_RESERVE_LAYERS") ? atoi(getenv("MFR_RESERVE_LAYERS")) : 4;
+  // for an SM is late by that CTA's whole share: the first kReservedLayers conv launches therefore leave `reserved_sms` SMs
+  // free (0 = use every SM).
+  int reserved_sms = 0;
   int conv_count = 0;
-  bool elu_in_attn = getenv("MFR_ELU_IN_ATTN") == nullptr || atoi(getenv("MFR_ELU_IN_ATTN")) != 0;
   struct Bf16Conv { std::string name; int cout, taps, cin, cin_pad; size_t off; };
   std::vector<Bf16Conv> bf16_convs;
   unsigned short* wblob16 = nullptr;
@@ -90,7 +83,8 @@ struct LoftrEngine {
   // buffers
   float* img = nullptr;
   float *a0, *a1, *a2, *b0, *b1, *b2, *c0, *c1, *c2, *fc, *p4a, *p4b, *p4c, *p2a, *p2b;
-  float *tok, *qkv, *msg, *mrg, *h1, *h2, *kvp, *kv, *S;
+  float *tok, *qkv, *msg, *kvp, *kv, *S;
+  float *mrg = nullptr, *h1 = nullptr, *h2 = nullptr;   // tf32 / fp32x3 only (unfused encoder tail)
   float *tokb = nullptr, *ftokb = nullptr;   // bf16 mode: bf16 shadows of tok / ftok (same shape; float-typed like the other bf16 buffers)
   size_t ftok_elems = 0;
   float* shadow(float* x) const {            // same element offset inside the shadow buffer
@@ -98,7 +92,8 @@ struct LoftrEngine {
     return tokb + (x - tok) / 2;
   }
   CoarseMatchBuffers cm;
-  float *cin, *cproj, *win, *ftok, *fqkv, *fmsg, *fmrg, *fh1, *fh2, *mk1f, *expec;
+  float *cin, *cproj, *win, *ftok, *fqkv, *fmsg, *mk1f, *expec;
+  float *fmrg = nullptr, *fh1 = nullptr, *fh2 = nullptr;   // tf32 / fp32x3 only
   // graph
   cudaGraphExec_t graph_exec = nullptr;
   bool use_graph = true;
@@ -190,7 +185,7 @@ struct LoftrEngine {
     ConvGemmParams p;
     int rc = conv_gemm_build(d, &p);
     if (rc != MFR_OK) { build_rc = rc; return; }
-    if (reserve_sms > 0 && conv_count < reserve_layers) p.grid_limit = conv_gemm_num_sms() - reserve_sms;
+    if (reserved_sms > 0 && conv_count < kReservedLayers) p.grid_limit = conv_gemm_num_sms() - reserved_sms;
     ++conv_count;
     steps.push_back([p](cudaStream_t st) { return conv_gemm_launch(p, st); });
     StepInfo inf;
@@ -258,36 +253,24 @@ struct LoftrEngine {
   // One LoFTREncoderLayer (transformer.py:35-58) on `n` "images" of `rows` tokens each.
   //   x, src : token buffers with row stride 2C (cols [0,C) = features, [C,2C) = message scratch)
   //   q/k/v live in `qkv_x` / `qkv_s` (row stride 3C) at the rows of the x / src images.
+  //   mrg_x, h1_x, h2_x : scratch of the unfused tail (tf32 / fp32x3 only, null in bf16 mode)
   void encoder_layer(const std::string& p, int C, float* x, float* src, float* qkv_x, float* qkv_s,
                      float* msg_x, float* mrg_x, float* h1_x, float* h2_x, int n, int rows,
                      const int* dyn_rows, const int* dyn_items, bool windows) {
     float* wq = W_(p + ".qkv.w");
     const long long ld2 = 2 * C, ld3 = 3 * C;
-    // bf16 mode: the big intermediates (q|k|v, attention message, MLP hidden) are stored in bf16 — these GEMMs and
-    // the attention kernels are HBM-bound — while the residual stream, LayerNorm inputs and outputs stay fp32.
+    // bf16 mode: q|k|v and the attention message are stored in bf16 — these GEMMs and the attention kernels are
+    // HBM-bound — while the residual stream, LayerNorm inputs and outputs stay fp32.
     // The buffers are float-typed: `tb` bf16 elements per float when converting element offsets.
     const int tbf = precision == 1 ? 1 : 0, tb = tbf ? 2 : 1;
     auto E = [tb](float* ptr, size_t elems) { return ptr + elems / tb; };
-    // bf16 mode: the GEMMs that read the token stream (q|k|v, mlp0) take their A operand from its bf16 shadow
-    // (written by the LayerNorms below): half the operand bytes and kind::f16 MMAs instead of kind::tf32.
+    // bf16 mode: the q|k|v GEMMs take their A operand from the bf16 shadow of the token stream (written by the fused
+    // tail): half the operand bytes and kind::f16 MMAs instead of kind::tf32. They store the raw projections, and the
+    // attention kernels apply elu + 1 to their mma fragments.
     float* xb = tbf ? shadow(x) : x;
     float* srcb = tbf ? shadow(src) : src;
     const std::string qn = p + ".qkv";
-    if (windows && tbf && fused_fine_attn) {
-      // fine level, bf16 mode: projection + window attention in one kernel (q, k, v stay on the SM; loftr_ops.cu)
-      const unsigned short* wq16 = w16(qn, 3 * C, C);
-      const int items_cap = rows / 25;
-      for (int side = 0; side < n; ++side) {
-        const size_t off2 = static_cast<size_t>(side) * rows * ld2, off1 = static_cast<size_t>(side) * rows * C;
-        const float *xq_ = E(xb, off2), *xs_ = E(srcb, off2);
-        float* mp = E(msg_x, off1);
-        push("fine_attn_fused", [=](cudaStream_t st) {
-          return fine_attention_fused(xq_, ld2, xs_, ld2, wq16, mp, C, dyn_items, items_cap, 25, st);
-        });
-      }
-    } else {
-    const bool raw = tbf && elu_in_attn;            // feature map applied by the attention kernels (bf16 = 2 below)
-    const int qk_act = raw ? ACT_NONE : ACT_ELU1, att_mode = raw ? 2 : tbf;
+    const int qk_act = tbf ? ACT_NONE : ACT_ELU1;
     if (x == src) {
       conv(qn, xb, n, 1, rows, C, ld2, 3 * C, 1, 1, false, nullptr, qk_act, qkv_x, ld3, 2 * C, dyn_rows, wq, nullptr, tbf, tbf,
            3 * C, 0);
@@ -301,7 +284,7 @@ struct LoftrEngine {
       const int Lr = rows, sk = splits_kv * NI / n;   // same partial-buffer footprint for n = B or n = 2B images
       float *kp = E(qkv_s, C), *vp = E(qkv_s, 2 * C);
       push("attn_long", [=](cudaStream_t st) {
-        return linear_attention_long(qkv_x, ld3, kp, ld3, vp, ld3, msg_x, C, kvp_, kv_, n, Lr, Lr, 8, 32, sk, st, att_mode);
+        return linear_attention_long(qkv_x, ld3, kp, ld3, vp, ld3, msg_x, C, kvp_, kv_, n, Lr, Lr, 8, 32, sk, st, tbf);
       }, 3);
     } else {
       const int items_cap = rows / 25;
@@ -310,14 +293,13 @@ struct LoftrEngine {
         const size_t off1 = static_cast<size_t>(side) * rows * C;
         float *qp = E(qkv_x, off3), *kp = E(qkv_s, off3 + C), *vp = E(qkv_s, off3 + 2 * C), *mp = E(msg_x, off1);
         push("attn_windows", [=](cudaStream_t st) {
-          return linear_attention_windows(qp, ld3, kp, ld3, vp, ld3, mp, C, dyn_items, items_cap, 25, st, att_mode);
+          return linear_attention_windows(qp, ld3, kp, ld3, vp, ld3, mp, C, dyn_items, items_cap, 25, st, tbf);
         });
       }
     }
-    }
     const float *g1 = W_(p + ".norm1.g"), *b1 = W_(p + ".norm1.b");
     const float *g2 = W_(p + ".norm2.g"), *b2 = W_(p + ".norm2.b");
-    if (tbf && fused_tail) {
+    if (tbf) {
       // merge -> norm1 -> mlp([x | message]) -> norm2 -> residual as ONE kernel: the merge output, the norm1 output, the
       // 2C-wide hidden tensor and the mlp output never leave the SM (encoder_tail.cu)
       EncoderTailDesc d{};
@@ -340,38 +322,32 @@ struct LoftrEngine {
       infos.push_back(inf);
       return;
     }
-    conv(p + ".merge", msg_x, n, 1, rows, C, C, C, 1, 1, false, nullptr, ACT_NONE, mrg_x, C, 0, dyn_rows, nullptr, nullptr,
-         tbf, 0);
+    // tf32 / fp32x3: merge, norm1 into the message half of x, mlp0 on [x | message], mlp2, norm2 + residual
+    conv(p + ".merge", msg_x, n, 1, rows, C, C, C, 1, 1, false, nullptr, ACT_NONE, mrg_x, C, 0, dyn_rows);
     const long long tot = static_cast<long long>(n) * rows;
-    // norm1(message) is only read by mlp0: in bf16 mode it goes straight to the shadow's message half
     if (dyn_rows == nullptr) {
       push("layernorm", [=](cudaStream_t st) {
-        if (tbf) return layernorm_rows(mrg_x, C, g1, b1, nullptr, 0, nullptr, 0, tot, C, nullptr, st, E(xb, C), ld2);
         return layernorm_rows(mrg_x, C, g1, b1, nullptr, 0, x + C, ld2, tot, C, nullptr, st);
       });
     } else {
       for (int side = 0; side < n; ++side) {
         const size_t o1 = static_cast<size_t>(side) * rows * C, o2 = static_cast<size_t>(side) * rows * ld2;
         push("layernorm", [=](cudaStream_t st) {
-          if (tbf) return layernorm_rows(mrg_x + o1, C, g1, b1, nullptr, 0, nullptr, 0, rows, C, dyn_rows, st, E(xb, o2 + C), ld2);
           return layernorm_rows(mrg_x + o1, C, g1, b1, nullptr, 0, x + o2 + C, ld2, rows, C, dyn_rows, st);
         });
       }
     }
-    conv(p + ".mlp0", xb, n, 1, rows, 2 * C, ld2, 2 * C, 1, 1, false, nullptr, ACT_RELU, h1_x, ld2, 0, dyn_rows, nullptr,
-         nullptr, tbf, tbf);
-    conv(p + ".mlp2", h1_x, n, 1, rows, 2 * C, ld2, C, 1, 1, false, nullptr, ACT_NONE, h2_x, C, 0, dyn_rows, nullptr,
-         nullptr, tbf, 0);
+    conv(p + ".mlp0", x, n, 1, rows, 2 * C, ld2, 2 * C, 1, 1, false, nullptr, ACT_RELU, h1_x, ld2, 0, dyn_rows);
+    conv(p + ".mlp2", h1_x, n, 1, rows, 2 * C, ld2, C, 1, 1, false, nullptr, ACT_NONE, h2_x, C, 0, dyn_rows);
     if (dyn_rows == nullptr) {
       push("layernorm", [=](cudaStream_t st) {
-        return layernorm_rows(h2_x, C, g2, b2, x, ld2, x, ld2, tot, C, nullptr, st, tbf ? xb : nullptr, ld2);
+        return layernorm_rows(h2_x, C, g2, b2, x, ld2, x, ld2, tot, C, nullptr, st);
       });
     } else {
       for (int side = 0; side < n; ++side) {
         const size_t o1 = static_cast<size_t>(side) * rows * C, o2 = static_cast<size_t>(side) * rows * ld2;
         push("layernorm", [=](cudaStream_t st) {
-          return layernorm_rows(h2_x + o1, C, g2, b2, x + o2, ld2, x + o2, ld2, rows, C, dyn_rows, st,
-                                tbf ? E(xb, o2) : nullptr, ld2);
+          return layernorm_rows(h2_x + o1, C, g2, b2, x + o2, ld2, x + o2, ld2, rows, C, dyn_rows, st);
         });
       }
     }
@@ -418,8 +394,10 @@ struct LoftrEngine {
     float* featf = alloc<float>(px2 * 128, "feat_f");
     tok = alloc<float>(px8 * 512, "tok");
     if (bf) tokb = reinterpret_cast<float*>(alloc<unsigned short>(px8 * 512, "tok_bf16"));
-    qkv = alloc<float>(px8 * 768, "qkv"); msg = alloc<float>(px8 * 256, "msg"); mrg = alloc<float>(px8 * 256, "mrg");
-    h1 = alloc<float>(px8 * 512, "h1"); h2 = alloc<float>(px8 * 256, "h2");
+    qkv = alloc<float>(px8 * 768, "qkv"); msg = alloc<float>(px8 * 256, "msg");
+    if (!bf) {   // the unfused encoder tail's scratch (bf16 mode runs the fused tail)
+      mrg = alloc<float>(px8 * 256, "mrg"); h1 = alloc<float>(px8 * 512, "h1"); h2 = alloc<float>(px8 * 256, "h2");
+    }
     splits_kv = std::max(1, std::min(L / 16, (2 * sm_count() + NI - 1) / NI));   // ~2 blocks per SM when all images run
     kvp = alloc<float>(static_cast<size_t>(NI) * 8 * splits_kv * 1056, "kvp");
     kv = alloc<float>(static_cast<size_t>(NI) * 8 * 1056, "kv");
@@ -442,8 +420,8 @@ struct LoftrEngine {
     ftok = alloc<float>(frows * 256, "fine_tok");
     ftok_elems = frows * 256;
     if (bf) ftokb = reinterpret_cast<float*>(alloc<unsigned short>(frows * 256, "fine_tok_bf16"));
-    fqkv = alloc<float>(frows * 384, "fine_qkv"); fmsg = alloc<float>(frows * 128); fmrg = alloc<float>(frows * 128);
-    fh1 = alloc<float>(frows * 256); fh2 = alloc<float>(frows * 128);
+    fqkv = alloc<float>(frows * 384, "fine_qkv"); fmsg = alloc<float>(frows * 128);
+    if (!bf) { fmrg = alloc<float>(frows * 128); fh1 = alloc<float>(frows * 256); fh2 = alloc<float>(frows * 128); }
     mk1f = alloc<float>(BL * 2, "mkpts1_f"); expec = alloc<float>(BL * 3, "expec_f");
     if (build_rc != MFR_OK) return build_rc;
 
@@ -452,8 +430,7 @@ struct LoftrEngine {
     {
       float *img_ = img, *a0_ = a0; float* ws = W_("stem.w"); float* bs = W_("stem.b");
       const int NI_ = NI, H_ = H, W_w = W, ob = B16, exact = precision == 2 ? 1 : 0;
-      const int stem_limit = reserve_sms > 0 ? conv_gemm_num_sms() - reserve_sms : 0;
-      push("stem", [=](cudaStream_t st) { return stem_conv7x7(img_, ws, bs, a0_, NI_, H_, W_w, st, ob, exact, stem_limit); });
+      push("stem", [=](cudaStream_t st) { return stem_conv7x7(img_, ws, bs, a0_, NI_, H_, W_w, st, ob, exact); });
     }
     auto bconv = [&](const std::string& name, const float* x, int Hh, int Ww, int Cin, int ldx, int Cout, int R,
                      int stride, bool bias, const float* res, int act, float* out, int ldo, int out16) {
@@ -501,16 +478,17 @@ struct LoftrEngine {
     }
     const size_t half_tok = static_cast<size_t>(B) * L * 512, half_qkv = static_cast<size_t>(B) * L * 768;
     const size_t half_c = static_cast<size_t>(B) * L * 256, half_2c = static_cast<size_t>(B) * L * 512;
+    const int tb = bf ? 2 : 1;   // qkv / msg hold bf16 in that mode (see encoder_layer)
+    auto at = [](float* p, size_t off) { return p ? p + off : p; };   // the unfused tail's scratch is null in bf16 mode
     for (int i = 0; i < 8; ++i) {
       const std::string p = "coarse." + std::to_string(i);
       if (i % 2 == 0) {  // self: both image sets at once
         encoder_layer(p, 256, tok, tok, qkv, qkv, msg, mrg, h1, h2, NI, L, nullptr, nullptr, false);
       } else {  // cross: feat0 <- (feat0, feat1), then feat1 <- (feat1, updated feat0)
-        const int tb = precision == 1 ? 2 : 1;   // qkv / msg / h1 hold bf16 in that mode (see encoder_layer)
         encoder_layer(p, 256, tok, tok + half_tok, qkv, qkv + half_qkv / tb, msg, mrg, h1, h2, B, L, nullptr,
                       nullptr, false);
-        encoder_layer(p, 256, tok + half_tok, tok, qkv + half_qkv / tb, qkv, msg + half_c / tb, mrg + half_c,
-                      h1 + half_2c / tb, h2 + half_c, B, L, nullptr, nullptr, false);
+        encoder_layer(p, 256, tok + half_tok, tok, qkv + half_qkv / tb, qkv, msg + half_c / tb, at(mrg, half_c),
+                      at(h1, half_2c), at(h2, half_c), B, L, nullptr, nullptr, false);
       }
     }
 
@@ -519,7 +497,8 @@ struct LoftrEngine {
       ConvGemmDesc d{};
       d.x = tok; d.N = B; d.H = 1; d.W = L; d.Cin = 256; d.ldx = 512;
       d.w = tok + half_tok; d.Cout = L; d.R = 1; d.S = 1; d.stride = 1; d.pad = 0;
-      if (kCorrelationBf16 && precision == 1) { d.x = tokb; d.w = tokb + half_tok / 2; d.in_bf16 = 1; }
+      // bf16 mode: the correlation reads the bf16 shadow of the final tokens (kind::f16, half the operand bytes)
+      if (bf) { d.x = tokb; d.w = tokb + half_tok / 2; d.in_bf16 = 1; }
       if (precision == 2) {   // 3xTF32: X -> [hi | lo | hi], Y -> [hi | hi | lo], one GEMM over K = 768
         const size_t BLr = static_cast<size_t>(B) * L;
         float *xa = x3, *xb = x3 + BLr * 768; const float *t0 = tok, *t1 = tok + half_tok; const int B_ = B, L_ = L;
@@ -572,11 +551,10 @@ struct LoftrEngine {
                    s_c = static_cast<size_t>(rows) * 128, s_2c = static_cast<size_t>(rows) * 256;
       encoder_layer("fine.0", 128, ftok, ftok, fqkv, fqkv, fmsg, fmrg, fh1, fh2, 2, rows, cm.m_total + 2,
                     cm.m_total, true);
-      const int tb = precision == 1 ? 2 : 1;   // qkv / msg / h1 hold bf16 in that mode (see encoder_layer)
       encoder_layer("fine.1", 128, ftok, ftok + s_tok, fqkv, fqkv + s_qkv / tb, fmsg, fmrg, fh1, fh2, 1, rows,
                     cm.m_total + 2, cm.m_total, true);
-      encoder_layer("fine.1", 128, ftok + s_tok, ftok, fqkv + s_qkv / tb, fqkv, fmsg + s_c / tb, fmrg + s_c,
-                    fh1 + s_2c / tb, fh2 + s_c, 1, rows, cm.m_total + 2, cm.m_total, true);
+      encoder_layer("fine.1", 128, ftok + s_tok, ftok, fqkv + s_qkv / tb, fqkv, fmsg + s_c / tb, at(fmrg, s_c),
+                    at(fh1, s_2c), at(fh2, s_c), 1, rows, cm.m_total + 2, cm.m_total, true);
       CoarseMatchBuffers cmb = cm; float *f0 = ftok, *f1 = ftok + s_tok, *mk = mk1f, *ex = expec;
       const int Mc = Mcap; const float scale_f = static_cast<float>(H) / static_cast<float>(H2);
       push("fine_match", [=](cudaStream_t st) {
@@ -710,11 +688,13 @@ struct LoftrEngine {
 };
 
 // ---------------------------------------------------------------------------------------------
-int loftr_create(int B, int H, int W, float thr, int border, float temperature, int precision, LoftrEngine** out) {
+int loftr_create(int B, int H, int W, float thr, int border, float temperature, int precision, int reserved_sms,
+                 LoftrEngine** out) {
   if (B < 1 || H % 8 || W % 8 || H < 32 || W < 32 || precision < 0 || precision > 2) return MFR_ERR_ARG;
+  if (reserved_sms < 0 || reserved_sms >= conv_gemm_num_sms()) return MFR_ERR_ARG;
   auto* e = new LoftrEngine();
   e->B = B; e->H = H; e->W = W; e->thr = thr; e->border = border; e->temperature = temperature;
-  e->precision = precision;
+  e->precision = precision; e->reserved_sms = reserved_sms;
   int rc = e->build();
   if (rc != MFR_OK) { delete e; return rc; }
   *out = e;

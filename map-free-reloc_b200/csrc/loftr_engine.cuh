@@ -16,7 +16,8 @@ struct LoftrOutputs {
   int capacity;
 };
 
-int loftr_create(int B, int H, int W, float thr, int border, float temperature, int precision, LoftrEngine** out);
+int loftr_create(int B, int H, int W, float thr, int border, float temperature, int precision, int reserved_sms,
+                 LoftrEngine** out);
 void loftr_destroy(LoftrEngine* e);
 int loftr_num_weights(const LoftrEngine* e);
 const char* loftr_weight_name(const LoftrEngine* e, int i);

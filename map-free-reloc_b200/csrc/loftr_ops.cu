@@ -210,7 +210,6 @@ __global__ void posenc_kernel(const float* __restrict__ feat, const float* __res
 // Both streaming kernels move their token rows with a 3-stage cp.async pipeline (16 tokens x 1 KB per
 // operand per stage), so the HBM latency is paid once per block, not once per slab.
 constexpr int kSlab = 16;     // tokens per pipeline stage
-constexpr bool kUseMmaAttention = true;   // bf16 mode: warp-level tensor-core linear attention (false: the SIMT kernels)
 constexpr int kAttStages = 3;
 
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc, bool valid) {
@@ -222,63 +221,40 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// rows [r0, r0+kSlab) of a [rows][256] matrix (fp32 or bf16, row stride ld elements) -> dst[kSlab][256];
+// rows [r0, r0+kSlab) of an fp32 [rows][256] matrix (row stride ld floats) -> dst[kSlab][256];
 // rows >= r_end are zero-filled
-template <bool BF>
 __device__ __forceinline__ void slab_load(void* dst, const void* __restrict__ src, long long ld, long long r0,
                                           long long r_end, int t) {
-  constexpr int kChunks = BF ? 32 : 64;             // 16-byte chunks per row
-  constexpr int kEs = BF ? 2 : 4;
+  constexpr int kChunks = 64;                       // 16-byte chunks per row
 #pragma unroll
   for (int i = 0; i < kSlab * kChunks / 256; ++i) {
     const int c = t + 256 * i;
     const int r = c / kChunks, ch = c % kChunks;
     const bool ok = r0 + r < r_end;
     cp_async16(static_cast<char*>(dst) + (r * kChunks + ch) * 16,
-               static_cast<const char*>(src) + ((ok ? (r0 + r) : r0) * ld) * kEs + ch * 16, ok);
+               static_cast<const char*>(src) + ((ok ? (r0 + r) : r0) * ld) * 4 + ch * 16, ok);
   }
 }
 // element t of row r / the 32 channels of head h of row r, from a staged slab
-template <bool BF>
 __device__ __forceinline__ float slab_elem(const void* slab, int r, int t) {
-  if constexpr (BF) return bf2f(static_cast<const unsigned short*>(slab)[r * 256 + t]);
-  else return static_cast<const float*>(slab)[r * 256 + t];
+  return static_cast<const float*>(slab)[r * 256 + t];
 }
-template <bool BF>
 __device__ __forceinline__ void slab_head(const void* slab, int r, int h, float (&o)[32]) {
-  if constexpr (BF) {
-    const uint4* p = reinterpret_cast<const uint4*>(static_cast<const unsigned short*>(slab) + r * 256 + h * 32);
+  const float4* p = reinterpret_cast<const float4*>(static_cast<const float*>(slab) + r * 256 + h * 32);
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const uint4 u = p[q];
-      const unsigned w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        o[8 * q + 2 * e] = __uint_as_float(w[e] << 16);
-        o[8 * q + 2 * e + 1] = __uint_as_float(w[e] & 0xffff0000u);
-      }
-    }
-  } else {
-    const float4* p = reinterpret_cast<const float4*>(static_cast<const float*>(slab) + r * 256 + h * 32);
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      const float4 f = p[q];
-      o[4 * q] = f.x; o[4 * q + 1] = f.y; o[4 * q + 2] = f.z; o[4 * q + 3] = f.w;
-    }
+  for (int q = 0; q < 8; ++q) {
+    const float4 f = p[q];
+    o[4 * q] = f.x; o[4 * q + 1] = f.y; o[4 * q + 2] = f.z; o[4 * q + 3] = f.w;
   }
 }
 
-template <bool BF>
 __global__ void __launch_bounds__(256) kv_partial_kernel(const void* __restrict__ K, long long ldk,
                                                          const void* __restrict__ V, long long ldv,
                                                          float* __restrict__ kv_part, int S, int splits) {
   extern __shared__ __align__(16) float att_smem[];
-  constexpr int kSlabBytes = kSlab * 256 * (BF ? 2 : 4);
+  constexpr int kSlabBytes = kSlab * 256 * 4;
   char* sK = reinterpret_cast<char*>(att_smem);                          // [stages][kSlab][256]
   char* sV = reinterpret_cast<char*>(att_smem) + kAttStages * kSlabBytes;
-  // bf16 operands: every K element is read by the 32 lanes of its head's warp, so it is widened to fp32 ONCE per slab
-  // into this buffer instead of 32 times in the inner loop (the kernel is ALU-bound)
-  float* sKf = reinterpret_cast<float*>(reinterpret_cast<char*>(att_smem) + 2 * kAttStages * kSlabBytes);   // [kSlab][256], BF only
   const int split = blockIdx.x, n = blockIdx.y;
   const int chunk = (S + splits - 1) / splits;
   const int s_beg = split * chunk, s_end = min(S, s_beg + chunk);
@@ -293,8 +269,8 @@ __global__ void __launch_bounds__(256) kv_partial_kernel(const void* __restrict_
 #pragma unroll
   for (int st = 0; st < kAttStages - 1; ++st) {
     if (st < nslab) {
-      slab_load<BF>(sK + st * kSlabBytes, K, ldk, base + s_beg + st * kSlab, base + s_end, t);
-      slab_load<BF>(sV + st * kSlabBytes, V, ldv, base + s_beg + st * kSlab, base + s_end, t);
+      slab_load(sK + st * kSlabBytes, K, ldk, base + s_beg + st * kSlab, base + s_end, t);
+      slab_load(sV + st * kSlabBytes, V, ldv, base + s_beg + st * kSlab, base + s_end, t);
     }
     cp_async_commit();
   }
@@ -305,39 +281,21 @@ __global__ void __launch_bounds__(256) kv_partial_kernel(const void* __restrict_
       const int nx = i + kAttStages - 1;
       if (nx < nslab) {
         const int st = nx % kAttStages;
-        slab_load<BF>(sK + st * kSlabBytes, K, ldk, base + s_beg + nx * kSlab, base + s_end, t);
-        slab_load<BF>(sV + st * kSlabBytes, V, ldv, base + s_beg + nx * kSlab, base + s_end, t);
+        slab_load(sK + st * kSlabBytes, K, ldk, base + s_beg + nx * kSlab, base + s_end, t);
+        slab_load(sV + st * kSlabBytes, V, ldv, base + s_beg + nx * kSlab, base + s_end, t);
       }
       cp_async_commit();
     }
     const char* k0 = sK + (i % kAttStages) * kSlabBytes;
     const char* v0 = sV + (i % kAttStages) * kSlabBytes;
-    const void* kc = k0;                       // what the inner loop reads K from
-    if constexpr (BF) {
-#pragma unroll
-      for (int e = 0; e < kSlab * 256 / 256 / 8; ++e) {           // 8 elements (16 bytes) per thread per step
-        const int idx = (t + 256 * e) * 8;
-        const uint4 u = *reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned short*>(k0) + idx);
-        const unsigned w[4] = {u.x, u.y, u.z, u.w};
-        float4 lo, hi;
-        lo.x = __uint_as_float(w[0] << 16); lo.y = __uint_as_float(w[0] & 0xffff0000u);
-        lo.z = __uint_as_float(w[1] << 16); lo.w = __uint_as_float(w[1] & 0xffff0000u);
-        hi.x = __uint_as_float(w[2] << 16); hi.y = __uint_as_float(w[2] & 0xffff0000u);
-        hi.z = __uint_as_float(w[3] << 16); hi.w = __uint_as_float(w[3] & 0xffff0000u);
-        *reinterpret_cast<float4*>(sKf + idx) = lo;
-        *reinterpret_cast<float4*>(sKf + idx + 4) = hi;
-      }
-      __syncthreads();
-      kc = sKf;
-    }
 #pragma unroll 4
     for (int r = 0; r < kSlab; ++r) {
-      const float vv = __fdiv_rn(slab_elem<BF>(v0, r, t), fS);     // values / v_length (linear_attention.py:40)
+      const float vv = __fdiv_rn(slab_elem(v0, r, t), fS);     // values / v_length (linear_attention.py:40)
       float kk[32];
-      slab_head<false>(kc, r, h, kk);
+      slab_head(k0, r, h, kk);
 #pragma unroll
       for (int d = 0; d < 32; ++d) acc[d] = fmaf(kk[d], vv, acc[d]);
-      ks += slab_elem<false>(kc, r, t);
+      ks += slab_elem(k0, r, t);
     }
   }
   float* o = kv_part + ((static_cast<size_t>(n) * splits + split) * 8 + h) * 1056;
@@ -357,15 +315,13 @@ __global__ void __launch_bounds__(256) kv_reduce_kernel(const float* __restrict_
   kv[static_cast<size_t>(n) * 8448 + e] = s;
 }
 
-template <bool BF>
 __global__ void __launch_bounds__(256) attn_apply_kernel(const void* __restrict__ Q, long long ldq,
                                                          const float* __restrict__ kv,
                                                          void* __restrict__ msg, long long ldm, int L,
                                                          int S, float eps, int splits) {
   extern __shared__ __align__(16) float att_smem[];
-  constexpr int kSlabBytes = kSlab * 256 * (BF ? 2 : 4);
+  constexpr int kSlabBytes = kSlab * 256 * 4;
   char* sQ = reinterpret_cast<char*>(att_smem);                           // [stages][kSlab][256]
-  float* sQf = reinterpret_cast<float*>(reinterpret_cast<char*>(att_smem) + kAttStages * kSlabBytes);   // [kSlab][256], BF only
   const int n = blockIdx.y;
   const int chunk = (L + splits - 1) / splits;
   const int l_beg = blockIdx.x * chunk, l_end = min(L, l_beg + chunk);
@@ -374,7 +330,7 @@ __global__ void __launch_bounds__(256) attn_apply_kernel(const void* __restrict_
   const long long base = static_cast<long long>(n) * L;
 #pragma unroll
   for (int st = 0; st < kAttStages - 1; ++st) {
-    if (st < nslab) slab_load<BF>(sQ + st * kSlabBytes, Q, ldq, base + l_beg + st * kSlab, base + l_end, t);
+    if (st < nslab) slab_load(sQ + st * kSlabBytes, Q, ldq, base + l_beg + st * kSlab, base + l_end, t);
     cp_async_commit();
   }
   const float* kvh = kv + (static_cast<size_t>(n) * 8 + h) * 1056;
@@ -388,49 +344,30 @@ __global__ void __launch_bounds__(256) attn_apply_kernel(const void* __restrict_
     __syncthreads();
     {
       const int nx = i + kAttStages - 1;
-      if (nx < nslab) slab_load<BF>(sQ + (nx % kAttStages) * kSlabBytes, Q, ldq, base + l_beg + nx * kSlab, base + l_end, t);
+      if (nx < nslab) slab_load(sQ + (nx % kAttStages) * kSlabBytes, Q, ldq, base + l_beg + nx * kSlab, base + l_end, t);
       cp_async_commit();
     }
     const char* q0 = sQ + (i % kAttStages) * kSlabBytes;
     const int cnt = min(kSlab, l_end - l_beg - i * kSlab);
-    const void* qc = q0;
-    if constexpr (BF) {                        // widen the slab once (every q element is read by a whole warp)
-#pragma unroll
-      for (int e = 0; e < kSlab * 256 / 256 / 8; ++e) {
-        const int idx = (t + 256 * e) * 8;
-        const uint4 u = *reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned short*>(q0) + idx);
-        const unsigned w[4] = {u.x, u.y, u.z, u.w};
-        float4 lo, hi;
-        lo.x = __uint_as_float(w[0] << 16); lo.y = __uint_as_float(w[0] & 0xffff0000u);
-        lo.z = __uint_as_float(w[1] << 16); lo.w = __uint_as_float(w[1] & 0xffff0000u);
-        hi.x = __uint_as_float(w[2] << 16); hi.y = __uint_as_float(w[2] & 0xffff0000u);
-        hi.z = __uint_as_float(w[3] << 16); hi.w = __uint_as_float(w[3] & 0xffff0000u);
-        *reinterpret_cast<float4*>(sQf + idx) = lo;
-        *reinterpret_cast<float4*>(sQf + idx + 4) = hi;
-      }
-      __syncthreads();
-      qc = sQf;
-    }
 #pragma unroll 4
     for (int r = 0; r < cnt; ++r) {
       float qq[32];
-      slab_head<false>(qc, r, h, qq);
+      slab_head(q0, r, h, qq);
       float a = 0.f;
 #pragma unroll
       for (int d = 0; d < 32; ++d) a = fmaf(qq[d], kvr[d], a);
-      const float den = warp_sum(slab_elem<false>(qc, r, t) * ksum);
+      const float den = warp_sum(slab_elem(q0, r, t) * ksum);
       const float o = a * (1.f / (den + eps)) * fS;
       const long long oi = (base + l_beg + i * kSlab + r) * ldm + t;
-      if constexpr (BF) static_cast<unsigned short*>(msg)[oi] = f2bf(o);
-      else static_cast<float*>(msg)[oi] = o;
+      static_cast<float*>(msg)[oi] = o;
     }
   }
 }
 
 
 // ------------------------------------------------------------------------------------------ linear attention on mma.sync (bf16 operands)
-// bf16 mode: q' = elu(q)+1, k' and v are already bf16 in HBM, so K'^T V (32 x 32 per head, reduction over the tokens)
-// and Q' (KV) are warp-level m16n8k16 tensor-core products with fp32 accumulation; the SIMT kernels above are
+// bf16 mode: q, k and v are bf16 in HBM, so K'^T V (32 x 32 per head, reduction over the tokens) and Q' (KV) are
+// warp-level m16n8k16 tensor-core products with fp32 accumulation; SIMT kernels like the fp32 ones above would be
 // issue-bound on shared-memory reads and fp32 FMAs. Slabs land by cp.async with the 16-byte chunk index XOR-ed by
 // (row & 7), which makes every ldmatrix phase (8 rows, one chunk column) bank-conflict free. The reference's
 // values / v_length ... * v_length pair (linear_attention.py:40-45) cancels and is not applied here.
@@ -476,7 +413,7 @@ __device__ __forceinline__ float elu1_fast(float v) {   // the token-GEMM epilog
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(fminf(v * 1.4426950408889634f, 0.f)));
   return fmaxf(v, 0.f) + e;
 }
-// RAW variants of the attention kernels take q and k as the projection GEMM leaves them and apply the feature map
+// The bf16 attention kernels take q and k as the projection GEMM leaves them and apply the feature map
 // elu(x) + 1 to the mma fragments in registers: the GEMM's 8 epilogue warps were bound by exactly this (MUFU + ALU issue),
 // while these kernels wait for HBM. keep_lo / keep_hi = false zeroes an element (token padding: K' rows past the end).
 __device__ __forceinline__ unsigned elu1_bf16x2(unsigned v, bool keep_lo = true, bool keep_hi = true) {
@@ -484,7 +421,6 @@ __device__ __forceinline__ unsigned elu1_bf16x2(unsigned v, bool keep_lo = true,
   return pack_bf16(keep_lo ? lo : 0.f, keep_hi ? hi : 0.f);
 }
 
-template <bool RAW>
 __global__ void __launch_bounds__(256) kv_partial_mma_kernel(const void* __restrict__ K, long long ldk,
                                                              const void* __restrict__ V, long long ldv,
                                                              float* __restrict__ kv_part, int S, int splits) {
@@ -537,16 +473,15 @@ __global__ void __launch_bounds__(256) kv_partial_mma_kernel(const void* __restr
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt)      // A = K'^T: m = channel d, k = token
         ldsm_x4_t(a[mt], sw_addr(k0, 16 * ks + r + 8 * (j >> 1), 4 * h + 2 * mt + (j & 1)));
-      if constexpr (RAW) {                // registers e = 0, 1 hold tokens 2 tq, 2 tq + 1 of the k-step, e = 2, 3 those + 8
-        const int tok = s_beg + i * kMS + 16 * ks + 2 * tq;
+      // registers e = 0, 1 hold tokens 2 tq, 2 tq + 1 of the k-step, e = 2, 3 those + 8
+      const int tok = s_beg + i * kMS + 16 * ks + 2 * tq;
 #pragma unroll
-        for (int mt = 0; mt < 2; ++mt)
+      for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int t0 = tok + 8 * (e >> 1);
-            a[mt][e] = elu1_bf16x2(a[mt][e], t0 < s_end, t0 + 1 < s_end);
-          }
-      }
+        for (int e = 0; e < 4; ++e) {
+          const int t0 = tok + 8 * (e >> 1);
+          a[mt][e] = elu1_bf16x2(a[mt][e], t0 < s_end, t0 + 1 < s_end);
+        }
 #pragma unroll
       for (int pp = 0; pp < 2; ++pp)      // B = V: k = token, n = channel v (two 8-wide tiles per ldmatrix)
         ldsm_x4_t(b[pp], sw_addr(v0, 16 * ks + r + 8 * (j & 1), 4 * h + 2 * pp + (j >> 1)));
@@ -574,7 +509,6 @@ __global__ void __launch_bounds__(256) kv_partial_mma_kernel(const void* __restr
 }
 
 // msg[l][32h+v] = (Q'[l] . KV[:, v]) / (Q'[l] . Ksum + eps), KV / Ksum rounded to bf16 as the B operand; warp = head
-template <bool RAW>
 __global__ void __launch_bounds__(256) attn_apply_mma_kernel(const void* __restrict__ Q, long long ldq,
                                                              const float* __restrict__ kv,
                                                              unsigned short* __restrict__ msg, long long ldm, int L,
@@ -629,10 +563,8 @@ __global__ void __launch_bounds__(256) attn_apply_mma_kernel(const void* __restr
       for (int ks = 0; ks < 2; ++ks) {
         unsigned a[4];                      // A = Q': m = token, k = channel d
         ldsm_x4(a, sw_addr(q0, 16 * mt + r + 8 * (j & 1), 4 * h + 2 * ks + (j >> 1)));
-        if constexpr (RAW) {
 #pragma unroll
-          for (int e = 0; e < 4; ++e) a[e] = elu1_bf16x2(a[e]);
-        }
+        for (int e = 0; e < 4; ++e) a[e] = elu1_bf16x2(a[e]);
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) mma_bf16(c[nt], a, bkv[ks][nt][0], bkv[ks][nt][1]);
         mma_bf16(cd, a, bden[ks][0], bden[ks][1]);
@@ -653,7 +585,7 @@ __global__ void __launch_bounds__(256) attn_apply_mma_kernel(const void* __restr
 
 // ------------------------------------------------------------------------------------------ linear attention (windows)
 // C = 128 (8 heads x 16), T tokens per item (T <= 32). One block (128 threads) per item.
-template <int T, bool BF>
+template <int T>
 __global__ void __launch_bounds__(128) attn_windows_kernel(const void* __restrict__ Qv, long long ldq,
                                                            const void* __restrict__ Kv, long long ldk,
                                                            const void* __restrict__ Vv, long long ldv,
@@ -668,31 +600,18 @@ __global__ void __launch_bounds__(128) attn_windows_kernel(const void* __restric
   const int t = threadIdx.x;
   const int hb = (t >> 4) << 4;  // first channel of this thread's head
   const float fT = static_cast<float>(T);
-  // cooperative 16-byte loads of the item's T x 128 q / k / v rows (fp32: 32 chunks per row, bf16: 16)
-  constexpr int CH = BF ? 16 : 32, EPC = BF ? 8 : 4;     // chunks per row, elements per chunk
+  // cooperative 16-byte loads of the item's T x 128 q / k / v rows
+  constexpr int CH = 32, EPC = 4;     // chunks per row, elements per chunk
   const size_t row0 = static_cast<size_t>(item) * T;
   for (int c = t; c < T * CH; c += 128) {
     const int r = c / CH, e0 = (c % CH) * EPC;
     float q[EPC], k[EPC], v[EPC];
-    if constexpr (BF) {
-      const uint4 uq = *reinterpret_cast<const uint4*>(static_cast<const unsigned short*>(Qv) + (row0 + r) * ldq + e0);
-      const uint4 uk = *reinterpret_cast<const uint4*>(static_cast<const unsigned short*>(Kv) + (row0 + r) * ldk + e0);
-      const uint4 uv = *reinterpret_cast<const uint4*>(static_cast<const unsigned short*>(Vv) + (row0 + r) * ldv + e0);
-      const unsigned wq[4] = {uq.x, uq.y, uq.z, uq.w}, wk[4] = {uk.x, uk.y, uk.z, uk.w}, wv[4] = {uv.x, uv.y, uv.z, uv.w};
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        q[2 * e] = __uint_as_float(wq[e] << 16); q[2 * e + 1] = __uint_as_float(wq[e] & 0xffff0000u);
-        k[2 * e] = __uint_as_float(wk[e] << 16); k[2 * e + 1] = __uint_as_float(wk[e] & 0xffff0000u);
-        v[2 * e] = __uint_as_float(wv[e] << 16); v[2 * e + 1] = __uint_as_float(wv[e] & 0xffff0000u);
-      }
-    } else {
-      const float4 fq = *reinterpret_cast<const float4*>(static_cast<const float*>(Qv) + (row0 + r) * ldq + e0);
-      const float4 fk = *reinterpret_cast<const float4*>(static_cast<const float*>(Kv) + (row0 + r) * ldk + e0);
-      const float4 fv = *reinterpret_cast<const float4*>(static_cast<const float*>(Vv) + (row0 + r) * ldv + e0);
-      q[0] = fq.x; q[1] = fq.y; q[2] = fq.z; q[3] = fq.w;
-      k[0] = fk.x; k[1] = fk.y; k[2] = fk.z; k[3] = fk.w;
-      v[0] = fv.x; v[1] = fv.y; v[2] = fv.z; v[3] = fv.w;
-    }
+    const float4 fq = *reinterpret_cast<const float4*>(static_cast<const float*>(Qv) + (row0 + r) * ldq + e0);
+    const float4 fk = *reinterpret_cast<const float4*>(static_cast<const float*>(Kv) + (row0 + r) * ldk + e0);
+    const float4 fv = *reinterpret_cast<const float4*>(static_cast<const float*>(Vv) + (row0 + r) * ldv + e0);
+    q[0] = fq.x; q[1] = fq.y; q[2] = fq.z; q[3] = fq.w;
+    k[0] = fk.x; k[1] = fk.y; k[2] = fk.z; k[3] = fk.w;
+    v[0] = fv.x; v[1] = fv.y; v[2] = fv.z; v[3] = fv.w;
 #pragma unroll
     for (int e = 0; e < EPC; e += 4) {                 // 16-byte shared-memory stores
       *reinterpret_cast<float4*>(&sQ[r][e0 + e]) = make_float4(q[e], q[e + 1], q[e + 2], q[e + 3]);
@@ -736,17 +655,8 @@ __global__ void __launch_bounds__(128) attn_windows_kernel(const void* __restric
   __syncthreads();
   for (int c = t; c < T * CH; c += 128) {              // 16-byte stores of the T x 128 message rows
     const int r = c / CH, e0 = (c % CH) * EPC;
-    if constexpr (BF) {
-      uint4 o;
-      o.x = static_cast<unsigned>(f2bf(sK[r][e0])) | (static_cast<unsigned>(f2bf(sK[r][e0 + 1])) << 16);
-      o.y = static_cast<unsigned>(f2bf(sK[r][e0 + 2])) | (static_cast<unsigned>(f2bf(sK[r][e0 + 3])) << 16);
-      o.z = static_cast<unsigned>(f2bf(sK[r][e0 + 4])) | (static_cast<unsigned>(f2bf(sK[r][e0 + 5])) << 16);
-      o.w = static_cast<unsigned>(f2bf(sK[r][e0 + 6])) | (static_cast<unsigned>(f2bf(sK[r][e0 + 7])) << 16);
-      *reinterpret_cast<uint4*>(static_cast<unsigned short*>(msgv) + (row0 + r) * ldm + e0) = o;
-    } else {
-      *reinterpret_cast<float4*>(static_cast<float*>(msgv) + (row0 + r) * ldm + e0) =
-          make_float4(sK[r][e0], sK[r][e0 + 1], sK[r][e0 + 2], sK[r][e0 + 3]);
-    }
+    *reinterpret_cast<float4*>(static_cast<float*>(msgv) + (row0 + r) * ldm + e0) =
+        make_float4(sK[r][e0], sK[r][e0 + 1], sK[r][e0 + 2], sK[r][e0 + 3]);
   }
 }
 
@@ -755,7 +665,7 @@ __global__ void __launch_bounds__(128) attn_windows_kernel(const void* __restric
 // rows. Per head: KV^T[v][d] = sum_s V[s][v] K'[s][d] (A = V^T, B = K') and Ksum through an A tile whose row 0 is all
 // ones; the accumulator fragments ARE the B fragments of the second product out[l][v] = Q'[l][d] KV[d][v] (transposed
 // accumulation puts (d pair, v) in the right lanes), so nothing goes back through shared memory.
-template <int T, bool RAW>
+template <int T>
 __global__ void __launch_bounds__(256) attn_windows_mma_kernel(const unsigned short* __restrict__ Q, long long ldq,
                                                                const unsigned short* __restrict__ K, long long ldk,
                                                                const unsigned short* __restrict__ V, long long ldv,
@@ -795,13 +705,12 @@ __global__ void __launch_bounds__(256) attn_windows_mma_kernel(const unsigned sh
     unsigned a[4], b[4];
     ldsm_x4_t(a, addr(2, 16 * ks + r + 8 * (j >> 1), 2 * h + (j & 1)));     // A = V^T: m = v, k = token
     ldsm_x4_t(b, addr(1, 16 * ks + r + 8 * (j & 1), 2 * h + (j >> 1)));     // B = K': k = token, n = d
-    if constexpr (RAW) {                  // b[2 nt] holds tokens 2 tq, 2 tq + 1 of the k-step, b[2 nt + 1] those + 8; rows >= T stay zero
-      const int tok = 16 * ks + 2 * tq;
+    // b[2 nt] holds tokens 2 tq, 2 tq + 1 of the k-step, b[2 nt + 1] those + 8; rows >= T stay zero
+    const int tok = 16 * ks + 2 * tq;
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int t0 = tok + 8 * (e & 1);
-        b[e] = elu1_bf16x2(b[e], t0 < T, t0 + 1 < T);
-      }
+    for (int e = 0; e < 4; ++e) {
+      const int t0 = tok + 8 * (e & 1);
+      b[e] = elu1_bf16x2(b[e], t0 < T, t0 + 1 < T);
     }
 #pragma unroll
     for (int nt = 0; nt < 2; ++nt) {
@@ -816,10 +725,8 @@ __global__ void __launch_bounds__(256) attn_windows_mma_kernel(const unsigned sh
   for (int mt = 0; mt < 2; ++mt) {
     unsigned a[4];
     ldsm_x4(a, addr(0, 16 * mt + r + 8 * (j & 1), 2 * h + (j >> 1)));       // A = Q': m = token, k = d
-    if constexpr (RAW) {
 #pragma unroll
-      for (int e = 0; e < 4; ++e) a[e] = elu1_bf16x2(a[e]);
-    }
+    for (int e = 0; e < 4; ++e) a[e] = elu1_bf16x2(a[e]);
     float c0[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f}, cd[4] = {0.f, 0.f, 0.f, 0.f};
     mma_bf16(c0, a, bv0[0], bv0[1]);
     mma_bf16(c1, a, bv1[0], bv1[1]);
@@ -840,153 +747,6 @@ __global__ void __launch_bounds__(256) attn_windows_mma_kernel(const unsigned sh
   }
 }
 
-// q|k|v projection + window attention of the fine level in ONE kernel (bf16 mode): q, k, v never go to HBM.
-// Persistent blocks, 8 warps = 8 heads. Warp h keeps rows [16 h, 16 h + 16) of Wq, Wk and Wv (its head's 16 output
-// channels, all 128 input channels) as mma.sync B fragments in 96 registers for the lifetime of the block. Per window:
-//   cp.async the 25 x 128 bf16 token rows of the query side and of the source side (the same for self attention) into
-//   shared memory (double-buffered across windows), project them with mma.sync m16n8k16 (tokens padded to 32, zero rows),
-//   elu + 1 on q and k in registers, write the head's Q', K', V slice (bf16) into the shared tile the attention part reads
-//   (only this warp touches its head's columns, so a __syncwarp orders the two), then the attention of
-//   attn_windows_mma_kernel above and the 25 message rows to global memory.
-template <int T>
-__global__ void __launch_bounds__(256, 1) fine_attn_fused_kernel(const unsigned short* __restrict__ xq, long long ldq,
-                                                                  const unsigned short* __restrict__ xs, long long lds,
-                                                                  const unsigned short* __restrict__ W,   // [3 * 128][128] bf16: Wq, Wk, Wv
-                                                                  unsigned short* __restrict__ msg, long long ldm,
-                                                                  const int* __restrict__ n_items_dev, float eps) {
-  static_assert(T <= 32, "window tokens are padded to 32");
-  extern __shared__ __align__(128) char smf[];            // x tiles [2 buffers][query, source][32][128] bf16, then Q', K', V tiles
-  char* sX = smf;
-  char* sP = smf + 4 * 8192;
-  const int n_items = *n_items_dev;
-  const bool self = xq == xs;
-  const int t = threadIdx.x, h = t >> 5, lane = t & 31;
-  const int j = lane >> 3, r = lane & 7, g = lane >> 2, tq = lane & 3;
-  unsigned wf[3][2][8][2];                                // B fragments: wf[matrix][n tile][k tile]: W[n = g][k = 2 tq (+1)], W[g][k + 8 ...]
-#pragma unroll
-  for (int m = 0; m < 3; ++m)
-#pragma unroll
-    for (int nt = 0; nt < 2; ++nt)
-#pragma unroll
-      for (int kt = 0; kt < 8; ++kt) {
-        const unsigned short* wr = W + static_cast<size_t>(m * 128 + 16 * h + 8 * nt + g) * 128 + 16 * kt + 2 * tq;
-        wf[m][nt][kt][0] = *reinterpret_cast<const unsigned*>(wr);
-        wf[m][nt][kt][1] = *reinterpret_cast<const unsigned*>(wr + 8);
-      }
-  for (int c = t; c < 4 * (32 - T) * 16; c += 256) {      // zero padding rows of the four x tiles (never written again)
-    const int which = c / ((32 - T) * 16), rc = c % ((32 - T) * 16), rr = T + (rc >> 4), ch = rc & 15;
-    *reinterpret_cast<uint4*>(sX + which * 8192 + rr * 256 + (ch << 4)) = make_uint4(0, 0, 0, 0);
-  }
-  auto load_x = [&](int item, int buf) {
-    const size_t row0 = static_cast<size_t>(item) * T;
-    const int n = (self ? 1 : 2) * T * 16;
-    for (int c = t; c < n; c += 256) {
-      const int which = c / (T * 16), rc = c % (T * 16), rr = rc >> 4, ch = rc & 15;
-      const unsigned short* src = (which == 0 ? xq + (row0 + rr) * ldq : xs + (row0 + rr) * lds) + ch * 8;
-      cp_async16(sX + (buf * 2 + which) * 8192 + rr * 256 + ((ch ^ (rr & 7)) << 4), src, true);
-    }
-    cp_async_commit();
-  };
-  auto addr = [&](int which, int row, int chunk) { return sP + which * 8192 + row * 256 + ((chunk ^ (row & 7)) << 4); };
-  int item = blockIdx.x, buf = 0;
-  if (item < n_items) load_x(item, 0);
-  for (; item < n_items; item += gridDim.x, buf ^= 1) {
-    cp_async_wait<0>();
-    __syncthreads();                                      // this window's rows have landed; everyone is done with the other buffer
-    if (item + static_cast<int>(gridDim.x) < n_items) load_x(item + gridDim.x, buf ^ 1);
-    const char* xqb = sX + (buf * 2) * 8192;
-    const char* xsb = self ? xqb : xqb + 8192;
-    // ---- projection: this head's 16 channels of Q', K', V for the 32 (padded) tokens
-#pragma unroll
-    for (int mt = 0; mt < 2; ++mt) {
-      float cq[2][4], ck[2][4], cv[2][4];
-#pragma unroll
-      for (int nt = 0; nt < 2; ++nt)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) { cq[nt][e] = 0.f; ck[nt][e] = 0.f; cv[nt][e] = 0.f; }
-      const int arow = 16 * mt + r + 8 * (j & 1);
-#pragma unroll
-      for (int kt = 0; kt < 8; ++kt) {
-        const int off = arow * 256 + (((2 * kt + (j >> 1)) ^ (arow & 7)) << 4);
-        unsigned aq[4], as[4];
-        ldsm_x4(aq, xqb + off);
-        if (self) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) as[e] = aq[e];
-        } else {
-          ldsm_x4(as, xsb + off);
-        }
-#pragma unroll
-        for (int nt = 0; nt < 2; ++nt) {
-          mma_bf16(cq[nt], aq, wf[0][nt][kt][0], wf[0][nt][kt][1]);
-          mma_bf16(ck[nt], as, wf[1][nt][kt][0], wf[1][nt][kt][1]);
-          mma_bf16(cv[nt], as, wf[2][nt][kt][0], wf[2][nt][kt][1]);
-        }
-      }
-      const int l0 = 16 * mt + g, l1 = l0 + 8;
-#pragma unroll
-      for (int nt = 0; nt < 2; ++nt) {
-        const int chunk = 2 * h + nt;
-        *reinterpret_cast<unsigned*>(addr(0, l0, chunk) + 4 * tq) = pack_bf16(elu1_fast(cq[nt][0]), elu1_fast(cq[nt][1]));
-        *reinterpret_cast<unsigned*>(addr(0, l1, chunk) + 4 * tq) = pack_bf16(elu1_fast(cq[nt][2]), elu1_fast(cq[nt][3]));
-        // padding rows of K' must be zero (elu(0) + 1 = 1 would count as tokens); those of V are zero already (zero x rows)
-        *reinterpret_cast<unsigned*>(addr(1, l0, chunk) + 4 * tq) = l0 < T ? pack_bf16(elu1_fast(ck[nt][0]), elu1_fast(ck[nt][1])) : 0u;
-        *reinterpret_cast<unsigned*>(addr(1, l1, chunk) + 4 * tq) = l1 < T ? pack_bf16(elu1_fast(ck[nt][2]), elu1_fast(ck[nt][3])) : 0u;
-        *reinterpret_cast<unsigned*>(addr(2, l0, chunk) + 4 * tq) = pack_bf16(cv[nt][0], cv[nt][1]);
-        *reinterpret_cast<unsigned*>(addr(2, l1, chunk) + 4 * tq) = pack_bf16(cv[nt][2], cv[nt][3]);
-      }
-    }
-    __syncwarp();
-    // ---- attention of this head (see attn_windows_mma_kernel)
-    float ckv[2][4], cks[2][4];
-#pragma unroll
-    for (int a = 0; a < 2; ++a) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) { ckv[a][e] = 0.f; cks[a][e] = 0.f; }
-    }
-    const unsigned one = (g == 0) ? 0x3F803F80u : 0u;
-    const unsigned aones[4] = {one, 0u, one, 0u};
-#pragma unroll
-    for (int ks = 0; ks < 2; ++ks) {
-      unsigned a[4], b[4];
-      ldsm_x4_t(a, addr(2, 16 * ks + r + 8 * (j >> 1), 2 * h + (j & 1)));     // A = V^T: m = v, k = token
-      ldsm_x4_t(b, addr(1, 16 * ks + r + 8 * (j & 1), 2 * h + (j >> 1)));     // B = K': k = token, n = d
-#pragma unroll
-      for (int nt = 0; nt < 2; ++nt) {
-        mma_bf16(ckv[nt], a, b[2 * nt], b[2 * nt + 1]);
-        mma_bf16(cks[nt], aones, b[2 * nt], b[2 * nt + 1]);
-      }
-    }
-    const unsigned bv0[2] = {pack_bf16(ckv[0][0], ckv[0][1]), pack_bf16(ckv[1][0], ckv[1][1])};
-    const unsigned bv1[2] = {pack_bf16(ckv[0][2], ckv[0][3]), pack_bf16(ckv[1][2], ckv[1][3])};
-    const unsigned bd[2] = {pack_bf16(cks[0][0], cks[0][1]), pack_bf16(cks[1][0], cks[1][1])};
-    const size_t row0 = static_cast<size_t>(item) * T;
-#pragma unroll
-    for (int mt = 0; mt < 2; ++mt) {
-      unsigned a[4];
-      ldsm_x4(a, addr(0, 16 * mt + r + 8 * (j & 1), 2 * h + (j >> 1)));       // A = Q': m = token, k = d
-      float c0[4] = {0.f, 0.f, 0.f, 0.f}, c1[4] = {0.f, 0.f, 0.f, 0.f}, cd[4] = {0.f, 0.f, 0.f, 0.f};
-      mma_bf16(c0, a, bv0[0], bv0[1]);
-      mma_bf16(c1, a, bv1[0], bv1[1]);
-      mma_bf16(cd, a, bd[0], bd[1]);
-      const float den_lo = __shfl_sync(0xffffffffu, cd[0], lane & ~3), den_hi = __shfl_sync(0xffffffffu, cd[2], lane & ~3);
-      const float z_lo = 1.f / (den_lo + eps), z_hi = 1.f / (den_hi + eps);
-      const int l0 = 16 * mt + g;
-      if (l0 < T) {
-        unsigned short* o = msg + (row0 + l0) * ldm + 16 * h + 2 * tq;
-        *reinterpret_cast<unsigned*>(o) = pack_bf16(c0[0] * z_lo, c0[1] * z_lo);
-        *reinterpret_cast<unsigned*>(o + 8) = pack_bf16(c1[0] * z_lo, c1[1] * z_lo);
-      }
-      if (l0 + 8 < T) {
-        unsigned short* o = msg + (row0 + l0 + 8) * ldm + 16 * h + 2 * tq;
-        *reinterpret_cast<unsigned*>(o) = pack_bf16(c0[2] * z_hi, c0[3] * z_hi);
-        *reinterpret_cast<unsigned*>(o + 8) = pack_bf16(c1[2] * z_hi, c1[3] * z_hi);
-      }
-    }
-    __syncwarp();                                         // the head's tiles are rewritten by the next window's projection
-  }
-}
-
 // ------------------------------------------------------------------------------------------ layernorm
 template <int C>
 __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ in, long long ldi,
@@ -994,8 +754,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
                                                         const float* __restrict__ beta,
                                                         const float* __restrict__ res, long long ldr,
                                                         float* __restrict__ out, long long ldo,
-                                                        long long rows, const int* __restrict__ dyn_rows,
-                                                        unsigned short* __restrict__ out16, long long ldo16) {
+                                                        long long rows, const int* __restrict__ dyn_rows) {
   constexpr int V = C / 128;  // float4 per lane
   long long lim = rows;
   if (dyn_rows) lim = min(lim, static_cast<long long>(*dyn_rows));
@@ -1033,13 +792,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
       const float4 r = *reinterpret_cast<const float4*>(res + row * ldr + c);
       o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
     }
-    if (out) *reinterpret_cast<float4*>(out + row * ldo + c) = o;
-    if (out16) {     // bf16 shadow of the row (A operand of the next token GEMMs in bf16 mode)
-      uint2 u;
-      u.x = static_cast<unsigned>(f2bf(o.x)) | (static_cast<unsigned>(f2bf(o.y)) << 16);
-      u.y = static_cast<unsigned>(f2bf(o.z)) | (static_cast<unsigned>(f2bf(o.w)) << 16);
-      *reinterpret_cast<uint2*>(out16 + row * ldo16 + c) = u;
-    }
+    *reinterpret_cast<float4*>(out + row * ldo + c) = o;
   }
   }
 }
@@ -1813,7 +1566,7 @@ __global__ void __launch_bounds__(128) stem_mma_kernel(const float* __restrict__
 // launch wrappers
 // ================================================================================================
 int stem_conv7x7(const float* img, const float* w, const float* bias, float* out, int NI, int H, int W,
-                 cudaStream_t st, int out_bf16, int exact_fp32, int grid_limit) {
+                 cudaStream_t st, int out_bf16, int exact_fp32) {
   const int Ho = (H + 6 - 7) / 2 + 1, Wo = (W + 6 - 7) / 2 + 1;
   if (kUseMmaStem && !exact_fp32) {
     const int PW = 32 * ((Wo + 15) / 16) + 8;                 // patch columns: 2 px + kx for every pixel of the padded row
@@ -1876,41 +1629,24 @@ int linear_attention_long(const void* Q, long long ldq, const void* K, long long
   if (dim != 32 || heads != 8) return MFR_ERR_UNSUPPORTED;
   if ((ldq | ldk | ldv) & (bf16 ? 7 : 3)) return MFR_ERR_ARG;                    // 16-byte cp.async chunks
   constexpr int kKvSmem = 2 * kAttStages * kSlab * 256 * 4, kApSmem = kAttStages * kSlab * 256 * 4;
-  constexpr int kWide = kSlab * 256 * 4;   // bf16 variants: one fp32 slab the K / Q rows are widened into
-  constexpr int kKvSmemBf = kKvSmem / 2 + kWide, kApSmemBf = kApSmem / 2 + kWide;
   static bool attr_seen[64] = {};
   if (first_call_on_device(attr_seen)) {
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(kv_partial_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kKvSmem));
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(attn_apply_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApSmem));
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(kv_partial_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kKvSmemBf));
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(attn_apply_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kApSmemBf));
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(kv_partial_mma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kMStages * kMSlabBytes));
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(attn_apply_mma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMStages * kMSlabBytes));
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(kv_partial_mma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kMStages * kMSlabBytes));
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(attn_apply_mma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMStages * kMSlabBytes));
+    MFR_CUDA_CHECK(cudaFuncSetAttribute(kv_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kKvSmem));
+    MFR_CUDA_CHECK(cudaFuncSetAttribute(attn_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kApSmem));
+    MFR_CUDA_CHECK(cudaFuncSetAttribute(kv_partial_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * kMStages * kMSlabBytes));
+    MFR_CUDA_CHECK(cudaFuncSetAttribute(attn_apply_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMStages * kMSlabBytes));
   }
-  const int asplits = std::max(1, std::min((L + kSlab - 1) / kSlab, (4 * sm_count() + n - 1) / n));
   if (bf16) {
-    if (kUseMmaAttention) {
-      const int msplits = std::max(1, std::min((L + kMS - 1) / kMS, (4 * sm_count() + n - 1) / n));
-      if (bf16 == 2) kv_partial_mma_kernel<true><<<dim3(splits, n), 256, 2 * kMStages * kMSlabBytes, st>>>(K, ldk, V, ldv, kv_part, S, splits);
-      else kv_partial_mma_kernel<false><<<dim3(splits, n), 256, 2 * kMStages * kMSlabBytes, st>>>(K, ldk, V, ldv, kv_part, S, splits);
-      kv_reduce_kernel<<<dim3((8 * 1056 + 255) / 256, n), 256, 0, st>>>(kv_part, kv, splits);
-      if (bf16 == 2)
-        attn_apply_mma_kernel<true><<<dim3(msplits, n), 256, kMStages * kMSlabBytes, st>>>(Q, ldq, kv, static_cast<unsigned short*>(msg), ldm, L,
-                                                                                          1e-6f, msplits);
-      else
-        attn_apply_mma_kernel<false><<<dim3(msplits, n), 256, kMStages * kMSlabBytes, st>>>(Q, ldq, kv, static_cast<unsigned short*>(msg), ldm, L,
-                                                                                           1e-6f, msplits);
-    } else {
-      kv_partial_kernel<true><<<dim3(splits, n), 256, kKvSmemBf, st>>>(K, ldk, V, ldv, kv_part, S, splits);
-      kv_reduce_kernel<<<dim3((8 * 1056 + 255) / 256, n), 256, 0, st>>>(kv_part, kv, splits);
-      attn_apply_kernel<true><<<dim3(asplits, n), 256, kApSmemBf, st>>>(Q, ldq, kv, msg, ldm, L, S, 1e-6f, asplits);
-    }
-  } else {
-    kv_partial_kernel<false><<<dim3(splits, n), 256, kKvSmem, st>>>(K, ldk, V, ldv, kv_part, S, splits);
+    const int msplits = std::max(1, std::min((L + kMS - 1) / kMS, (4 * sm_count() + n - 1) / n));
+    kv_partial_mma_kernel<<<dim3(splits, n), 256, 2 * kMStages * kMSlabBytes, st>>>(K, ldk, V, ldv, kv_part, S, splits);
     kv_reduce_kernel<<<dim3((8 * 1056 + 255) / 256, n), 256, 0, st>>>(kv_part, kv, splits);
-    attn_apply_kernel<false><<<dim3(asplits, n), 256, kApSmem, st>>>(Q, ldq, kv, msg, ldm, L, S, 1e-6f, asplits);
+    attn_apply_mma_kernel<<<dim3(msplits, n), 256, kMStages * kMSlabBytes, st>>>(Q, ldq, kv, static_cast<unsigned short*>(msg), ldm, L,
+                                                                               1e-6f, msplits);
+  } else {
+    const int asplits = std::max(1, std::min((L + kSlab - 1) / kSlab, (4 * sm_count() + n - 1) / n));
+    kv_partial_kernel<<<dim3(splits, n), 256, kKvSmem, st>>>(K, ldk, V, ldv, kv_part, S, splits);
+    kv_reduce_kernel<<<dim3((8 * 1056 + 255) / 256, n), 256, 0, st>>>(kv_part, kv, splits);
+    attn_apply_kernel<<<dim3(asplits, n), 256, kApSmem, st>>>(Q, ldq, kv, msg, ldm, L, S, 1e-6f, asplits);
   }
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
@@ -1920,52 +1656,28 @@ int linear_attention_windows(const void* Q, long long ldq, const void* K, long l
                              long long ldv, void* msg, long long ldm, const int* n_items_dev,
                              int max_items, int T, cudaStream_t st, int bf16) {
   if (T != 25 || max_items <= 0) return MFR_ERR_UNSUPPORTED;
-  if (bf16 && kUseMmaAttention) {
+  if (bf16) {
     if ((ldq | ldk | ldv) & 7) return MFR_ERR_ARG;
-    if (bf16 == 2)
-      attn_windows_mma_kernel<25, true><<<max_items, 256, 0, st>>>(static_cast<const unsigned short*>(Q), ldq, static_cast<const unsigned short*>(K), ldk,
-                                                                  static_cast<const unsigned short*>(V), ldv, static_cast<unsigned short*>(msg), ldm,
-                                                                  n_items_dev, 1e-6f);
-    else
-      attn_windows_mma_kernel<25, false><<<max_items, 256, 0, st>>>(static_cast<const unsigned short*>(Q), ldq, static_cast<const unsigned short*>(K), ldk,
-                                                                   static_cast<const unsigned short*>(V), ldv, static_cast<unsigned short*>(msg), ldm,
-                                                                   n_items_dev, 1e-6f);
-  } else if (bf16) attn_windows_kernel<25, true><<<max_items, 128, 0, st>>>(Q, ldq, K, ldk, V, ldv, msg, ldm, n_items_dev, 1e-6f);
-  else attn_windows_kernel<25, false><<<max_items, 128, 0, st>>>(Q, ldq, K, ldk, V, ldv, msg, ldm, n_items_dev, 1e-6f);
-  MFR_CUDA_CHECK(cudaGetLastError());
-  return MFR_OK;
-}
-
-int fine_attention_fused(const void* xq, long long ldq, const void* xs, long long lds, const void* w_qkv, void* msg,
-                         long long ldm, const int* n_items_dev, int max_items, int T, cudaStream_t st) {
-  if (T != 25 || max_items <= 0) return MFR_ERR_UNSUPPORTED;
-  if (((ldq | lds | ldm) & 7) || ((reinterpret_cast<uintptr_t>(xq) | reinterpret_cast<uintptr_t>(xs) | reinterpret_cast<uintptr_t>(w_qkv)) & 15))
-    return MFR_ERR_ARG;
-  constexpr int kSmem = 7 * 8192;
-  static bool attr_seen[64] = {};
-  if (first_call_on_device(attr_seen)) {
-    MFR_CUDA_CHECK(cudaFuncSetAttribute(fine_attn_fused_kernel<25>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+    attn_windows_mma_kernel<25><<<max_items, 256, 0, st>>>(static_cast<const unsigned short*>(Q), ldq, static_cast<const unsigned short*>(K), ldk,
+                                                           static_cast<const unsigned short*>(V), ldv, static_cast<unsigned short*>(msg), ldm,
+                                                           n_items_dev, 1e-6f);
+  } else {
+    attn_windows_kernel<25><<<max_items, 128, 0, st>>>(Q, ldq, K, ldk, V, ldv, msg, ldm, n_items_dev, 1e-6f);
   }
-  const int grid = std::min(max_items, 2 * sm_count());
-  fine_attn_fused_kernel<25><<<grid, 256, kSmem, st>>>(static_cast<const unsigned short*>(xq), ldq, static_cast<const unsigned short*>(xs), lds,
-                                                       static_cast<const unsigned short*>(w_qkv), static_cast<unsigned short*>(msg), ldm,
-                                                       n_items_dev, 1e-6f);
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
 }
 
 int layernorm_rows(const float* in, long long ldi, const float* gamma, const float* beta,
                    const float* res, long long ldr, float* out, long long ldo, long long rows, int C,
-                   const int* dyn_rows, cudaStream_t st, void* out16, long long ldo16) {
+                   const int* dyn_rows, cudaStream_t st) {
   unsigned grid = static_cast<unsigned>(std::min<long long>((rows + 7) / 8, static_cast<long long>(sm_count()) * 16));
   if (grid == 0) return MFR_OK;
-  if (out == nullptr && out16 == nullptr) return MFR_ERR_ARG;
-  if (out16 != nullptr && ((ldo16 & 3) || (reinterpret_cast<uintptr_t>(out16) & 7))) return MFR_ERR_ARG;
-  unsigned short* o16 = static_cast<unsigned short*>(out16);
+  if (out == nullptr) return MFR_ERR_ARG;
   if (C == 256)
-    layernorm_kernel<256><<<grid, 256, 0, st>>>(in, ldi, gamma, beta, res, ldr, out, ldo, rows, dyn_rows, o16, ldo16);
+    layernorm_kernel<256><<<grid, 256, 0, st>>>(in, ldi, gamma, beta, res, ldr, out, ldo, rows, dyn_rows);
   else if (C == 128)
-    layernorm_kernel<128><<<grid, 256, 0, st>>>(in, ldi, gamma, beta, res, ldr, out, ldo, rows, dyn_rows, o16, ldo16);
+    layernorm_kernel<128><<<grid, 256, 0, st>>>(in, ldi, gamma, beta, res, ldr, out, ldo, rows, dyn_rows);
   else
     return MFR_ERR_UNSUPPORTED;
   MFR_CUDA_CHECK(cudaGetLastError());

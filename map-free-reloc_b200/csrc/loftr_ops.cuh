@@ -8,7 +8,7 @@ namespace mfr {
 // stem: conv7x7 stride 2 pad 3, 1 -> 128 channels, folded BN bias, ReLU (resnet_fpn.py:60-62,102)
 // exact_fp32: plain fp32 FMA kernel instead of the tensor-core one (bf16 hi/lo split, ~2^-16 relative)
 int stem_conv7x7(const float* img, const float* w /*[128][49]*/, const float* bias, float* out,
-                 int NI, int H, int W, cudaStream_t st, int out_bf16 = 0, int exact_fp32 = 0, int grid_limit = 0);
+                 int NI, int H, int W, cudaStream_t st, int out_bf16 = 0, int exact_fp32 = 0);
 
 // dst[n,y,x,:] += bilinear_x2_align_corners(src)[n,y,x,:]   (resnet_fpn.py:110,114)
 // pixel strides lds / ldd in elements; src / dst fp32 or bf16
@@ -25,27 +25,24 @@ int posenc_tokens(const float* feat, const float* pe, float* tok, long long ldt,
 //   K,V: [n][S][H*D] (row strides ldk, ldv), already elu+1'd K.  Q: [n][L][H*D].
 //   msg[n,l,h,:] = (Q . KV) / (Q . Ksum + eps),  KV = sum_s K^T (V/S) * S
 // scratch: kv_part [n][H][splits][(D+1)*D], kv [n][H][(D+1)*D]
-// bf16 != 0: Q / K / V / msg are bf16 (strides in elements), sums stay fp32
+// bf16 != 0: Q / K / V / msg are bf16 (strides in elements), sums stay fp32, and Q and K are the raw projections:
+// the kernels apply elu(x) + 1 themselves
 int linear_attention_long(const void* Q, long long ldq, const void* K, long long ldk, const void* V,
                           long long ldv, void* msg, long long ldm, float* kv_part, float* kv, int n,
                           int L, int S, int heads, int dim, int splits, cudaStream_t st, int bf16 = 0);
 
 // Linear attention for many short sequences (fine level): items of `T` tokens (T <= 32), C = 128,
 // 8 heads x 16. x-side item i attends to src-side item i. n_items read from device (*n_items_dev).
+// bf16 as for linear_attention_long.
 int linear_attention_windows(const void* Q, long long ldq, const void* K, long long ldk, const void* V,
                              long long ldv, void* msg, long long ldm, const int* n_items_dev,
                              int max_items, int T, cudaStream_t st, int bf16 = 0);
-// bf16 mode, fine level: q|k|v projection (w_qkv = [3 * 128][128] bf16: Wq, Wk, Wv rows) + window attention in one kernel.
-// xq / xs: bf16 token rows of the query / source side (equal pointers = self attention), 25 rows per window.
-int fine_attention_fused(const void* xq, long long ldq, const void* xs, long long lds, const void* w_qkv, void* msg,
-                         long long ldm, const int* n_items_dev, int max_items, int T, cudaStream_t st);
 
 // out[r,:] = (res ? res[r,:] : 0) + LayerNorm(in[r,:]) * gamma + beta, C in {128, 256}; rows may be
 // limited by *dyn_rows (device) when non-null.
 int layernorm_rows(const float* in, long long ldi, const float* gamma, const float* beta,
                    const float* res, long long ldr, float* out, long long ldo, long long rows, int C,
-                   const int* dyn_rows, cudaStream_t st, void* out16 = nullptr, long long ldo16 = 0);
-// out may be NULL when only the bf16 copy out16 (row stride ldo16 elements) is wanted.
+                   const int* dyn_rows, cudaStream_t st);
 // dst16[row][0..C) = bf16(src[row][0..C)); rows optionally capped by *dyn_rows
 int rows_to_bf16(const float* src, long long lds, void* dst, long long ldd, long long rows, int C, const int* dyn_rows,
                  cudaStream_t st);

@@ -46,7 +46,7 @@ SIGNATURES = {
                                      c_vp, c_ll, c_vp]),
     "mfr_conv2d_nhwc_bf16": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_ll, c_vp, c_ll, c_int, c_int, c_int,
                                      c_int, c_int, c_vp, c_vp, c_ll, c_int, c_float, c_vp, c_ll, c_int, c_vp]),
-    "mfr_loftr_create": (c_int, [c_int, c_int, c_int, c_float, c_int, c_float, c_int, c_pp]),
+    "mfr_loftr_create": (c_int, [c_int, c_int, c_int, c_float, c_int, c_float, c_int, c_int, c_pp]),
     "mfr_loftr_destroy": (None, [c_vp]),
     "mfr_loftr_num_weights": (c_int, [c_vp]),
     "mfr_loftr_weight_name": (ctypes.c_char_p, [c_vp, c_int]),
@@ -93,7 +93,6 @@ SIGNATURES = {
                                c_float, ctypes.c_ulonglong, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "mfr_linear_attention": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
     "mfr_stem_conv7x7": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
-    "mfr_fine_attention_fused": (c_int, [c_vp, c_ll, c_vp, c_ll, c_vp, c_vp, c_ll, c_int, c_vp]),
     "mfr_icp_refine": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_float, c_int, c_float, c_float,
                                c_vp, c_vp, c_vp, c_vp]),
     "mfr_jpeg_info": (c_int, [c_vp, c_ll, c_vp, c_vp, c_vp]),

@@ -6,7 +6,6 @@ All network arithmetic runs in libmfr_b200.so (hand-written sm_90a kernels); tor
 device memory and streams only. There is no CPU fallback.
 """
 import ctypes
-import os
 import math
 
 import numpy as np
@@ -293,18 +292,12 @@ class LoFTR:
         self.precision = {"tf32": 0, "bf16": 1, "fp32x3": 2, "fp32": 2}[precision]
         self.precision_name = {0: "tf32", 1: "bf16", 2: "fp32x3"}[self.precision]
         # pipelined: the engine will run under RelocPipeline, where the pose back end of the previous batch shares the GPU
-        # with the first layers of this batch's matcher: those launches then leave 8 SMs to it (loftr_engine.cu,
-        # MFR_RESERVE_SMS; measured +0.8 % pairs/s in the pipeline, -0.6 % for a matcher running alone)
-        prev = os.environ.get("MFR_RESERVE_SMS")
-        if pipelined and prev is None:
-            os.environ["MFR_RESERVE_SMS"] = "8"
-        try:
-            _lib.check(self._l.mfr_loftr_create(self.B, self.H, self.W, float(self.cfg["thr"]),
-                                                int(self.cfg["border_rm"]), float(self.cfg["temperature"]),
-                                                self.precision, ctypes.byref(h)), "mfr_loftr_create")
-        finally:
-            if pipelined and prev is None:
-                del os.environ["MFR_RESERVE_SMS"]
+        # with the first layers of this batch's matcher: those launches then leave 8 SMs to it (reserved_sms of
+        # mfr_loftr_create; measured +0.8 % pairs/s in the pipeline, -0.6 % for a matcher running alone)
+        reserved_sms = 8 if pipelined else 0
+        _lib.check(self._l.mfr_loftr_create(self.B, self.H, self.W, float(self.cfg["thr"]),
+                                            int(self.cfg["border_rm"]), float(self.cfg["temperature"]),
+                                            self.precision, reserved_sms, ctypes.byref(h)), "mfr_loftr_create")
         self._h = h
         self._l.mfr_loftr_set_graph(self._h, int(bool(graph)))
         self.load_state_dict(state_dict)

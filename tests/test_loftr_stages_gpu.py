@@ -5,10 +5,11 @@ the GPU with ``oracle/loftr_oracle.py``'s functions, so the error of one stage d
 stages before it and the bars can follow each precision's rounding model. All checks run for the three engine
 precisions, with two pairs per batch (B = 2) whose match sets differ, so that a mix-up of ``b_ids`` shows.
 
-One encoder layer at a time: a layer whose norm2 gain and bias are zero returns ``x + 0 = x`` exactly (the unfused
-LayerNorm, the fused encoder tail and the bf16 shadow rewrite all compute ``(x - mean) * rstd * 0 + 0``), so with
-norm2 zeroed in every layer but k the transformer's output is layer k applied to its input
-(``tests/test_loftr_stages_host.py`` checks that on the oracle).
+One encoder layer at a time: a layer whose norm2 gain and bias are zero returns ``x + 0 = x`` exactly (the LayerNorm
+kernel of tf32 / fp32x3 and bf16's fused encoder tail, which also rewrites the bf16 shadow, both compute
+``(x - mean) * rstd * 0 + 0``), so with norm2 zeroed in every layer but k the transformer's output is layer k applied
+to its input (``tests/test_loftr_stages_host.py`` checks that on the oracle). Every bf16 check runs the one bf16 path
+the engine has: raw q, k into the tensor-core attention kernels, then the fused tail.
 
 Bars. Single-kernel stages have bounds derived from the kernel's arithmetic (a K-term fp32 dot product is within
 ``(c_op + K * 2^-24) * sum |a| |b|`` of the exact one, with c_op the operand rounding of the precision). The encoder
@@ -211,56 +212,39 @@ def test_coarse_layer_bench_frame(precision, layer):
     torch.cuda.empty_cache()
 
 
-@pytest.mark.parametrize("env,layer", [("MFR_FUSED_TAIL", 0), ("MFR_FUSED_TAIL", 1), ("MFR_ELU_IN_ATTN", 0),
-                                       ("MFR_ELU_IN_ATTN", 1)])
-def test_coarse_layer_bf16_variants(monkeypatch, env, layer):
-    """bf16 with the unfused tail (merge GEMM, LayerNorm kernels writing the shadow) or with the feature map applied by
-    the q|k|v GEMM epilogue instead of the attention kernel. Bar 4 u = 1.56e-2; measured maxima: unfused tail 5.1e-3,
-    feature map in the epilogue 4.9e-3."""
+@pytest.mark.parametrize("layer", [0, 1])
+@pytest.mark.parametrize("precision", PRECISIONS)
+def test_coarse_layer_small_message(precision, layer):
+    """Layer 0 (self) or 1 (cross) with merge.weight scaled by 2^-10: the LayerNorm1 input of layer 1 then has a variance
+    of about 8e-6 per row (8.3 at scale 1 in the oracle), the size of LayerNorm's eps = 1e-5, so a LayerNorm path with
+    another eps or a mis-rounded variance fails here (layernorm_kernel in tf32 / fp32x3, the fused tail in bf16). Bars as
+    for the other coarse layers; measured maxima for layer 1: tf32 5.8e-4, bf16 4.8e-3, fp32x3 2.8e-6."""
     from mfr_b200 import loftr
-    monkeypatch.setenv(env, "0")          # read by the engine's constructor
     H, W = 160, 120
     sd = loftr.synthetic_state_dict(0)
-    eng = engine(sd, "bf16", H, W, {"thr": 0.0})
-    x_in, x_out, ref = _coarse_layer(eng, sd, layer, H, W)
-    err = branch_err(x_in, x_out, ref)
-    print(f"coarse bf16 {env}=0 layer {layer}: branch err {err:.3e}")
-    assert err < COARSE_BAR["bf16"], err
-    eng.close()
-
-
-@pytest.mark.parametrize("precision,fused_tail", [("tf32", "1"), ("bf16", "1"), ("bf16", "0"), ("fp32x3", "1")])
-def test_coarse_layer_small_message(monkeypatch, precision, fused_tail):
-    """Layer 1 with merge.weight scaled by 2^-10: the LayerNorm1 input then has a variance of about 8e-6 per row (8.3 at
-    scale 1 in the oracle), the size of LayerNorm's eps = 1e-5, so a LayerNorm path with another eps or a mis-rounded
-    variance fails here. bf16 with the fused tail and with MFR_FUSED_TAIL=0 (layernorm_kernel). Bars as for the other
-    coarse layers; measured maxima: tf32 5.8e-4, bf16 4.8e-3 (both tails), fp32x3 2.8e-6."""
-    from mfr_b200 import loftr
-    monkeypatch.setenv("MFR_FUSED_TAIL", fused_tail)
-    H, W = 160, 120
-    sd = loftr.synthetic_state_dict(0)
-    k = "loftr_coarse.layers.1.merge.weight"
+    k = f"loftr_coarse.layers.{layer}.merge.weight"
     sd[k] = sd[k] * 2.0 ** -10
     eng = engine(sd, precision, H, W, {"thr": 0.0})
-    x_in, x_out, ref = _coarse_layer(eng, sd, 1, H, W)
+    x_in, x_out, ref = _coarse_layer(eng, sd, layer, H, W)
     err = branch_err(x_in, x_out, ref)
-    print(f"coarse small message {precision} fused_tail={fused_tail}: branch err {err:.3e}")
+    print(f"coarse small message {precision} layer {layer}: branch err {err:.3e}")
     assert err < COARSE_BAR[precision], err
     eng.close()
 
 
 # ------------------------------------------------------------------------------------------------ bf16 shadows
-@pytest.mark.parametrize("fused_tail", ["1", "0"])
-def test_bf16_shadows_coherent(monkeypatch, fused_tail):
+FINE_CASES = [("shifted", 160, 120), ("identical", 96, 128)]
+
+
+@pytest.mark.parametrize("kind,H,W", FINE_CASES)
+def test_bf16_shadows_coherent(kind, H, W):
     """After a bf16 forward, the bf16 copies the token GEMMs read are the round-to-nearest-even bf16 of the fp32 tokens,
     bit for bit: the coarse tokens on all 2B * L rows, the fine tokens on the 25 * M live rows of both sides (last
-    written by the fused tail, or by layernorm_kernel with MFR_FUSED_TAIL=0)."""
+    written by the fused tail). "identical" fills M close to the capacity B * L."""
     from mfr_b200 import loftr
-    monkeypatch.setenv("MFR_FUSED_TAIL", fused_tail)
-    H, W = 160, 120
-    L = 300
+    L = (H // 8) * (W // 8)
     eng = engine(loftr.synthetic_state_dict(0), "bf16", H, W, {"thr": 0.0, "border_rm": 0})
-    out = eng.forward(*images("shifted", H, W))
+    out = eng.forward(*images(kind, H, W))
     M = out["M"]
     assert M > 0
     tok = eng.debug_tensor("tok", (4, L, 512))[:, :, :256]
@@ -341,9 +325,6 @@ def test_selection_on_engine_sim(precision, thr, border):
 
 
 # ------------------------------------------------------------------------------------------------ fine level
-FINE_CASES = [("shifted", 160, 120), ("identical", 96, 128)]
-
-
 def _edge_matches(out, w8):
     """Matches whose window reaches outside the 1/2-resolution map (cell row or column 0 on either side)."""
     i, j = out["i_ids"].long(), out["j_ids"].long()
@@ -390,17 +371,15 @@ def test_fine_gather_and_projections(precision, kind, H, W):
 
 
 @pytest.mark.parametrize("layer", [0, 1])
-@pytest.mark.parametrize("precision,fused", [("tf32", "0"), ("bf16", "0"), ("bf16", "1"), ("fp32x3", "0")])
-def test_fine_layer(monkeypatch, precision, fused, layer):
+@pytest.mark.parametrize("kind,H,W", FINE_CASES)
+@pytest.mark.parametrize("precision", PRECISIONS)
+def test_fine_layer(precision, kind, H, W, layer):
     """One fine encoder layer (0 = self, 1 = cross over the 5x5 windows) on the merge_feat output of the same engine
-    (both fine layers zeroed), residual branch against fp64; bf16 with the unfused window attention and with
-    MFR_FUSED_FINE_ATTN=1. Bars as for the coarse layers; measured maxima: tf32 6.4e-4, bf16 4.5e-3 (both attention
-    paths), fp32x3 2.8e-6."""
-    monkeypatch.setenv("MFR_FUSED_FINE_ATTN", fused)
-    H, W = 160, 120
+    (both fine layers zeroed), residual branch against fp64. "identical" fills M close to the capacity B * L. Bars as
+    for the coarse layers; measured maxima on "shifted": tf32 6.4e-4, bf16 4.5e-3, fp32x3 2.8e-6."""
     base = hybrid_state_dict()
     eng = engine(base, precision, H, W, {"thr": 0.2, "border_rm": 0})
-    ims = images("shifted", H, W)
+    ims = images(kind, H, W)
     eng.load_state_dict(isolate_layer(base, "loftr_fine", 2, None))
     M = eng.forward(*ims)["M"]
     a = live(eng, M)
@@ -418,7 +397,7 @@ def test_fine_layer(monkeypatch, precision, fused, layer):
     else:
         r = torch.stack([lo.encoder_layer(x[0], x[1], s64, p, 8), lo.encoder_layer(x[1], y[0].double(), s64, p, 8)])
     err = branch_err(x, y, r)
-    print(f"fine {precision} fused={fused} layer {layer}: M {M} branch err {err:.3e}")
+    print(f"fine {precision} {kind} layer {layer}: M {M} branch err {err:.3e}")
     assert err < FINE_BAR[precision], err
     eng.close()
 

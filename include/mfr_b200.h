@@ -133,8 +133,17 @@ typedef struct {
 } mfr_spsg_outputs;
 int mfr_spsg_create(int B, int H, int W, int max_keypoints, int nms_radius, float keypoint_threshold,
                     int remove_borders, int sinkhorn_iterations, float match_threshold, mfr_spsg** out);
-/* same with the GEMM precision: MFR_PRECISION_TF32 (what mfr_spsg_create uses) or MFR_PRECISION_FP32X3 (every conv /
- * linear / attention / score GEMM as a 3xTF32 split product: the fp32-faithful parity mode) */
+/* same with the GEMM precision: MFR_PRECISION_TF32 (what mfr_spsg_create uses), MFR_PRECISION_FP32X3 (every conv /
+ * linear / attention / score GEMM as a 3xTF32 split product: the fp32-faithful parity mode) or MFR_PRECISION_BF16
+ * (throughput mode). In bf16 mode:
+ *  - bf16 operands and outputs: conv1a's output, conv1b .. conv4b, convPa, convDa (ReLU in the epilogue), the 2x2
+ *    max-pools, the inputs of convPb / convDb (whose outputs stay fp32), and in every GNN layer q|k|v, the attention
+ *    message (mfr_superglue_attention: one fused launch, scores never stored), merge, mlp.0, and the input of mlp.3;
+ *  - the token stream is fp32 with a bf16 shadow [x | message] refreshed after the keypoint encoder and after every
+ *    layer's mlp.3 (which adds its output to the fp32 stream);
+ *  - fp32 / tf32 as in MFR_PRECISION_TF32: the detector head and NMS, keypoint selection, descriptor normalisation and
+ *    sampling, the keypoint encoder, final_proj, the score matrix, Sinkhorn and match extraction.
+ * The "attn_scores" and "attn_vt" debug tensors do not exist in bf16 mode; "qkv" and "msg" hold bf16 there. */
 int mfr_spsg_create_ex(int B, int H, int W, int max_keypoints, int nms_radius, float keypoint_threshold,
                        int remove_borders, int sinkhorn_iterations, float match_threshold, int precision,
                        mfr_spsg** out);
@@ -298,6 +307,15 @@ float mfr_debug_time_conv(const float* x, int N, int H, int W, int Cin, const fl
  * pre-mapped q, k) returns MFR_ERR_UNSUPPORTED. Device pointers, dense rows. */
 int mfr_linear_attention(const void* q, const void* k, const void* v, void* msg, int n, int L, int S, int windows,
                          int bf16, void* stream);
+
+/* Stage entry for tests: SuperGlue's multi-head softmax attention (SuperGlue/models/superglue.py:85-89), the fused
+ * kernel of the bf16 engine mode. qkv: device bf16 [n_img][max_kp][ldq], columns q | k | v (0-255, 256-511, 512-767;
+ * head h at 64 h), counts: device int[n_img]. Image i attends to the first counts[i ^ cross] keys / values of image
+ * i ^ cross (cross 0 or 1; images pair-interleaved). msg: device bf16 [n_img][max_kp][ldo], channel 64 h + d;
+ * rows >= counts[i], and every row when counts[i ^ cross] == 0, are written as zeros. max_kp: multiple of 16 in
+ * [16, 2048]; ldq >= 768 and a multiple of 8, ldo >= 256 and even; qkv 16-byte aligned. */
+int mfr_superglue_attention(const void* qkv, long long ldq, const int* counts, int n_img, int max_kp, int cross,
+                            void* msg, long long ldo, void* stream);
 
 /* Stage entry for tests: the backbone stem, conv 7x7 stride 2 pad 3, 1 -> 128 channels, folded-BN bias, ReLU
  * (LoFTR/src/loftr/backbone/resnet_fpn.py:52-62,102). img fp32 [NI][H][W]; w fp32 [128][49]; out [NI][H/2][W/2][128], bf16 when

@@ -9,6 +9,7 @@
 #include "loftr_engine.cuh"
 #include "loftr_ops.cuh"
 #include "spsg_engine.cuh"
+#include "sg_attention.cuh"
 #include "geometry_solvers.cuh"
 #include "geometry.cuh"
 #include "descriptor_match.cuh"
@@ -332,6 +333,14 @@ int mfr_linear_attention(const void* q, const void* k, const void* v, void* msg,
   cudaStreamSynchronize(st);
   cudaFree(kv_part); cudaFree(kv);
   return r;
+}
+
+int mfr_superglue_attention(const void* qkv, long long ldq, const int* counts, int n_img, int max_kp, int cross,
+                            void* msg, long long ldo, void* stream) {
+  mfr::SgAttentionParams p;
+  const int r = mfr::sg_attention_build(qkv, ldq, counts, n_img, max_kp, cross, msg, ldo, &p);
+  if (r != MFR_OK) return r;
+  return mfr::sg_attention_launch(p, static_cast<cudaStream_t>(stream));
 }
 
 int mfr_icp_refine(mfr_pose_solver* s, const float* depth0, const float* depth1, int H, int W, int P, const float* K0,

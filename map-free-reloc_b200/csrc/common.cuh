@@ -121,6 +121,17 @@ __device__ __forceinline__ void mbar_wait_inl(uint32_t bar, uint32_t parity, int
   while (!mbar_try_wait(bar, parity))
     if (clock64() - t0 > MFR_SPIN_TIMEOUT_CYCLES) __trap();
 }
+// mbar_wait_inl with the trap after the spin loop rather than inside it, for warp-specialised kernels: a trap inside the
+// loop makes ptxas allocate the whole kernel at the launch-bounds register count (168 at 384 threads), ignoring the
+// consumers' setmaxnreg.inc
+__device__ __forceinline__ void wait_bounded(uint32_t bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  bool ok;
+  while (!(ok = mbar_try_wait(bar, parity)) && clock64() - t0 <= MFR_SPIN_TIMEOUT_CYCLES) {
+  }
+  if (!ok) __trap();
+}
 
 // One lane of a converged warp (elect.sync): lets ptxas emit a single UTMALDG instead of the
 // per-active-thread loop it wraps around uniform-datapath instructions in divergent code.

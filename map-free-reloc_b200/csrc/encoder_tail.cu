@@ -124,17 +124,6 @@ __device__ __forceinline__ const float* opaque(const float* v) {
   return v;
 }
 
-// mbar_wait_inl with the trap after the spin loop rather than inside it: a trap inside the loop makes ptxas allocate the
-// whole kernel at the launch-bounds register count (168 at 384 threads), ignoring the consumers' setmaxnreg.inc
-__device__ __forceinline__ void wait_bounded(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  bool ok;
-  while (!(ok = mbar_try_wait(bar, parity)) && clock64() - t0 <= MFR_SPIN_TIMEOUT_CYCLES) {
-  }
-  if (!ok) __trap();
-}
-
 __device__ __forceinline__ void prefetch_l2(const void* ptr, uint32_t bytes) {
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(ptr), "r"(bytes) : "memory");
 }

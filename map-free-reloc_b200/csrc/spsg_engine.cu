@@ -13,7 +13,8 @@
 #include <vector>
 
 #include "conv_gemm.cuh"
-#include "loftr_ops.cuh"   // rows_split3 (3xTF32 operand split of the fp32-faithful mode)
+#include "loftr_ops.cuh"   // rows_split3 (3xTF32 operand split of the fp32-faithful mode), weights_to_bf16, rows_to_bf16
+#include "sg_attention.cuh"
 #include "spsg_ops.cuh"
 
 namespace mfr {
@@ -50,6 +51,10 @@ struct SpsgEngine {
   bool w3_ready = false;
   struct W3 { std::string name; long long rows; int cin; };
   std::vector<W3> w3_list;
+  // precision 1 (MFR_PRECISION_BF16): bf16 copy of the whole weight blob at the same offsets (every bf16 GEMM has a
+  // Cin that is a multiple of 8, so rows need no padding), converted once per upload
+  unsigned short* wblob16 = nullptr;
+  bool w16_ready = false;
 
   void add(const std::string& n, size_t numel) {
     idx[n] = specs.size();
@@ -73,10 +78,15 @@ struct SpsgEngine {
   void push(std::function<int(cudaStream_t)> f, int n_launch = 1) { steps.push_back(std::move(f)); launches += n_launch; }
 
   void gemm(const std::string& w, const float* x, int N, int Hh, int Ww, int Cin, long long ldx, int Cout, int R,
-            int act, const float* residual, float* out, long long ldo, long long ldr = 0) {
+            int act, const float* residual, float* out, long long ldo, long long ldr = 0, int in_bf16 = 0,
+            int out_bf16 = 0) {
     ConvGemmDesc d{};
     d.x = x; d.N = N; d.H = Hh; d.W = Ww; d.Cin = Cin; d.ldx = ldx;
     d.w = Wp(w + ".w");
+    if (in_bf16) {   // bf16 x and weights (ldw = Cin); out / residual bf16 when out_bf16
+      d.in_bf16 = 1; d.out_bf16 = out_bf16;
+      d.w = reinterpret_cast<const float*>(wblob16 + (d.w - wblob));
+    }
     if (precision == 2) {
       const long long rows_img = static_cast<long long>(Hh) * Ww;
       if (static_cast<size_t>(N) * rows_img * 3 * Cin > x3_cap || (Cin & 3)) { rc = MFR_ERR_ARG; return; }
@@ -112,6 +122,8 @@ struct SpsgEngine {
     cv("final_proj", 256, 256, 1);
     add("bin_score", 1);
     wblob = alloc<float>(wtotal, "weights");
+    const bool bf = precision == 1;
+    if (bf) wblob16 = alloc<unsigned short>(wtotal, "weights_bf16");
     if (precision == 2) {
       wblob3 = alloc<float>(3 * wtotal, "weights_split3");
       const size_t act = static_cast<size_t>(2) * B * H * W * 64;                         // largest conv input (conv1b)
@@ -124,14 +136,18 @@ struct SpsgEngine {
     const int Hs = h8 * 8, Ws = w8 * 8;
     auto px = [&](int hh, int ww) { return static_cast<size_t>(NI) * hh * ww; };
     img = alloc<float>(px(H, W), "img");
-    float* x1a = alloc<float>(px(H, W) * 64, "x1a"); float* x1b = alloc<float>(px(H, W) * 64);
-    float* p1 = alloc<float>(px(H2, W2) * 64); float* x2a = alloc<float>(px(H2, W2) * 64); float* x2b = alloc<float>(px(H2, W2) * 64);
-    float* p2 = alloc<float>(px(H4, W4) * 64); float* x3a = alloc<float>(px(H4, W4) * 128); float* x3b = alloc<float>(px(H4, W4) * 128);
-    float* p3 = alloc<float>(px(h8, w8) * 128); float* x4a = alloc<float>(px(h8, w8) * 128); float* x4b = alloc<float>(px(h8, w8) * 128, "x4b");
-    float* cPa = alloc<float>(px(h8, w8) * 256); float* logits = alloc<float>(px(h8, w8) * 65, "logits");
+    // SuperPoint activations up to the heads' inputs: bf16 storage in bf16 mode (float-typed pointers)
+    auto act = [&](size_t n, const char* name = nullptr) {
+      return bf ? reinterpret_cast<float*>(alloc<unsigned short>(n, name)) : alloc<float>(n, name);
+    };
+    float* x1a = act(px(H, W) * 64, "x1a"); float* x1b = act(px(H, W) * 64);
+    float* p1 = act(px(H2, W2) * 64); float* x2a = act(px(H2, W2) * 64); float* x2b = act(px(H2, W2) * 64);
+    float* p2 = act(px(H4, W4) * 64); float* x3a = act(px(H4, W4) * 128); float* x3b = act(px(H4, W4) * 128);
+    float* p3 = act(px(h8, w8) * 128); float* x4a = act(px(h8, w8) * 128); float* x4b = act(px(h8, w8) * 128, "x4b");
+    float* cPa = act(px(h8, w8) * 256); float* logits = alloc<float>(px(h8, w8) * 65, "logits");
     float* scores = alloc<float>(px(Hs, Ws), "scores"); float* mask = alloc<float>(px(Hs, Ws), "nms_mask");
     float* t0 = alloc<float>(px(Hs, Ws)); float* t1 = alloc<float>(px(Hs, Ws)); float* t2 = alloc<float>(px(Hs, Ws)); float* t3 = alloc<float>(px(Hs, Ws));
-    float* cDa = alloc<float>(px(h8, w8) * 256); float* dense = alloc<float>(px(h8, w8) * 256, "dense_desc");
+    float* cDa = act(px(h8, w8) * 256); float* dense = alloc<float>(px(h8, w8) * 256, "dense_desc");
     kpts = alloc<float>(static_cast<size_t>(NI) * K * 2, "keypoints"); kscores = alloc<float>(static_cast<size_t>(NI) * K, "kscores");
     counts = alloc<int>(NI);
     X = alloc<float>(static_cast<size_t>(NI) * K * 512, "tokens");
@@ -139,11 +155,20 @@ struct SpsgEngine {
     const size_t rows = static_cast<size_t>(NI) * K;
     float* kin = alloc<float>(rows * 4); float* k1 = alloc<float>(rows * 32); float* k2 = alloc<float>(rows * 64);
     float* k3 = alloc<float>(rows * 128); float* k4 = alloc<float>(rows * 256);
-    float* qkv = alloc<float>(rows * 768, "qkv"); float* msg = alloc<float>(rows * 256, "msg"); float* h1 = alloc<float>(rows * 512);
+    float *qkv = nullptr, *msg = nullptr, *h1 = nullptr, *Xb = nullptr, *Sat = nullptr, *Vt = nullptr;
+    if (!bf) {
+      qkv = alloc<float>(rows * 768, "qkv"); msg = alloc<float>(rows * 256, "msg"); h1 = alloc<float>(rows * 512);
+    } else {   // bf16 storage: q|k|v, the attention message, the hidden layer, and the token shadow [x | message]
+      qkv = reinterpret_cast<float*>(alloc<unsigned short>(rows * 768, "qkv"));
+      msg = reinterpret_cast<float*>(alloc<unsigned short>(rows * 256, "msg"));
+      h1 = reinterpret_cast<float*>(alloc<unsigned short>(rows * 512));
+      Xb = reinterpret_cast<float*>(alloc<unsigned short>(rows * 512, "tokens_bf16"));
+    }
     float* Mb = alloc<float>(rows * 256, "mdesc");
-    // tensor-core attention: scores / probabilities [NI][4 heads][K][K] and V transposed [NI][256][K]
-    float* Sat = alloc<float>(static_cast<size_t>(NI) * 4 * K * K, "attn_scores");
-    float* Vt = alloc<float>(static_cast<size_t>(NI) * 256 * K, "attn_vt");
+    if (!bf) {   // tensor-core attention: scores / probabilities [NI][4 heads][K][K] and V transposed [NI][256][K]
+      Sat = alloc<float>(static_cast<size_t>(NI) * 4 * K * K, "attn_scores");
+      Vt = alloc<float>(static_cast<size_t>(NI) * 256 * K, "attn_vt");
+    }
     float* S = alloc<float>(static_cast<size_t>(B) * K * K, "sg_scores");
     float* u = alloc<float>(static_cast<size_t>(B) * (K + 1), "sk_u"); float* v = alloc<float>(static_cast<size_t>(B) * (K + 1), "sk_v");
     float* rmax = alloc<float>(static_cast<size_t>(B) * K); int* rarg = alloc<int>(static_cast<size_t>(B) * K); int* carg = alloc<int>(static_cast<size_t>(B) * K);
@@ -155,24 +180,27 @@ struct SpsgEngine {
     // ---- SuperPoint (superpoint.py:145-196)
     {
       float *w = Wp("conv1a.w"), *b = Wp("conv1a.b"), *im = img; const int n = NI, hh = H, ww = W;
-      push([=](cudaStream_t st) { return sp_conv1a(im, w, b, x1a, n, hh, ww, st); });
+      if (bf) push([=](cudaStream_t st) { return sp_conv1a_bf16(im, w, b, x1a, n, hh, ww, st); });
+      else push([=](cudaStream_t st) { return sp_conv1a(im, w, b, x1a, n, hh, ww, st); });
     }
     auto pool = [&](float* in, float* out, int hh, int ww, int c) {
       const int n = NI;
-      push([=](cudaStream_t st) { return maxpool2x2(in, out, n, hh, ww, c, st); });
+      if (bf) push([=](cudaStream_t st) { return maxpool2x2_bf16(in, out, n, hh, ww, c, st); });
+      else push([=](cudaStream_t st) { return maxpool2x2(in, out, n, hh, ww, c, st); });
     };
-    gemm("conv1b", x1a, NI, H, W, 64, 64, 64, 3, ACT_RELU, nullptr, x1b, 64);
+    const int b16 = bf ? 1 : 0;   // bf16 operands (and outputs, up to the heads' inputs) in bf16 mode
+    gemm("conv1b", x1a, NI, H, W, 64, 64, 64, 3, ACT_RELU, nullptr, x1b, 64, 0, b16, b16);
     pool(x1b, p1, H, W, 64);
-    gemm("conv2a", p1, NI, H2, W2, 64, 64, 64, 3, ACT_RELU, nullptr, x2a, 64);
-    gemm("conv2b", x2a, NI, H2, W2, 64, 64, 64, 3, ACT_RELU, nullptr, x2b, 64);
+    gemm("conv2a", p1, NI, H2, W2, 64, 64, 64, 3, ACT_RELU, nullptr, x2a, 64, 0, b16, b16);
+    gemm("conv2b", x2a, NI, H2, W2, 64, 64, 64, 3, ACT_RELU, nullptr, x2b, 64, 0, b16, b16);
     pool(x2b, p2, H2, W2, 64);
-    gemm("conv3a", p2, NI, H4, W4, 64, 64, 128, 3, ACT_RELU, nullptr, x3a, 128);
-    gemm("conv3b", x3a, NI, H4, W4, 128, 128, 128, 3, ACT_RELU, nullptr, x3b, 128);
+    gemm("conv3a", p2, NI, H4, W4, 64, 64, 128, 3, ACT_RELU, nullptr, x3a, 128, 0, b16, b16);
+    gemm("conv3b", x3a, NI, H4, W4, 128, 128, 128, 3, ACT_RELU, nullptr, x3b, 128, 0, b16, b16);
     pool(x3b, p3, H4, W4, 128);
-    gemm("conv4a", p3, NI, h8, w8, 128, 128, 128, 3, ACT_RELU, nullptr, x4a, 128);
-    gemm("conv4b", x4a, NI, h8, w8, 128, 128, 128, 3, ACT_RELU, nullptr, x4b, 128);
-    gemm("convPa", x4b, NI, h8, w8, 128, 128, 256, 3, ACT_RELU, nullptr, cPa, 256);
-    gemm("convPb", cPa, NI, h8, w8, 256, 256, 65, 1, ACT_NONE, nullptr, logits, 65);
+    gemm("conv4a", p3, NI, h8, w8, 128, 128, 128, 3, ACT_RELU, nullptr, x4a, 128, 0, b16, b16);
+    gemm("conv4b", x4a, NI, h8, w8, 128, 128, 128, 3, ACT_RELU, nullptr, x4b, 128, 0, b16, b16);
+    gemm("convPa", x4b, NI, h8, w8, 128, 128, 256, 3, ACT_RELU, nullptr, cPa, 256, 0, b16, b16);
+    gemm("convPb", cPa, NI, h8, w8, 256, 256, 65, 1, ACT_NONE, nullptr, logits, 65, 0, b16, 0);
     {
       const int n = NI, hh = h8, ww = w8, r = nms_r, bd = border, kk = K; const float th = kp_thr;
       float* kp = kpts; float* ks = kscores; int* cn = counts;
@@ -180,8 +208,8 @@ struct SpsgEngine {
       push([=](cudaStream_t st) { return sp_nms(scores, mask, t0, t1, t2, t3, n, hh * 8, ww * 8, r, st); }, 15);
       push([=](cudaStream_t st) { return sp_select_keypoints(scores, mask, n, hh * 8, ww * 8, th, bd, kk, kp, ks, cn, st); });
     }
-    gemm("convDa", x4b, NI, h8, w8, 128, 128, 256, 3, ACT_RELU, nullptr, cDa, 256);
-    gemm("convDb", cDa, NI, h8, w8, 256, 256, 256, 1, ACT_NONE, nullptr, dense, 256);
+    gemm("convDa", x4b, NI, h8, w8, 128, 128, 256, 3, ACT_RELU, nullptr, cDa, 256, 0, b16, b16);
+    gemm("convDb", cDa, NI, h8, w8, 256, 256, 256, 1, ACT_NONE, nullptr, dense, 256, 0, b16, 0);
     {
       const int n = NI, hh = h8, ww = w8, kk = K; float* kp = kpts; int* cn = counts; float* Dp = D;
       const size_t rws = px(h8, w8);
@@ -199,7 +227,8 @@ struct SpsgEngine {
     gemm("kenc.2", k2, NI, 1, K, 64, 64, 128, 1, ACT_RELU, nullptr, k3, 128);
     gemm("kenc.3", k3, NI, 1, K, 128, 128, 256, 1, ACT_RELU, nullptr, k4, 256);
     gemm("kenc.4", k4, NI, 1, K, 256, 256, 256, 1, ACT_NONE, D, X, 512, 256);   // X[:, :256] = desc + kenc
-    for (int i = 0; i < 18; ++i) {
+    if (bf) build_gnn_bf16(qkv, msg, h1, Xb);
+    else for (int i = 0; i < 18; ++i) {   // tf32 / fp32x3 GNN layers
       const std::string p = "gnn." + std::to_string(i);
       gemm(p + ".qkv", X, NI, 1, K, 256, 512, 768, 1, ACT_NONE, nullptr, qkv, 768);
       {
@@ -282,6 +311,29 @@ struct SpsgEngine {
     return rc;
   }
 
+  // the 18 GNN layers in bf16 mode. The fp32 token stream X [NI][K][512] keeps x in its first 256 columns; its bf16
+  // shadow Xb [NI][K][512] = [x | message] is the operand of qkv and mlp.0. Per layer: qkv (bf16), the fused attention
+  // (sg_attention.cu) into msg, merge into the message half of Xb, mlp.0 (ReLU) into h1, mlp.3 added to X in fp32, and
+  // the x half of Xb refreshed from X (not after the last layer: final_proj reads X).
+  void build_gnn_bf16(float* qkv, float* msg, float* h1, float* Xb) {
+    const long long rows = static_cast<long long>(NI) * K;
+    float* x = X;
+    push([=](cudaStream_t st) { return rows_to_bf16(x, 512, Xb, 512, rows, 256, nullptr, st); });
+    float* xb_msg = reinterpret_cast<float*>(reinterpret_cast<unsigned short*>(Xb) + 256);
+    for (int i = 0; i < 18; ++i) {
+      const std::string p = "gnn." + std::to_string(i);
+      gemm(p + ".qkv", Xb, NI, 1, K, 256, 512, 768, 1, ACT_NONE, nullptr, qkv, 768, 0, 1, 1);
+      SgAttentionParams ap;
+      int r = sg_attention_build(qkv, 768, counts, NI, K, i % 2, msg, 256, &ap);
+      if (r != MFR_OK) { rc = r; return; }
+      push([ap](cudaStream_t st) { return sg_attention_launch(ap, st); });
+      gemm(p + ".merge", msg, NI, 1, K, 256, 256, 256, 1, ACT_NONE, nullptr, xb_msg, 512, 0, 1, 1);
+      gemm(p + ".mlp0", Xb, NI, 1, K, 512, 512, 512, 1, ACT_RELU, nullptr, h1, 512, 0, 1, 1);
+      gemm(p + ".mlp3", h1, NI, 1, K, 512, 512, 256, 1, ACT_NONE, X, X, 512, 0, 1, 0);   // x + delta (fp32, in place)
+      if (i < 17) push([=](cudaStream_t st) { return rows_to_bf16(x, 512, Xb, 512, rows, 256, nullptr, st); });
+    }
+  }
+
   int run(cudaStream_t st) {
     int r = prepare_weights(st);
     if (r != MFR_OK) return r;
@@ -289,6 +341,11 @@ struct SpsgEngine {
     return MFR_OK;
   }
   int prepare_weights(cudaStream_t st) {
+    if (precision == 1 && !w16_ready) {   // the blob is a whole number of 64-element rows
+      int r = weights_to_bf16(wblob, wblob16, wtotal / 64, 64, 64, st);
+      if (r != MFR_OK) return r;
+      w16_ready = true;
+    }
     if (precision != 2 || w3_ready) return MFR_OK;
     for (const auto& e : w3_list) {
       const size_t off = specs[idx[e.name + ".w"]].offset;
@@ -355,7 +412,8 @@ struct SpsgEngine {
 int spsg_create(int B, int H, int W, int max_kp, int nms_radius, float kp_thr, int border, int sinkhorn_iters,
                 float match_thr, int precision, SpsgEngine** out) {
   if (B < 1 || H < 64 || W < 64 || max_kp < 16 || max_kp > 2048 || (max_kp % 16)) return MFR_ERR_ARG;
-  if (precision != 0 && precision != 2) return MFR_ERR_ARG;   // 0 = TF32 GEMM inputs, 2 = 3xTF32 split (fp32-faithful)
+  // 0 = TF32 GEMM inputs, 1 = bf16 operands and fused attention (see mfr_b200.h), 2 = 3xTF32 split (fp32-faithful)
+  if (precision < 0 || precision > 2) return MFR_ERR_ARG;
   auto* e = new SpsgEngine();
   e->precision = precision;
   e->B = B; e->H = H; e->W = W; e->K = max_kp; e->nms_r = nms_radius; e->kp_thr = kp_thr; e->border = border;
@@ -374,6 +432,7 @@ int spsg_set_weight(SpsgEngine* e, int i, const float* host, long long numel, cu
   MFR_CUDA_CHECK(cudaMemcpyAsync(e->wblob + e->specs[i].offset, host, numel * 4, cudaMemcpyHostToDevice, st));
   MFR_CUDA_CHECK(cudaStreamSynchronize(st));
   e->w3_ready = false;
+  e->w16_ready = false;
   if (e->specs[i].name == "bin_score") e->bin_score = host[0];
   if (i == static_cast<int>(e->specs.size()) - 1) e->loaded = true;
   return MFR_OK;

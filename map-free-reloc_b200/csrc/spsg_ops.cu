@@ -2,7 +2,10 @@
 // Reference: etc/feature_matching_baselines/SuperGlue/models/{superpoint,superglue}.py.
 #include "spsg_ops.cuh"
 
+#include <cuda_bf16.h>
+
 #include <algorithm>
+#include <type_traits>
 
 namespace mfr {
 
@@ -20,9 +23,10 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 
 // ------------------------------------------------------------------------------------------ conv1a
-// 3x3, pad 1, 1 -> 64 channels, bias, ReLU (superpoint.py:119,148). thread = output channel.
+// 3x3, pad 1, 1 -> 64 channels, bias, ReLU (superpoint.py:119,148). thread = output channel. OutT: float or bf16
+template <typename OutT>
 __global__ void __launch_bounds__(64) conv1a_kernel(const float* __restrict__ img, const float* __restrict__ w,
-                                                    const float* __restrict__ bias, float* __restrict__ out,
+                                                    const float* __restrict__ bias, OutT* __restrict__ out,
                                                     int H, int W) {
   __shared__ float patch[3][66];
   const int n = blockIdx.z, y = blockIdx.y, x0 = blockIdx.x * 64;
@@ -44,7 +48,9 @@ __global__ void __launch_bounds__(64) conv1a_kernel(const float* __restrict__ im
     for (int ky = 0; ky < 3; ++ky)
 #pragma unroll
       for (int kx = 0; kx < 3; ++kx) a = fmaf(wr[ky * 3 + kx], patch[ky][px + kx], a);
-    out[((static_cast<size_t>(n) * H + y) * W + x0 + px) * 64 + c] = fmaxf(a, 0.f);
+    const float r = fmaxf(a, 0.f);
+    if constexpr (std::is_same<OutT, float>::value) out[((static_cast<size_t>(n) * H + y) * W + x0 + px) * 64 + c] = r;
+    else out[((static_cast<size_t>(n) * H + y) * W + x0 + px) * 64 + c] = __float2bfloat16_rn(r);
   }
 }
 
@@ -68,6 +74,31 @@ __global__ void maxpool2_kernel(const float* __restrict__ in, float* __restrict_
   o.z = fmaxf(fmaxf(a.z, b.z), fmaxf(c.z, d.z));
   o.w = fmaxf(fmaxf(a.w, b.w), fmaxf(c.w, d.w));
   reinterpret_cast<float4*>(out)[idx] = o;
+}
+
+// bf16 [N][H][W][8 C8] -> [N][H/2][W/2][8 C8], 8 channels per thread (the max of bf16 values is exact)
+__global__ void maxpool2_bf16_kernel(const uint4* __restrict__ in, uint4* __restrict__ out, int N, int H, int W, int C8) {
+  const int Ho = H / 2, Wo = W / 2;
+  const size_t total = static_cast<size_t>(N) * Ho * Wo * C8;
+  const size_t idx = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int c8 = static_cast<int>(idx % C8);
+  size_t p = idx / C8;
+  const int x = static_cast<int>(p % Wo); p /= Wo;
+  const int y = static_cast<int>(p % Ho);
+  const int n = static_cast<int>(p / Ho);
+  const uint4* s = in + (static_cast<size_t>(n) * H + 2 * y) * W * C8;
+  uint4 v[4] = {s[(2 * x) * C8 + c8], s[(2 * x + 1) * C8 + c8], s[(static_cast<size_t>(W) + 2 * x) * C8 + c8],
+                s[(static_cast<size_t>(W) + 2 * x + 1) * C8 + c8]};
+  const __nv_bfloat162* a = reinterpret_cast<const __nv_bfloat162*>(&v[0]);
+  const __nv_bfloat162* b = reinterpret_cast<const __nv_bfloat162*>(&v[1]);
+  const __nv_bfloat162* c = reinterpret_cast<const __nv_bfloat162*>(&v[2]);
+  const __nv_bfloat162* d = reinterpret_cast<const __nv_bfloat162*>(&v[3]);
+  uint4 o;
+  __nv_bfloat162* r = reinterpret_cast<__nv_bfloat162*>(&o);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) r[i] = __hmax2(__hmax2(a[i], b[i]), __hmax2(c[i], d[i]));
+  out[idx] = o;
 }
 
 // ------------------------------------------------------------------------------------------ detector head
@@ -301,123 +332,6 @@ __global__ void kenc_input_kernel(const float* __restrict__ kpts, const float* _
   o.z = kscores[i];
   o.w = 0.f;
   reinterpret_cast<float4*>(out)[i] = o;
-}
-
-// ------------------------------------------------------------------------------------------ softmax attention
-// 4 heads x 64 (superglue.py:85-89): out[q, h, :] = softmax_k(q.k / 8) v. 32 queries per block: 8 lanes per PAIR
-// of queries (q, q + 16) — every key / value row read from shared memory feeds two queries, which halves the
-// shared-memory traffic the kernel is bound by. Key/value tiles of 64 rows in shared memory, online softmax.
-constexpr int kAtQ = 32, kAtK = 64;
-__global__ void __launch_bounds__(128) sg_attention_kernel(const float* __restrict__ qkv, long long ld,
-                                                           const int* __restrict__ counts, int src_xor,
-                                                           int max_kp, float* __restrict__ out, long long ldo) {
-  // row stride 68 floats: 16-byte aligned rows, and the 8 key rows a quarter-warp reads at once (kk = sub + 8j) start
-  // 4 banks apart, so a 128-bit read of all of them is conflict-free
-  __shared__ __align__(16) float sK[kAtK][68];
-  __shared__ __align__(16) float sV[kAtK][68];
-  __shared__ float sP[kAtQ][kAtK + 1];
-  const int img = blockIdx.z, head = blockIdx.y;
-  const int src = img ^ src_xor;
-  const int nq = counts[img], nk = counts[src];
-  const int q0 = blockIdx.x * kAtQ;
-  if (q0 >= nq) return;
-  const int t = threadIdx.x, qi = t >> 3, sub = t & 7;
-  const int qa = q0 + qi, qb = q0 + qi + 16;
-  float qr[2][64];
-#pragma unroll
-  for (int u = 0; u < 2; ++u) {
-    const int q = u == 0 ? qa : qb;
-    const float* qp = qkv + (static_cast<size_t>(img) * max_kp + (q < nq ? q : q0)) * ld + head * 64;
-#pragma unroll
-    for (int d4 = 0; d4 < 16; ++d4) {
-      const float4 f = *reinterpret_cast<const float4*>(qp + 4 * d4);
-      qr[u][4 * d4] = f.x * 0.125f; qr[u][4 * d4 + 1] = f.y * 0.125f; qr[u][4 * d4 + 2] = f.z * 0.125f; qr[u][4 * d4 + 3] = f.w * 0.125f;
-    }
-  }
-  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-  float o[2][8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) { o[0][j] = 0.f; o[1][j] = 0.f; }
-  const float* kbase = qkv + static_cast<size_t>(src) * max_kp * ld + 256 + head * 64;
-  const float* vbase = qkv + static_cast<size_t>(src) * max_kp * ld + 512 + head * 64;
-  for (int k0 = 0; k0 < nk; k0 += kAtK) {
-    __syncthreads();
-    for (int idx = t; idx < kAtK * 16; idx += 128) {
-      const int r = idx >> 4, c4 = idx & 15;
-      float4 kk = make_float4(0.f, 0.f, 0.f, 0.f), vv = kk;
-      if (k0 + r < nk) {
-        kk = *reinterpret_cast<const float4*>(kbase + static_cast<size_t>(k0 + r) * ld + 4 * c4);
-        vv = *reinterpret_cast<const float4*>(vbase + static_cast<size_t>(k0 + r) * ld + 4 * c4);
-      }
-      *reinterpret_cast<float4*>(&sK[r][4 * c4]) = kk;
-      *reinterpret_cast<float4*>(&sV[r][4 * c4]) = vv;
-    }
-    __syncthreads();
-    float s[2][8];
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int kk = sub + 8 * j;
-      float a0 = 0.f, a1 = 0.f;
-      const float4* kr = reinterpret_cast<const float4*>(&sK[kk][0]);
-#pragma unroll
-      for (int d4 = 0; d4 < 16; ++d4) {            // same accumulation order as a scalar loop over d
-        const float4 kv = kr[d4];
-        a0 = fmaf(qr[0][4 * d4], kv.x, a0); a0 = fmaf(qr[0][4 * d4 + 1], kv.y, a0);
-        a0 = fmaf(qr[0][4 * d4 + 2], kv.z, a0); a0 = fmaf(qr[0][4 * d4 + 3], kv.w, a0);
-        a1 = fmaf(qr[1][4 * d4], kv.x, a1); a1 = fmaf(qr[1][4 * d4 + 1], kv.y, a1);
-        a1 = fmaf(qr[1][4 * d4 + 2], kv.z, a1); a1 = fmaf(qr[1][4 * d4 + 3], kv.w, a1);
-      }
-      const bool ok = k0 + kk < nk;
-      s[0][j] = ok ? a0 : -INFINITY; s[1][j] = ok ? a1 : -INFINITY;
-      mx[0] = fmaxf(mx[0], s[0][j]); mx[1] = fmaxf(mx[1], s[1][j]);
-    }
-    float corr[2];
-#pragma unroll
-    for (int u = 0; u < 2; ++u) {
-      float m = mx[u];
-      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
-      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
-      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
-      const float m_new = fmaxf(m_run[u], m);
-      corr[u] = __expf(m_run[u] - m_new);
-      float ps = 0.f;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float pv = __expf(s[u][j] - m_new);
-        sP[qi + 16 * u][sub + 8 * j] = pv;
-        ps += pv;
-      }
-      ps += __shfl_xor_sync(0xffffffffu, ps, 1);
-      ps += __shfl_xor_sync(0xffffffffu, ps, 2);
-      ps += __shfl_xor_sync(0xffffffffu, ps, 4);
-      l_run[u] = l_run[u] * corr[u] + ps;
-      m_run[u] = m_new;
-    }
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { o[0][j] *= corr[0]; o[1][j] *= corr[1]; }
-    for (int kk = 0; kk < kAtK; ++kk) {
-      const float p0 = sP[qi][kk], p1 = sP[qi + 16][kk];
-      const float4 v0 = *reinterpret_cast<const float4*>(&sV[kk][sub * 8]);
-      const float4 v1 = *reinterpret_cast<const float4*>(&sV[kk][sub * 8 + 4]);
-      o[0][0] = fmaf(p0, v0.x, o[0][0]); o[0][1] = fmaf(p0, v0.y, o[0][1]); o[0][2] = fmaf(p0, v0.z, o[0][2]); o[0][3] = fmaf(p0, v0.w, o[0][3]);
-      o[0][4] = fmaf(p0, v1.x, o[0][4]); o[0][5] = fmaf(p0, v1.y, o[0][5]); o[0][6] = fmaf(p0, v1.z, o[0][6]); o[0][7] = fmaf(p0, v1.w, o[0][7]);
-      o[1][0] = fmaf(p1, v0.x, o[1][0]); o[1][1] = fmaf(p1, v0.y, o[1][1]); o[1][2] = fmaf(p1, v0.z, o[1][2]); o[1][3] = fmaf(p1, v0.w, o[1][3]);
-      o[1][4] = fmaf(p1, v1.x, o[1][4]); o[1][5] = fmaf(p1, v1.y, o[1][5]); o[1][6] = fmaf(p1, v1.z, o[1][6]); o[1][7] = fmaf(p1, v1.w, o[1][7]);
-    }
-    __syncwarp();
-  }
-#pragma unroll
-  for (int u = 0; u < 2; ++u) {
-    const int q = u == 0 ? qa : qb;
-    if (q < nq) {
-      const float inv = l_run[u] > 0.f ? 1.f / l_run[u] : 0.f;
-      float* op = out + (static_cast<size_t>(img) * max_kp + q) * ldo + head * 64 + sub * 8;
-      *reinterpret_cast<float4*>(op) = make_float4(o[u][0] * inv, o[u][1] * inv, o[u][2] * inv, o[u][3] * inv);
-      *reinterpret_cast<float4*>(op + 4) = make_float4(o[u][4] * inv, o[u][5] * inv, o[u][6] * inv, o[u][7] * inv);
-    }
-  }
 }
 
 // ------------------------------------------------------------------------------------------ softmax attention on the tensor cores
@@ -711,7 +625,12 @@ __global__ void __launch_bounds__(1024) sg_matches_kernel(const int* __restrict_
 #define GRID1(n, b) static_cast<unsigned>(((n) + (b) - 1) / (b))
 
 int sp_conv1a(const float* img, const float* w, const float* bias, float* out, int N, int H, int W, cudaStream_t st) {
-  conv1a_kernel<<<dim3((W + 63) / 64, H, N), 64, 0, st>>>(img, w, bias, out, H, W);
+  conv1a_kernel<float><<<dim3((W + 63) / 64, H, N), 64, 0, st>>>(img, w, bias, out, H, W);
+  MFR_CUDA_CHECK(cudaGetLastError());
+  return MFR_OK;
+}
+int sp_conv1a_bf16(const float* img, const float* w, const float* bias, void* out, int N, int H, int W, cudaStream_t st) {
+  conv1a_kernel<__nv_bfloat16><<<dim3((W + 63) / 64, H, N), 64, 0, st>>>(img, w, bias, static_cast<__nv_bfloat16*>(out), H, W);
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
 }
@@ -719,6 +638,13 @@ int maxpool2x2(const float* in, float* out, int N, int H, int W, int C, cudaStre
   if (C % 4) return MFR_ERR_ARG;
   const size_t total = static_cast<size_t>(N) * (H / 2) * (W / 2) * (C / 4);
   maxpool2_kernel<<<GRID1(total, 256), 256, 0, st>>>(in, out, N, H, W, C / 4);
+  MFR_CUDA_CHECK(cudaGetLastError());
+  return MFR_OK;
+}
+int maxpool2x2_bf16(const void* in, void* out, int N, int H, int W, int C, cudaStream_t st) {
+  if (C % 8) return MFR_ERR_ARG;
+  const size_t total = static_cast<size_t>(N) * (H / 2) * (W / 2) * (C / 8);
+  maxpool2_bf16_kernel<<<GRID1(total, 256), 256, 0, st>>>(static_cast<const uint4*>(in), static_cast<uint4*>(out), N, H, W, C / 8);
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
 }
@@ -769,12 +695,6 @@ int sp_sample_descriptors(const float* dense, const float* kpts, const int* coun
 int sg_kenc_input(const float* kpts, const float* kscores, float* out, int total, int H, int W, cudaStream_t st) {
   const float sc = 1.f / (0.7f * static_cast<float>(std::max(H, W)));
   kenc_input_kernel<<<GRID1(total, 256), 256, 0, st>>>(kpts, kscores, out, total, W * 0.5f, H * 0.5f, sc);
-  MFR_CUDA_CHECK(cudaGetLastError());
-  return MFR_OK;
-}
-int sg_attention(const float* qkv, long long ld, const int* counts, int cross, int max_kp, int n_img, float* out,
-                 long long ldo, cudaStream_t st) {
-  sg_attention_kernel<<<dim3((max_kp + kAtQ - 1) / kAtQ, 4, n_img), 128, 0, st>>>(qkv, ld, counts, cross ? 1 : 0, max_kp, out, ldo);
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
 }

@@ -1,4 +1,4 @@
-// SIMT kernels of the SuperPoint + SuperGlue matcher (launch wrappers). fp32, channel-last.
+// SIMT kernels of the SuperPoint + SuperGlue matcher (launch wrappers). fp32 unless named bf16, channel-last.
 #pragma once
 #include "common.cuh"
 
@@ -7,6 +7,9 @@ namespace mfr {
 int sp_conv1a(const float* img, const float* w /*[64][9]*/, const float* bias, float* out, int N, int H, int W,
               cudaStream_t st);
 int maxpool2x2(const float* in, float* out, int N, int H, int W, int C, cudaStream_t st);
+// bf16 variants of the engine's bf16 mode: conv1a with a bf16 output, 2x2 max-pool over bf16 (C % 8 == 0)
+int sp_conv1a_bf16(const float* img, const float* w, const float* bias, void* out, int N, int H, int W, cudaStream_t st);
+int maxpool2x2_bf16(const void* in, void* out, int N, int H, int W, int C, cudaStream_t st);
 // softmax over 65 logits (row stride ldc), drop dustbin, depth-to-space -> scores [N][8h][8w]
 int sp_score_map(const float* logits, int ldc, float* scores, int N, int h, int w, cudaStream_t st);
 // simple_nms (superpoint.py:47-62): mask (0/1 floats); t0..t3 scratch of the same size
@@ -20,9 +23,6 @@ int sp_sample_descriptors(const float* dense, const float* kpts, const int* coun
                           float* out, long long ldo, cudaStream_t st);
 // SuperGlue
 int sg_kenc_input(const float* kpts, const float* kscores, float* out, int total, int H, int W, cudaStream_t st);
-// images are stored pair-interleaved (2p, 2p+1); cross != 0: image i attends to image i^1
-int sg_attention(const float* qkv, long long ld, const int* counts, int cross, int max_kp, int n_img, float* out,
-                 long long ldo, cudaStream_t st);
 // tensor-core attention helpers (see spsg_ops.cu): in-place row softmax of the [img][4][K][K] scores, V transpose
 int sg_softmax_rows(float* S, const int* counts, int cross, int max_kp, int n_img, cudaStream_t st);
 int sg_transpose_v(const float* qkv, long long ld, float* vt, int max_kp, int n_img, cudaStream_t st);

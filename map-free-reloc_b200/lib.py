@@ -92,6 +92,7 @@ SIGNATURES = {
     "mfr_pnp_ransac": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_int,
                                c_float, ctypes.c_ulonglong, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "mfr_linear_attention": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
+    "mfr_superglue_attention": (c_int, [c_vp, c_ll, c_vp, c_int, c_int, c_int, c_vp, c_ll, c_vp]),
     "mfr_stem_conv7x7": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
     "mfr_icp_refine": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_float, c_int, c_float, c_float,
                                c_vp, c_vp, c_vp, c_vp]),

@@ -142,7 +142,7 @@ class SuperPointSuperGlue:
         self.stream = torch.cuda.Stream(device=self.device)
         h = ctypes.c_void_p()
         c = self.cfg
-        self.precision = {"tf32": 0, "fp32x3": 2, "fp32": 2}[precision]
+        self.precision = {"tf32": 0, "bf16": 1, "fp32x3": 2, "fp32": 2}[precision]
         _lib.check(self._l.mfr_spsg_create_ex(self.B, self.H, self.W, self.K, int(c["nms_radius"]),
                                               float(c["keypoint_threshold"]), int(c["remove_borders"]),
                                               int(c["sinkhorn_iterations"]), float(c["match_threshold"]),
@@ -169,15 +169,24 @@ class SuperPointSuperGlue:
         class _A:
             pass
         a = _A()
-        a.__cuda_array_interface__ = {"shape": (int(np.prod(shape)),), "typestr": "<f4" if dtype == torch.float32 else "<i4",
+        typestr = {torch.float32: "<f4", torch.int32: "<i4", torch.bfloat16: "<i2"}[dtype]
+        a.__cuda_array_interface__ = {"shape": (int(np.prod(shape)),), "typestr": typestr,
                                       "data": (int(ptr), False), "version": 2}
-        return torch.as_tensor(a, device=self.device).view(*shape)
+        t = torch.as_tensor(a, device=self.device)
+        return (t.view(torch.bfloat16) if dtype == torch.bfloat16 else t).view(*shape)
+
+    # buffers stored in bf16 in bf16 mode: the SuperPoint activations, q|k|v, the attention message, the token shadow
+    BF16_TENSORS = ("x1a", "x4b", "qkv", "msg", "tokens_bf16")
 
     def debug_tensor(self, name, shape):
+        """Named engine buffer as a device tensor view. fp32, except in bf16 mode (precision="bf16"), where the
+        buffers named in BF16_TENSORS ("qkv" [2B][K][768], "msg" [2B][K][256], ...) are torch.bfloat16 views, and
+        "attn_scores" / "attn_vt" do not exist (the fused attention never stores them)."""
         p, n = ctypes.c_void_p(), ctypes.c_longlong()
         _lib.check(self._l.mfr_spsg_debug_tensor(self._h, name.encode(), ctypes.byref(p), ctypes.byref(n)), name)
         assert int(np.prod(shape)) <= n.value
-        return self._wrap(p.value, shape, torch.float32)
+        bf = self.precision == 1 and name in self.BF16_TENSORS
+        return self._wrap(p.value, shape, torch.bfloat16 if bf else torch.float32)
 
     def device_outputs(self):
         o, B, K = self._o, self.B, self.K
@@ -237,14 +246,15 @@ class SuperGlue_matcher:
     holds superpoint_v1.pth and superglue_{indoor,outdoor}.pth (SuperGlue/models/weights in the
     reference tree)."""
 
-    def __init__(self, resize, outdoor=False, weights_dir="SuperGlue/models/weights", state_dicts=None):
+    def __init__(self, resize, outdoor=False, weights_dir="SuperGlue/models/weights", state_dicts=None, precision="tf32"):
         if state_dicts is None:
             sp = torch.load(os.path.join(weights_dir, "superpoint_v1.pth"), map_location="cpu")
             sg = torch.load(os.path.join(weights_dir, f"superglue_{'outdoor' if outdoor else 'indoor'}.pth"), map_location="cpu")
         else:
             sp, sg = state_dicts
         self.resize = resize
-        self.engine = SuperPointSuperGlue(sp, sg, batch=1, height=int(resize[1]), width=int(resize[0]))
+        # precision: "tf32" (default), "bf16" (throughput mode, see include/mfr_b200.h) or "fp32x3"
+        self.engine = SuperPointSuperGlue(sp, sg, batch=1, height=int(resize[1]), width=int(resize[0]), precision=precision)
 
     def match(self, pair_path):
         """matchers.py:93-120; images decoded (JPEG: nvJPEG) and resized on the GPU (mfr_b200.image_io)."""

@@ -99,6 +99,15 @@ long long mfr_loftr_weight_numel(const mfr_loftr* h, int i);
 int mfr_loftr_set_weight(mfr_loftr* h, int i, const float* host, long long numel, void* stream);
 int mfr_loftr_forward(mfr_loftr* h, const float* img0, const float* img1, int src_h, int src_w,
                       void* stream);
+/* Shared map frame (Map-free: every query of a scene is matched against the same reference image).
+ * mfr_loftr_set_map encodes one map image img0 [src_h][src_w] (device float32) — backbone, position encoding and the
+ * first coarse layer, which depend on that image alone — into buffers of its own; they stay valid until the next
+ * set_map or weight upload, and a paired mfr_loftr_forward in between does not disturb them. Runs eagerly.
+ * mfr_loftr_forward_shared(h, img1 [B][src_h][src_w]) then writes outputs bit-identical, in every precision, to
+ * mfr_loftr_forward(h, img0 repeated B times, img1), and runs as its own CUDA graph. It returns MFR_ERR_ARG before any
+ * set_map or when (src_h, src_w) differs from the map's. */
+int mfr_loftr_set_map(mfr_loftr* h, const float* img0, int src_h, int src_w, void* stream);
+int mfr_loftr_forward_shared(mfr_loftr* h, const float* img1, int src_h, int src_w, void* stream);
 void mfr_loftr_set_graph(mfr_loftr* h, int enabled);
 int mfr_loftr_get_outputs(mfr_loftr* h, mfr_loftr_outputs* out);
 /* named intermediate buffers for stage-wise parity tests ("feat_c_backbone", "feat_f", "tok", "sim", ...) */
@@ -153,6 +162,13 @@ const char* mfr_spsg_weight_name(const mfr_spsg* h, int i);
 long long mfr_spsg_weight_numel(const mfr_spsg* h, int i);
 int mfr_spsg_set_weight(mfr_spsg* h, int i, const float* host, long long numel, void* stream);
 int mfr_spsg_forward(mfr_spsg* h, const float* img0, const float* img1, void* stream);
+/* Shared map frame: mfr_spsg_set_map runs SuperPoint once on the map image img0 [H][W] (device float32, eagerly) and
+ * keeps its keypoints, scores and descriptors until the next set_map or weight upload; a paired mfr_spsg_forward in
+ * between does not disturb them. mfr_spsg_forward_shared(h, img1 [B][H][W]) runs SuperPoint on the queries only, then
+ * SuperGlue on every pair, and writes outputs bit-identical, in every precision, to mfr_spsg_forward(h, img0 repeated
+ * B times, img1); it runs as its own CUDA graph and returns MFR_ERR_ARG before any set_map. */
+int mfr_spsg_set_map(mfr_spsg* h, const float* img0, void* stream);
+int mfr_spsg_forward_shared(mfr_spsg* h, const float* img1, void* stream);
 void mfr_spsg_set_graph(mfr_spsg* h, int enabled);
 int mfr_spsg_get_outputs(mfr_spsg* h, mfr_spsg_outputs* out);
 int mfr_spsg_debug_tensor(mfr_spsg* h, const char* name, float** ptr, long long* numel);

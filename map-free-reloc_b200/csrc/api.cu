@@ -91,6 +91,14 @@ int mfr_loftr_set_weight(mfr_loftr* h, int i, const float* host, long long numel
 int mfr_loftr_forward(mfr_loftr* h, const float* img0, const float* img1, int src_h, int src_w, void* stream) {
   return mfr::loftr_forward(h->e, img0, img1, src_h, src_w, static_cast<cudaStream_t>(stream));
 }
+int mfr_loftr_set_map(mfr_loftr* h, const float* img0, int src_h, int src_w, void* stream) {
+  if (!h || !img0) return MFR_ERR_ARG;
+  return mfr::loftr_set_map(h->e, img0, src_h, src_w, static_cast<cudaStream_t>(stream));
+}
+int mfr_loftr_forward_shared(mfr_loftr* h, const float* img1, int src_h, int src_w, void* stream) {
+  if (!h || !img1) return MFR_ERR_ARG;
+  return mfr::loftr_forward_shared(h->e, img1, src_h, src_w, static_cast<cudaStream_t>(stream));
+}
 void mfr_loftr_set_graph(mfr_loftr* h, int enabled) { mfr::loftr_set_graph(h->e, enabled); }
 int mfr_loftr_get_outputs(mfr_loftr* h, mfr_loftr_outputs* out) {
   if (!h || !out) return MFR_ERR_ARG;
@@ -138,6 +146,14 @@ int mfr_spsg_set_weight(mfr_spsg* h, int i, const float* host, long long numel, 
 }
 int mfr_spsg_forward(mfr_spsg* h, const float* img0, const float* img1, void* stream) {
   return mfr::spsg_forward(h->e, img0, img1, static_cast<cudaStream_t>(stream));
+}
+int mfr_spsg_set_map(mfr_spsg* h, const float* img0, void* stream) {
+  if (!h || !img0) return MFR_ERR_ARG;
+  return mfr::spsg_set_map(h->e, img0, static_cast<cudaStream_t>(stream));
+}
+int mfr_spsg_forward_shared(mfr_spsg* h, const float* img1, void* stream) {
+  if (!h || !img1) return MFR_ERR_ARG;
+  return mfr::spsg_forward_shared(h->e, img1, static_cast<cudaStream_t>(stream));
 }
 void mfr_spsg_set_graph(mfr_spsg* h, int enabled) { mfr::spsg_set_graph(h->e, enabled); }
 int mfr_spsg_get_outputs(mfr_spsg* h, mfr_spsg_outputs* out) {

@@ -72,8 +72,13 @@ struct LoftrEngine {
 
   std::vector<void*> allocs;
   std::map<std::string, DebugTensor> dbg;
-  std::vector<std::function<int(cudaStream_t)>> steps;
+  using StepList = std::vector<std::function<int(cudaStream_t)>>;
+  StepList steps;              // the paired forward; conv() and push() append here
   std::vector<StepInfo> infos;
+  // Shared map frame (set_map / forward_shared): map_steps encodes one image up to coarse layer 0 into the map_*
+  // buffers; shared_steps runs the query half of a batch, broadcasts the map into the image-0 half and continues with
+  // the paired list's own steps from coarse layer 1 on.
+  StepList map_steps, shared_steps;
   void push(const std::string& name, std::function<int(cudaStream_t)> f, int launches = 1) {
     steps.push_back(std::move(f));
     StepInfo inf{name, 0, 0.0, nullptr, 0};
@@ -87,15 +92,21 @@ struct LoftrEngine {
   float *mrg = nullptr, *h1 = nullptr, *h2 = nullptr;   // tf32 / fp32x3 only (unfused encoder tail)
   float *tokb = nullptr, *ftokb = nullptr;   // bf16 mode: bf16 shadows of tok / ftok (same shape; float-typed like the other bf16 buffers)
   size_t ftok_elems = 0;
+  float *featf = nullptr;
+  // the encoded map frame: its [H][W] input, tokens after coarse layer 0 ([L][512], + bf16 shadow), fine map [H/2][W/2][128]
+  float *map_img = nullptr, *map_tok = nullptr, *map_tokb = nullptr, *map_featf = nullptr;
+  bool map_ready = false;
+  int map_src_h = -1, map_src_w = -1;
   float* shadow(float* x) const {            // same element offset inside the shadow buffer
     if (x >= ftok && x < ftok + ftok_elems) return ftokb + (x - ftok) / 2;
+    if (x >= map_tok && x < map_tok + static_cast<size_t>(L) * 512) return map_tokb + (x - map_tok) / 2;
     return tokb + (x - tok) / 2;
   }
   CoarseMatchBuffers cm;
   float *cin, *cproj, *win, *ftok, *fqkv, *fmsg, *mk1f, *expec;
   float *fmrg = nullptr, *fh1 = nullptr, *fh2 = nullptr;   // tf32 / fp32x3 only
   // graph
-  cudaGraphExec_t graph_exec = nullptr;
+  cudaGraphExec_t graph_exec = nullptr, shared_exec = nullptr;
   bool use_graph = true;
   int build_rc = MFR_OK;
 
@@ -256,7 +267,7 @@ struct LoftrEngine {
   //   mrg_x, h1_x, h2_x : scratch of the unfused tail (tf32 / fp32x3 only, null in bf16 mode)
   void encoder_layer(const std::string& p, int C, float* x, float* src, float* qkv_x, float* qkv_s,
                      float* msg_x, float* mrg_x, float* h1_x, float* h2_x, int n, int rows,
-                     const int* dyn_rows, const int* dyn_items, bool windows) {
+                     const int* dyn_rows, const int* dyn_items, bool windows, int kv_splits = 0) {
     float* wq = W_(p + ".qkv.w");
     const long long ld2 = 2 * C, ld3 = 3 * C;
     // bf16 mode: q|k|v and the attention message are stored in bf16 — these GEMMs and the attention kernels are
@@ -281,7 +292,8 @@ struct LoftrEngine {
     }
     if (!windows) {
       float* kvp_ = kvp; float* kv_ = kv;
-      const int Lr = rows, sk = splits_kv * NI / n;   // same partial-buffer footprint for n = B or n = 2B images
+      // same partial-buffer footprint for n = B or n = 2B images, unless the caller pins the split count
+      const int Lr = rows, sk = kv_splits > 0 ? kv_splits : splits_kv * NI / n;
       float *kp = E(qkv_s, C), *vp = E(qkv_s, 2 * C);
       push("attn_long", [=](cudaStream_t st) {
         return linear_attention_long(qkv_x, ld3, kp, ld3, vp, ld3, msg_x, C, kvp_, kv_, n, Lr, Lr, 8, 32, sk, st, tbf);
@@ -353,6 +365,80 @@ struct LoftrEngine {
     }
   }
 
+  // Stem + ResNet-FPN (resnet_fpn.py:100-119) over the N images of `input` ([N][H][W]): the 1/8 map goes to feat_c
+  // ([N][L][256] fp32), the 1/2 map to feat_f ([N][H/2][W/2][128] fp32). The other activations live in the shared
+  // scratch buffers a0 ... p2b.
+  void backbone(float* input, int N, float* feat_c, float* feat_f) {
+    const bool bf = precision == 1;
+    const int c196 = bf ? 200 : 196;
+    const int B16 = bf ? 1 : 0;
+    {
+      float *img_ = input, *a0_ = a0; float* ws = W_("stem.w"); float* bs = W_("stem.b");
+      const int NI_ = N, H_ = H, W_w = W, ob = B16, exact = precision == 2 ? 1 : 0;
+      push("stem", [=](cudaStream_t st) { return stem_conv7x7(img_, ws, bs, a0_, NI_, H_, W_w, st, ob, exact); });
+    }
+    auto bconv = [&](const std::string& name, const float* x, int Hh, int Ww, int Cin, int ldx, int Cout, int R,
+                     int stride, bool bias, const float* res, int act, float* out, int ldo, int out16) {
+      conv(name, x, N, Hh, Ww, Cin, ldx, Cout, R, stride, bias, res, act, out, ldo, 0, nullptr, nullptr, nullptr, B16,
+           out16);
+    };
+    bconv("layer1.0.conv1", a0, H2, W2, 128, 128, 128, 3, 1, true, nullptr, ACT_RELU, a1, 128, B16);
+    bconv("layer1.0.conv2", a1, H2, W2, 128, 128, 128, 3, 1, true, a0, ACT_RELU, a2, 128, B16);
+    bconv("layer1.1.conv1", a2, H2, W2, 128, 128, 128, 3, 1, true, nullptr, ACT_RELU, a1, 128, B16);
+    bconv("layer1.1.conv2", a1, H2, W2, 128, 128, 128, 3, 1, true, a2, ACT_RELU, a0, 128, B16);  // x1 = a0
+    bconv("layer2.0.conv1", a0, H2, W2, 128, 128, 196, 3, 2, true, nullptr, ACT_RELU, b1, c196, B16);
+    bconv("layer2.0.down", a0, H2, W2, 128, 128, 196, 1, 2, true, nullptr, ACT_NONE, b2, c196, B16);
+    bconv("layer2.0.conv2", b1, H4, W4, 196, c196, 196, 3, 1, true, b2, ACT_RELU, b0, c196, B16);
+    bconv("layer2.1.conv1", b0, H4, W4, 196, c196, 196, 3, 1, true, nullptr, ACT_RELU, b1, c196, B16);
+    bconv("layer2.1.conv2", b1, H4, W4, 196, c196, 196, 3, 1, true, b0, ACT_RELU, b2, c196, B16);  // x2 = b2
+    bconv("layer3.0.conv1", b2, H4, W4, 196, c196, 256, 3, 2, true, nullptr, ACT_RELU, c1, 256, B16);
+    bconv("layer3.0.down", b2, H4, W4, 196, c196, 256, 1, 2, true, nullptr, ACT_NONE, c2, 256, B16);
+    bconv("layer3.0.conv2", c1, H8, W8, 256, 256, 256, 3, 1, true, c2, ACT_RELU, c0, 256, B16);
+    bconv("layer3.1.conv1", c0, H8, W8, 256, 256, 256, 3, 1, true, nullptr, ACT_RELU, c1, 256, B16);
+    bconv("layer3.1.conv2", c1, H8, W8, 256, 256, 256, 3, 1, true, c0, ACT_RELU, c2, 256, B16);  // x3 = c2
+    bconv("layer3_outconv", c2, H8, W8, 256, 256, 256, 1, 1, false, nullptr, ACT_NONE, feat_c, 256, 0);   // fp32 out
+    bconv("layer2_outconv", b2, H4, W4, 196, c196, 256, 1, 1, false, nullptr, ACT_NONE, p4a, 256, B16);
+    {
+      float *s_ = feat_c, *d_ = p4a; const int n = N, hs = H8, wsz = W8, ob = B16;
+      push("upsample", [=](cudaStream_t st) { return upsample2x_add(s_, d_, n, hs, wsz, 256, 256, 256, 0, ob, st); });
+    }
+    bconv("layer2_outconv2.0", p4a, H4, W4, 256, 256, 256, 3, 1, true, nullptr, ACT_LEAKY, p4b, 256, B16);
+    bconv("layer2_outconv2.3", p4b, H4, W4, 256, 256, 196, 3, 1, false, nullptr, ACT_NONE, p4c, c196, B16);
+    bconv("layer1_outconv", a0, H2, W2, 128, 128, 196, 1, 1, false, nullptr, ACT_NONE, p2a, c196, B16);
+    {
+      float *s_ = p4c, *d_ = p2a; const int n = N, hs = H4, wsz = W4, ld = c196, ob = B16;
+      push("upsample", [=](cudaStream_t st) { return upsample2x_add(s_, d_, n, hs, wsz, 196, ld, ld, ob, ob, st); });
+    }
+    bconv("layer1_outconv2.0", p2a, H2, W2, 196, c196, 196, 3, 1, true, nullptr, ACT_LEAKY, p2b, c196, B16);
+    bconv("layer1_outconv2.3", p2b, H2, W2, 196, c196, 128, 3, 1, false, nullptr, ACT_NONE, feat_f, 128, 0);   // fp32 out
+  }
+
+  // pos-enc add (loftr.py:58-59) of N images' 1/8 maps into token rows t (row stride 512), and its bf16 shadow
+  void coarse_tokens(float* feat_c, int N, float* t) {
+    float* pe = W_("pos_enc"); const int n = N, l = L;
+    push("posenc", [=](cudaStream_t st) { return posenc_tokens(feat_c, pe, t, 512, n, l, 256, st); });
+    if (precision == 1) {
+      float* tb_ = shadow(t);
+      push("to_bf16", [=](cudaStream_t st) { return rows_to_bf16(t, 512, tb_, 512, static_cast<long long>(n) * l, 256, nullptr, st); });
+    }
+  }
+
+  // Coarse layer 0 (a self layer) on n images of token rows t. The K'ᵀV sums are split into splits_kv parts whatever n
+  // is — the split count of the paired list's self layers — so an image gives the same bits alone as inside a batch.
+  void coarse_layer0(float* t, int n) {
+    encoder_layer("coarse.0", 256, t, t, qkv, qkv, msg, mrg, h1, h2, n, L, nullptr, nullptr, false, splits_kv);
+  }
+
+  // 5x5 windows of the fine maps around every coarse match: side s reads pair b's map at feat_f_s + b * stride_s
+  void fine_windows(const float* f0, long long stride0, const float* f1, long long stride1) {
+    CoarseMatchBuffers cmb = cm; float *cproj_ = cproj, *win_ = win;
+    const int Mc = Mcap, Hf = H2, Wf = W2, wc = W8;
+    push("fine_gather_windows", [=](cudaStream_t st) {
+      return fine_gather_windows(f0, stride0, f1, stride1, Hf, Wf, wc, cmb.b_ids, cmb.i_ids, cmb.j_ids, cmb.m_total, Mc,
+                                 cproj_, win_, st);
+    });
+  }
+
   int build() {
     NI = 2 * B;
     H2 = H / 2; W2 = W / 2; H4 = H / 4; W4 = W / 4; H8 = H / 8; W8 = W / 8;
@@ -391,9 +477,13 @@ struct LoftrEngine {
     fc = alloc<float>(px8 * 256, "feat_c_backbone");
     p4a = balloc(px4 * 256, "p4a"); p4b = balloc(px4 * 256, "p4b"); p4c = balloc(px4 * c196, "p4c");
     p2a = balloc(px2 * c196, "p2a"); p2b = balloc(px2 * c196, "p2b");
-    float* featf = alloc<float>(px2 * 128, "feat_f");
+    featf = alloc<float>(px2 * 128, "feat_f");
     tok = alloc<float>(px8 * 512, "tok");
     if (bf) tokb = reinterpret_cast<float*>(alloc<unsigned short>(px8 * 512, "tok_bf16"));
+    map_img = alloc<float>(static_cast<size_t>(H) * W, "map_img");
+    map_tok = alloc<float>(static_cast<size_t>(L) * 512, "map_tok");
+    if (bf) map_tokb = reinterpret_cast<float*>(alloc<unsigned short>(static_cast<size_t>(L) * 512, "map_tok_bf16"));
+    map_featf = alloc<float>(static_cast<size_t>(H2) * W2 * 128, "map_feat_f");
     qkv = alloc<float>(px8 * 768, "qkv"); msg = alloc<float>(px8 * 256, "msg");
     if (!bf) {   // the unfused encoder tail's scratch (bf16 mode runs the fused tail)
       mrg = alloc<float>(px8 * 256, "mrg"); h1 = alloc<float>(px8 * 512, "h1"); h2 = alloc<float>(px8 * 256, "h2");
@@ -425,62 +515,18 @@ struct LoftrEngine {
     mk1f = alloc<float>(BL * 2, "mkpts1_f"); expec = alloc<float>(BL * 3, "expec_f");
     if (build_rc != MFR_OK) return build_rc;
 
-    // ---------------------------------------------------------------- backbone (resnet_fpn.py:100-119)
-    const int B16 = bf ? 1 : 0;
-    {
-      float *img_ = img, *a0_ = a0; float* ws = W_("stem.w"); float* bs = W_("stem.b");
-      const int NI_ = NI, H_ = H, W_w = W, ob = B16, exact = precision == 2 ? 1 : 0;
-      push("stem", [=](cudaStream_t st) { return stem_conv7x7(img_, ws, bs, a0_, NI_, H_, W_w, st, ob, exact); });
-    }
-    auto bconv = [&](const std::string& name, const float* x, int Hh, int Ww, int Cin, int ldx, int Cout, int R,
-                     int stride, bool bias, const float* res, int act, float* out, int ldo, int out16) {
-      conv(name, x, NI, Hh, Ww, Cin, ldx, Cout, R, stride, bias, res, act, out, ldo, 0, nullptr, nullptr, nullptr, B16,
-           out16);
-    };
-    bconv("layer1.0.conv1", a0, H2, W2, 128, 128, 128, 3, 1, true, nullptr, ACT_RELU, a1, 128, B16);
-    bconv("layer1.0.conv2", a1, H2, W2, 128, 128, 128, 3, 1, true, a0, ACT_RELU, a2, 128, B16);
-    bconv("layer1.1.conv1", a2, H2, W2, 128, 128, 128, 3, 1, true, nullptr, ACT_RELU, a1, 128, B16);
-    bconv("layer1.1.conv2", a1, H2, W2, 128, 128, 128, 3, 1, true, a2, ACT_RELU, a0, 128, B16);  // x1 = a0
-    bconv("layer2.0.conv1", a0, H2, W2, 128, 128, 196, 3, 2, true, nullptr, ACT_RELU, b1, c196, B16);
-    bconv("layer2.0.down", a0, H2, W2, 128, 128, 196, 1, 2, true, nullptr, ACT_NONE, b2, c196, B16);
-    bconv("layer2.0.conv2", b1, H4, W4, 196, c196, 196, 3, 1, true, b2, ACT_RELU, b0, c196, B16);
-    bconv("layer2.1.conv1", b0, H4, W4, 196, c196, 196, 3, 1, true, nullptr, ACT_RELU, b1, c196, B16);
-    bconv("layer2.1.conv2", b1, H4, W4, 196, c196, 196, 3, 1, true, b0, ACT_RELU, b2, c196, B16);  // x2 = b2
-    bconv("layer3.0.conv1", b2, H4, W4, 196, c196, 256, 3, 2, true, nullptr, ACT_RELU, c1, 256, B16);
-    bconv("layer3.0.down", b2, H4, W4, 196, c196, 256, 1, 2, true, nullptr, ACT_NONE, c2, 256, B16);
-    bconv("layer3.0.conv2", c1, H8, W8, 256, 256, 256, 3, 1, true, c2, ACT_RELU, c0, 256, B16);
-    bconv("layer3.1.conv1", c0, H8, W8, 256, 256, 256, 3, 1, true, nullptr, ACT_RELU, c1, 256, B16);
-    bconv("layer3.1.conv2", c1, H8, W8, 256, 256, 256, 3, 1, true, c0, ACT_RELU, c2, 256, B16);  // x3 = c2
-    bconv("layer3_outconv", c2, H8, W8, 256, 256, 256, 1, 1, false, nullptr, ACT_NONE, fc, 256, 0);   // fp32 out
-    bconv("layer2_outconv", b2, H4, W4, 196, c196, 256, 1, 1, false, nullptr, ACT_NONE, p4a, 256, B16);
-    {
-      float *s_ = fc, *d_ = p4a; const int n = NI, hs = H8, wsz = W8, ob = B16;
-      push("upsample", [=](cudaStream_t st) { return upsample2x_add(s_, d_, n, hs, wsz, 256, 256, 256, 0, ob, st); });
-    }
-    bconv("layer2_outconv2.0", p4a, H4, W4, 256, 256, 256, 3, 1, true, nullptr, ACT_LEAKY, p4b, 256, B16);
-    bconv("layer2_outconv2.3", p4b, H4, W4, 256, 256, 196, 3, 1, false, nullptr, ACT_NONE, p4c, c196, B16);
-    bconv("layer1_outconv", a0, H2, W2, 128, 128, 196, 1, 1, false, nullptr, ACT_NONE, p2a, c196, B16);
-    {
-      float *s_ = p4c, *d_ = p2a; const int n = NI, hs = H4, wsz = W4, ld = c196, ob = B16;
-      push("upsample", [=](cudaStream_t st) { return upsample2x_add(s_, d_, n, hs, wsz, 196, ld, ld, ob, ob, st); });
-    }
-    bconv("layer1_outconv2.0", p2a, H2, W2, 196, c196, 196, 3, 1, true, nullptr, ACT_LEAKY, p2b, c196, B16);
-    bconv("layer1_outconv2.3", p2b, H2, W2, 196, c196, 128, 3, 1, false, nullptr, ACT_NONE, featf, 128, 0);   // fp32 out
-
-    // ---------------------------------------------------------------- pos-enc + coarse transformer
-    {
-      float *f = fc, *t = tok; float* pe = W_("pos_enc"); const int n = NI, l = L;
-      push("posenc", [=](cudaStream_t st) { return posenc_tokens(f, pe, t, 512, n, l, 256, st); });
-      if (bf) {
-        float* tb_ = tokb;
-        push("to_bf16", [=](cudaStream_t st) { return rows_to_bf16(t, 512, tb_, 512, static_cast<long long>(n) * l, 256, nullptr, st); });
-      }
-    }
+    // ---------------------------------------------------------------- backbone, pos-enc, coarse layer 0
+    conv_count = 0;
+    backbone(img, NI, fc, featf);
+    coarse_tokens(fc, NI, tok);
+    coarse_layer0(tok, NI);
+    const size_t img_f = static_cast<size_t>(H2) * W2 * 128;   // floats of one image's fine map
     const size_t half_tok = static_cast<size_t>(B) * L * 512, half_qkv = static_cast<size_t>(B) * L * 768;
     const size_t half_c = static_cast<size_t>(B) * L * 256, half_2c = static_cast<size_t>(B) * L * 512;
     const int tb = bf ? 2 : 1;   // qkv / msg hold bf16 in that mode (see encoder_layer)
     auto at = [](float* p, size_t off) { return p ? p + off : p; };   // the unfused tail's scratch is null in bf16 mode
-    for (int i = 0; i < 8; ++i) {
+    const size_t layer1_begin = steps.size();
+    for (int i = 1; i < 8; ++i) {
       const std::string p = "coarse." + std::to_string(i);
       if (i % 2 == 0) {  // self: both image sets at once
         encoder_layer(p, 256, tok, tok, qkv, qkv, msg, mrg, h1, h2, NI, L, nullptr, nullptr, false);
@@ -523,17 +569,17 @@ struct LoftrEngine {
 
     // ---------------------------------------------------------------- fine level
     {
-      CoarseMatchBuffers cmb = cm; float *tok_ = tok, *cin_ = cin, *cproj_ = cproj, *win_ = win;
-      const int B_ = B, L_ = L, Mc = Mcap, Hf = H2, Wf = W2, wc = W8;
+      CoarseMatchBuffers cmb = cm; float *tok_ = tok, *cin_ = cin;
+      const int B_ = B, L_ = L, Mc = Mcap;
       push("fine_gather_coarse", [=](cudaStream_t st) {
         return fine_gather_coarse(tok_, 512, B_, L_, cmb.b_ids, cmb.i_ids, cmb.j_ids, cmb.m_total, Mc, cin_, st);
       });
       conv("fine.down_proj", cin, 2, 1, Mcap, 256, 256, 128, 1, 1, true, nullptr, ACT_NONE, cproj, 128, 0,
            cm.m_total);
-      push("fine_gather_windows", [=](cudaStream_t st) {
-        return fine_gather_windows(featf, B_, Hf, Wf, wc, cmb.b_ids, cmb.i_ids, cmb.j_ids, cmb.m_total, Mc,
-                                   cproj_, win_, st);
-      });
+    }
+    const size_t windows_step = steps.size();
+    fine_windows(featf, img_f, featf + B * img_f, img_f);
+    {
       conv("fine.merge_feat", win, 2, 1, Mcap * 25, 256, 256, 128, 1, 1, true, nullptr, ACT_NONE, ftok, 256, 0,
            cm.m_total + 2);
     }
@@ -561,6 +607,39 @@ struct LoftrEngine {
         return fine_match(f0, f1, 256, cmb.mkpts1_c, cmb.m_total, Mc, scale_f, mk, ex, st);
       });
     }
+    if (build_rc != MFR_OK) return build_rc;
+
+    // ---------------------------------------------------------------- shared map frame
+    StepList paired = std::move(steps);
+    std::vector<StepInfo> paired_infos = std::move(infos);
+    steps.clear(); infos.clear();
+    conv_count = kReservedLayers;   // the map encode runs once per scene, on its own: no SMs to leave free
+    backbone(map_img, 1, fc, map_featf);
+    coarse_tokens(fc, 1, map_tok);
+    coarse_layer0(map_tok, 1);
+    map_steps = std::move(steps);
+    steps.clear(); infos.clear();
+    conv_count = 0;
+    const size_t half_img = static_cast<size_t>(B) * H * W;
+    backbone(img + half_img, B, fc + half_c, featf + B * img_f);
+    coarse_tokens(fc + half_c, B, tok + half_tok);
+    {
+      float *mt = map_tok, *mtb = map_tokb, *t0 = tok, *tb0 = tokb; const long long bytes = static_cast<long long>(L) * 512 * 4;
+      const int nb = B;
+      push("map_broadcast", [=](cudaStream_t st) {
+        int rc = broadcast_copies(mt, bytes, t0, nb, st);
+        if (rc == MFR_OK && mtb) rc = broadcast_copies(mtb, bytes / 2, tb0, nb, st);
+        return rc;
+      }, bf ? 2 : 1);
+    }
+    coarse_layer0(tok + half_tok, B);
+    for (size_t i = layer1_begin; i < windows_step; ++i) steps.push_back(paired[i]);
+    fine_windows(map_featf, 0, featf + B * img_f, img_f);
+    for (size_t i = windows_step + 1; i < paired.size(); ++i) steps.push_back(paired[i]);
+    shared_steps = std::move(steps);
+    steps = std::move(paired);
+    infos = std::move(paired_infos);
+
     if (precision == 2 && w16_total > wtotal * 3 + 64 * specs.size()) {
       fprintf(stderr, "[mfr_b200] split weight blob too small\n");
       return MFR_ERR_ARG;
@@ -572,22 +651,42 @@ struct LoftrEngine {
     return build_rc;
   }
 
-  int run_steps(cudaStream_t st) {
-    for (auto& s : steps) {
+  int run_steps(const StepList& list, cudaStream_t st) {
+    for (auto& s : list) {
       int rc = s(st);
       if (rc != MFR_OK) return rc;
     }
     return MFR_OK;
   }
 
-  // src images are [B][src_h][src_w] (src_h <= H, src_w <= W); the right/bottom remainder of the
-  // engine's [H][W] frame stays zero: the reference's ConstantPad2d (matchers.py:41-46).
-  int forward(const float* img0, const float* img1, int src_h, int src_w, cudaStream_t st) {
-    if (!weights_loaded) {
-      fprintf(stderr, "[mfr_b200] loftr forward before weights were loaded\n");
-      return MFR_ERR_ARG;
+  // Runs `list` through its CUDA graph `exec`, capturing it on the first call.
+  int launch(const StepList& list, cudaGraphExec_t& exec, cudaStream_t st) {
+    if (!use_graph) return run_steps(list, st);
+    if (!exec) {
+      // warm (sets function attributes outside capture), then capture the launch list once
+      int rc = run_steps(list, st);
+      if (rc != MFR_OK) return rc;
+      MFR_CUDA_CHECK(cudaStreamSynchronize(st));
+      cudaGraph_t g;
+      MFR_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+      rc = run_steps(list, st);
+      cudaError_t e = cudaStreamEndCapture(st, &g);
+      if (rc != MFR_OK || e != cudaSuccess) {
+        fprintf(stderr, "[mfr_b200] graph capture failed (%d, %s); running eagerly\n", rc, cudaGetErrorString(e));
+        use_graph = false;
+        cudaGetLastError();
+        return run_steps(list, st);
+      }
+      MFR_CUDA_CHECK(cudaGraphInstantiate(&exec, g, 0));
+      cudaGraphDestroy(g);
+      return MFR_OK;  // the warm-up pass above already produced this call's results
     }
-    if (src_h > H || src_w > W || src_h < 1 || src_w < 1) return MFR_ERR_ARG;
+    MFR_CUDA_CHECK(cudaGraphLaunch(exec, st));
+    return MFR_OK;
+  }
+
+  // bf16 / split copies of the weights, rebuilt after every weight upload
+  int prepare_weights(cudaStream_t st) {
     if (precision == 1 && !w16_ready) {   // bf16 copies of the (folded) backbone conv weights
       for (const auto& bc : bf16_convs) {
         int rc = weights_to_bf16(W_(bc.name + ".w"), wblob16 + bc.off, static_cast<size_t>(bc.cout) * bc.taps, bc.cin,
@@ -604,45 +703,72 @@ struct LoftrEngine {
       }
       w16_ready = true;
     }
+    return MFR_OK;
+  }
+
+  // Copies `n` source images [n][src_h][src_w] into the engine frames dst [n][H][W]; the right/bottom remainder of a
+  // frame stays zero: the reference's ConstantPad2d (matchers.py:41-46).
+  int copy_frames(float* dst, const float* src, int n, int src_h, int src_w, cudaStream_t st) {
+    if (src_h == H && src_w == W) {
+      MFR_CUDA_CHECK(cudaMemcpyAsync(dst, src, static_cast<size_t>(n) * H * W * 4, cudaMemcpyDeviceToDevice, st));
+      return MFR_OK;
+    }
+    for (int b = 0; b < n; ++b)
+      MFR_CUDA_CHECK(cudaMemcpy2DAsync(dst + static_cast<size_t>(b) * H * W, static_cast<size_t>(W) * 4,
+                                       src + static_cast<size_t>(b) * src_h * src_w, static_cast<size_t>(src_w) * 4,
+                                       static_cast<size_t>(src_w) * 4, src_h, cudaMemcpyDeviceToDevice, st));
+    return MFR_OK;
+  }
+
+  // Stages the batch into `img` (img0 == nullptr: the query half only). The pad of every frame in `img` is zero as
+  // long as each call writes frames of the size of the previous call; a change of size clears the whole buffer.
+  int stage(const float* img0, const float* img1, int src_h, int src_w, cudaStream_t st) {
+    if (src_h > H || src_w > W || src_h < 1 || src_w < 1) return MFR_ERR_ARG;
     const size_t half = static_cast<size_t>(B) * H * W;
     if ((src_h != H || src_w != W) && (src_h != last_src_h || src_w != last_src_w) && last_src_h > 0)
       MFR_CUDA_CHECK(cudaMemsetAsync(img, 0, 2 * half * 4, st));   // a smaller source than last time: clear the old pixels of the pad
     last_src_h = src_h; last_src_w = src_w;
-    if (src_h == H && src_w == W) {
-      MFR_CUDA_CHECK(cudaMemcpyAsync(img, img0, half * 4, cudaMemcpyDeviceToDevice, st));
-      MFR_CUDA_CHECK(cudaMemcpyAsync(img + half, img1, half * 4, cudaMemcpyDeviceToDevice, st));
-    } else {
-      for (int b = 0; b < B; ++b) {
-        MFR_CUDA_CHECK(cudaMemcpy2DAsync(img + static_cast<size_t>(b) * H * W, static_cast<size_t>(W) * 4,
-                                         img0 + static_cast<size_t>(b) * src_h * src_w, static_cast<size_t>(src_w) * 4,
-                                         static_cast<size_t>(src_w) * 4, src_h, cudaMemcpyDeviceToDevice, st));
-        MFR_CUDA_CHECK(cudaMemcpy2DAsync(img + half + static_cast<size_t>(b) * H * W, static_cast<size_t>(W) * 4,
-                                         img1 + static_cast<size_t>(b) * src_h * src_w, static_cast<size_t>(src_w) * 4,
-                                         static_cast<size_t>(src_w) * 4, src_h, cudaMemcpyDeviceToDevice, st));
-      }
+    int rc = MFR_OK;
+    if (img0) rc = copy_frames(img, img0, B, src_h, src_w, st);
+    if (rc == MFR_OK) rc = copy_frames(img + half, img1, B, src_h, src_w, st);
+    return rc;
+  }
+
+  // src images are [B][src_h][src_w] (src_h <= H, src_w <= W), zero-padded to the engine's [H][W] frame
+  int forward(const float* img0, const float* img1, int src_h, int src_w, cudaStream_t st) {
+    if (!weights_loaded) {
+      fprintf(stderr, "[mfr_b200] loftr forward before weights were loaded\n");
+      return MFR_ERR_ARG;
     }
-    if (!use_graph) return run_steps(st);
-    if (!graph_exec) {
-      // warm (sets function attributes outside capture), then capture the launch list once
-      int rc = run_steps(st);
-      if (rc != MFR_OK) return rc;
-      MFR_CUDA_CHECK(cudaStreamSynchronize(st));
-      cudaGraph_t g;
-      MFR_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      rc = run_steps(st);
-      cudaError_t e = cudaStreamEndCapture(st, &g);
-      if (rc != MFR_OK || e != cudaSuccess) {
-        fprintf(stderr, "[mfr_b200] graph capture failed (%d, %s); running eagerly\n", rc, cudaGetErrorString(e));
-        use_graph = false;
-        cudaGetLastError();
-        return run_steps(st);
-      }
-      MFR_CUDA_CHECK(cudaGraphInstantiate(&graph_exec, g, 0));
-      cudaGraphDestroy(g);
-      return MFR_OK;  // the warm-up pass above already produced this call's results
-    }
-    MFR_CUDA_CHECK(cudaGraphLaunch(graph_exec, st));
+    int rc = stage(img0, img1, src_h, src_w, st);
+    if (rc == MFR_OK) rc = prepare_weights(st);
+    if (rc != MFR_OK) return rc;
+    return launch(steps, graph_exec, st);
+  }
+
+  // Encodes one map image [src_h][src_w] (eagerly) into the map buffers, which forward_shared reads until the next
+  // set_map. The pixels of the frame outside the source stay zero, as in forward.
+  int set_map(const float* img0, int src_h, int src_w, cudaStream_t st) {
+    if (!weights_loaded) return MFR_ERR_ARG;
+    if (src_h > H || src_w > W || src_h < 1 || src_w < 1) return MFR_ERR_ARG;
+    map_ready = false;
+    int rc = prepare_weights(st);
+    if (rc != MFR_OK) return rc;
+    if (src_h != H || src_w != W) MFR_CUDA_CHECK(cudaMemsetAsync(map_img, 0, static_cast<size_t>(H) * W * 4, st));
+    rc = copy_frames(map_img, img0, 1, src_h, src_w, st);
+    if (rc == MFR_OK) rc = run_steps(map_steps, st);
+    if (rc != MFR_OK) return rc;
+    map_src_h = src_h; map_src_w = src_w;
+    map_ready = true;
     return MFR_OK;
+  }
+
+  // forward(map repeated B times, img1) without encoding the map again: the same bits in every output
+  int forward_shared(const float* img1, int src_h, int src_w, cudaStream_t st) {
+    if (!weights_loaded || !map_ready || src_h != map_src_h || src_w != map_src_w) return MFR_ERR_ARG;
+    int rc = stage(nullptr, img1, src_h, src_w, st);
+    if (rc != MFR_OK) return rc;
+    return launch(shared_steps, shared_exec, st);
   }
 
   // eager run with a CUDA event pair around every step; ms[i] = device time of step i
@@ -683,6 +809,7 @@ struct LoftrEngine {
 
   ~LoftrEngine() {
     if (graph_exec) cudaGraphExecDestroy(graph_exec);
+    if (shared_exec) cudaGraphExecDestroy(shared_exec);
     for (void* p : allocs) cudaFree(p);
   }
 };
@@ -710,6 +837,7 @@ int loftr_set_weight(LoftrEngine* e, int i, const float* host, long long numel, 
   MFR_CUDA_CHECK(cudaMemcpyAsync(e->wblob + e->specs[i].offset, host, numel * 4, cudaMemcpyHostToDevice, st));
   MFR_CUDA_CHECK(cudaStreamSynchronize(st));
   e->w16_ready = false;                       // derived copies (bf16 / split operands) are rebuilt by the next forward
+  e->map_ready = false;                       // a map encoded with the old weights is stale
   if (e->weight_set.size() != e->specs.size()) e->weight_set.assign(e->specs.size(), 0);
   e->weight_set[i] = 1;
   bool all = true;
@@ -720,6 +848,12 @@ int loftr_set_weight(LoftrEngine* e, int i, const float* host, long long numel, 
 void loftr_mark_weights_loaded(LoftrEngine* e) { e->weights_loaded = true; }
 int loftr_forward(LoftrEngine* e, const float* img0, const float* img1, int src_h, int src_w, cudaStream_t st) {
   return e->forward(img0, img1, src_h, src_w, st);
+}
+int loftr_set_map(LoftrEngine* e, const float* img0, int src_h, int src_w, cudaStream_t st) {
+  return e->set_map(img0, src_h, src_w, st);
+}
+int loftr_forward_shared(LoftrEngine* e, const float* img1, int src_h, int src_w, cudaStream_t st) {
+  return e->forward_shared(img1, src_h, src_w, st);
 }
 void loftr_set_graph(LoftrEngine* e, int on) { e->use_graph = on != 0; }
 LoftrOutputs loftr_outputs(LoftrEngine* e) {

@@ -24,6 +24,8 @@ const char* loftr_weight_name(const LoftrEngine* e, int i);
 long long loftr_weight_numel(const LoftrEngine* e, int i);
 int loftr_set_weight(LoftrEngine* e, int i, const float* host, long long numel, cudaStream_t st);
 int loftr_forward(LoftrEngine* e, const float* img0, const float* img1, int src_h, int src_w, cudaStream_t st);
+int loftr_set_map(LoftrEngine* e, const float* img0, int src_h, int src_w, cudaStream_t st);
+int loftr_forward_shared(LoftrEngine* e, const float* img1, int src_h, int src_w, cudaStream_t st);
 void loftr_set_graph(LoftrEngine* e, int on);
 LoftrOutputs loftr_outputs(LoftrEngine* e);
 int loftr_debug_tensor(LoftrEngine* e, const char* name, float** ptr, long long* numel);

@@ -1401,8 +1401,18 @@ __global__ void __launch_bounds__(64) fine_gather_coarse_kernel(const float* __r
   *reinterpret_cast<float4*>(cin + (static_cast<size_t>(s) * Mcap + m) * 256 + threadIdx.x * 4) = v;
 }
 
+// dst[k][0:n16) = src[0:n16) for k = blockIdx.y (16-byte elements; grid-stride over x)
+__global__ void __launch_bounds__(256) broadcast_copies_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst,
+                                                               long long n16) {
+  uint4* d = dst + static_cast<size_t>(blockIdx.y) * n16;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n16;
+       i += static_cast<long long>(gridDim.x) * blockDim.x)
+    d[i] = src[i];
+}
+
 __global__ void __launch_bounds__(128) fine_gather_windows_kernel(
-    const float* __restrict__ featf, int B, int Hf, int Wf, int w_c, int stride,
+    const float* __restrict__ featf0, long long img_stride0, const float* __restrict__ featf1, long long img_stride1,
+    int Hf, int Wf, int w_c, int stride,
     const int* __restrict__ b_ids, const int* __restrict__ i_ids, const int* __restrict__ j_ids,
     const int* __restrict__ m_total, int Mcap, const float* __restrict__ cproj, float* __restrict__ win) {
   const int m = blockIdx.x, s = blockIdx.y;
@@ -1410,7 +1420,7 @@ __global__ void __launch_bounds__(128) fine_gather_windows_kernel(
   const int b = b_ids[m];
   const int idx = s == 0 ? i_ids[m] : j_ids[m];
   const int cy = idx / w_c, cx = idx - cy * w_c;
-  const int img = s == 0 ? b : B + b;
+  const float* featf = s == 0 ? featf0 + b * img_stride0 : featf1 + b * img_stride1;
   const int c = threadIdx.x;
   const float cp = cproj[(static_cast<size_t>(s) * Mcap + m) * 128 + c];
   float* o = win + (static_cast<size_t>(s) * Mcap + m) * 25 * 256;
@@ -1419,7 +1429,7 @@ __global__ void __launch_bounds__(128) fine_gather_windows_kernel(
     const int y = cy * stride - 2 + tap / 5, x = cx * stride - 2 + tap % 5;
     float v = 0.f;
     if (y >= 0 && y < Hf && x >= 0 && x < Wf)
-      v = featf[((static_cast<size_t>(img) * Hf + y) * Wf + x) * 128 + c];
+      v = featf[(static_cast<size_t>(y) * Wf + x) * 128 + c];
     o[tap * 256 + c] = v;
     o[tap * 256 + 128 + c] = cp;
   }
@@ -1694,6 +1704,17 @@ int rows_to_bf16(const float* src, long long lds, void* dst, long long ldd, long
   return MFR_OK;
 }
 
+int broadcast_copies(const void* src, long long bytes, void* dst, int copies, cudaStream_t st) {
+  if ((bytes & 15) || (reinterpret_cast<uintptr_t>(src) & 15) || (reinterpret_cast<uintptr_t>(dst) & 15) || copies < 1)
+    return MFR_ERR_ARG;
+  const long long n16 = bytes / 16;
+  const unsigned gx = static_cast<unsigned>(std::min<long long>((n16 + 255) / 256, std::max(1LL, static_cast<long long>(sm_count()) * 16 / copies)));
+  broadcast_copies_kernel<<<dim3(gx, static_cast<unsigned>(copies)), 256, 0, st>>>(static_cast<const uint4*>(src),
+                                                                                  static_cast<uint4*>(dst), n16);
+  MFR_CUDA_CHECK(cudaGetLastError());
+  return MFR_OK;
+}
+
 int rows_split3(const float* src, long long lds, long long src_img_stride, float* dst, long long rows_per_img,
                 int images, int C, int pattern, const int* dyn_rows, cudaStream_t st) {
   if ((C & 3) || (lds & 3) || (src_img_stride & 3) || rows_per_img <= 0 || images <= 0 || images > 65535) return MFR_ERR_ARG;
@@ -1782,14 +1803,12 @@ int fine_gather_coarse(const float* tok, long long ldt, int B, int L, const int*
   return MFR_OK;
 }
 
-int fine_gather_windows(const float* featf, int B, int Hf, int Wf, int w_c, const int* b_ids,
-                        const int* i_ids, const int* j_ids, const int* m_total, int Mcap,
-                        const float* cproj, float* win, cudaStream_t st) {
-  const int h_c_times_stride = Hf;  // stride = Hf / h_c, computed by the caller through w_c
-  (void)h_c_times_stride;
+int fine_gather_windows(const float* featf0, long long img_stride0, const float* featf1, long long img_stride1, int Hf,
+                        int Wf, int w_c, const int* b_ids, const int* i_ids, const int* j_ids, const int* m_total,
+                        int Mcap, const float* cproj, float* win, cudaStream_t st) {
   const int stride = Wf / w_c;
-  fine_gather_windows_kernel<<<dim3(Mcap, 2), 128, 0, st>>>(featf, B, Hf, Wf, w_c, stride, b_ids, i_ids,
-                                                            j_ids, m_total, Mcap, cproj, win);
+  fine_gather_windows_kernel<<<dim3(Mcap, 2), 128, 0, st>>>(featf0, img_stride0, featf1, img_stride1, Hf, Wf, w_c, stride,
+                                                            b_ids, i_ids, j_ids, m_total, Mcap, cproj, win);
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
 }

@@ -47,6 +47,9 @@ int layernorm_rows(const float* in, long long ldi, const float* gamma, const flo
 int rows_to_bf16(const float* src, long long lds, void* dst, long long ldd, long long rows, int C, const int* dyn_rows,
                  cudaStream_t st);
 
+// dst[k * bytes .. (k + 1) * bytes) = src[0 .. bytes) for k < copies (16-byte aligned, bytes a multiple of 16)
+int broadcast_copies(const void* src, long long bytes, void* dst, int copies, cudaStream_t st);
+
 // 3xTF32 operand split: dst[img][row][0:3C] = [hi | lo | hi] (pattern 0) or [hi | hi | lo] (pattern 1) of
 // src[img][row][0:C]; hi = tf32(x), lo = tf32(x - hi). Rows per image optionally capped by *dyn_rows.
 int rows_split3(const float* src, long long lds, long long src_img_stride, float* dst, long long rows_per_img,
@@ -79,10 +82,12 @@ void coarse_match_free(CoarseMatchBuffers* b);
 // cin[(s*Mcap + m), 0:256] = feat_c{s}[b, i or j, :]   (fine_preprocess.py:51-52), tokens ld = ldt
 int fine_gather_coarse(const float* tok, long long ldt, int B, int L, const int* b_ids, const int* i_ids,
                        const int* j_ids, const int* m_total, int Mcap, float* cin, cudaStream_t st);
-// win[(s*Mcap + m)*25 + tap, 0:128] = 5x5 stride-4 window of feat_f (zero padded), [128:256] = cproj
-int fine_gather_windows(const float* featf, int B, int Hf, int Wf, int w_c, const int* b_ids,
-                        const int* i_ids, const int* j_ids, const int* m_total, int Mcap,
-                        const float* cproj, float* win, cudaStream_t st);
+// win[(s*Mcap + m)*25 + tap, 0:128] = 5x5 stride-4 window of feat_f (zero padded), [128:256] = cproj.
+// Side s reads the fine map of pair b at featf_s + b * img_stride_s ([Hf][Wf][128] fp32); a stride of 0 makes every
+// pair read the same map.
+int fine_gather_windows(const float* featf0, long long img_stride0, const float* featf1, long long img_stride1, int Hf,
+                        int Wf, int w_c, const int* b_ids, const int* i_ids, const int* j_ids, const int* m_total,
+                        int Mcap, const float* cproj, float* win, cudaStream_t st);
 // fine_matching.py:43-69: expectation over the 5x5 heat map, mkpts1_f = mkpts1_c + coords * 2 * scale
 int fine_match(const float* f0, const float* f1, long long ldf, const float* mkpts1_c,
                const int* m_total, int Mcap, float scale_f, float* mkpts1_f, float* expec,

@@ -32,11 +32,19 @@ struct SpsgEngine {
   float bin_score = 1.f;
   std::vector<void*> allocs;
   std::map<std::string, std::pair<float*, long long>> dbg;
-  std::vector<std::function<int(cudaStream_t)>> steps;
+  using StepList = std::vector<std::function<int(cudaStream_t)>>;
+  StepList steps;        // the paired forward
   int launches = 0;
   size_t sg_begin = 0;   // first step of the SuperGlue part
+  // Shared map frame (set_map / forward_shared): map_steps runs SuperPoint on one image into the map_* buffers;
+  // shared_steps runs it on the B queries into the q_* buffers, interleaves map and queries into the pair layout and
+  // continues with the paired list's SuperGlue steps.
+  StepList map_steps, shared_steps;
+  int *map_counts = nullptr, *q_counts = nullptr;
+  float *map_kpts = nullptr, *map_kscores = nullptr, *map_D = nullptr, *q_kpts = nullptr, *q_kscores = nullptr, *q_D = nullptr;
+  bool map_ready = false;
   int rc = MFR_OK;
-  cudaGraphExec_t graph = nullptr;
+  cudaGraphExec_t graph = nullptr, shared_graph = nullptr;
   bool use_graph = true;
   // buffers
   float* img;
@@ -175,47 +183,55 @@ struct SpsgEngine {
     matches0 = alloc<int>(static_cast<size_t>(B) * K); mscores0 = alloc<float>(static_cast<size_t>(B) * K, "mscores0");
     mk0 = alloc<float>(static_cast<size_t>(B) * K * 2); mk1 = alloc<float>(static_cast<size_t>(B) * K * 2);
     m_offsets = alloc<int>(B + 1);
+    map_counts = alloc<int>(1); q_counts = alloc<int>(B);
+    map_kpts = alloc<float>(static_cast<size_t>(K) * 2); map_kscores = alloc<float>(K);
+    map_D = alloc<float>(static_cast<size_t>(K) * 256);
+    q_kpts = alloc<float>(static_cast<size_t>(B) * K * 2); q_kscores = alloc<float>(static_cast<size_t>(B) * K);
+    q_D = alloc<float>(static_cast<size_t>(B) * K * 256);
     if (rc != MFR_OK) return rc;
 
-    // ---- SuperPoint (superpoint.py:145-196)
+    // ---- SuperPoint (superpoint.py:145-196) on the N frames of `im` -> counts, keypoints, scores, descriptors
+    auto superpoint = [&](float* im, int N, int* counts_, float* kpts_, float* kscores_, float* D_) {
     {
-      float *w = Wp("conv1a.w"), *b = Wp("conv1a.b"), *im = img; const int n = NI, hh = H, ww = W;
+      float *w = Wp("conv1a.w"), *b = Wp("conv1a.b"); const int n = N, hh = H, ww = W;
       if (bf) push([=](cudaStream_t st) { return sp_conv1a_bf16(im, w, b, x1a, n, hh, ww, st); });
       else push([=](cudaStream_t st) { return sp_conv1a(im, w, b, x1a, n, hh, ww, st); });
     }
     auto pool = [&](float* in, float* out, int hh, int ww, int c) {
-      const int n = NI;
+      const int n = N;
       if (bf) push([=](cudaStream_t st) { return maxpool2x2_bf16(in, out, n, hh, ww, c, st); });
       else push([=](cudaStream_t st) { return maxpool2x2(in, out, n, hh, ww, c, st); });
     };
     const int b16 = bf ? 1 : 0;   // bf16 operands (and outputs, up to the heads' inputs) in bf16 mode
-    gemm("conv1b", x1a, NI, H, W, 64, 64, 64, 3, ACT_RELU, nullptr, x1b, 64, 0, b16, b16);
+    gemm("conv1b", x1a, N, H, W, 64, 64, 64, 3, ACT_RELU, nullptr, x1b, 64, 0, b16, b16);
     pool(x1b, p1, H, W, 64);
-    gemm("conv2a", p1, NI, H2, W2, 64, 64, 64, 3, ACT_RELU, nullptr, x2a, 64, 0, b16, b16);
-    gemm("conv2b", x2a, NI, H2, W2, 64, 64, 64, 3, ACT_RELU, nullptr, x2b, 64, 0, b16, b16);
+    gemm("conv2a", p1, N, H2, W2, 64, 64, 64, 3, ACT_RELU, nullptr, x2a, 64, 0, b16, b16);
+    gemm("conv2b", x2a, N, H2, W2, 64, 64, 64, 3, ACT_RELU, nullptr, x2b, 64, 0, b16, b16);
     pool(x2b, p2, H2, W2, 64);
-    gemm("conv3a", p2, NI, H4, W4, 64, 64, 128, 3, ACT_RELU, nullptr, x3a, 128, 0, b16, b16);
-    gemm("conv3b", x3a, NI, H4, W4, 128, 128, 128, 3, ACT_RELU, nullptr, x3b, 128, 0, b16, b16);
+    gemm("conv3a", p2, N, H4, W4, 64, 64, 128, 3, ACT_RELU, nullptr, x3a, 128, 0, b16, b16);
+    gemm("conv3b", x3a, N, H4, W4, 128, 128, 128, 3, ACT_RELU, nullptr, x3b, 128, 0, b16, b16);
     pool(x3b, p3, H4, W4, 128);
-    gemm("conv4a", p3, NI, h8, w8, 128, 128, 128, 3, ACT_RELU, nullptr, x4a, 128, 0, b16, b16);
-    gemm("conv4b", x4a, NI, h8, w8, 128, 128, 128, 3, ACT_RELU, nullptr, x4b, 128, 0, b16, b16);
-    gemm("convPa", x4b, NI, h8, w8, 128, 128, 256, 3, ACT_RELU, nullptr, cPa, 256, 0, b16, b16);
-    gemm("convPb", cPa, NI, h8, w8, 256, 256, 65, 1, ACT_NONE, nullptr, logits, 65, 0, b16, 0);
+    gemm("conv4a", p3, N, h8, w8, 128, 128, 128, 3, ACT_RELU, nullptr, x4a, 128, 0, b16, b16);
+    gemm("conv4b", x4a, N, h8, w8, 128, 128, 128, 3, ACT_RELU, nullptr, x4b, 128, 0, b16, b16);
+    gemm("convPa", x4b, N, h8, w8, 128, 128, 256, 3, ACT_RELU, nullptr, cPa, 256, 0, b16, b16);
+    gemm("convPb", cPa, N, h8, w8, 256, 256, 65, 1, ACT_NONE, nullptr, logits, 65, 0, b16, 0);
     {
-      const int n = NI, hh = h8, ww = w8, r = nms_r, bd = border, kk = K; const float th = kp_thr;
-      float* kp = kpts; float* ks = kscores; int* cn = counts;
+      const int n = N, hh = h8, ww = w8, r = nms_r, bd = border, kk = K; const float th = kp_thr;
+      float* kp = kpts_; float* ks = kscores_; int* cn = counts_;
       push([=](cudaStream_t st) { return sp_score_map(logits, 65, scores, n, hh, ww, st); });
       push([=](cudaStream_t st) { return sp_nms(scores, mask, t0, t1, t2, t3, n, hh * 8, ww * 8, r, st); }, 15);
       push([=](cudaStream_t st) { return sp_select_keypoints(scores, mask, n, hh * 8, ww * 8, th, bd, kk, kp, ks, cn, st); });
     }
-    gemm("convDa", x4b, NI, h8, w8, 128, 128, 256, 3, ACT_RELU, nullptr, cDa, 256, 0, b16, b16);
-    gemm("convDb", cDa, NI, h8, w8, 256, 256, 256, 1, ACT_NONE, nullptr, dense, 256, 0, b16, 0);
+    gemm("convDa", x4b, N, h8, w8, 128, 128, 256, 3, ACT_RELU, nullptr, cDa, 256, 0, b16, b16);
+    gemm("convDb", cDa, N, h8, w8, 256, 256, 256, 1, ACT_NONE, nullptr, dense, 256, 0, b16, 0);
     {
-      const int n = NI, hh = h8, ww = w8, kk = K; float* kp = kpts; int* cn = counts; float* Dp = D;
-      const size_t rws = px(h8, w8);
+      const int n = N, hh = h8, ww = w8, kk = K; float* kp = kpts_; int* cn = counts_; float* Dp = D_;
+      const size_t rws = static_cast<size_t>(N) * h8 * w8;
       push([=](cudaStream_t st) { return l2norm256(dense, rws, st); });
       push([=](cudaStream_t st) { return sp_sample_descriptors(dense, kp, cn, n, hh, ww, kk, Dp, 256, st); });
     }
+    };
+    superpoint(img, NI, counts, kpts, kscores, D);
     // ---- SuperGlue (superglue.py:228-283). Token buffer X: [NI][K][512] = [desc | message]
     sg_begin = steps.size();
     {
@@ -308,6 +324,26 @@ struct SpsgEngine {
         return sg_extract_matches(S, kk, cn, u, v, th, kp, kk, rmax, rarg, carg, m0, ms, a0, a1, mo, nb, st);
       }, 3);
     }
+    if (rc != MFR_OK) return rc;
+
+    // ---- shared map frame
+    StepList paired = std::move(steps);
+    const int paired_launches = launches;
+    steps.clear();
+    superpoint(img, 1, map_counts, map_kpts, map_kscores, map_D);   // the map image is staged in frame 0
+    map_steps = std::move(steps);
+    steps.clear();
+    superpoint(img, B, q_counts, q_kpts, q_kscores, q_D);            // the queries in frames 0 .. B-1
+    {
+      int *mc = map_counts, *qc = q_counts, *cn = counts; const int nb = B, kk = K;
+      float *mk = map_kpts, *ms = map_kscores, *md = map_D, *qk = q_kpts, *qs = q_kscores, *qd = q_D;
+      float *kp = kpts, *ks = kscores, *Dp = D;
+      push([=](cudaStream_t st) { return sp_pair_interleave(mc, mk, ms, md, qc, qk, qs, qd, nb, kk, cn, kp, ks, Dp, st); });
+    }
+    for (size_t i = sg_begin; i < paired.size(); ++i) steps.push_back(paired[i]);
+    shared_steps = std::move(steps);
+    steps = std::move(paired);
+    launches = paired_launches;
     return rc;
   }
 
@@ -334,10 +370,10 @@ struct SpsgEngine {
     }
   }
 
-  int run(cudaStream_t st) {
+  int run(const StepList& list, cudaStream_t st) {
     int r = prepare_weights(st);
     if (r != MFR_OK) return r;
-    for (auto& s : steps) { r = s(st); if (r != MFR_OK) return r; }
+    for (auto& s : list) { r = s(st); if (r != MFR_OK) return r; }
     return MFR_OK;
   }
   int prepare_weights(cudaStream_t st) {
@@ -356,34 +392,57 @@ struct SpsgEngine {
     return MFR_OK;
   }
 
+  // Runs `list` through its CUDA graph `exec`, capturing it on the first call.
+  int launch(const StepList& list, cudaGraphExec_t& exec, cudaStream_t st) {
+    { int r0 = prepare_weights(st); if (r0 != MFR_OK) return r0; }   // outside any capture
+    if (!use_graph) return run(list, st);
+    if (!exec) {
+      int r = run(list, st);
+      if (r != MFR_OK) return r;
+      MFR_CUDA_CHECK(cudaStreamSynchronize(st));
+      cudaGraph_t g;
+      MFR_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+      r = run(list, st);
+      cudaError_t e = cudaStreamEndCapture(st, &g);
+      if (r != MFR_OK || e != cudaSuccess) {
+        fprintf(stderr, "[mfr_b200] spsg graph capture failed (%d, %s); running eagerly\n", r, cudaGetErrorString(e));
+        use_graph = false;
+        cudaGetLastError();
+        return run(list, st);
+      }
+      MFR_CUDA_CHECK(cudaGraphInstantiate(&exec, g, 0));
+      cudaGraphDestroy(g);
+      return MFR_OK;
+    }
+    MFR_CUDA_CHECK(cudaGraphLaunch(exec, st));
+    return MFR_OK;
+  }
+
   // img0/img1: device [B][H][W]; copied into the pair-interleaved frame buffer
   int forward(const float* img0, const float* img1, cudaStream_t st) {
     if (!loaded) return MFR_ERR_ARG;
     const size_t hw = static_cast<size_t>(H) * W;
     MFR_CUDA_CHECK(cudaMemcpy2DAsync(img, 2 * hw * 4, img0, hw * 4, hw * 4, B, cudaMemcpyDeviceToDevice, st));
     MFR_CUDA_CHECK(cudaMemcpy2DAsync(img + hw, 2 * hw * 4, img1, hw * 4, hw * 4, B, cudaMemcpyDeviceToDevice, st));
-    { int r0 = prepare_weights(st); if (r0 != MFR_OK) return r0; }   // outside any capture
-    if (!use_graph) return run(st);
-    if (!graph) {
-      int r = run(st);
-      if (r != MFR_OK) return r;
-      MFR_CUDA_CHECK(cudaStreamSynchronize(st));
-      cudaGraph_t g;
-      MFR_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      r = run(st);
-      cudaError_t e = cudaStreamEndCapture(st, &g);
-      if (r != MFR_OK || e != cudaSuccess) {
-        fprintf(stderr, "[mfr_b200] spsg graph capture failed (%d, %s); running eagerly\n", r, cudaGetErrorString(e));
-        use_graph = false;
-        cudaGetLastError();
-        return run(st);
-      }
-      MFR_CUDA_CHECK(cudaGraphInstantiate(&graph, g, 0));
-      cudaGraphDestroy(g);
-      return MFR_OK;
-    }
-    MFR_CUDA_CHECK(cudaGraphLaunch(graph, st));
+    return launch(steps, graph, st);
+  }
+
+  // Runs SuperPoint (eagerly) on one map image [H][W]; forward_shared reads its keypoints until the next set_map.
+  int set_map(const float* img0, cudaStream_t st) {
+    if (!loaded) return MFR_ERR_ARG;
+    map_ready = false;
+    MFR_CUDA_CHECK(cudaMemcpyAsync(img, img0, static_cast<size_t>(H) * W * 4, cudaMemcpyDeviceToDevice, st));
+    int r = run(map_steps, st);
+    if (r != MFR_OK) return r;
+    map_ready = true;
     return MFR_OK;
+  }
+
+  // forward(map repeated B times, img1) without running SuperPoint on the map again: the same bits in every output
+  int forward_shared(const float* img1, cudaStream_t st) {
+    if (!loaded || !map_ready) return MFR_ERR_ARG;
+    MFR_CUDA_CHECK(cudaMemcpyAsync(img, img1, static_cast<size_t>(B) * H * W * 4, cudaMemcpyDeviceToDevice, st));
+    return launch(shared_steps, shared_graph, st);
   }
 
   // SuperGlue only, on keypoints / scores / descriptors / counts uploaded by the caller (host arrays,
@@ -405,6 +464,7 @@ struct SpsgEngine {
 
   ~SpsgEngine() {
     if (graph) cudaGraphExecDestroy(graph);
+    if (shared_graph) cudaGraphExecDestroy(shared_graph);
     for (void* p : allocs) cudaFree(p);
   }
 };
@@ -433,11 +493,14 @@ int spsg_set_weight(SpsgEngine* e, int i, const float* host, long long numel, cu
   MFR_CUDA_CHECK(cudaStreamSynchronize(st));
   e->w3_ready = false;
   e->w16_ready = false;
+  e->map_ready = false;   // a map encoded with the old weights is stale
   if (e->specs[i].name == "bin_score") e->bin_score = host[0];
   if (i == static_cast<int>(e->specs.size()) - 1) e->loaded = true;
   return MFR_OK;
 }
 int spsg_forward(SpsgEngine* e, const float* img0, const float* img1, cudaStream_t st) { return e->forward(img0, img1, st); }
+int spsg_set_map(SpsgEngine* e, const float* img0, cudaStream_t st) { return e->set_map(img0, st); }
+int spsg_forward_shared(SpsgEngine* e, const float* img1, cudaStream_t st) { return e->forward_shared(img1, st); }
 void spsg_set_graph(SpsgEngine* e, int on) { e->use_graph = on != 0; }
 SpsgOutputs spsg_outputs(SpsgEngine* e) {
   SpsgOutputs o;

@@ -27,6 +27,8 @@ const char* spsg_weight_name(const SpsgEngine* e, int i);
 long long spsg_weight_numel(const SpsgEngine* e, int i);
 int spsg_set_weight(SpsgEngine* e, int i, const float* host, long long numel, cudaStream_t st);
 int spsg_forward(SpsgEngine* e, const float* img0, const float* img1, cudaStream_t st);
+int spsg_set_map(SpsgEngine* e, const float* img0, cudaStream_t st);
+int spsg_forward_shared(SpsgEngine* e, const float* img1, cudaStream_t st);
 void spsg_set_graph(SpsgEngine* e, int on);
 SpsgOutputs spsg_outputs(SpsgEngine* e);
 int spsg_debug_tensor(SpsgEngine* e, const char* name, float** ptr, long long* numel);

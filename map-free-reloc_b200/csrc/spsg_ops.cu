@@ -617,6 +617,28 @@ __global__ void __launch_bounds__(1024) sg_matches_kernel(const int* __restrict_
   }
 }
 
+// ------------------------------------------------------------------------------------------ shared map frame
+// Pair-interleaved SuperPoint outputs from one map image and B queries: image 2b <- the map, 2b + 1 <- query b.
+// blockIdx.y = output image; x grid-strides over the image's descriptors, keypoints and scores as 16-byte elements.
+__global__ void __launch_bounds__(256) pair_interleave_kernel(
+    const int* __restrict__ m_cnt, const float4* __restrict__ m_kp, const float4* __restrict__ m_ks,
+    const float4* __restrict__ m_d, const int* __restrict__ q_cnt, const float4* __restrict__ q_kp,
+    const float4* __restrict__ q_ks, const float4* __restrict__ q_d, int max_kp, int* __restrict__ cnt,
+    float4* __restrict__ kp, float4* __restrict__ ks, float4* __restrict__ d) {
+  const int img = blockIdx.y, b = img >> 1;
+  const bool q = img & 1;
+  const int nd = max_kp * 64, nkp = max_kp / 2, nks = max_kp / 4;   // float4 per image
+  if (blockIdx.x == 0 && threadIdx.x == 0) cnt[img] = q ? q_cnt[b] : m_cnt[0];
+  const float4* sd = q ? q_d + static_cast<size_t>(b) * nd : m_d;
+  const float4* skp = q ? q_kp + static_cast<size_t>(b) * nkp : m_kp;
+  const float4* sks = q ? q_ks + static_cast<size_t>(b) * nks : m_ks;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nd + nkp + nks; i += gridDim.x * blockDim.x) {
+    if (i < nd) d[static_cast<size_t>(img) * nd + i] = sd[i];
+    else if (i < nd + nkp) kp[static_cast<size_t>(img) * nkp + i - nd] = skp[i - nd];
+    else ks[static_cast<size_t>(img) * nks + i - nd - nkp] = sks[i - nd - nkp];
+  }
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -728,6 +750,20 @@ int sg_extract_matches(const float* S, int ldS, const int* counts, const float* 
   sg_colarg_kernel<<<dim3((max_kp + 31) / 32, n_pairs), 256, 0, st>>>(S, ldS, counts, u, carg);
   sg_matches_kernel<<<1, 1024, 0, st>>>(counts, rmax, rarg, carg, thr, kpts, max_kp, matches0, mscores0, mk0, mk1,
                                         m_offsets, n_pairs);
+  MFR_CUDA_CHECK(cudaGetLastError());
+  return MFR_OK;
+}
+
+int sp_pair_interleave(const int* map_counts, const float* map_kpts, const float* map_scores, const float* map_desc,
+                       const int* q_counts, const float* q_kpts, const float* q_scores, const float* q_desc, int B, int max_kp,
+                       int* counts, float* kpts, float* scores, float* desc, cudaStream_t st) {
+  if (B < 1 || (max_kp % 4)) return MFR_ERR_ARG;
+  const int per_img = max_kp * 64 + max_kp / 2 + max_kp / 4;
+  pair_interleave_kernel<<<dim3(GRID1(per_img, 256 * 4), 2 * B), 256, 0, st>>>(
+      map_counts, reinterpret_cast<const float4*>(map_kpts), reinterpret_cast<const float4*>(map_scores),
+      reinterpret_cast<const float4*>(map_desc), q_counts, reinterpret_cast<const float4*>(q_kpts),
+      reinterpret_cast<const float4*>(q_scores), reinterpret_cast<const float4*>(q_desc), max_kp, counts,
+      reinterpret_cast<float4*>(kpts), reinterpret_cast<float4*>(scores), reinterpret_cast<float4*>(desc));
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
 }

@@ -21,6 +21,11 @@ int sp_select_keypoints(const float* scores, const float* mask, int N, int H, in
 int l2norm256(float* x, size_t rows, cudaStream_t st);
 int sp_sample_descriptors(const float* dense, const float* kpts, const int* counts, int N, int h, int w, int max_kp,
                           float* out, long long ldo, cudaStream_t st);
+// shared map frame: pair-interleaved counts [2B], kpts [2B][K][2], scores [2B][K], desc [2B][K][256] with image 2b =
+// the map's SuperPoint outputs (counts [1], kpts [K][2], ...) and image 2b + 1 = query b's (q_* [B][...])
+int sp_pair_interleave(const int* map_counts, const float* map_kpts, const float* map_scores, const float* map_desc,
+                       const int* q_counts, const float* q_kpts, const float* q_scores, const float* q_desc, int B, int max_kp,
+                       int* counts, float* kpts, float* scores, float* desc, cudaStream_t st);
 // SuperGlue
 int sg_kenc_input(const float* kpts, const float* kscores, float* out, int total, int H, int W, cudaStream_t st);
 // tensor-core attention helpers (see spsg_ops.cu): in-place row softmax of the [img][4][K][K] scores, V transpose

@@ -53,6 +53,8 @@ SIGNATURES = {
     "mfr_loftr_weight_numel": (c_ll, [c_vp, c_int]),
     "mfr_loftr_set_weight": (c_int, [c_vp, c_int, c_vp, c_ll, c_vp]),
     "mfr_loftr_forward": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_vp]),
+    "mfr_loftr_set_map": (c_int, [c_vp, c_vp, c_int, c_int, c_vp]),
+    "mfr_loftr_forward_shared": (c_int, [c_vp, c_vp, c_int, c_int, c_vp]),
     "mfr_loftr_set_graph": (None, [c_vp, c_int]),
     "mfr_loftr_get_outputs": (c_int, [c_vp, ctypes.POINTER(LoftrOutputs)]),
     "mfr_loftr_debug_tensor": (c_int, [c_vp, ctypes.c_char_p, c_pp, ctypes.POINTER(c_ll)]),
@@ -67,6 +69,8 @@ SIGNATURES = {
     "mfr_spsg_weight_numel": (c_ll, [c_vp, c_int]),
     "mfr_spsg_set_weight": (c_int, [c_vp, c_int, c_vp, c_ll, c_vp]),
     "mfr_spsg_forward": (c_int, [c_vp, c_vp, c_vp, c_vp]),
+    "mfr_spsg_set_map": (c_int, [c_vp, c_vp, c_vp]),
+    "mfr_spsg_forward_shared": (c_int, [c_vp, c_vp, c_vp]),
     "mfr_spsg_set_graph": (None, [c_vp, c_int]),
     "mfr_spsg_get_outputs": (c_int, [c_vp, ctypes.POINTER(SpsgOutputs)]),
     "mfr_spsg_debug_tensor": (c_int, [c_vp, ctypes.c_char_p, c_pp, ctypes.POINTER(c_ll)]),

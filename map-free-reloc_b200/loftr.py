@@ -400,9 +400,41 @@ class LoFTR:
             "expec_f": self._wrap(o.expec_f, (cap, 3), torch.float32),
         }
 
+    def set_map(self, img0):
+        """Encodes the map image img0 (CUDA float32 [(1,)(1,)h,w], h <= H, w <= W) once, eagerly, on the engine stream.
+        Until the next set_map or weight upload, ``forward_shared[_async](img1)`` gives the bits ``forward[_async]`` gives
+        with img0 repeated for every pair; a paired forward in between does not disturb the map."""
+        h, w = img0.shape[-2:]
+        img0 = img0.reshape(h, w).contiguous()
+        assert img0.is_cuda and img0.dtype == torch.float32
+        self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(self.stream):
+            _lib.check(self._l.mfr_loftr_set_map(self._h, _lib.ptr(img0), int(h), int(w),
+                                                 ctypes.c_void_p(self.stream.cuda_stream)), "loftr set_map")
+        img0.record_stream(self.stream)
+
+    def forward_shared_async(self, img1):
+        """Enqueues one batch of B query images [B,(1,)h,w] against the map of ``set_map`` (same h, w; else MfrError)."""
+        h, w = img1.shape[-2:]
+        img1 = img1.reshape(self.B, h, w).contiguous()
+        assert img1.is_cuda and img1.dtype == torch.float32
+        self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(self.stream):
+            _lib.check(self._l.mfr_loftr_forward_shared(self._h, _lib.ptr(img1), int(h), int(w),
+                                                        ctypes.c_void_p(self.stream.cuda_stream)), "loftr forward_shared")
+        img1.record_stream(self.stream)
+
+    def forward_shared(self, img1):
+        """forward_shared_async + the live matches, as ``forward`` returns them."""
+        self.forward_shared_async(img1)
+        return self._live_outputs()
+
     def forward(self, img0, img1):
         """Runs the batch and returns the live matches (device tensors, sliced to M)."""
         self.forward_async(img0, img1)
+        return self._live_outputs()
+
+    def _live_outputs(self):
         d = self.device_outputs()
         with torch.cuda.stream(self.stream):
             self._host_counts[:4].copy_(d["m_total"], non_blocking=True)
@@ -469,7 +501,19 @@ class LoFTR_matcher:
         from . import image_io
         im0 = image_io.read_image(pair_path[0], self.resize, True, self.engine.device)
         im1 = image_io.read_image(pair_path[1], self.resize, True, self.engine.device)
-        out = self.engine.forward(im0[None], im1[None])
+        return self._result(self.engine.forward(im0[None], im1[None]))
+
+    def match_scene(self, ref_path, query_paths):
+        """``[self.match((ref_path, q)) for q in query_paths]``, array for array, with the reference image decoded and
+        encoded once (Map-free: every pair of a scene shares its first image)."""
+        from . import image_io
+        dev = self.engine.device
+        self.engine.set_map(image_io.read_image(ref_path, self.resize, True, dev)[None])
+        return [self._result(self.engine.forward_shared(image_io.read_image(q, self.resize, True, dev)[None]))
+                for q in query_paths]
+
+    @staticmethod
+    def _result(out):
         if out["M"] > 0:
             return torch.cat([out["mkpts0_f"], out["mkpts1_f"]], 1).cpu().numpy()
         return np.full((1, 4), np.nan)
@@ -478,7 +522,4 @@ class LoFTR_matcher:
         dev = self.engine.device
         t0 = torch.from_numpy(np.ascontiguousarray(im0, dtype=np.float32))[None].to(dev)
         t1 = torch.from_numpy(np.ascontiguousarray(im1, dtype=np.float32))[None].to(dev)
-        out = self.engine.forward(t0, t1)     # padding to the engine frame happens on the device
-        if out["M"] > 0:
-            return torch.cat([out["mkpts0_f"], out["mkpts1_f"]], 1).cpu().numpy()
-        return np.full((1, 4), np.nan)
+        return self._result(self.engine.forward(t0, t1))     # padding to the engine frame happens on the device

@@ -10,7 +10,11 @@ a *stream* of pairs they are overlapped:
     solver stream : essential-matrix RANSAC + scale-from-depth of batch i-1 (reads slot (i-1) % 2)
 
 ``submit()`` enqueues a batch and returns the finished result of the batch submitted one call earlier
-(None on the first call); ``drain()`` returns the last one. Results are ``(R [B,3,3], t [B,3], inliers [B])``
+(None on the first call); ``drain()`` returns the last one.
+
+Map-free scenes match every query against one map frame. ``set_map(g0, d0, K0)`` encodes that frame once on every
+engine; ``submit_host_queries`` / ``submit_device_queries`` then copy and match only the query side, with results
+bit-identical to submitting the map frame with every pair. Results are ``(R [B,3,3], t [B,3], inliers [B])``
 float32 / int32 tensors in pinned host memory, written by an asynchronous device->host copy that is
 complete when they are handed out.
 """
@@ -52,6 +56,11 @@ class RelocPipeline:
                           for _ in range(2)]
         self.i = 0
         self._outs_all = [e.device_outputs() for e in self.engines]
+        # shared map frame: its depth / intrinsics, a generation counter bumped by set_map, and per slot the [B,...]
+        # copies the solver reads, refilled when the slot's generation is behind (the slot's last batch must be solved)
+        self.map_gen, self.map_d0, self.map_K0 = 0, None, None
+        self.ev_map = torch.cuda.Event()
+        self.map_slots = [{"d0": None, "K0": None, "gen": 0} for _ in range(2)]
 
     # ---------------------------------------------------------------- stages
     def _enqueue(self, g0, g1, d0, d1, K0, K1):
@@ -63,7 +72,10 @@ class RelocPipeline:
         outs = self._outs_all[self.i % len(self.engines)]
         if slot["busy"]:                              # the solver of batch i-2 must be done with this slot
             eng.stream.wait_event(slot["ev_solved"])
-        eng.forward_async(g0, g1)
+        if g0 is None:
+            eng.forward_shared_async(g1)
+        else:
+            eng.forward_async(g0, g1)
         with torch.cuda.stream(eng.stream):
             slot["k0"].copy_(outs["mkpts0_f"], non_blocking=True)
             slot["k1"].copy_(outs["mkpts1_f"], non_blocking=True)
@@ -91,13 +103,84 @@ class RelocPipeline:
         B = self.eng.B
         return rec[:, :9].reshape(B, 3, 3).clone(), rec[:, 9:12].clone(), rec[:, 12].to(torch.int32)
 
+    def _submit(self, g0, g1, d0, d1, K0, K1):
+        self._enqueue(g0, g1, d0, d1, K0, K1)
+        self.i += 1
+        return self._collect(self.i - 2) if self.i >= 2 else None
+
+    def _stage_copy(self, st, items):
+        for k, src in items:
+            if isinstance(src, (list, tuple)):    # one pinned tensor per pair
+                for j, row in enumerate(src):
+                    st[k][j].copy_(row, non_blocking=True)
+            else:
+                st[k].copy_(src, non_blocking=True)
+
+    def _map_inputs(self, stream):
+        """The map depth / intrinsics of this batch's slot as [B,h,w] / [B,3,3], refilled on `stream` when set_map ran
+        since the slot was last filled. `stream` must already wait for the slot's previous solve."""
+        assert self.map_d0 is not None, "call set_map before submitting queries"
+        ms = self.map_slots[self.i % 2]
+        if ms["gen"] != self.map_gen:
+            B, (h, w) = self.eng.B, self.map_d0.shape
+            if ms["d0"] is None or ms["d0"].shape[1:] != (h, w):
+                ms["d0"] = torch.empty(B, h, w, device=self.dev)
+                ms["K0"] = torch.empty(B, 3, 3, device=self.dev)
+            with torch.cuda.stream(stream):
+                stream.wait_event(self.ev_map)
+                ms["d0"].copy_(self.map_d0.expand(B, h, w), non_blocking=True)
+                ms["K0"].copy_(self.map_K0.expand(B, 3, 3), non_blocking=True)
+            for x in (self.map_d0, self.map_K0, ms["d0"], ms["K0"]):
+                x.record_stream(stream)
+            ms["gen"] = self.map_gen
+        return ms["d0"], ms["K0"]
+
     # ---------------------------------------------------------------- public
     def submit_device(self, g0, g1, d0, d1, K0, K1=None):
         """Batch already resident on the device ([B,3,3] float32 intrinsics per image; K1=None: both frames share
         K0). Returns the result of the previous batch (or None)."""
-        self._enqueue(g0, g1, d0, d1, K0, K0 if K1 is None else K1)
-        self.i += 1
-        return self._collect(self.i - 2) if self.i >= 2 else None
+        return self._submit(g0, g1, d0, d1, K0, K0 if K1 is None else K1)
+
+    def set_map(self, g0, d0, K0):
+        """Map frame of the batches submitted from now on: gray image g0 [(1,)h,w], depth d0 [(1,)h,w] and intrinsics
+        K0 [(1,)3,3], float32, on the host or the device. g0 is encoded once on every engine; batches already submitted
+        keep the map they were submitted with."""
+        cur = torch.cuda.current_stream(self.dev)
+        h, w = g0.shape[-2:]
+        g0 = g0.reshape(h, w).to(self.dev, torch.float32)
+        self.map_d0 = torch.empty(d0.shape[-2:], device=self.dev)
+        self.map_d0.copy_(d0.reshape(self.map_d0.shape))
+        self.map_K0 = torch.empty(3, 3, device=self.dev)
+        self.map_K0.copy_(K0.reshape(3, 3))
+        for e in self.engines:
+            e.set_map(g0)
+        self.ev_map.record(cur)
+        self.map_gen += 1
+
+    def submit_device_queries(self, g1, d1, K1):
+        """Query side of a batch already resident on the device (g1, d1 [B,h,w], K1 [B,3,3]), matched against the map
+        of the last set_map. Returns the result of the previous batch (or None)."""
+        slot = self.slots[self.i % 2]
+        cur = torch.cuda.current_stream(self.dev)
+        if slot["busy"]:                              # the slot's map copies are read by the solver of batch i-2
+            cur.wait_event(slot["ev_solved"])
+        d0, K0 = self._map_inputs(cur)
+        return self._submit(None, g1, d0, d1, K0, K1)
+
+    def submit_host_queries(self, g1, d1, K1):
+        """Query side of a batch in pinned host memory (as in submit_host), matched against the map of the last
+        set_map: only the queries are copied to the device."""
+        assert self.stage is not None, "construct the pipeline with depth_hw=(h, w) to feed host batches"
+        st, slot = self.stage[self.i % 2], self.slots[self.i % 2]
+        with torch.cuda.stream(self.s_copy):
+            if slot["busy"]:                          # staging tensors of batch i-2 are read by its solver
+                self.s_copy.wait_event(slot["ev_solved"])
+            self._stage_copy(st, (("g1", g1), ("d1", d1), ("K1", K1)))
+            d0, K0 = self._map_inputs(self.s_copy)
+            slot["ev_in"].record(self.s_copy)
+        self.engines[self.i % len(self.engines)].stream.wait_event(slot["ev_in"])
+        self.s_solve.wait_event(slot["ev_in"])
+        return self._submit(None, st["g1"], d0, st["d1"], K0, st["K1"])
 
     def submit_host(self, g0, g1, d0, d1, K0, K1=None):
         """Batch in pinned host memory ([B,h,w] float32 images / depths, [B,3,3] intrinsics of each frame; K1=None:
@@ -108,12 +191,8 @@ class RelocPipeline:
         with torch.cuda.stream(self.s_copy):
             if slot["busy"]:                          # staging tensors of batch i-2 are read by its solver
                 self.s_copy.wait_event(slot["ev_solved"])
-            for k, src in (("g0", g0), ("g1", g1), ("d0", d0), ("d1", d1), ("K0", K0), ("K1", K0 if K1 is None else K1)):
-                if isinstance(src, (list, tuple)):    # one pinned tensor per pair
-                    for j, row in enumerate(src):
-                        st[k][j].copy_(row, non_blocking=True)
-                else:
-                    st[k].copy_(src, non_blocking=True)
+            self._stage_copy(st, (("g0", g0), ("g1", g1), ("d0", d0), ("d1", d1), ("K0", K0),
+                                  ("K1", K0 if K1 is None else K1)))
             slot["ev_in"].record(self.s_copy)
         self.engines[self.i % len(self.engines)].stream.wait_event(slot["ev_in"])
         self.s_solve.wait_event(slot["ev_in"])

@@ -211,6 +211,33 @@ class SuperPointSuperGlue:
         img0.record_stream(self.stream)
         img1.record_stream(self.stream)
 
+    def set_map(self, img0):
+        """Runs SuperPoint once, eagerly on the engine stream, on the map image img0 (CUDA float32 [(1,)(1,)H,W]). Until
+        the next set_map, ``forward_shared[_async](img1)`` gives the bits ``forward[_async]`` gives with img0 repeated for
+        every pair; a paired forward in between does not disturb the map."""
+        img0 = img0.reshape(self.H, self.W).contiguous()
+        assert img0.is_cuda and img0.dtype == torch.float32
+        self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(self.stream):
+            _lib.check(self._l.mfr_spsg_set_map(self._h, _lib.ptr(img0), ctypes.c_void_p(self.stream.cuda_stream)),
+                       "spsg set_map")
+        img0.record_stream(self.stream)
+
+    def forward_shared_async(self, img1):
+        """Enqueues one batch of B query images [B,(1,)H,W] against the map of ``set_map``."""
+        img1 = img1.reshape(self.B, self.H, self.W).contiguous()
+        assert img1.is_cuda and img1.dtype == torch.float32
+        self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(self.stream):
+            _lib.check(self._l.mfr_spsg_forward_shared(self._h, _lib.ptr(img1), ctypes.c_void_p(self.stream.cuda_stream)),
+                       "spsg forward_shared")
+        img1.record_stream(self.stream)
+
+    def forward_shared(self, img1):
+        self.forward_shared_async(img1)
+        self.stream.synchronize()
+        return self.device_outputs()
+
     def forward_superglue(self, counts, kpts, scores, desc):
         """SuperGlue only on host numpy arrays: counts [2B] int32, kpts [2B,K,2], scores [2B,K],
         desc [2B,K,256] float32 (pair-interleaved image order)."""
@@ -262,6 +289,15 @@ class SuperGlue_matcher:
         dev = self.engine.device
         return self._result(self.engine.forward(image_io.read_image(pair_path[0], self.resize, True, dev)[None],
                                                 image_io.read_image(pair_path[1], self.resize, True, dev)[None]))
+
+    def match_scene(self, ref_path, query_paths):
+        """``[self.match((ref_path, q)) for q in query_paths]``, array for array, with the reference image decoded and
+        run through SuperPoint once (Map-free: every pair of a scene shares its first image)."""
+        from . import image_io
+        dev = self.engine.device
+        self.engine.set_map(image_io.read_image(ref_path, self.resize, True, dev)[None])
+        return [self._result(self.engine.forward_shared(image_io.read_image(q, self.resize, True, dev)[None]))
+                for q in query_paths]
 
     def match_arrays(self, im0, im1):
         dev = self.engine.device

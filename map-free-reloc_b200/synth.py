@@ -112,6 +112,29 @@ def make_pair(i, h=H, w=W, K=None):
     }
 
 
+def make_scene(seed, n_queries, h=H, w=W, K=None):
+    """A Map-free-style scene (lib/datasets/mapfree.py:148-165: every pair of a scene shares its first frame): one map
+    frame and ``n_queries`` query frames rendered from it with ``warp_forward``, each with its own ground-truth pose.
+    Drawn from ``np.random.default_rng(seed)`` in ``make_pair``'s order (depth, texture, then one pose per query), so
+    ``make_scene(1000 + i, 1)`` holds ``make_pair(i)``. Returns {"image0" [3,h,w], "gray0" [h,w] float32 in [0,1] (the
+    BT.601 gray the matchers read), "depth0", "K_color0", "queries": [{"image1", "gray1", "depth1", "K_color1", "R_gt",
+    "t_gt"}, ...]}."""
+    rng = np.random.default_rng(seed)
+    K = (K_DEFAULT if K is None else np.asarray(K, dtype=np.float64)).copy()
+    depth0 = make_depth(rng, h, w)
+    tex0 = make_texture(rng, h, w)
+    image0 = np.ascontiguousarray(tex0.transpose(2, 0, 1)).astype(np.float32) / 255.0
+    queries = []
+    for _ in range(n_queries):
+        R, t = random_pose(rng)
+        tex1, depth1 = warp_forward(tex0, depth0, R, t, K)
+        image1 = np.ascontiguousarray(tex1.transpose(2, 0, 1)).astype(np.float32) / 255.0
+        queries.append({"image1": image1, "gray1": rgb_to_gray_u8(image1).astype(np.float32) / 255.0, "depth1": depth1,
+                        "K_color1": K.astype(np.float32), "R_gt": R, "t_gt": t})
+    return {"image0": image0, "gray0": rgb_to_gray_u8(image0).astype(np.float32) / 255.0, "depth0": depth0,
+            "K_color0": K.astype(np.float32), "queries": queries}
+
+
 def rgb_to_gray_u8(img_chw):
     """OpenCV COLOR_RGB2GRAY (BT.601 fixed point) of a float [3,H,W] image in [0,1] -> uint8 [H,W]
     (reference lib/models/matching/feature_matching.py:61-65)."""

@@ -110,7 +110,8 @@ int mfr_loftr_set_map(mfr_loftr* h, const float* img0, int src_h, int src_w, voi
 int mfr_loftr_forward_shared(mfr_loftr* h, const float* img1, int src_h, int src_w, void* stream);
 void mfr_loftr_set_graph(mfr_loftr* h, int enabled);
 int mfr_loftr_get_outputs(mfr_loftr* h, mfr_loftr_outputs* out);
-/* named intermediate buffers for stage-wise parity tests ("feat_c_backbone", "feat_f", "tok", "sim", ...) */
+/* named intermediate buffers for stage-wise parity tests ("feat_c_backbone", "feat_f", "tok", "sim", ...). In every
+ * engine's *_debug_tensor, numel counts 4-byte words, whatever the buffer's element type. */
 int mfr_loftr_debug_tensor(mfr_loftr* h, const char* name, float** ptr, long long* numel);
 int mfr_loftr_num_kernels(const mfr_loftr* h);  /* steps of the launch list per forward */
 int mfr_loftr_num_launches(const mfr_loftr* h); /* kernel launches per forward */

@@ -6,6 +6,7 @@
 #include "common.cuh"
 #include "conv_gemm.cuh"
 #include "encoder_tail.cuh"
+#include "engine_core.cuh"
 #include "loftr_engine.cuh"
 #include "loftr_ops.cuh"
 #include "spsg_engine.cuh"
@@ -25,6 +26,11 @@ namespace mfr {   // metrics.cu
 int pose_metrics(const double* q_gt, const double* t_gt, const double* q_est, const double* t_est, const double* K, int W, int H,
                  int n, double* trans_err, double* rot_err, double* reproj_err, cudaStream_t st);
 }
+
+// The engine operations every engine shares (weight enumeration and upload, debug buffers, the graph switch, launch
+// counts) act on its EngineCore.
+template <class Handle>
+static mfr::EngineCore& core(const Handle* h) { return mfr::engine_core(h->e); }
 
 extern "C" {
 
@@ -82,11 +88,11 @@ void mfr_loftr_destroy(mfr_loftr* h) {
   mfr::loftr_destroy(h->e);
   delete h;
 }
-int mfr_loftr_num_weights(const mfr_loftr* h) { return mfr::loftr_num_weights(h->e); }
-const char* mfr_loftr_weight_name(const mfr_loftr* h, int i) { return mfr::loftr_weight_name(h->e, i); }
-long long mfr_loftr_weight_numel(const mfr_loftr* h, int i) { return mfr::loftr_weight_numel(h->e, i); }
+int mfr_loftr_num_weights(const mfr_loftr* h) { return core(h).weights.count(); }
+const char* mfr_loftr_weight_name(const mfr_loftr* h, int i) { return core(h).weights.name(i); }
+long long mfr_loftr_weight_numel(const mfr_loftr* h, int i) { return core(h).weights.numel(i); }
 int mfr_loftr_set_weight(mfr_loftr* h, int i, const float* host, long long numel, void* stream) {
-  return mfr::loftr_set_weight(h->e, i, host, numel, static_cast<cudaStream_t>(stream));
+  return core(h).weights.set(i, host, numel, static_cast<cudaStream_t>(stream));
 }
 int mfr_loftr_forward(mfr_loftr* h, const float* img0, const float* img1, int src_h, int src_w, void* stream) {
   return mfr::loftr_forward(h->e, img0, img1, src_h, src_w, static_cast<cudaStream_t>(stream));
@@ -99,20 +105,18 @@ int mfr_loftr_forward_shared(mfr_loftr* h, const float* img1, int src_h, int src
   if (!h || !img1) return MFR_ERR_ARG;
   return mfr::loftr_forward_shared(h->e, img1, src_h, src_w, static_cast<cudaStream_t>(stream));
 }
-void mfr_loftr_set_graph(mfr_loftr* h, int enabled) { mfr::loftr_set_graph(h->e, enabled); }
+void mfr_loftr_set_graph(mfr_loftr* h, int enabled) { if (h) core(h).use_graph = enabled != 0; }
 int mfr_loftr_get_outputs(mfr_loftr* h, mfr_loftr_outputs* out) {
   if (!h || !out) return MFR_ERR_ARG;
-  mfr::LoftrOutputs o = mfr::loftr_outputs(h->e);
-  out->m_total = o.m_total; out->m_offsets = o.m_offsets; out->b_ids = o.b_ids; out->i_ids = o.i_ids;
-  out->j_ids = o.j_ids; out->mconf = o.mconf; out->mkpts0_f = o.mkpts0_f; out->mkpts1_f = o.mkpts1_f;
-  out->mkpts1_c = o.mkpts1_c; out->expec_f = o.expec_f; out->capacity = o.capacity;
+  mfr::loftr_outputs(h->e, out);
   return MFR_OK;
 }
 int mfr_loftr_debug_tensor(mfr_loftr* h, const char* name, float** ptr, long long* numel) {
-  return mfr::loftr_debug_tensor(h->e, name, ptr, numel);
+  if (!h) return MFR_ERR_ARG;
+  return core(h).mem.debug_tensor(name, ptr, numel);
 }
-int mfr_loftr_num_kernels(const mfr_loftr* h) { return mfr::loftr_num_steps(h->e); }
-int mfr_loftr_num_launches(const mfr_loftr* h) { return mfr::loftr_num_launches(h->e); }
+int mfr_loftr_num_kernels(const mfr_loftr* h) { return core(h).steps.size(); }
+int mfr_loftr_num_launches(const mfr_loftr* h) { return core(h).steps.launches(); }
 int mfr_loftr_profile(mfr_loftr* h, const float* img0, const float* img1, int src_h, int src_w, void* stream,
                       int max_steps, float* ms, double* flops, int* kinds, char* names) {
   return mfr::loftr_profile(h->e, img0, img1, src_h, src_w, static_cast<cudaStream_t>(stream), max_steps, ms, flops,
@@ -138,11 +142,11 @@ int mfr_spsg_create(int B, int H, int W, int max_keypoints, int nms_radius, floa
                             sinkhorn_iterations, match_threshold, MFR_PRECISION_TF32, out);
 }
 void mfr_spsg_destroy(mfr_spsg* h) { if (h) { mfr::spsg_destroy(h->e); delete h; } }
-int mfr_spsg_num_weights(const mfr_spsg* h) { return mfr::spsg_num_weights(h->e); }
-const char* mfr_spsg_weight_name(const mfr_spsg* h, int i) { return mfr::spsg_weight_name(h->e, i); }
-long long mfr_spsg_weight_numel(const mfr_spsg* h, int i) { return mfr::spsg_weight_numel(h->e, i); }
+int mfr_spsg_num_weights(const mfr_spsg* h) { return core(h).weights.count(); }
+const char* mfr_spsg_weight_name(const mfr_spsg* h, int i) { return core(h).weights.name(i); }
+long long mfr_spsg_weight_numel(const mfr_spsg* h, int i) { return core(h).weights.numel(i); }
 int mfr_spsg_set_weight(mfr_spsg* h, int i, const float* host, long long numel, void* stream) {
-  return mfr::spsg_set_weight(h->e, i, host, numel, static_cast<cudaStream_t>(stream));
+  return core(h).weights.set(i, host, numel, static_cast<cudaStream_t>(stream));
 }
 int mfr_spsg_forward(mfr_spsg* h, const float* img0, const float* img1, void* stream) {
   return mfr::spsg_forward(h->e, img0, img1, static_cast<cudaStream_t>(stream));
@@ -155,19 +159,17 @@ int mfr_spsg_forward_shared(mfr_spsg* h, const float* img1, void* stream) {
   if (!h || !img1) return MFR_ERR_ARG;
   return mfr::spsg_forward_shared(h->e, img1, static_cast<cudaStream_t>(stream));
 }
-void mfr_spsg_set_graph(mfr_spsg* h, int enabled) { mfr::spsg_set_graph(h->e, enabled); }
+void mfr_spsg_set_graph(mfr_spsg* h, int enabled) { if (h) core(h).use_graph = enabled != 0; }
 int mfr_spsg_get_outputs(mfr_spsg* h, mfr_spsg_outputs* out) {
   if (!h || !out) return MFR_ERR_ARG;
-  mfr::SpsgOutputs o = mfr::spsg_outputs(h->e);
-  out->counts = o.counts; out->keypoints = o.keypoints; out->scores = o.scores; out->descriptors = o.descriptors;
-  out->desc_ld = o.desc_ld; out->matches0 = o.matches0; out->matching_scores0 = o.matching_scores0;
-  out->m_offsets = o.m_offsets; out->mkpts0 = o.mkpts0; out->mkpts1 = o.mkpts1; out->max_keypoints = o.max_keypoints;
+  mfr::spsg_outputs(h->e, out);
   return MFR_OK;
 }
 int mfr_spsg_debug_tensor(mfr_spsg* h, const char* name, float** ptr, long long* numel) {
-  return mfr::spsg_debug_tensor(h->e, name, ptr, numel);
+  if (!h) return MFR_ERR_ARG;
+  return core(h).mem.debug_tensor(name, ptr, numel);
 }
-int mfr_spsg_num_launches(const mfr_spsg* h) { return mfr::spsg_num_launches(h->e); }
+int mfr_spsg_num_launches(const mfr_spsg* h) { return core(h).steps.launches(); }
 int mfr_spsg_forward_superglue(mfr_spsg* h, const int* counts, const float* keypoints, const float* scores,
                                const float* descriptors, void* stream) {
   return mfr::spsg_forward_superglue(h->e, counts, keypoints, scores, descriptors, static_cast<cudaStream_t>(stream));
@@ -219,12 +221,10 @@ int mfr_sift_detect(mfr_sift* h, const unsigned char* imgs, void* stream) {
   if (!h) return MFR_ERR_ARG;
   return mfr::sift_detect(h->e, imgs, static_cast<cudaStream_t>(stream));
 }
-void mfr_sift_set_graph(mfr_sift* h, int enabled) { if (h) mfr::sift_set_graph(h->e, enabled); }
+void mfr_sift_set_graph(mfr_sift* h, int enabled) { if (h) core(h).use_graph = enabled != 0; }
 int mfr_sift_get_outputs(mfr_sift* h, mfr_sift_outputs* out) {
   if (!h || !out) return MFR_ERR_ARG;
-  mfr::SiftOutputs o = mfr::sift_outputs(h->e);
-  out->counts = o.counts; out->raw_counts = o.raw_counts; out->extrema_counts = o.extrema_counts;
-  out->keypoints = o.keypoints; out->octaves = o.octaves; out->descriptors = o.descriptors; out->capacity = o.capacity;
+  mfr::sift_outputs(h->e, out);
   return MFR_OK;
 }
 int mfr_sift_match_pairs(mfr_sift* h, float ratio, float* kpts0, float* kpts1, int* offsets, void* stream) {
@@ -232,8 +232,8 @@ int mfr_sift_match_pairs(mfr_sift* h, float ratio, float* kpts0, float* kpts1, i
   return mfr::sift_match_pairs(h->e, ratio, kpts0, kpts1, offsets, static_cast<cudaStream_t>(stream));
 }
 int mfr_sift_debug_tensor(mfr_sift* h, const char* name, float** ptr, long long* numel) {
-  if (!h || !name || !ptr || !numel) return MFR_ERR_ARG;
-  return mfr::sift_debug_tensor(h->e, name, ptr, numel);
+  if (!h) return MFR_ERR_ARG;
+  return core(h).mem.debug_tensor(name, ptr, numel);
 }
 int mfr_sift_profile(mfr_sift* h, const unsigned char* imgs, float* ms, void* stream) {
   if (!h) return MFR_ERR_ARG;

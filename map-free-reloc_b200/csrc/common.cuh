@@ -10,10 +10,7 @@
 #include <stdint.h>
 #include <stdio.h>
 
-#define MFR_OK 0
-#define MFR_ERR_CUDA 1
-#define MFR_ERR_ARG 2
-#define MFR_ERR_UNSUPPORTED 3
+#include "../../include/mfr_b200.h"   // MFR_OK, MFR_ERR_*
 
 #define MFR_CUDA_CHECK(expr)                                                         \
   do {                                                                               \

@@ -6,41 +6,19 @@
 #include "loftr_engine.cuh"
 
 #include <cstring>
-#include <functional>
-#include <map>
 #include <string>
 #include <vector>
 
 #include "conv_gemm.cuh"
 #include "encoder_tail.cuh"
+#include "engine_core.cuh"
 #include "loftr_ops.cuh"
 
 namespace mfr {
 
-struct WeightSpec {
-  std::string name;
-  size_t numel;
-  size_t offset;  // floats, 64-float aligned
-};
-
-struct DebugTensor {
-  float* ptr;
-  long long numel;
-};
-
-struct StepInfo {
-  std::string name;
-  int kind;             // 1 = tensor-core conv/GEMM launch, 0 = SIMT kernel(s)
-  double flops;         // algorithmic FLOPs (static part); for dyn steps: FLOPs per live row
-  const int* dyn_rows;  // device row count (per image) or null
-  int dyn_images;
-  int launches = 1;     // kernels this step launches
-};
-
-constexpr size_t kW16Capacity = static_cast<size_t>(16) * 1024 * 1024;   // bf16 weight copies (elements): ~11.5 M used
 constexpr int kReservedLayers = 4;   // conv launches at the start of the list that leave LoftrEngine::reserved_sms SMs free
 
-struct LoftrEngine {
+struct LoftrEngine : EngineCore {
   int B, H, W, NI;
   int H2, W2, H4, W4, H8, W8, L, Mcap;
   float thr, temperature;
@@ -53,37 +31,19 @@ struct LoftrEngine {
   // free (0 = use every SM).
   int reserved_sms = 0;
   int conv_count = 0;
-  struct Bf16Conv { std::string name; int cout, taps, cin, cin_pad; size_t off; };
-  std::vector<Bf16Conv> bf16_convs;
-  unsigned short* wblob16 = nullptr;
-  float* wblob3 = nullptr;     // precision 2: [hi | hi | lo] split of every GEMM weight (3 * Cin per row)
+  DerivedWeights derived{&rc};   // precision 1: bf16 GEMM weights; precision 2: their [hi | hi | lo] split
   float* x3 = nullptr;         // precision 2: scratch for the [hi | lo | hi] split of a GEMM's activations
   size_t x3_cap = 0;
-  size_t w16_total = 0;
-  bool w16_ready = false;
-
-  std::vector<WeightSpec> specs;
-  std::map<std::string, size_t> spec_index;
-  float* wblob = nullptr;
-  size_t wtotal = 0;
-  bool weights_loaded = false;
-  std::vector<char> weight_set;   // per weight tensor: uploaded at least once
   int last_src_h = -1, last_src_w = -1;
 
-  std::vector<void*> allocs;
-  std::map<std::string, DebugTensor> dbg;
-  using StepList = std::vector<std::function<int(cudaStream_t)>>;
-  StepList steps;              // the paired forward; conv() and push() append here
-  std::vector<StepInfo> infos;
+  // `steps` is the paired forward; conv() and push() append to it.
   // Shared map frame (set_map / forward_shared): map_steps encodes one image up to coarse layer 0 into the map_*
   // buffers; shared_steps runs the query half of a batch, broadcasts the map into the image-0 half and continues with
   // the paired list's own steps from coarse layer 1 on.
-  StepList map_steps, shared_steps;
+  LaunchList map_steps, shared_steps;
+  GraphExec graph, shared_graph;
   void push(const std::string& name, std::function<int(cudaStream_t)> f, int launches = 1) {
-    steps.push_back(std::move(f));
-    StepInfo inf{name, 0, 0.0, nullptr, 0};
-    inf.launches = launches;
-    infos.push_back(inf);
+    steps.push(std::move(f), name, launches);
   }
   // buffers
   float* img = nullptr;
@@ -95,7 +55,7 @@ struct LoftrEngine {
   float *featf = nullptr;
   // the encoded map frame: its [H][W] input, tokens after coarse layer 0 ([L][512], + bf16 shadow), fine map [H/2][W/2][128]
   float *map_img = nullptr, *map_tok = nullptr, *map_tokb = nullptr, *map_featf = nullptr;
-  bool map_ready = false;
+  long long map_gen = -1;   // weight generation the map was encoded with (-1: no map)
   int map_src_h = -1, map_src_w = -1;
   float* shadow(float* x) const {            // same element offset inside the shadow buffer
     if (x >= ftok && x < ftok + ftok_elems) return ftokb + (x - ftok) / 2;
@@ -105,39 +65,6 @@ struct LoftrEngine {
   CoarseMatchBuffers cm;
   float *cin, *cproj, *win, *ftok, *fqkv, *fmsg, *mk1f, *expec;
   float *fmrg = nullptr, *fh1 = nullptr, *fh2 = nullptr;   // tf32 / fp32x3 only
-  // graph
-  cudaGraphExec_t graph_exec = nullptr, shared_exec = nullptr;
-  bool use_graph = true;
-  int build_rc = MFR_OK;
-
-  float* W_(const std::string& n) {
-    auto it = spec_index.find(n);
-    if (it == spec_index.end()) {
-      fprintf(stderr, "[mfr_b200] unknown weight %s\n", n.c_str());
-      build_rc = MFR_ERR_ARG;
-      return wblob;
-    }
-    return wblob + specs[it->second].offset;
-  }
-  void add_spec(const std::string& n, size_t numel) {
-    WeightSpec s{n, numel, wtotal};
-    spec_index[n] = specs.size();
-    specs.push_back(s);
-    wtotal += (numel + 63) / 64 * 64;
-  }
-  template <typename T>
-  T* alloc(size_t n, const char* name = nullptr) {
-    void* p = nullptr;
-    if (cudaMalloc(&p, n * sizeof(T)) != cudaSuccess) {
-      fprintf(stderr, "[mfr_b200] cudaMalloc of %zu bytes failed (%s)\n", n * sizeof(T), name ? name : "");
-      build_rc = MFR_ERR_CUDA;
-      return nullptr;
-    }
-    cudaMemset(p, 0, n * sizeof(T));
-    allocs.push_back(p);
-    if (name) dbg[name] = DebugTensor{reinterpret_cast<float*>(p), static_cast<long long>(n)};
-    return reinterpret_cast<T*>(p);
-  }
 
   // ---- step builders -----------------------------------------------------------------------
   void conv(const std::string& wname, const float* x, int N, int Hh, int Ww, int Cin, long long ldx,
@@ -147,84 +74,54 @@ struct LoftrEngine {
             int w_row_off = 0) {
     ConvGemmDesc d{};
     int cin_gemm = Cin;                       // K of the GEMM per tap (3 * Cin in the 3xTF32 mode)
+    // a GEMM may use a row window [w_row_off, w_row_off + Cout) of a larger weight (q / k|v parts of qkv); cross layers
+    // ask for the same weights twice and share one derived copy
+    const long long w_rows = static_cast<long long>(w_rows_total > 0 ? w_rows_total : Cout) * R * R;
     if (precision == 2 && !in_bf16) {
       // fp32-faithful mode: A = [hi | lo | hi] of the activations (split into the scratch x3 right before the GEMM),
-      // B = [hi | hi | lo] of the weights (wblob3, built once per weight upload) -> one TF32 GEMM over 3 * Cin
+      // B = [hi | hi | lo] of the weights (derived, rebuilt after every weight upload) -> one TF32 GEMM over 3 * Cin
       const long long rows_img = static_cast<long long>(Hh) * Ww;
       if (static_cast<size_t>(N) * rows_img * 3 * Cin > x3_cap) {
         fprintf(stderr, "[mfr_b200] split scratch too small for %s\n", wname.c_str());
-        build_rc = MFR_ERR_ARG;
+        rc = MFR_ERR_ARG;
         return;
       }
       float* x3_ = x3; const float* xs = x; const int N_ = N, C_ = Cin; const long long ldx_ = ldx;
       push("split3", [=](cudaStream_t st) { return rows_split3(xs, ldx_, rows_img * ldx_, x3_, rows_img, N_, C_, 0, dyn_w, st); });
-      size_t off = w16_total;
-      bool found = false;
-      for (const auto& e : bf16_convs)
-        if (e.name == wname) { off = e.off; found = true; }
-      if (!found) {
-        const int rows_total = w_rows_total > 0 ? w_rows_total : Cout;
-        bf16_convs.push_back(Bf16Conv{wname, rows_total, R * R, Cin, 3 * Cin, off});
-        w16_total += (static_cast<size_t>(rows_total) * R * R * 3 * Cin + 63) / 64 * 64;
-      }
-      w_override = wblob3 + off + static_cast<size_t>(w_row_off) * R * R * 3 * Cin;
+      w_override = derived.get(weights, wname + ".w", w_rows, Cin, static_cast<long long>(w_row_off) * R * R);
       x = x3; ldx = 3 * Cin; cin_gemm = 3 * Cin;
     }
     d.x = x; d.N = N; d.H = Hh; d.W = Ww; d.Cin = cin_gemm; d.ldx = ldx;
     d.in_bf16 = in_bf16; d.out_bf16 = out_bf16;
     if (in_bf16) {   // bf16 copy of the weights, Cin padded to a multiple of 8 (16-byte TMA strides)
-      const int cin_pad = (Cin + 7) / 8 * 8;
-      size_t off = w16_total;
-      bool found = false;
-      for (const auto& e : bf16_convs)
-        if (e.name == wname) { off = e.off; found = true; }     // cross layers build the same weights twice
-      if (!found) {
-        // a GEMM may use a row window [w_row_off, w_row_off + Cout) of a larger weight (q / k|v parts of qkv)
-        const int rows_total = w_rows_total > 0 ? w_rows_total : Cout;
-        bf16_convs.push_back(Bf16Conv{wname, rows_total, R * R, Cin, cin_pad, off});
-        w16_total += (static_cast<size_t>(rows_total) * R * R * cin_pad + 63) / 64 * 64;
-      }
-      d.ldw = cin_pad;
-      w_override = reinterpret_cast<const float*>(wblob16 + off + static_cast<size_t>(w_row_off) * R * R * cin_pad);
+      d.ldw = derived.ld(Cin);
+      w_override = derived.get(weights, wname + ".w", w_rows, Cin, static_cast<long long>(w_row_off) * R * R);
     }
-    d.w = w_override ? w_override : W_(wname + ".w");
+    d.w = w_override ? w_override : weights[wname + ".w"];
     d.Cout = Cout; d.R = R; d.S = R; d.stride = stride; d.pad = R / 2;
     d.b_batched = 0; if (!in_bf16) d.ldw = 0; d.act_cols = act_cols; d.dyn_w = dyn_w;
-    d.bias = bias ? (bias_override ? bias_override : W_(wname + ".b")) : nullptr;
+    d.bias = bias ? (bias_override ? bias_override : weights[wname + ".b"]) : nullptr;
     d.residual = residual; d.ldr = ldo;
     d.act = act; d.alpha = 1.f; d.out = out; d.ldo = ldo;
     ConvGemmParams p;
-    int rc = conv_gemm_build(d, &p);
-    if (rc != MFR_OK) { build_rc = rc; return; }
+    const int r = conv_gemm_build(d, &p);
+    if (r != MFR_OK) { rc = r; return; }
     if (reserved_sms > 0 && conv_count < kReservedLayers) p.grid_limit = conv_gemm_num_sms() - reserved_sms;
     ++conv_count;
-    steps.push_back([p](cudaStream_t st) { return conv_gemm_launch(p, st); });
-    StepInfo inf;
-    inf.name = wname.empty() ? "qkv" : wname;
-    inf.kind = 1;
-    inf.dyn_rows = dyn_w;
-    inf.dyn_images = N;
+    Step& s = steps.push([p](cudaStream_t st) { return conv_gemm_launch(p, st); }, wname.empty() ? "qkv" : wname);
+    s.kind = 1;
+    s.dyn_rows = dyn_w;
+    s.dyn_images = N;
     const double per_pixel = 2.0 * Cout * Cin * R * R;
-    inf.flops = dyn_w ? per_pixel : per_pixel * N * p.Ho * p.Wo;
-    infos.push_back(inf);
-  }
-
-  // bf16 copy of a GEMM weight [rows][cin] in wblob16 (converted from the fp32 blob by the next forward)
-  const unsigned short* w16(const std::string& wname, int rows, int cin) {
-    for (const auto& e : bf16_convs)
-      if (e.name == wname) return wblob16 + e.off;
-    const size_t off = w16_total;
-    bf16_convs.push_back(Bf16Conv{wname, rows, 1, cin, cin, off});
-    w16_total += (static_cast<size_t>(rows) * cin + 63) / 64 * 64;
-    return wblob16 + off;
+    s.flops = dyn_w ? per_pixel : per_pixel * N * p.Ho * p.Wo;
   }
 
   void specs_backbone() {
-    add_spec("stem.w", 128 * 49);
-    add_spec("stem.b", 128);
+    weights.add("stem.w", 128 * 49);
+    weights.add("stem.b", 128);
     auto cv = [&](const std::string& n, int cin, int cout, int r, bool bias) {
-      add_spec(n + ".w", static_cast<size_t>(cout) * r * r * cin);
-      if (bias) add_spec(n + ".b", cout);
+      weights.add(n + ".w", static_cast<size_t>(cout) * r * r * cin);
+      if (bias) weights.add(n + ".b", cout);
     };
     int cin = 128;
     const int dims[3] = {128, 196, 256};
@@ -245,19 +142,19 @@ struct LoftrEngine {
     cv("layer1_outconv", 128, 196, 1, false);
     cv("layer1_outconv2.0", 196, 196, 3, true);
     cv("layer1_outconv2.3", 196, 128, 3, false);
-    add_spec("pos_enc", static_cast<size_t>(L) * 256);
+    weights.add("pos_enc", static_cast<size_t>(L) * 256);
   }
   void specs_transformer(const std::string& pre, int C, int layers) {
     for (int i = 0; i < layers; ++i) {
       const std::string p = pre + "." + std::to_string(i);
-      add_spec(p + ".qkv.w", static_cast<size_t>(3) * C * C);
-      add_spec(p + ".merge.w", static_cast<size_t>(C) * C);
-      add_spec(p + ".mlp0.w", static_cast<size_t>(4) * C * C);
-      add_spec(p + ".mlp2.w", static_cast<size_t>(2) * C * C);
-      add_spec(p + ".norm1.g", C);
-      add_spec(p + ".norm1.b", C);
-      add_spec(p + ".norm2.g", C);
-      add_spec(p + ".norm2.b", C);
+      weights.add(p + ".qkv.w", static_cast<size_t>(3) * C * C);
+      weights.add(p + ".merge.w", static_cast<size_t>(C) * C);
+      weights.add(p + ".mlp0.w", static_cast<size_t>(4) * C * C);
+      weights.add(p + ".mlp2.w", static_cast<size_t>(2) * C * C);
+      weights.add(p + ".norm1.g", C);
+      weights.add(p + ".norm1.b", C);
+      weights.add(p + ".norm2.g", C);
+      weights.add(p + ".norm2.b", C);
     }
   }
 
@@ -268,7 +165,7 @@ struct LoftrEngine {
   void encoder_layer(const std::string& p, int C, float* x, float* src, float* qkv_x, float* qkv_s,
                      float* msg_x, float* mrg_x, float* h1_x, float* h2_x, int n, int rows,
                      const int* dyn_rows, const int* dyn_items, bool windows, int kv_splits = 0) {
-    float* wq = W_(p + ".qkv.w");
+    float* wq = weights[p + ".qkv.w"];
     const long long ld2 = 2 * C, ld3 = 3 * C;
     // bf16 mode: q|k|v and the attention message are stored in bf16 — these GEMMs and the attention kernels are
     // HBM-bound — while the residual stream, LayerNorm inputs and outputs stay fp32.
@@ -309,29 +206,28 @@ struct LoftrEngine {
         });
       }
     }
-    const float *g1 = W_(p + ".norm1.g"), *b1 = W_(p + ".norm1.b");
-    const float *g2 = W_(p + ".norm2.g"), *b2 = W_(p + ".norm2.b");
+    const float *g1 = weights[p + ".norm1.g"], *b1 = weights[p + ".norm1.b"];
+    const float *g2 = weights[p + ".norm2.g"], *b2 = weights[p + ".norm2.b"];
     if (tbf) {
       // merge -> norm1 -> mlp([x | message]) -> norm2 -> residual as ONE kernel: the merge output, the norm1 output, the
       // 2C-wide hidden tensor and the mlp output never leave the SM (encoder_tail.cu)
       EncoderTailDesc d{};
       d.msg = msg_x; d.ld_msg = C; d.xb_in = xb; d.ld_xb = ld2;
-      d.w_merge = w16(p + ".merge", C, C); d.w_mlp0 = w16(p + ".mlp0", 2 * C, 2 * C); d.w_mlp2 = w16(p + ".mlp2", C, 2 * C);
+      d.w_merge = derived.get(weights, p + ".merge.w", C, C);
+      d.w_mlp0 = derived.get(weights, p + ".mlp0.w", 2 * C, 2 * C);
+      d.w_mlp2 = derived.get(weights, p + ".mlp2.w", C, 2 * C);
       d.g1 = g1; d.b1 = b1; d.g2 = g2; d.b2 = b2; d.x = x; d.ldx = ld2; d.C = C;
       if (dyn_rows) { d.n_img = n; d.rows_cap = rows; d.dyn_rows = dyn_rows; }
       else { d.n_img = 1; d.rows_cap = static_cast<long long>(n) * rows; d.dyn_rows = nullptr; }
       EncoderTailParams tp;
-      int rc = encoder_tail_build(d, &tp);
-      if (rc != MFR_OK) { build_rc = rc; return; }
-      steps.push_back([tp](cudaStream_t st) { return encoder_tail_launch(tp, st); });
-      StepInfo inf;
-      inf.name = p + ".tail";
-      inf.kind = 1;
-      inf.dyn_rows = dyn_rows;
-      inf.dyn_images = n;
+      const int r = encoder_tail_build(d, &tp);
+      if (r != MFR_OK) { rc = r; return; }
+      Step& s = steps.push([tp](cudaStream_t st) { return encoder_tail_launch(tp, st); }, p + ".tail");
+      s.kind = 1;
+      s.dyn_rows = dyn_rows;
+      s.dyn_images = n;
       const double per_row = 14.0 * C * C;      // 2 * (C*C + 2C*2C + 2C*C)
-      inf.flops = dyn_rows ? per_row : per_row * n * rows;
-      infos.push_back(inf);
+      s.flops = dyn_rows ? per_row : per_row * n * rows;
       return;
     }
     // tf32 / fp32x3: merge, norm1 into the message half of x, mlp0 on [x | message], mlp2, norm2 + residual
@@ -373,7 +269,7 @@ struct LoftrEngine {
     const int c196 = bf ? 200 : 196;
     const int B16 = bf ? 1 : 0;
     {
-      float *img_ = input, *a0_ = a0; float* ws = W_("stem.w"); float* bs = W_("stem.b");
+      float *img_ = input, *a0_ = a0; float* ws = weights["stem.w"]; float* bs = weights["stem.b"];
       const int NI_ = N, H_ = H, W_w = W, ob = B16, exact = precision == 2 ? 1 : 0;
       push("stem", [=](cudaStream_t st) { return stem_conv7x7(img_, ws, bs, a0_, NI_, H_, W_w, st, ob, exact); });
     }
@@ -415,7 +311,7 @@ struct LoftrEngine {
 
   // pos-enc add (loftr.py:58-59) of N images' 1/8 maps into token rows t (row stride 512), and its bf16 shadow
   void coarse_tokens(float* feat_c, int N, float* t) {
-    float* pe = W_("pos_enc"); const int n = N, l = L;
+    float* pe = weights["pos_enc"]; const int n = N, l = L;
     push("posenc", [=](cudaStream_t st) { return posenc_tokens(feat_c, pe, t, 512, n, l, 256, st); });
     if (precision == 1) {
       float* tb_ = shadow(t);
@@ -446,74 +342,72 @@ struct LoftrEngine {
     Mcap = B * L;
     specs_backbone();
     specs_transformer("coarse", 256, 8);
-    add_spec("fine.down_proj.w", 128 * 256);
-    add_spec("fine.down_proj.b", 128);
-    add_spec("fine.merge_feat.w", 128 * 256);
-    add_spec("fine.merge_feat.b", 128);
+    weights.add("fine.down_proj.w", 128 * 256);
+    weights.add("fine.down_proj.b", 128);
+    weights.add("fine.merge_feat.w", 128 * 256);
+    weights.add("fine.merge_feat.b", 128);
     specs_transformer("fine", 128, 2);
-    wblob = alloc<float>(wtotal, "weights");
+    weights.alloc(mem);
 
     const size_t px2 = static_cast<size_t>(NI) * H2 * W2, px4 = static_cast<size_t>(NI) * H4 * W4,
                  px8 = static_cast<size_t>(NI) * H8 * W8;
-    img = alloc<float>(static_cast<size_t>(NI) * H * W, "img");
+    img = mem.alloc<float>(static_cast<size_t>(NI) * H * W, "img");
     const bool bf = precision == 1;
     const int c196 = bf ? 200 : 196;                  // pixel stride of the 196-channel maps (16-byte rows in bf16)
     const size_t esz = bf ? 2 : 4;
     auto balloc = [&](size_t elems, const char* name) {  // backbone activation buffer (fp32 or bf16 storage)
-      return reinterpret_cast<float*>(alloc<unsigned char>(elems * esz, name));
+      return reinterpret_cast<float*>(mem.alloc<unsigned char>(elems * esz, name));
     };
-    // the bf16 weight blob must exist before the conv steps are built (its size is known only afterwards:
-    // reserve the upper bound = all backbone conv weights)
-    if (bf) wblob16 = alloc<unsigned short>(kW16Capacity, "weights_bf16");
+    if (bf) derived.alloc(mem, weights, DerivedWeights::kBf16);
     if (precision == 2) {
-      wblob3 = alloc<float>(wtotal * 3 + 64 * specs.size(), "weights_split3");
+      derived.alloc(mem, weights, DerivedWeights::kSplit3);
       const size_t frows_ = static_cast<size_t>(2) * Mcap * 25;
       x3_cap = 3 * std::max(std::max(px2 * 196, px4 * 256), std::max(px8 * 512, frows_ * 256));
-      x3 = alloc<float>(x3_cap, "split3_scratch");
+      x3 = mem.alloc<float>(x3_cap, "split3_scratch");
     }
     a0 = balloc(px2 * 128, "a0"); a1 = balloc(px2 * 128, "a1"); a2 = balloc(px2 * 128, "a2");
     b0 = balloc(px4 * c196, "b0"); b1 = balloc(px4 * c196, "b1"); b2 = balloc(px4 * c196, "b2");
     c0 = balloc(px8 * 256, "c0"); c1 = balloc(px8 * 256, "c1"); c2 = balloc(px8 * 256, "c2");
-    fc = alloc<float>(px8 * 256, "feat_c_backbone");
+    fc = mem.alloc<float>(px8 * 256, "feat_c_backbone");
     p4a = balloc(px4 * 256, "p4a"); p4b = balloc(px4 * 256, "p4b"); p4c = balloc(px4 * c196, "p4c");
     p2a = balloc(px2 * c196, "p2a"); p2b = balloc(px2 * c196, "p2b");
-    featf = alloc<float>(px2 * 128, "feat_f");
-    tok = alloc<float>(px8 * 512, "tok");
-    if (bf) tokb = reinterpret_cast<float*>(alloc<unsigned short>(px8 * 512, "tok_bf16"));
-    map_img = alloc<float>(static_cast<size_t>(H) * W, "map_img");
-    map_tok = alloc<float>(static_cast<size_t>(L) * 512, "map_tok");
-    if (bf) map_tokb = reinterpret_cast<float*>(alloc<unsigned short>(static_cast<size_t>(L) * 512, "map_tok_bf16"));
-    map_featf = alloc<float>(static_cast<size_t>(H2) * W2 * 128, "map_feat_f");
-    qkv = alloc<float>(px8 * 768, "qkv"); msg = alloc<float>(px8 * 256, "msg");
+    featf = mem.alloc<float>(px2 * 128, "feat_f");
+    tok = mem.alloc<float>(px8 * 512, "tok");
+    if (bf) tokb = reinterpret_cast<float*>(mem.alloc<unsigned short>(px8 * 512, "tok_bf16"));
+    map_img = mem.alloc<float>(static_cast<size_t>(H) * W, "map_img");
+    map_tok = mem.alloc<float>(static_cast<size_t>(L) * 512, "map_tok");
+    if (bf) map_tokb = reinterpret_cast<float*>(mem.alloc<unsigned short>(static_cast<size_t>(L) * 512, "map_tok_bf16"));
+    map_featf = mem.alloc<float>(static_cast<size_t>(H2) * W2 * 128, "map_feat_f");
+    qkv = mem.alloc<float>(px8 * 768, "qkv"); msg = mem.alloc<float>(px8 * 256, "msg");
     if (!bf) {   // the unfused encoder tail's scratch (bf16 mode runs the fused tail)
-      mrg = alloc<float>(px8 * 256, "mrg"); h1 = alloc<float>(px8 * 512, "h1"); h2 = alloc<float>(px8 * 256, "h2");
+      mrg = mem.alloc<float>(px8 * 256, "mrg"); h1 = mem.alloc<float>(px8 * 512, "h1"); h2 = mem.alloc<float>(px8 * 256, "h2");
     }
     splits_kv = std::max(1, std::min(L / 16, (2 * sm_count() + NI - 1) / NI));   // ~2 blocks per SM when all images run
-    kvp = alloc<float>(static_cast<size_t>(NI) * 8 * splits_kv * 1056, "kvp");
-    kv = alloc<float>(static_cast<size_t>(NI) * 8 * 1056, "kv");
-    S = alloc<float>(static_cast<size_t>(B) * L * L, "sim");
+    kvp = mem.alloc<float>(static_cast<size_t>(NI) * 8 * splits_kv * 1056, "kvp");
+    kv = mem.alloc<float>(static_cast<size_t>(NI) * 8 * 1056, "kv");
+    S = mem.alloc<float>(static_cast<size_t>(B) * L * L, "sim");
     const size_t BL = static_cast<size_t>(B) * L;
-    cm.row_max = alloc<float>(BL); cm.row_rsum = alloc<float>(BL);
-    cm.col_max = alloc<float>(BL); cm.col_rsum = alloc<float>(BL);
+    cm.row_max = mem.alloc<float>(BL); cm.row_rsum = mem.alloc<float>(BL);
+    cm.col_max = mem.alloc<float>(BL); cm.col_rsum = mem.alloc<float>(BL);
     splits_col = coarse_match_splits(B, L);
-    cm.col_part = alloc<float>(BL * splits_col * 2);
-    cm.rconf_max = alloc<float>(BL); cm.rconf_arg = alloc<int>(BL); cm.rconf_ties = alloc<int>(BL);
-    cm.cconf_max = alloc<float>(BL); cm.jsel = alloc<int>(BL);
-    cm.m_total = alloc<int>(4); cm.m_offsets = alloc<int>(B + 1);
-    cm.b_ids = alloc<int>(BL); cm.i_ids = alloc<int>(BL); cm.j_ids = alloc<int>(BL);
-    cm.mconf = alloc<float>(BL, "mconf"); cm.mkpts0_c = alloc<float>(BL * 2, "mkpts0_c");
-    cm.mkpts1_c = alloc<float>(BL * 2, "mkpts1_c");
+    cm.col_part = mem.alloc<float>(BL * splits_col * 2);
+    cm.rconf_max = mem.alloc<float>(BL); cm.rconf_arg = mem.alloc<int>(BL); cm.rconf_ties = mem.alloc<int>(BL);
+    cm.cconf_max = mem.alloc<float>(BL); cm.jsel = mem.alloc<int>(BL);
+    cm.m_total = mem.alloc<int>(4); cm.m_offsets = mem.alloc<int>(B + 1);
+    cm.b_ids = mem.alloc<int>(BL); cm.i_ids = mem.alloc<int>(BL); cm.j_ids = mem.alloc<int>(BL);
+    cm.mconf = mem.alloc<float>(BL, "mconf"); cm.mkpts0_c = mem.alloc<float>(BL * 2, "mkpts0_c");
+    cm.mkpts1_c = mem.alloc<float>(BL * 2, "mkpts1_c");
     const size_t frows = static_cast<size_t>(2) * Mcap * 25;
-    cin = alloc<float>(static_cast<size_t>(2) * Mcap * 256, "fine_cin");
-    cproj = alloc<float>(static_cast<size_t>(2) * Mcap * 128, "fine_cproj");
-    win = alloc<float>(frows * 256, "fine_win");
-    ftok = alloc<float>(frows * 256, "fine_tok");
+    cin = mem.alloc<float>(static_cast<size_t>(2) * Mcap * 256, "fine_cin");
+    cproj = mem.alloc<float>(static_cast<size_t>(2) * Mcap * 128, "fine_cproj");
+    win = mem.alloc<float>(frows * 256, "fine_win");
+    ftok = mem.alloc<float>(frows * 256, "fine_tok");
     ftok_elems = frows * 256;
-    if (bf) ftokb = reinterpret_cast<float*>(alloc<unsigned short>(frows * 256, "fine_tok_bf16"));
-    fqkv = alloc<float>(frows * 384, "fine_qkv"); fmsg = alloc<float>(frows * 128);
-    if (!bf) { fmrg = alloc<float>(frows * 128); fh1 = alloc<float>(frows * 256); fh2 = alloc<float>(frows * 128); }
-    mk1f = alloc<float>(BL * 2, "mkpts1_f"); expec = alloc<float>(BL * 3, "expec_f");
-    if (build_rc != MFR_OK) return build_rc;
+    if (bf) ftokb = reinterpret_cast<float*>(mem.alloc<unsigned short>(frows * 256, "fine_tok_bf16"));
+    fqkv = mem.alloc<float>(frows * 384, "fine_qkv"); fmsg = mem.alloc<float>(frows * 128);
+    if (!bf) { fmrg = mem.alloc<float>(frows * 128); fh1 = mem.alloc<float>(frows * 256); fh2 = mem.alloc<float>(frows * 128); }
+    mk1f = mem.alloc<float>(BL * 2, "mkpts1_f"); expec = mem.alloc<float>(BL * 3, "expec_f");
+    if (rc != MFR_OK) return rc;
 
     // ---------------------------------------------------------------- backbone, pos-enc, coarse layer 0
     conv_count = 0;
@@ -555,10 +449,11 @@ struct LoftrEngine {
       d.b_batched = 1; if (precision != 2) d.ldw = 512; d.act = ACT_NONE; d.alpha = 1.f / (256.f * temperature);
       d.out = S; d.ldo = L; d.ldr = L;
       ConvGemmParams p;
-      int rc = conv_gemm_build(d, &p);
-      if (rc != MFR_OK) return rc;
-      steps.push_back([p](cudaStream_t st) { return conv_gemm_launch(p, st); });
-      infos.push_back(StepInfo{"correlation", 1, 2.0 * B * static_cast<double>(L) * L * 256, nullptr, 0});
+      const int r = conv_gemm_build(d, &p);
+      if (r != MFR_OK) return r;
+      Step& s = steps.push([p](cudaStream_t st) { return conv_gemm_launch(p, st); }, "correlation");
+      s.kind = 1;
+      s.flops = 2.0 * B * static_cast<double>(L) * L * 256;
       CoarseMatchBuffers cmb = cm; float* S_ = S;
       const int B_ = B, L_ = L, hc = H8, wc = W8, bd = border, sc = splits_col; const float th = thr;
       const float scale = static_cast<float>(H) / static_cast<float>(H8);
@@ -607,18 +502,17 @@ struct LoftrEngine {
         return fine_match(f0, f1, 256, cmb.mkpts1_c, cmb.m_total, Mc, scale_f, mk, ex, st);
       });
     }
-    if (build_rc != MFR_OK) return build_rc;
+    if (rc != MFR_OK) return rc;
 
     // ---------------------------------------------------------------- shared map frame
-    StepList paired = std::move(steps);
-    std::vector<StepInfo> paired_infos = std::move(infos);
-    steps.clear(); infos.clear();
+    LaunchList paired = std::move(steps);
+    steps = LaunchList();
     conv_count = kReservedLayers;   // the map encode runs once per scene, on its own: no SMs to leave free
     backbone(map_img, 1, fc, map_featf);
     coarse_tokens(fc, 1, map_tok);
     coarse_layer0(map_tok, 1);
     map_steps = std::move(steps);
-    steps.clear(); infos.clear();
+    steps = LaunchList();
     conv_count = 0;
     const size_t half_img = static_cast<size_t>(B) * H * W;
     backbone(img + half_img, B, fc + half_c, featf + B * img_f);
@@ -633,77 +527,12 @@ struct LoftrEngine {
       }, bf ? 2 : 1);
     }
     coarse_layer0(tok + half_tok, B);
-    for (size_t i = layer1_begin; i < windows_step; ++i) steps.push_back(paired[i]);
+    steps.append(paired, layer1_begin, windows_step);
     fine_windows(map_featf, 0, featf + B * img_f, img_f);
-    for (size_t i = windows_step + 1; i < paired.size(); ++i) steps.push_back(paired[i]);
+    steps.append(paired, windows_step + 1, paired.steps.size());
     shared_steps = std::move(steps);
     steps = std::move(paired);
-    infos = std::move(paired_infos);
-
-    if (precision == 2 && w16_total > wtotal * 3 + 64 * specs.size()) {
-      fprintf(stderr, "[mfr_b200] split weight blob too small\n");
-      return MFR_ERR_ARG;
-    }
-    if (bf && w16_total > kW16Capacity) {
-      fprintf(stderr, "[mfr_b200] bf16 weight blob too small\n");
-      return MFR_ERR_ARG;
-    }
-    return build_rc;
-  }
-
-  int run_steps(const StepList& list, cudaStream_t st) {
-    for (auto& s : list) {
-      int rc = s(st);
-      if (rc != MFR_OK) return rc;
-    }
-    return MFR_OK;
-  }
-
-  // Runs `list` through its CUDA graph `exec`, capturing it on the first call.
-  int launch(const StepList& list, cudaGraphExec_t& exec, cudaStream_t st) {
-    if (!use_graph) return run_steps(list, st);
-    if (!exec) {
-      // warm (sets function attributes outside capture), then capture the launch list once
-      int rc = run_steps(list, st);
-      if (rc != MFR_OK) return rc;
-      MFR_CUDA_CHECK(cudaStreamSynchronize(st));
-      cudaGraph_t g;
-      MFR_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      rc = run_steps(list, st);
-      cudaError_t e = cudaStreamEndCapture(st, &g);
-      if (rc != MFR_OK || e != cudaSuccess) {
-        fprintf(stderr, "[mfr_b200] graph capture failed (%d, %s); running eagerly\n", rc, cudaGetErrorString(e));
-        use_graph = false;
-        cudaGetLastError();
-        return run_steps(list, st);
-      }
-      MFR_CUDA_CHECK(cudaGraphInstantiate(&exec, g, 0));
-      cudaGraphDestroy(g);
-      return MFR_OK;  // the warm-up pass above already produced this call's results
-    }
-    MFR_CUDA_CHECK(cudaGraphLaunch(exec, st));
-    return MFR_OK;
-  }
-
-  // bf16 / split copies of the weights, rebuilt after every weight upload
-  int prepare_weights(cudaStream_t st) {
-    if (precision == 1 && !w16_ready) {   // bf16 copies of the (folded) backbone conv weights
-      for (const auto& bc : bf16_convs) {
-        int rc = weights_to_bf16(W_(bc.name + ".w"), wblob16 + bc.off, static_cast<size_t>(bc.cout) * bc.taps, bc.cin,
-                                 bc.cin_pad, st);
-        if (rc != MFR_OK) return rc;
-      }
-      w16_ready = true;
-    }
-    if (precision == 2 && !w16_ready) {   // [hi | hi | lo] split of every GEMM weight
-      for (const auto& bc : bf16_convs) {
-        int rc = rows_split3(W_(bc.name + ".w"), bc.cin, 0, wblob3 + bc.off, static_cast<long long>(bc.cout) * bc.taps, 1, bc.cin,
-                             1, nullptr, st);
-        if (rc != MFR_OK) return rc;
-      }
-      w16_ready = true;
-    }
-    return MFR_OK;
+    return rc;
   }
 
   // Copies `n` source images [n][src_h][src_w] into the engine frames dst [n][H][W]; the right/bottom remainder of a
@@ -736,39 +565,39 @@ struct LoftrEngine {
 
   // src images are [B][src_h][src_w] (src_h <= H, src_w <= W), zero-padded to the engine's [H][W] frame
   int forward(const float* img0, const float* img1, int src_h, int src_w, cudaStream_t st) {
-    if (!weights_loaded) {
+    if (!weights.complete()) {
       fprintf(stderr, "[mfr_b200] loftr forward before weights were loaded\n");
       return MFR_ERR_ARG;
     }
-    int rc = stage(img0, img1, src_h, src_w, st);
-    if (rc == MFR_OK) rc = prepare_weights(st);
-    if (rc != MFR_OK) return rc;
-    return launch(steps, graph_exec, st);
+    int r = stage(img0, img1, src_h, src_w, st);
+    if (r == MFR_OK) r = derived.rebuild(weights, st);
+    if (r != MFR_OK) return r;
+    return graph.launch(steps, st, use_graph, "loftr");
   }
 
   // Encodes one map image [src_h][src_w] (eagerly) into the map buffers, which forward_shared reads until the next
-  // set_map. The pixels of the frame outside the source stay zero, as in forward.
+  // set_map or weight upload. The pixels of the frame outside the source stay zero, as in forward.
   int set_map(const float* img0, int src_h, int src_w, cudaStream_t st) {
-    if (!weights_loaded) return MFR_ERR_ARG;
+    if (!weights.complete()) return MFR_ERR_ARG;
     if (src_h > H || src_w > W || src_h < 1 || src_w < 1) return MFR_ERR_ARG;
-    map_ready = false;
-    int rc = prepare_weights(st);
-    if (rc != MFR_OK) return rc;
+    map_gen = -1;
+    int r = derived.rebuild(weights, st);
+    if (r != MFR_OK) return r;
     if (src_h != H || src_w != W) MFR_CUDA_CHECK(cudaMemsetAsync(map_img, 0, static_cast<size_t>(H) * W * 4, st));
-    rc = copy_frames(map_img, img0, 1, src_h, src_w, st);
-    if (rc == MFR_OK) rc = run_steps(map_steps, st);
-    if (rc != MFR_OK) return rc;
+    r = copy_frames(map_img, img0, 1, src_h, src_w, st);
+    if (r == MFR_OK) r = map_steps.run(st);
+    if (r != MFR_OK) return r;
     map_src_h = src_h; map_src_w = src_w;
-    map_ready = true;
+    map_gen = weights.generation;
     return MFR_OK;
   }
 
   // forward(map repeated B times, img1) without encoding the map again: the same bits in every output
   int forward_shared(const float* img1, int src_h, int src_w, cudaStream_t st) {
-    if (!weights_loaded || !map_ready || src_h != map_src_h || src_w != map_src_w) return MFR_ERR_ARG;
-    int rc = stage(nullptr, img1, src_h, src_w, st);
-    if (rc != MFR_OK) return rc;
-    return launch(shared_steps, shared_exec, st);
+    if (!weights.complete() || map_gen != weights.generation || src_h != map_src_h || src_w != map_src_w) return MFR_ERR_ARG;
+    const int r = stage(nullptr, img1, src_h, src_w, st);
+    if (r != MFR_OK) return r;
+    return shared_graph.launch(shared_steps, st, use_graph, "loftr");
   }
 
   // eager run with a CUDA event pair around every step; ms[i] = device time of step i
@@ -776,41 +605,22 @@ struct LoftrEngine {
               float* ms, double* flops, int* kinds, char* names) {
     const bool g = use_graph;
     use_graph = false;
-    int rc = forward(img0, img1, src_h, src_w, st);  // warm
-    if (rc != MFR_OK) { use_graph = g; return -rc; }
-    const int n = static_cast<int>(steps.size());
-    std::vector<cudaEvent_t> ev(n + 1);
-    for (auto& e : ev) cudaEventCreate(&e);
-    cudaEventRecord(ev[0], st);
-    for (int i = 0; i < n; ++i) {
-      rc = steps[i](st);
-      if (rc != MFR_OK) break;
-      cudaEventRecord(ev[i + 1], st);
-    }
-    cudaStreamSynchronize(st);
+    int r = forward(img0, img1, src_h, src_w, st);  // warm
+    std::vector<float> t;
+    if (r == MFR_OK) r = timed_run(steps, st, t);
+    use_graph = g;
+    if (r != MFR_OK) return -r;
     int m_total_h[4] = {0, 0, 0, 0};
     cudaMemcpy(m_total_h, cm.m_total, sizeof(m_total_h), cudaMemcpyDeviceToHost);
-    for (int i = 0; i < n && i < max_steps && rc == MFR_OK; ++i) {
-      cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]);
-      double f = infos[i].flops;
-      if (infos[i].dyn_rows) {
-        const int idx = static_cast<int>(infos[i].dyn_rows - cm.m_total);
-        f *= static_cast<double>(m_total_h[idx]) * infos[i].dyn_images;
-      }
-      flops[i] = f;
-      kinds[i] = infos[i].kind;
-      strncpy(names + 32 * i, infos[i].name.c_str(), 31);
+    for (int i = 0; i < steps.size() && i < max_steps; ++i) {
+      const Step& s = steps.steps[i];
+      ms[i] = t[i];
+      flops[i] = s.dyn_rows ? s.flops * (static_cast<double>(m_total_h[s.dyn_rows - cm.m_total]) * s.dyn_images) : s.flops;
+      kinds[i] = s.kind;
+      strncpy(names + 32 * i, s.name.c_str(), 31);
       names[32 * i + 31] = 0;
     }
-    for (auto& e : ev) cudaEventDestroy(e);
-    use_graph = g;
-    return rc == MFR_OK ? n : -rc;
-  }
-
-  ~LoftrEngine() {
-    if (graph_exec) cudaGraphExecDestroy(graph_exec);
-    if (shared_exec) cudaGraphExecDestroy(shared_exec);
-    for (void* p : allocs) cudaFree(p);
+    return steps.size();
   }
 };
 
@@ -822,30 +632,13 @@ int loftr_create(int B, int H, int W, float thr, int border, float temperature, 
   auto* e = new LoftrEngine();
   e->B = B; e->H = H; e->W = W; e->thr = thr; e->border = border; e->temperature = temperature;
   e->precision = precision; e->reserved_sms = reserved_sms;
-  int rc = e->build();
+  const int rc = e->build();
   if (rc != MFR_OK) { delete e; return rc; }
   *out = e;
   return MFR_OK;
 }
 void loftr_destroy(LoftrEngine* e) { delete e; }
-int loftr_num_weights(const LoftrEngine* e) { return static_cast<int>(e->specs.size()); }
-const char* loftr_weight_name(const LoftrEngine* e, int i) { return e->specs[i].name.c_str(); }
-long long loftr_weight_numel(const LoftrEngine* e, int i) { return static_cast<long long>(e->specs[i].numel); }
-int loftr_set_weight(LoftrEngine* e, int i, const float* host, long long numel, cudaStream_t st) {
-  if (i < 0 || i >= static_cast<int>(e->specs.size()) || numel != static_cast<long long>(e->specs[i].numel))
-    return MFR_ERR_ARG;
-  MFR_CUDA_CHECK(cudaMemcpyAsync(e->wblob + e->specs[i].offset, host, numel * 4, cudaMemcpyHostToDevice, st));
-  MFR_CUDA_CHECK(cudaStreamSynchronize(st));
-  e->w16_ready = false;                       // derived copies (bf16 / split operands) are rebuilt by the next forward
-  e->map_ready = false;                       // a map encoded with the old weights is stale
-  if (e->weight_set.size() != e->specs.size()) e->weight_set.assign(e->specs.size(), 0);
-  e->weight_set[i] = 1;
-  bool all = true;
-  for (char c : e->weight_set) all = all && c;
-  e->weights_loaded = all;                    // every tensor of the state dict has arrived
-  return MFR_OK;
-}
-void loftr_mark_weights_loaded(LoftrEngine* e) { e->weights_loaded = true; }
+EngineCore& engine_core(LoftrEngine* e) { return *e; }
 int loftr_forward(LoftrEngine* e, const float* img0, const float* img1, int src_h, int src_w, cudaStream_t st) {
   return e->forward(img0, img1, src_h, src_w, st);
 }
@@ -855,27 +648,11 @@ int loftr_set_map(LoftrEngine* e, const float* img0, int src_h, int src_w, cudaS
 int loftr_forward_shared(LoftrEngine* e, const float* img1, int src_h, int src_w, cudaStream_t st) {
   return e->forward_shared(img1, src_h, src_w, st);
 }
-void loftr_set_graph(LoftrEngine* e, int on) { e->use_graph = on != 0; }
-LoftrOutputs loftr_outputs(LoftrEngine* e) {
-  LoftrOutputs o;
-  o.m_total = e->cm.m_total; o.m_offsets = e->cm.m_offsets; o.b_ids = e->cm.b_ids;
-  o.i_ids = e->cm.i_ids; o.j_ids = e->cm.j_ids; o.mconf = e->cm.mconf;
-  o.mkpts0_f = e->cm.mkpts0_c; o.mkpts1_f = e->mk1f; o.mkpts1_c = e->cm.mkpts1_c; o.expec_f = e->expec;
-  o.capacity = e->Mcap;
-  return o;
-}
-int loftr_debug_tensor(LoftrEngine* e, const char* name, float** ptr, long long* numel) {
-  auto it = e->dbg.find(name);
-  if (it == e->dbg.end()) return MFR_ERR_ARG;
-  *ptr = it->second.ptr;
-  *numel = it->second.numel;
-  return MFR_OK;
-}
-int loftr_num_steps(const LoftrEngine* e) { return static_cast<int>(e->steps.size()); }
-int loftr_num_launches(const LoftrEngine* e) {
-  int n = 0;
-  for (const auto& i : e->infos) n += i.launches;
-  return n;
+void loftr_outputs(LoftrEngine* e, mfr_loftr_outputs* o) {
+  o->m_total = e->cm.m_total; o->m_offsets = e->cm.m_offsets; o->b_ids = e->cm.b_ids;
+  o->i_ids = e->cm.i_ids; o->j_ids = e->cm.j_ids; o->mconf = e->cm.mconf;
+  o->mkpts0_f = e->cm.mkpts0_c; o->mkpts1_f = e->mk1f; o->mkpts1_c = e->cm.mkpts1_c; o->expec_f = e->expec;
+  o->capacity = e->Mcap;
 }
 int loftr_profile(LoftrEngine* e, const float* img0, const float* img1, int src_h, int src_w, cudaStream_t st,
                   int max_steps, float* ms, double* flops, int* kinds, char* names) {

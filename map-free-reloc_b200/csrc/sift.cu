@@ -29,6 +29,7 @@
 #include <vector>
 
 #include "descriptor_match.cuh"
+#include "engine_core.cuh"
 
 namespace mfr {
 
@@ -617,16 +618,11 @@ Kernel1D gaussian_kernel(double sigma) {
 
 }  // namespace
 
-struct SiftEngine {
+// the launch list's steps are grouped by stage: pyramid, extrema + refinement, orientation, selection, descriptors
+struct SiftEngine : EngineCore {
   int B, H, W, nfeat, cap, cap2, root, nOct;
   int oh[kMaxOct], ow[kMaxOct];
-  std::vector<void*> allocs;
-  std::map<std::string, std::pair<float*, long long>> dbg;
-  struct Step { std::function<int(cudaStream_t)> f; int stage; };
-  std::vector<Step> steps;
-  int rc = MFR_OK;
-  cudaGraphExec_t graph = nullptr;
-  bool use_graph = true;
+  GraphExec graph;
   cudaStream_t own = nullptr;
   cudaEvent_t ev_in = nullptr, ev_out = nullptr;
   unsigned char* img_u8 = nullptr;
@@ -640,16 +636,7 @@ struct SiftEngine {
   // match_pairs scratch
   int *m_i1 = nullptr, *m_i2 = nullptr, *pair_n = nullptr; float *m_d1 = nullptr, *m_d2 = nullptr; unsigned char* m_good = nullptr;
 
-  template <typename T>
-  T* alloc(size_t n, const char* name = nullptr) {
-    void* p = nullptr;
-    if (cudaMalloc(&p, n * sizeof(T)) != cudaSuccess) { rc = MFR_ERR_CUDA; return nullptr; }
-    cudaMemset(p, 0, n * sizeof(T));
-    allocs.push_back(p);
-    if (name) dbg[name] = {reinterpret_cast<float*>(p), static_cast<long long>(n * sizeof(T) / 4)};
-    return reinterpret_cast<T*>(p);
-  }
-  void push(int stage, std::function<int(cudaStream_t)> f) { steps.push_back({std::move(f), stage}); }
+  void push(int stage, std::function<int(cudaStream_t)> f) { steps.push(std::move(f)).group = stage; }
   Pyr pyr() const {
     Pyr p{};
     p.n = nOct;
@@ -667,25 +654,25 @@ struct SiftEngine {
     while (cap2 < cap) cap2 <<= 1;
     oh[0] = 2 * H; ow[0] = 2 * W;
     for (int o = 1; o < nOct; ++o) { oh[o] = oh[o - 1] / 2; ow[o] = ow[o - 1] / 2; }
-    img_u8 = alloc<unsigned char>(static_cast<size_t>(B) * H * W);
-    up = alloc<float>(static_cast<size_t>(B) * oh[0] * ow[0], "upscaled");
+    img_u8 = mem.alloc<unsigned char>(static_cast<size_t>(B) * H * W);
+    up = mem.alloc<float>(static_cast<size_t>(B) * oh[0] * ow[0], "upscaled");
     for (int o = 0; o < nOct; ++o) {
       const size_t plane = static_cast<size_t>(oh[o]) * ow[o];
-      gauss[o] = alloc<float>(static_cast<size_t>(B) * kLevels * plane, ("gauss_" + std::to_string(o)).c_str());
-      dog[o] = alloc<float>(static_cast<size_t>(B) * kDogs * plane, ("dog_" + std::to_string(o)).c_str());
+      gauss[o] = mem.alloc<float>(static_cast<size_t>(B) * kLevels * plane, ("gauss_" + std::to_string(o)).c_str());
+      dog[o] = mem.alloc<float>(static_cast<size_t>(B) * kDogs * plane, ("dog_" + std::to_string(o)).c_str());
     }
-    counters = alloc<int>(3 * B, "counters");
+    counters = mem.alloc<int>(3 * B, "counters");
     const size_t bc = static_cast<size_t>(B) * cap;
-    ext_f = alloc<float4>(bc, "extrema_f"); ext_i = alloc<int4>(bc, "extrema_i");
-    kp = alloc<float>(bc * 5, "kp_pre"); kp_oct = alloc<int>(bc, "kp_pre_octave");
-    keys = alloc<unsigned long long>(static_cast<size_t>(B) * cap2); sidx = alloc<int>(static_cast<size_t>(B) * cap2);
-    rank = alloc<int>(bc);
-    out_kp = alloc<float>(bc * 5, "keypoints"); out_oct = alloc<int>(bc, "octaves"); desc = alloc<float>(bc * 128, "descriptors");
+    ext_f = mem.alloc<float4>(bc, "extrema_f"); ext_i = mem.alloc<int4>(bc, "extrema_i");
+    kp = mem.alloc<float>(bc * 5, "kp_pre"); kp_oct = mem.alloc<int>(bc, "kp_pre_octave");
+    keys = mem.alloc<unsigned long long>(static_cast<size_t>(B) * cap2); sidx = mem.alloc<int>(static_cast<size_t>(B) * cap2);
+    rank = mem.alloc<int>(bc);
+    out_kp = mem.alloc<float>(bc * 5, "keypoints"); out_oct = mem.alloc<int>(bc, "octaves"); desc = mem.alloc<float>(bc * 128, "descriptors");
     const int P = B / 2;
     if (P > 0) {
       const size_t pc = static_cast<size_t>(P) * cap;
-      m_i1 = alloc<int>(pc); m_i2 = alloc<int>(pc); m_d1 = alloc<float>(pc); m_d2 = alloc<float>(pc);
-      m_good = alloc<unsigned char>(pc); pair_n = alloc<int>(P);
+      m_i1 = mem.alloc<int>(pc); m_i2 = mem.alloc<int>(pc); m_d1 = mem.alloc<float>(pc); m_d2 = mem.alloc<float>(pc);
+      m_good = mem.alloc<unsigned char>(pc); pair_n = mem.alloc<int>(P);
     }
     if (rc != MFR_OK) return rc;
 
@@ -783,11 +770,6 @@ struct SiftEngine {
     return rc;
   }
 
-  int run(cudaStream_t st) {
-    for (auto& s : steps) { const int r = s.f(st); if (r != MFR_OK) return r; }
-    return MFR_OK;
-  }
-
   // The launch list runs on the engine's own stream, ordered after / before the caller's stream by events: a graph
   // cannot be captured on the legacy default stream a caller may pass.
   int detect(const unsigned char* imgs, cudaStream_t st) {
@@ -795,51 +777,19 @@ struct SiftEngine {
     MFR_CUDA_CHECK(cudaEventRecord(ev_in, st));
     MFR_CUDA_CHECK(cudaStreamWaitEvent(own, ev_in, 0));
     MFR_CUDA_CHECK(cudaMemcpyAsync(img_u8, imgs, static_cast<size_t>(B) * H * W, cudaMemcpyDeviceToDevice, own));
-    int r = launch(own);
+    const int r = graph.launch(steps, own, use_graph, "sift");
     if (r != MFR_OK) return r;
     MFR_CUDA_CHECK(cudaEventRecord(ev_out, own));
     MFR_CUDA_CHECK(cudaStreamWaitEvent(st, ev_out, 0));
     return MFR_OK;
   }
-  int launch(cudaStream_t st) {
-    if (!use_graph) return run(st);
-    if (!graph) {
-      int r0 = run(st);   // first run eagerly: loads every kernel before the capture
-      if (r0 != MFR_OK) return r0;
-      MFR_CUDA_CHECK(cudaStreamSynchronize(st));
-      cudaGraph_t g;
-      MFR_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      int r = run(st);
-      cudaError_t e = cudaStreamEndCapture(st, &g);
-      if (r != MFR_OK || e != cudaSuccess) {
-        fprintf(stderr, "[mfr_b200] sift graph capture failed (%d, %s); running eagerly\n", r, cudaGetErrorString(e));
-        use_graph = false;
-        cudaGetLastError();
-        return run(st);
-      }
-      MFR_CUDA_CHECK(cudaGraphInstantiate(&graph, g, 0));
-      cudaGraphDestroy(g);
-    }
-    MFR_CUDA_CHECK(cudaGraphLaunch(graph, st));
-    return MFR_OK;
-  }
-
   // eager run with an event pair around each stage: ms[5] = pyramid, extrema + refinement, orientation, selection, descriptors
   int profile(const unsigned char* imgs, float* ms, cudaStream_t st) {
     if (!imgs || !ms) return MFR_ERR_ARG;
     MFR_CUDA_CHECK(cudaMemcpyAsync(img_u8, imgs, static_cast<size_t>(B) * H * W, cudaMemcpyDeviceToDevice, st));
-    cudaEvent_t ev[6];
-    for (auto& e : ev) MFR_CUDA_CHECK(cudaEventCreate(&e));
-    int stage = 0, r = MFR_OK;
-    MFR_CUDA_CHECK(cudaEventRecord(ev[0], st));
-    for (auto& s : steps) {
-      while (stage < s.stage) MFR_CUDA_CHECK(cudaEventRecord(ev[++stage], st));
-      if ((r = s.f(st)) != MFR_OK) break;
-    }
-    while (stage < 5) MFR_CUDA_CHECK(cudaEventRecord(ev[++stage], st));
-    MFR_CUDA_CHECK(cudaEventSynchronize(ev[5]));
-    for (int i = 0; i < 5; ++i) cudaEventElapsedTime(ms + i, ev[i], ev[i + 1]);
-    for (auto& e : ev) cudaEventDestroy(e);
+    std::vector<float> t;
+    const int r = timed_run(steps, st, t);
+    if (r == MFR_OK) std::copy(t.begin(), t.end(), ms);
     return r;
   }
 
@@ -857,11 +807,9 @@ struct SiftEngine {
   }
 
   ~SiftEngine() {
-    if (graph) cudaGraphExecDestroy(graph);
     if (own) cudaStreamDestroy(own);
     if (ev_in) cudaEventDestroy(ev_in);
     if (ev_out) cudaEventDestroy(ev_out);
-    for (void* p : allocs) cudaFree(p);
   }
 };
 
@@ -875,22 +823,14 @@ int sift_create(int B, int H, int W, int nfeatures, int max_candidates, int root
   return MFR_OK;
 }
 void sift_destroy(SiftEngine* e) { delete e; }
+EngineCore& engine_core(SiftEngine* e) { return *e; }
 int sift_detect(SiftEngine* e, const unsigned char* imgs, cudaStream_t st) { return e->detect(imgs, st); }
-void sift_set_graph(SiftEngine* e, int on) { e->use_graph = on != 0; }
-SiftOutputs sift_outputs(SiftEngine* e) {
-  SiftOutputs o;
-  o.counts = e->counters + 2 * e->B; o.raw_counts = e->counters + e->B; o.extrema_counts = e->counters;
-  o.keypoints = e->out_kp; o.octaves = e->out_oct; o.descriptors = e->desc; o.capacity = e->cap;
-  return o;
+void sift_outputs(SiftEngine* e, mfr_sift_outputs* o) {
+  o->counts = e->counters + 2 * e->B; o->raw_counts = e->counters + e->B; o->extrema_counts = e->counters;
+  o->keypoints = e->out_kp; o->octaves = e->out_oct; o->descriptors = e->desc; o->capacity = e->cap;
 }
 int sift_match_pairs(SiftEngine* e, float ratio, float* kpts0, float* kpts1, int* offsets, cudaStream_t st) {
   return e->match_pairs(ratio, kpts0, kpts1, offsets, st);
-}
-int sift_debug_tensor(SiftEngine* e, const char* name, float** ptr, long long* numel) {
-  auto it = e->dbg.find(name);
-  if (it == e->dbg.end()) return MFR_ERR_ARG;
-  *ptr = it->second.first; *numel = it->second.second;
-  return MFR_OK;
 }
 int sift_profile(SiftEngine* e, const unsigned char* imgs, float* ms, cudaStream_t st) { return e->profile(imgs, ms, st); }
 

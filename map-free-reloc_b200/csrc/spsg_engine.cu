@@ -6,108 +6,66 @@
 // (image 2p = pair p's image0, 2p+1 = image1) so that the cross-attention partner is `img ^ 1`.
 #include "spsg_engine.cuh"
 
-#include <cstring>
-#include <functional>
-#include <map>
 #include <string>
-#include <vector>
 
 #include "conv_gemm.cuh"
-#include "loftr_ops.cuh"   // rows_split3 (3xTF32 operand split of the fp32-faithful mode), weights_to_bf16, rows_to_bf16
+#include "engine_core.cuh"
+#include "loftr_ops.cuh"   // rows_split3 (3xTF32 operand split of the fp32-faithful mode), rows_to_bf16
 #include "sg_attention.cuh"
 #include "spsg_ops.cuh"
 
 namespace mfr {
 
-struct SpsgEngine {
+struct SpsgEngine : EngineCore {
   int B, H, W, NI, K;  // K = max keypoints per image
   float kp_thr, match_thr;
   int nms_r, border, sk_iters;
-  struct Spec { std::string name; size_t numel, offset; };
-  std::vector<Spec> specs;
-  std::map<std::string, size_t> idx;
-  float* wblob = nullptr;
-  size_t wtotal = 0;
-  bool loaded = false;
   float bin_score = 1.f;
-  std::vector<void*> allocs;
-  std::map<std::string, std::pair<float*, long long>> dbg;
-  using StepList = std::vector<std::function<int(cudaStream_t)>>;
-  StepList steps;        // the paired forward
-  int launches = 0;
+  long long bin_gen = -1;   // weight generation bin_score was read from
   size_t sg_begin = 0;   // first step of the SuperGlue part
   // Shared map frame (set_map / forward_shared): map_steps runs SuperPoint on one image into the map_* buffers;
   // shared_steps runs it on the B queries into the q_* buffers, interleaves map and queries into the pair layout and
   // continues with the paired list's SuperGlue steps.
-  StepList map_steps, shared_steps;
+  LaunchList map_steps, shared_steps;
+  GraphExec graph, shared_graph;
   int *map_counts = nullptr, *q_counts = nullptr;
   float *map_kpts = nullptr, *map_kscores = nullptr, *map_D = nullptr, *q_kpts = nullptr, *q_kscores = nullptr, *q_D = nullptr;
-  bool map_ready = false;
-  int rc = MFR_OK;
-  cudaGraphExec_t graph = nullptr, shared_graph = nullptr;
-  bool use_graph = true;
+  long long map_gen = -1;   // weight generation the map was encoded with (-1: no map)
   // buffers
   float* img;
   float *kpts, *kscores, *X, *D, *mk0, *mk1, *mscores0;
   int *counts, *matches0, *m_offsets;
   // precision 2 (fp32-faithful, MFR_PRECISION_FP32X3): every tensor-core GEMM runs as a 3xTF32 split product over 3x the
   // K extent; A operands are split [hi | lo | hi] into the scratch x3 right before the GEMM, weights [hi | hi | lo] into
-  // wblob3 once per upload (see loftr_ops.cu: rows_split3)
+  // `derived` once per upload (see loftr_ops.cu: rows_split3)
+  // precision 1 (MFR_PRECISION_BF16): `derived` holds bf16 copies of the GEMM weights (every bf16 GEMM has a Cin that
+  // is a multiple of 8, so rows need no padding), converted once per upload
   int precision = 0;
   float* x3 = nullptr; size_t x3_cap = 0;
-  float* wblob3 = nullptr;
-  bool w3_ready = false;
-  struct W3 { std::string name; long long rows; int cin; };
-  std::vector<W3> w3_list;
-  // precision 1 (MFR_PRECISION_BF16): bf16 copy of the whole weight blob at the same offsets (every bf16 GEMM has a
-  // Cin that is a multiple of 8, so rows need no padding), converted once per upload
-  unsigned short* wblob16 = nullptr;
-  bool w16_ready = false;
+  DerivedWeights derived{&rc};
 
-  void add(const std::string& n, size_t numel) {
-    idx[n] = specs.size();
-    specs.push_back({n, numel, wtotal});
-    wtotal += (numel + 63) / 64 * 64;
-  }
-  float* Wp(const std::string& n) {
-    auto it = idx.find(n);
-    if (it == idx.end()) { fprintf(stderr, "[mfr_b200] spsg: unknown weight %s\n", n.c_str()); rc = MFR_ERR_ARG; return wblob; }
-    return wblob + specs[it->second].offset;
-  }
-  template <typename T>
-  T* alloc(size_t n, const char* name = nullptr) {
-    void* p = nullptr;
-    if (cudaMalloc(&p, n * sizeof(T)) != cudaSuccess) { rc = MFR_ERR_CUDA; return nullptr; }
-    cudaMemset(p, 0, n * sizeof(T));
-    allocs.push_back(p);
-    if (name) dbg[name] = {reinterpret_cast<float*>(p), static_cast<long long>(n)};
-    return reinterpret_cast<T*>(p);
-  }
-  void push(std::function<int(cudaStream_t)> f, int n_launch = 1) { steps.push_back(std::move(f)); launches += n_launch; }
+  void push(std::function<int(cudaStream_t)> f, int n_launch = 1) { steps.push(std::move(f), "", n_launch); }
 
   void gemm(const std::string& w, const float* x, int N, int Hh, int Ww, int Cin, long long ldx, int Cout, int R,
             int act, const float* residual, float* out, long long ldo, long long ldr = 0, int in_bf16 = 0,
             int out_bf16 = 0) {
     ConvGemmDesc d{};
     d.x = x; d.N = N; d.H = Hh; d.W = Ww; d.Cin = Cin; d.ldx = ldx;
-    d.w = Wp(w + ".w");
+    d.w = weights[w + ".w"];
     if (in_bf16) {   // bf16 x and weights (ldw = Cin); out / residual bf16 when out_bf16
       d.in_bf16 = 1; d.out_bf16 = out_bf16;
-      d.w = reinterpret_cast<const float*>(wblob16 + (d.w - wblob));
+      d.w = derived.get(weights, w + ".w", static_cast<long long>(Cout) * R * R, Cin);
     }
     if (precision == 2) {
       const long long rows_img = static_cast<long long>(Hh) * Ww;
       if (static_cast<size_t>(N) * rows_img * 3 * Cin > x3_cap || (Cin & 3)) { rc = MFR_ERR_ARG; return; }
       float* x3_ = x3; const int N_ = N, C_ = Cin;
       push([=](cudaStream_t st) { return rows_split3(x, ldx, rows_img * ldx, x3_, rows_img, N_, C_, 0, nullptr, st); });
-      bool found = false;
-      for (const auto& e : w3_list) found = found || e.name == w;
-      if (!found) w3_list.push_back(W3{w, static_cast<long long>(Cout) * R * R, Cin});
       d.x = x3; d.Cin = 3 * Cin; d.ldx = 3 * Cin;
-      d.w = wblob3 + 3 * specs[idx[w + ".w"]].offset;
+      d.w = derived.get(weights, w + ".w", static_cast<long long>(Cout) * R * R, Cin);
     }
     d.Cout = Cout; d.R = R; d.S = R; d.stride = 1; d.pad = R / 2;
-    d.bias = Wp(w + ".b"); d.residual = residual; d.ldr = ldr > 0 ? ldr : ldo; d.act = act; d.alpha = 1.f; d.out = out; d.ldo = ldo;
+    d.bias = weights[w + ".b"]; d.residual = residual; d.ldr = ldr > 0 ? ldr : ldo; d.act = act; d.alpha = 1.f; d.out = out; d.ldo = ldo;
     ConvGemmParams p;
     int r = conv_gemm_build(d, &p);
     if (r != MFR_OK) { rc = r; return; }
@@ -117,8 +75,11 @@ struct SpsgEngine {
   int build() {
     NI = 2 * B;
     // ---- weight table
-    add("conv1a.w", 64 * 9); add("conv1a.b", 64);
-    auto cv = [&](const std::string& n, int ci, int co, int r) { add(n + ".w", static_cast<size_t>(co) * r * r * ci); add(n + ".b", co); };
+    weights.add("conv1a.w", 64 * 9); weights.add("conv1a.b", 64);
+    auto cv = [&](const std::string& n, int ci, int co, int r) {
+      weights.add(n + ".w", static_cast<size_t>(co) * r * r * ci);
+      weights.add(n + ".b", co);
+    };
     cv("conv1b", 64, 64, 3); cv("conv2a", 64, 64, 3); cv("conv2b", 64, 64, 3); cv("conv3a", 64, 128, 3);
     cv("conv3b", 128, 128, 3); cv("conv4a", 128, 128, 3); cv("conv4b", 128, 128, 3);
     cv("convPa", 128, 256, 3); cv("convPb", 256, 65, 1); cv("convDa", 128, 256, 3); cv("convDb", 256, 256, 1);
@@ -128,72 +89,72 @@ struct SpsgEngine {
       cv(p + ".qkv", 256, 768, 1); cv(p + ".merge", 256, 256, 1); cv(p + ".mlp0", 512, 512, 1); cv(p + ".mlp3", 512, 256, 1);
     }
     cv("final_proj", 256, 256, 1);
-    add("bin_score", 1);
-    wblob = alloc<float>(wtotal, "weights");
+    weights.add("bin_score", 1);
+    weights.alloc(mem);
     const bool bf = precision == 1;
-    if (bf) wblob16 = alloc<unsigned short>(wtotal, "weights_bf16");
+    if (bf) derived.alloc(mem, weights, DerivedWeights::kBf16);
     if (precision == 2) {
-      wblob3 = alloc<float>(3 * wtotal, "weights_split3");
+      derived.alloc(mem, weights, DerivedWeights::kSplit3);
       const size_t act = static_cast<size_t>(2) * B * H * W * 64;                         // largest conv input (conv1b)
       const size_t att = static_cast<size_t>(2) * B * (4 * static_cast<size_t>(K) * K + 256 * static_cast<size_t>(K));   // P + V^T
       x3_cap = 3 * std::max(act, std::max(att, static_cast<size_t>(2) * B * K * 768));
-      x3 = alloc<float>(x3_cap, "split3_scratch");
+      x3 = mem.alloc<float>(x3_cap, "split3_scratch");
     }
 
     const int H2 = H / 2, W2 = W / 2, H4 = H2 / 2, W4 = W2 / 2, h8 = H4 / 2, w8 = W4 / 2;
     const int Hs = h8 * 8, Ws = w8 * 8;
     auto px = [&](int hh, int ww) { return static_cast<size_t>(NI) * hh * ww; };
-    img = alloc<float>(px(H, W), "img");
+    img = mem.alloc<float>(px(H, W), "img");
     // SuperPoint activations up to the heads' inputs: bf16 storage in bf16 mode (float-typed pointers)
     auto act = [&](size_t n, const char* name = nullptr) {
-      return bf ? reinterpret_cast<float*>(alloc<unsigned short>(n, name)) : alloc<float>(n, name);
+      return bf ? reinterpret_cast<float*>(mem.alloc<unsigned short>(n, name)) : mem.alloc<float>(n, name);
     };
     float* x1a = act(px(H, W) * 64, "x1a"); float* x1b = act(px(H, W) * 64);
     float* p1 = act(px(H2, W2) * 64); float* x2a = act(px(H2, W2) * 64); float* x2b = act(px(H2, W2) * 64);
     float* p2 = act(px(H4, W4) * 64); float* x3a = act(px(H4, W4) * 128); float* x3b = act(px(H4, W4) * 128);
     float* p3 = act(px(h8, w8) * 128); float* x4a = act(px(h8, w8) * 128); float* x4b = act(px(h8, w8) * 128, "x4b");
-    float* cPa = act(px(h8, w8) * 256); float* logits = alloc<float>(px(h8, w8) * 65, "logits");
-    float* scores = alloc<float>(px(Hs, Ws), "scores"); float* mask = alloc<float>(px(Hs, Ws), "nms_mask");
-    float* t0 = alloc<float>(px(Hs, Ws)); float* t1 = alloc<float>(px(Hs, Ws)); float* t2 = alloc<float>(px(Hs, Ws)); float* t3 = alloc<float>(px(Hs, Ws));
-    float* cDa = act(px(h8, w8) * 256); float* dense = alloc<float>(px(h8, w8) * 256, "dense_desc");
-    kpts = alloc<float>(static_cast<size_t>(NI) * K * 2, "keypoints"); kscores = alloc<float>(static_cast<size_t>(NI) * K, "kscores");
-    counts = alloc<int>(NI);
-    X = alloc<float>(static_cast<size_t>(NI) * K * 512, "tokens");
-    D = alloc<float>(static_cast<size_t>(NI) * K * 256, "descriptors");
+    float* cPa = act(px(h8, w8) * 256); float* logits = mem.alloc<float>(px(h8, w8) * 65, "logits");
+    float* scores = mem.alloc<float>(px(Hs, Ws), "scores"); float* mask = mem.alloc<float>(px(Hs, Ws), "nms_mask");
+    float* t0 = mem.alloc<float>(px(Hs, Ws)); float* t1 = mem.alloc<float>(px(Hs, Ws)); float* t2 = mem.alloc<float>(px(Hs, Ws)); float* t3 = mem.alloc<float>(px(Hs, Ws));
+    float* cDa = act(px(h8, w8) * 256); float* dense = mem.alloc<float>(px(h8, w8) * 256, "dense_desc");
+    kpts = mem.alloc<float>(static_cast<size_t>(NI) * K * 2, "keypoints"); kscores = mem.alloc<float>(static_cast<size_t>(NI) * K, "kscores");
+    counts = mem.alloc<int>(NI);
+    X = mem.alloc<float>(static_cast<size_t>(NI) * K * 512, "tokens");
+    D = mem.alloc<float>(static_cast<size_t>(NI) * K * 256, "descriptors");
     const size_t rows = static_cast<size_t>(NI) * K;
-    float* kin = alloc<float>(rows * 4); float* k1 = alloc<float>(rows * 32); float* k2 = alloc<float>(rows * 64);
-    float* k3 = alloc<float>(rows * 128); float* k4 = alloc<float>(rows * 256);
+    float* kin = mem.alloc<float>(rows * 4); float* k1 = mem.alloc<float>(rows * 32); float* k2 = mem.alloc<float>(rows * 64);
+    float* k3 = mem.alloc<float>(rows * 128); float* k4 = mem.alloc<float>(rows * 256);
     float *qkv = nullptr, *msg = nullptr, *h1 = nullptr, *Xb = nullptr, *Sat = nullptr, *Vt = nullptr;
     if (!bf) {
-      qkv = alloc<float>(rows * 768, "qkv"); msg = alloc<float>(rows * 256, "msg"); h1 = alloc<float>(rows * 512);
+      qkv = mem.alloc<float>(rows * 768, "qkv"); msg = mem.alloc<float>(rows * 256, "msg"); h1 = mem.alloc<float>(rows * 512);
     } else {   // bf16 storage: q|k|v, the attention message, the hidden layer, and the token shadow [x | message]
-      qkv = reinterpret_cast<float*>(alloc<unsigned short>(rows * 768, "qkv"));
-      msg = reinterpret_cast<float*>(alloc<unsigned short>(rows * 256, "msg"));
-      h1 = reinterpret_cast<float*>(alloc<unsigned short>(rows * 512));
-      Xb = reinterpret_cast<float*>(alloc<unsigned short>(rows * 512, "tokens_bf16"));
+      qkv = reinterpret_cast<float*>(mem.alloc<unsigned short>(rows * 768, "qkv"));
+      msg = reinterpret_cast<float*>(mem.alloc<unsigned short>(rows * 256, "msg"));
+      h1 = reinterpret_cast<float*>(mem.alloc<unsigned short>(rows * 512));
+      Xb = reinterpret_cast<float*>(mem.alloc<unsigned short>(rows * 512, "tokens_bf16"));
     }
-    float* Mb = alloc<float>(rows * 256, "mdesc");
+    float* Mb = mem.alloc<float>(rows * 256, "mdesc");
     if (!bf) {   // tensor-core attention: scores / probabilities [NI][4 heads][K][K] and V transposed [NI][256][K]
-      Sat = alloc<float>(static_cast<size_t>(NI) * 4 * K * K, "attn_scores");
-      Vt = alloc<float>(static_cast<size_t>(NI) * 256 * K, "attn_vt");
+      Sat = mem.alloc<float>(static_cast<size_t>(NI) * 4 * K * K, "attn_scores");
+      Vt = mem.alloc<float>(static_cast<size_t>(NI) * 256 * K, "attn_vt");
     }
-    float* S = alloc<float>(static_cast<size_t>(B) * K * K, "sg_scores");
-    float* u = alloc<float>(static_cast<size_t>(B) * (K + 1), "sk_u"); float* v = alloc<float>(static_cast<size_t>(B) * (K + 1), "sk_v");
-    float* rmax = alloc<float>(static_cast<size_t>(B) * K); int* rarg = alloc<int>(static_cast<size_t>(B) * K); int* carg = alloc<int>(static_cast<size_t>(B) * K);
-    matches0 = alloc<int>(static_cast<size_t>(B) * K); mscores0 = alloc<float>(static_cast<size_t>(B) * K, "mscores0");
-    mk0 = alloc<float>(static_cast<size_t>(B) * K * 2); mk1 = alloc<float>(static_cast<size_t>(B) * K * 2);
-    m_offsets = alloc<int>(B + 1);
-    map_counts = alloc<int>(1); q_counts = alloc<int>(B);
-    map_kpts = alloc<float>(static_cast<size_t>(K) * 2); map_kscores = alloc<float>(K);
-    map_D = alloc<float>(static_cast<size_t>(K) * 256);
-    q_kpts = alloc<float>(static_cast<size_t>(B) * K * 2); q_kscores = alloc<float>(static_cast<size_t>(B) * K);
-    q_D = alloc<float>(static_cast<size_t>(B) * K * 256);
+    float* S = mem.alloc<float>(static_cast<size_t>(B) * K * K, "sg_scores");
+    float* u = mem.alloc<float>(static_cast<size_t>(B) * (K + 1), "sk_u"); float* v = mem.alloc<float>(static_cast<size_t>(B) * (K + 1), "sk_v");
+    float* rmax = mem.alloc<float>(static_cast<size_t>(B) * K); int* rarg = mem.alloc<int>(static_cast<size_t>(B) * K); int* carg = mem.alloc<int>(static_cast<size_t>(B) * K);
+    matches0 = mem.alloc<int>(static_cast<size_t>(B) * K); mscores0 = mem.alloc<float>(static_cast<size_t>(B) * K, "mscores0");
+    mk0 = mem.alloc<float>(static_cast<size_t>(B) * K * 2); mk1 = mem.alloc<float>(static_cast<size_t>(B) * K * 2);
+    m_offsets = mem.alloc<int>(B + 1);
+    map_counts = mem.alloc<int>(1); q_counts = mem.alloc<int>(B);
+    map_kpts = mem.alloc<float>(static_cast<size_t>(K) * 2); map_kscores = mem.alloc<float>(K);
+    map_D = mem.alloc<float>(static_cast<size_t>(K) * 256);
+    q_kpts = mem.alloc<float>(static_cast<size_t>(B) * K * 2); q_kscores = mem.alloc<float>(static_cast<size_t>(B) * K);
+    q_D = mem.alloc<float>(static_cast<size_t>(B) * K * 256);
     if (rc != MFR_OK) return rc;
 
     // ---- SuperPoint (superpoint.py:145-196) on the N frames of `im` -> counts, keypoints, scores, descriptors
     auto superpoint = [&](float* im, int N, int* counts_, float* kpts_, float* kscores_, float* D_) {
     {
-      float *w = Wp("conv1a.w"), *b = Wp("conv1a.b"); const int n = N, hh = H, ww = W;
+      float *w = weights["conv1a.w"], *b = weights["conv1a.b"]; const int n = N, hh = H, ww = W;
       if (bf) push([=](cudaStream_t st) { return sp_conv1a_bf16(im, w, b, x1a, n, hh, ww, st); });
       else push([=](cudaStream_t st) { return sp_conv1a(im, w, b, x1a, n, hh, ww, st); });
     }
@@ -327,12 +288,11 @@ struct SpsgEngine {
     if (rc != MFR_OK) return rc;
 
     // ---- shared map frame
-    StepList paired = std::move(steps);
-    const int paired_launches = launches;
-    steps.clear();
+    LaunchList paired = std::move(steps);
+    steps = LaunchList();
     superpoint(img, 1, map_counts, map_kpts, map_kscores, map_D);   // the map image is staged in frame 0
     map_steps = std::move(steps);
-    steps.clear();
+    steps = LaunchList();
     superpoint(img, B, q_counts, q_kpts, q_kscores, q_D);            // the queries in frames 0 .. B-1
     {
       int *mc = map_counts, *qc = q_counts, *cn = counts; const int nb = B, kk = K;
@@ -340,10 +300,9 @@ struct SpsgEngine {
       float *kp = kpts, *ks = kscores, *Dp = D;
       push([=](cudaStream_t st) { return sp_pair_interleave(mc, mk, ms, md, qc, qk, qs, qd, nb, kk, cn, kp, ks, Dp, st); });
     }
-    for (size_t i = sg_begin; i < paired.size(); ++i) steps.push_back(paired[i]);
+    steps.append(paired, sg_begin, paired.steps.size());
     shared_steps = std::move(steps);
     steps = std::move(paired);
-    launches = paired_launches;
     return rc;
   }
 
@@ -370,102 +329,60 @@ struct SpsgEngine {
     }
   }
 
-  int run(const StepList& list, cudaStream_t st) {
-    int r = prepare_weights(st);
-    if (r != MFR_OK) return r;
-    for (auto& s : list) { r = s(st); if (r != MFR_OK) return r; }
-    return MFR_OK;
-  }
-  int prepare_weights(cudaStream_t st) {
-    if (precision == 1 && !w16_ready) {   // the blob is a whole number of 64-element rows
-      int r = weights_to_bf16(wblob, wblob16, wtotal / 64, 64, 64, st);
-      if (r != MFR_OK) return r;
-      w16_ready = true;
+  // brings the derived weights and bin_score up to the last upload; runs outside any capture
+  int prepare(cudaStream_t st) {
+    if (bin_gen != weights.generation) {
+      MFR_CUDA_CHECK(cudaMemcpy(&bin_score, weights["bin_score"], sizeof(float), cudaMemcpyDeviceToHost));
+      bin_gen = weights.generation;
     }
-    if (precision != 2 || w3_ready) return MFR_OK;
-    for (const auto& e : w3_list) {
-      const size_t off = specs[idx[e.name + ".w"]].offset;
-      int r = rows_split3(wblob + off, e.cin, 0, wblob3 + 3 * off, e.rows, 1, e.cin, 1, nullptr, st);
-      if (r != MFR_OK) return r;
-    }
-    w3_ready = true;
-    return MFR_OK;
-  }
-
-  // Runs `list` through its CUDA graph `exec`, capturing it on the first call.
-  int launch(const StepList& list, cudaGraphExec_t& exec, cudaStream_t st) {
-    { int r0 = prepare_weights(st); if (r0 != MFR_OK) return r0; }   // outside any capture
-    if (!use_graph) return run(list, st);
-    if (!exec) {
-      int r = run(list, st);
-      if (r != MFR_OK) return r;
-      MFR_CUDA_CHECK(cudaStreamSynchronize(st));
-      cudaGraph_t g;
-      MFR_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      r = run(list, st);
-      cudaError_t e = cudaStreamEndCapture(st, &g);
-      if (r != MFR_OK || e != cudaSuccess) {
-        fprintf(stderr, "[mfr_b200] spsg graph capture failed (%d, %s); running eagerly\n", r, cudaGetErrorString(e));
-        use_graph = false;
-        cudaGetLastError();
-        return run(list, st);
-      }
-      MFR_CUDA_CHECK(cudaGraphInstantiate(&exec, g, 0));
-      cudaGraphDestroy(g);
-      return MFR_OK;
-    }
-    MFR_CUDA_CHECK(cudaGraphLaunch(exec, st));
-    return MFR_OK;
+    return derived.rebuild(weights, st);
   }
 
   // img0/img1: device [B][H][W]; copied into the pair-interleaved frame buffer
   int forward(const float* img0, const float* img1, cudaStream_t st) {
-    if (!loaded) return MFR_ERR_ARG;
+    if (!weights.complete()) return MFR_ERR_ARG;
     const size_t hw = static_cast<size_t>(H) * W;
     MFR_CUDA_CHECK(cudaMemcpy2DAsync(img, 2 * hw * 4, img0, hw * 4, hw * 4, B, cudaMemcpyDeviceToDevice, st));
     MFR_CUDA_CHECK(cudaMemcpy2DAsync(img + hw, 2 * hw * 4, img1, hw * 4, hw * 4, B, cudaMemcpyDeviceToDevice, st));
-    return launch(steps, graph, st);
+    const int r = prepare(st);
+    if (r != MFR_OK) return r;
+    return graph.launch(steps, st, use_graph, "spsg");
   }
 
-  // Runs SuperPoint (eagerly) on one map image [H][W]; forward_shared reads its keypoints until the next set_map.
+  // Runs SuperPoint (eagerly) on one map image [H][W]; forward_shared reads its keypoints until the next set_map or
+  // weight upload.
   int set_map(const float* img0, cudaStream_t st) {
-    if (!loaded) return MFR_ERR_ARG;
-    map_ready = false;
+    if (!weights.complete()) return MFR_ERR_ARG;
+    map_gen = -1;
     MFR_CUDA_CHECK(cudaMemcpyAsync(img, img0, static_cast<size_t>(H) * W * 4, cudaMemcpyDeviceToDevice, st));
-    int r = run(map_steps, st);
+    int r = prepare(st);
+    if (r == MFR_OK) r = map_steps.run(st);
     if (r != MFR_OK) return r;
-    map_ready = true;
+    map_gen = weights.generation;
     return MFR_OK;
   }
 
   // forward(map repeated B times, img1) without running SuperPoint on the map again: the same bits in every output
   int forward_shared(const float* img1, cudaStream_t st) {
-    if (!loaded || !map_ready) return MFR_ERR_ARG;
+    if (!weights.complete() || map_gen != weights.generation) return MFR_ERR_ARG;
     MFR_CUDA_CHECK(cudaMemcpyAsync(img, img1, static_cast<size_t>(B) * H * W * 4, cudaMemcpyDeviceToDevice, st));
-    return launch(shared_steps, shared_graph, st);
+    const int r = prepare(st);
+    if (r != MFR_OK) return r;
+    return shared_graph.launch(shared_steps, st, use_graph, "spsg");
   }
 
-  // SuperGlue only, on keypoints / scores / descriptors / counts uploaded by the caller (host arrays,
-  // pair-interleaved image order) -- stage-boundary entry point for parity tests
+  // SuperGlue only (the paired list from sg_begin on), on keypoints / scores / descriptors / counts uploaded by the
+  // caller (host arrays, pair-interleaved image order) -- stage-boundary entry point for parity tests
   int forward_superglue(const int* h_counts, const float* h_kpts, const float* h_scores, const float* h_desc,
                         cudaStream_t st) {
-    if (!loaded) return MFR_ERR_ARG;
+    if (!weights.complete()) return MFR_ERR_ARG;
     MFR_CUDA_CHECK(cudaMemcpyAsync(counts, h_counts, sizeof(int) * NI, cudaMemcpyHostToDevice, st));
     MFR_CUDA_CHECK(cudaMemcpyAsync(kpts, h_kpts, sizeof(float) * NI * K * 2, cudaMemcpyHostToDevice, st));
     MFR_CUDA_CHECK(cudaMemcpyAsync(kscores, h_scores, sizeof(float) * NI * K, cudaMemcpyHostToDevice, st));
     MFR_CUDA_CHECK(cudaMemcpyAsync(D, h_desc, sizeof(float) * NI * K * 256, cudaMemcpyHostToDevice, st));
-    { int r0 = prepare_weights(st); if (r0 != MFR_OK) return r0; }
-    for (size_t i = sg_begin; i < steps.size(); ++i) {
-      int r = steps[i](st);
-      if (r != MFR_OK) return r;
-    }
-    return MFR_OK;
-  }
-
-  ~SpsgEngine() {
-    if (graph) cudaGraphExecDestroy(graph);
-    if (shared_graph) cudaGraphExecDestroy(shared_graph);
-    for (void* p : allocs) cudaFree(p);
+    const int r = prepare(st);
+    if (r != MFR_OK) return r;
+    return steps.run(st, sg_begin);
   }
 };
 
@@ -478,44 +395,21 @@ int spsg_create(int B, int H, int W, int max_kp, int nms_radius, float kp_thr, i
   e->precision = precision;
   e->B = B; e->H = H; e->W = W; e->K = max_kp; e->nms_r = nms_radius; e->kp_thr = kp_thr; e->border = border;
   e->sk_iters = sinkhorn_iters; e->match_thr = match_thr;
-  int rc = e->build();
+  const int rc = e->build();
   if (rc != MFR_OK) { delete e; return rc; }
   *out = e;
   return MFR_OK;
 }
 void spsg_destroy(SpsgEngine* e) { delete e; }
-int spsg_num_weights(const SpsgEngine* e) { return static_cast<int>(e->specs.size()); }
-const char* spsg_weight_name(const SpsgEngine* e, int i) { return e->specs[i].name.c_str(); }
-long long spsg_weight_numel(const SpsgEngine* e, int i) { return static_cast<long long>(e->specs[i].numel); }
-int spsg_set_weight(SpsgEngine* e, int i, const float* host, long long numel, cudaStream_t st) {
-  if (i < 0 || i >= static_cast<int>(e->specs.size()) || numel != static_cast<long long>(e->specs[i].numel)) return MFR_ERR_ARG;
-  MFR_CUDA_CHECK(cudaMemcpyAsync(e->wblob + e->specs[i].offset, host, numel * 4, cudaMemcpyHostToDevice, st));
-  MFR_CUDA_CHECK(cudaStreamSynchronize(st));
-  e->w3_ready = false;
-  e->w16_ready = false;
-  e->map_ready = false;   // a map encoded with the old weights is stale
-  if (e->specs[i].name == "bin_score") e->bin_score = host[0];
-  if (i == static_cast<int>(e->specs.size()) - 1) e->loaded = true;
-  return MFR_OK;
-}
+EngineCore& engine_core(SpsgEngine* e) { return *e; }
 int spsg_forward(SpsgEngine* e, const float* img0, const float* img1, cudaStream_t st) { return e->forward(img0, img1, st); }
 int spsg_set_map(SpsgEngine* e, const float* img0, cudaStream_t st) { return e->set_map(img0, st); }
 int spsg_forward_shared(SpsgEngine* e, const float* img1, cudaStream_t st) { return e->forward_shared(img1, st); }
-void spsg_set_graph(SpsgEngine* e, int on) { e->use_graph = on != 0; }
-SpsgOutputs spsg_outputs(SpsgEngine* e) {
-  SpsgOutputs o;
-  o.counts = e->counts; o.keypoints = e->kpts; o.scores = e->kscores; o.descriptors = e->D; o.desc_ld = 256;
-  o.matches0 = e->matches0; o.matching_scores0 = e->mscores0; o.m_offsets = e->m_offsets; o.mkpts0 = e->mk0;
-  o.mkpts1 = e->mk1; o.max_keypoints = e->K;
-  return o;
+void spsg_outputs(SpsgEngine* e, mfr_spsg_outputs* o) {
+  o->counts = e->counts; o->keypoints = e->kpts; o->scores = e->kscores; o->descriptors = e->D; o->desc_ld = 256;
+  o->matches0 = e->matches0; o->matching_scores0 = e->mscores0; o->m_offsets = e->m_offsets; o->mkpts0 = e->mk0;
+  o->mkpts1 = e->mk1; o->max_keypoints = e->K;
 }
-int spsg_debug_tensor(SpsgEngine* e, const char* name, float** ptr, long long* numel) {
-  auto it = e->dbg.find(name);
-  if (it == e->dbg.end()) return MFR_ERR_ARG;
-  *ptr = it->second.first; *numel = it->second.second;
-  return MFR_OK;
-}
-int spsg_num_launches(const SpsgEngine* e) { return e->launches; }
 int spsg_forward_superglue(SpsgEngine* e, const int* counts, const float* kpts, const float* scores, const float* desc,
                            cudaStream_t st) {
   return e->forward_superglue(counts, kpts, scores, desc, st);

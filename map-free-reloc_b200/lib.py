@@ -1,6 +1,7 @@
 """ctypes binding of libmfr_b200.so. There is NO CPU fallback: if the library is missing or a
 CUDA device is absent, compute entry points raise."""
 import ctypes
+import math
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -152,3 +153,44 @@ def ptr(t):
 def cur_stream():
     import torch
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def device_view(addr, shape, dtype, device):
+    """Zero-copy torch view (float32, int32 or bfloat16) of an engine-owned device buffer, valid while the engine
+    lives."""
+    import torch
+
+    class _A:   # __cuda_array_interface__ carrier
+        pass
+    a = _A()
+    typestr = {torch.float32: "<f4", torch.int32: "<i4", torch.bfloat16: "<i2"}[dtype]
+    a.__cuda_array_interface__ = {"shape": (int(math.prod(shape)),), "typestr": typestr, "data": (int(addr), False),
+                                  "version": 2}
+    t = torch.as_tensor(a, device=device)
+    return (t.view(torch.bfloat16) if dtype == torch.bfloat16 else t).view(*shape)
+
+
+def debug_tensor(l, engine, h, name, shape, dtype, device):
+    """View of the named buffer of engine handle ``h`` (mfr_<engine>_debug_tensor, which reports its size in 4-byte
+    words); ``shape`` must fit in it."""
+    import torch
+    p, n = ctypes.c_void_p(), ctypes.c_longlong()
+    check(getattr(l, f"mfr_{engine}_debug_tensor")(h, name.encode(), ctypes.byref(p), ctypes.byref(n)),
+          f"debug tensor {name}")
+    assert math.prod(shape) * (2 if dtype == torch.bfloat16 else 4) <= 4 * n.value, (name, shape, n.value)
+    return device_view(p.value, shape, dtype, device)
+
+
+def upload_weights(l, engine, h, weights, stream):
+    """Uploads ``weights`` ({name: float32 ndarray}) into engine handle ``h`` in the engine's order; a tensor the
+    engine expects that is missing or of another size raises MfrError naming it."""
+    for i in range(getattr(l, f"mfr_{engine}_num_weights")(h)):
+        name = getattr(l, f"mfr_{engine}_weight_name")(h, i).decode()
+        numel = getattr(l, f"mfr_{engine}_weight_numel")(h, i)
+        if name not in weights:
+            raise MfrError(f"missing weight tensor {name}")
+        a = weights[name].reshape(-1)
+        if a.size != numel:
+            raise MfrError(f"weight {name}: {a.size} elements, engine expects {numel}")
+        check(getattr(l, f"mfr_{engine}_set_weight")(h, i, a.ctypes.data_as(ctypes.c_void_p), numel, stream),
+              f"set_weight {name}")

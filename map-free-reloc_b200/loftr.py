@@ -308,19 +308,8 @@ class LoFTR:
         self._host_counts = torch.zeros(4 + self.B + 1, dtype=torch.int32).pin_memory()
 
     def load_state_dict(self, state_dict):
-        w = prepare_weights(state_dict, self.H // 8, self.W // 8)
-        n = self._l.mfr_loftr_num_weights(self._h)
-        sp = ctypes.c_void_p(self.stream.cuda_stream)
-        for i in range(n):
-            name = self._l.mfr_loftr_weight_name(self._h, i).decode()
-            numel = self._l.mfr_loftr_weight_numel(self._h, i)
-            if name not in w:
-                raise _lib.MfrError(f"missing weight tensor {name}")
-            a = w[name].reshape(-1)
-            if a.size != numel:
-                raise _lib.MfrError(f"weight {name}: {a.size} elements, engine expects {numel}")
-            _lib.check(self._l.mfr_loftr_set_weight(self._h, i, a.ctypes.data_as(ctypes.c_void_p),
-                                                    numel, sp), f"set_weight {name}")
+        _lib.upload_weights(self._l, "loftr", self._h, prepare_weights(state_dict, self.H // 8, self.W // 8),
+                            ctypes.c_void_p(self.stream.cuda_stream))
 
     def num_kernels(self):
         return self._l.mfr_loftr_num_kernels(self._h)
@@ -350,24 +339,10 @@ class LoFTR:
                 for i in range(rc)]
 
     def _wrap(self, ptr, shape, dtype):
-        """Zero-copy torch view of an engine-owned device buffer."""
-        n = int(np.prod(shape))
-        itemsize = 4
-        class _Arr:  # __cuda_array_interface__ carrier
-            pass
-        a = _Arr()
-        a.__cuda_array_interface__ = {
-            "shape": (n,), "typestr": "<f4" if dtype == torch.float32 else "<i4",
-            "data": (int(ptr), False), "version": 2}
-        return torch.as_tensor(a, device=self.device).view(*shape)
+        return _lib.device_view(ptr, shape, dtype, self.device)
 
     def debug_tensor(self, name, shape):
-        p = ctypes.c_void_p()
-        n = ctypes.c_longlong()
-        _lib.check(self._l.mfr_loftr_debug_tensor(self._h, name.encode(), ctypes.byref(p), ctypes.byref(n)),
-                   f"debug tensor {name}")
-        assert int(np.prod(shape)) <= n.value, (name, shape, n.value)
-        return self._wrap(p.value, shape, torch.float32)
+        return _lib.debug_tensor(self._l, "loftr", self._h, name, shape, torch.float32, self.device)
 
     def forward_async(self, img0, img1):
         """Enqueues one batch on the engine stream. img0/img1: CUDA float32 [B,(1,)h,w] with h <= H,

@@ -38,20 +38,11 @@ class SIFT:
         self._desc = self._wrap(o.descriptors, (B, cap, 128), torch.float32)
 
     def _wrap(self, addr, shape, dtype):
-        """Zero-copy torch view of an engine-owned device buffer (valid while the engine lives)."""
-        class _A:
-            pass
-        a = _A()
-        a.__cuda_array_interface__ = {"shape": (int(np.prod(shape)),), "typestr": "<f4" if dtype == torch.float32 else "<i4",
-                                      "data": (int(addr), False), "version": 2}
-        return torch.as_tensor(a, device=self.device).view(*shape)
+        return _lib.device_view(addr, shape, dtype, self.device)
 
     def debug_tensor(self, name, shape, dtype=torch.float32):
         """Named intermediate buffer (see mfr_sift_debug_tensor): "gauss_<o>", "dog_<o>", "kp_pre", "kp_pre_octave"."""
-        p, n = ctypes.c_void_p(), ctypes.c_longlong()
-        _lib.check(self.l.mfr_sift_debug_tensor(self.h, name.encode(), ctypes.byref(p), ctypes.byref(n)), name)
-        assert int(np.prod(shape)) <= n.value, (name, shape, n.value)
-        return self._wrap(p.value, shape, dtype)
+        return _lib.debug_tensor(self.l, "sift", self.h, name, shape, dtype, self.device)
 
     def octave_shapes(self):
         """(h, w) of every octave's levels, octave 0 = the doubled image."""

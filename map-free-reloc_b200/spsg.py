@@ -149,15 +149,7 @@ class SuperPointSuperGlue:
                                               self.precision, ctypes.byref(h)), "mfr_spsg_create_ex")
         self._h = h
         self._l.mfr_spsg_set_graph(self._h, int(bool(graph)))
-        w = prepare_weights(sp_sd, sg_sd)
-        sp = ctypes.c_void_p(self.stream.cuda_stream)
-        for i in range(self._l.mfr_spsg_num_weights(self._h)):
-            name = self._l.mfr_spsg_weight_name(self._h, i).decode()
-            numel = self._l.mfr_spsg_weight_numel(self._h, i)
-            a = w[name].reshape(-1)
-            if a.size != numel:
-                raise _lib.MfrError(f"weight {name}: {a.size} elements, engine expects {numel}")
-            _lib.check(self._l.mfr_spsg_set_weight(self._h, i, a.ctypes.data_as(ctypes.c_void_p), numel, sp), name)
+        _lib.upload_weights(self._l, "spsg", self._h, prepare_weights(sp_sd, sg_sd), ctypes.c_void_p(self.stream.cuda_stream))
         o = _lib.SpsgOutputs()
         _lib.check(self._l.mfr_spsg_get_outputs(self._h, ctypes.byref(o)))
         self._o = o
@@ -166,14 +158,7 @@ class SuperPointSuperGlue:
         return self._l.mfr_spsg_num_launches(self._h)
 
     def _wrap(self, ptr, shape, dtype):
-        class _A:
-            pass
-        a = _A()
-        typestr = {torch.float32: "<f4", torch.int32: "<i4", torch.bfloat16: "<i2"}[dtype]
-        a.__cuda_array_interface__ = {"shape": (int(np.prod(shape)),), "typestr": typestr,
-                                      "data": (int(ptr), False), "version": 2}
-        t = torch.as_tensor(a, device=self.device)
-        return (t.view(torch.bfloat16) if dtype == torch.bfloat16 else t).view(*shape)
+        return _lib.device_view(ptr, shape, dtype, self.device)
 
     # buffers stored in bf16 in bf16 mode: the SuperPoint activations, q|k|v, the attention message, the token shadow
     BF16_TENSORS = ("x1a", "x4b", "qkv", "msg", "tokens_bf16")
@@ -182,11 +167,9 @@ class SuperPointSuperGlue:
         """Named engine buffer as a device tensor view. fp32, except in bf16 mode (precision="bf16"), where the
         buffers named in BF16_TENSORS ("qkv" [2B][K][768], "msg" [2B][K][256], ...) are torch.bfloat16 views, and
         "attn_scores" / "attn_vt" do not exist (the fused attention never stores them)."""
-        p, n = ctypes.c_void_p(), ctypes.c_longlong()
-        _lib.check(self._l.mfr_spsg_debug_tensor(self._h, name.encode(), ctypes.byref(p), ctypes.byref(n)), name)
-        assert int(np.prod(shape)) <= n.value
         bf = self.precision == 1 and name in self.BF16_TENSORS
-        return self._wrap(p.value, shape, torch.bfloat16 if bf else torch.float32)
+        return _lib.debug_tensor(self._l, "spsg", self._h, name, shape, torch.bfloat16 if bf else torch.float32,
+                                 self.device)
 
     def device_outputs(self):
         o, B, K = self._o, self.B, self.K

@@ -113,10 +113,10 @@ struct SpsgEngine : EngineCore {
     float* p1 = act(px(H2, W2) * 64); float* x2a = act(px(H2, W2) * 64); float* x2b = act(px(H2, W2) * 64);
     float* p2 = act(px(H4, W4) * 64); float* x3a = act(px(H4, W4) * 128); float* x3b = act(px(H4, W4) * 128);
     float* p3 = act(px(h8, w8) * 128); float* x4a = act(px(h8, w8) * 128); float* x4b = act(px(h8, w8) * 128, "x4b");
-    float* cPa = act(px(h8, w8) * 256); float* logits = mem.alloc<float>(px(h8, w8) * 65, "logits");
+    float* cPa = act(px(h8, w8) * 256, "cPa"); float* logits = mem.alloc<float>(px(h8, w8) * 65, "logits");
     float* scores = mem.alloc<float>(px(Hs, Ws), "scores"); float* mask = mem.alloc<float>(px(Hs, Ws), "nms_mask");
     float* t0 = mem.alloc<float>(px(Hs, Ws)); float* t1 = mem.alloc<float>(px(Hs, Ws)); float* t2 = mem.alloc<float>(px(Hs, Ws)); float* t3 = mem.alloc<float>(px(Hs, Ws));
-    float* cDa = act(px(h8, w8) * 256); float* dense = mem.alloc<float>(px(h8, w8) * 256, "dense_desc");
+    float* cDa = act(px(h8, w8) * 256, "cDa"); float* dense = mem.alloc<float>(px(h8, w8) * 256, "dense_desc");
     kpts = mem.alloc<float>(static_cast<size_t>(NI) * K * 2, "keypoints"); kscores = mem.alloc<float>(static_cast<size_t>(NI) * K, "kscores");
     counts = mem.alloc<int>(NI);
     X = mem.alloc<float>(static_cast<size_t>(NI) * K * 512, "tokens");
@@ -389,6 +389,7 @@ struct SpsgEngine : EngineCore {
 int spsg_create(int B, int H, int W, int max_kp, int nms_radius, float kp_thr, int border, int sinkhorn_iters,
                 float match_thr, int precision, SpsgEngine** out) {
   if (B < 1 || H < 64 || W < 64 || max_kp < 16 || max_kp > 2048 || (max_kp % 16)) return MFR_ERR_ARG;
+  if (nms_radius < 0 || border < 0) return MFR_ERR_ARG;
   // 0 = TF32 GEMM inputs, 1 = bf16 operands and fused attention (see mfr_b200.h), 2 = 3xTF32 split (fp32-faithful)
   if (precision < 0 || precision > 2) return MFR_ERR_ARG;
   auto* e = new SpsgEngine();

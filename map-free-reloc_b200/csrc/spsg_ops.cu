@@ -167,13 +167,51 @@ __global__ void nms_update_kernel(const float* __restrict__ supp_scores, const f
 // then the max_kp highest scores in descending order (torch.topk), or all of them in row-major order
 // when there are not more than max_kp (superpoint.py:170-187). One block per image.
 constexpr int kMaxCand = 16384;
-__global__ void __launch_bounds__(1024) select_keypoints_kernel(
+constexpr int kRadixBits = 11;
+
+__device__ __forceinline__ bool is_candidate(float s, float m, int i, int H, int W, float thr, int border) {
+  const int y = i / W, x = i - y * W;
+  return m > 0.f && s > thr && y >= border && y < H - border && x >= border && x < W - border;
+}
+// sort key: descending key order = descending score, then lower pixel index first (scores are >= 0, so their bits
+// order like the values)
+__device__ __forceinline__ unsigned long long cand_key(float s, int i) {
+  return (static_cast<unsigned long long>(__float_as_uint(s)) << 32) |
+         static_cast<unsigned long long>(0xffffffffu - static_cast<unsigned>(i));
+}
+// inclusive prefix sum over a block of 1024 threads; wsum must not be in use by another scan
+__device__ __forceinline__ int block_scan1024(int v, int* wsum) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, v, o);
+    if (lane >= o) v += t;
+  }
+  if (lane == 31) wsum[wid] = v;
+  __syncthreads();
+  if (wid == 0) {
+    int ws = wsum[lane];
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, ws, o);
+      if (lane >= o) ws += t;
+    }
+    wsum[lane] = ws;
+  }
+  __syncthreads();
+  return v + (wid > 0 ? wsum[wid - 1] : 0);
+}
+
+// Shared memory: 128 KB of keys (dynamic) and the 8 KB radix histogram: one block per SM, so the register budget is
+// that of one 1024-thread block.
+__global__ void __launch_bounds__(1024, 1) select_keypoints_kernel(
     const float* __restrict__ scores, const float* __restrict__ mask, int H, int W, float thr, int border,
     int max_kp, float* __restrict__ kpts /*[N][max_kp][2]*/, float* __restrict__ kscores /*[N][max_kp]*/,
     int* __restrict__ counts) {
-  extern __shared__ unsigned long long s_key[];   // (score bits << 32) | (0xffffffff - pixel index)
+  extern __shared__ unsigned long long s_key[];   // cand_key of the first kMaxCand candidates
   __shared__ int wsum[32];
   __shared__ int base;
+  __shared__ unsigned hist[1 << kRadixBits];
+  __shared__ unsigned long long sel_prefix;
+  __shared__ int sel_rank, gathered;
   const int n = blockIdx.x;
   const float* sc = scores + static_cast<size_t>(n) * H * W;
   const float* mk = mask + static_cast<size_t>(n) * H * W;
@@ -186,9 +224,8 @@ __global__ void __launch_bounds__(1024) select_keypoints_kernel(
     int flag = 0;
     float s = 0.f;
     if (i < total) {
-      const int y = i / W, x = i - y * W;
       s = sc[i];
-      flag = (mk[i] > 0.f && s > thr && y >= border && y < H - border && x >= border && x < W - border) ? 1 : 0;
+      flag = is_candidate(s, mk[i], i, H, W, thr, border) ? 1 : 0;
     }
     int inc = flag;
     for (int o = 1; o < 32; o <<= 1) {
@@ -208,18 +245,65 @@ __global__ void __launch_bounds__(1024) select_keypoints_kernel(
     __syncthreads();
     if (flag) {
       const int slot = base + (wid > 0 ? wsum[wid - 1] : 0) + inc - 1;
-      if (slot < kMaxCand)
-        s_key[slot] = (static_cast<unsigned long long>(__float_as_uint(s)) << 32) |
-                      static_cast<unsigned long long>(0xffffffffu - static_cast<unsigned>(i));
+      if (slot < kMaxCand) s_key[slot] = cand_key(s, i);
     }
     __syncthreads();
     if (threadIdx.x == 0) base += wsum[31];
     __syncthreads();
   }
-  const int ncand = min(base, kMaxCand);
+  int ncand = min(base, kMaxCand);
+  const bool row_major = base <= max_kp;
+  if (base > kMaxCand) {
+    // s_key holds only the first kMaxCand candidates in row-major order. Radix-select the max_kp-th largest key
+    // over the whole image, most significant 11-bit digit first (digits [53, 64), [42, 53), ..., [0, 9)), then
+    // gather the max_kp keys at or above it (keys are distinct) for the sort below.
+    unsigned long long prefix = 0ull, pmask = 0ull;   // the selected key's digits found so far
+    int rank = max_kp;                                // its rank among the keys that match them
+    for (int hi = 64; hi > 0; hi -= kRadixBits) {
+      const int lo = max(hi - kRadixBits, 0);
+      const unsigned dmask = (1u << (hi - lo)) - 1u;
+      for (int b = threadIdx.x; b < (1 << kRadixBits); b += 1024) hist[b] = 0u;
+      __syncthreads();
+      for (int i = threadIdx.x; i < total; i += 1024) {
+        const float s = sc[i];
+        if (!is_candidate(s, mk[i], i, H, W, thr, border)) continue;
+        const unsigned long long key = cand_key(s, i);
+        if ((key & pmask) == prefix) atomicAdd(&hist[static_cast<unsigned>(key >> lo) & dmask], 1u);
+      }
+      __syncthreads();
+      // thread t holds digits 2047 - 2t and 2046 - 2t: the scan counts the keys above each digit
+      const int d1 = 2047 - 2 * static_cast<int>(threadIdx.x), d0 = d1 - 1;
+      const int c1 = static_cast<int>(hist[d1]), c = c1 + static_cast<int>(hist[d0]);
+      const int incl = block_scan1024(c, wsum);
+      const int excl = incl - c;
+      if (excl < rank && rank <= incl) {
+        const bool top = excl + c1 >= rank;
+        sel_prefix = prefix | (static_cast<unsigned long long>(top ? d1 : d0) << lo);
+        sel_rank = rank - (top ? excl : excl + c1);
+      }
+      __syncthreads();
+      prefix = sel_prefix;
+      rank = sel_rank;
+      pmask |= static_cast<unsigned long long>(dmask) << lo;
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) gathered = 0;
+    __syncthreads();
+    for (int i = threadIdx.x; i < total; i += 1024) {
+      const float s = sc[i];
+      if (!is_candidate(s, mk[i], i, H, W, thr, border)) continue;
+      const unsigned long long key = cand_key(s, i);
+      if (key >= prefix) {
+        const int slot = atomicAdd(&gathered, 1);
+        if (slot < max_kp) s_key[slot] = key;
+      }
+    }
+    __syncthreads();
+    ncand = max_kp;
+  }
   float* ko = kpts + static_cast<size_t>(n) * max_kp * 2;
   float* so = kscores + static_cast<size_t>(n) * max_kp;
-  if (ncand <= max_kp) {   // keep torch.nonzero (row-major) order
+  if (row_major) {   // keep torch.nonzero (row-major) order
     for (int k = threadIdx.x; k < max_kp; k += blockDim.x) {
       float x = 0.f, y = 0.f, s = 0.f;
       if (k < ncand) {

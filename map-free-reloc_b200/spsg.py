@@ -149,10 +149,14 @@ class SuperPointSuperGlue:
                                               self.precision, ctypes.byref(h)), "mfr_spsg_create_ex")
         self._h = h
         self._l.mfr_spsg_set_graph(self._h, int(bool(graph)))
-        _lib.upload_weights(self._l, "spsg", self._h, prepare_weights(sp_sd, sg_sd), ctypes.c_void_p(self.stream.cuda_stream))
+        self.load_state_dicts(sp_sd, sg_sd)
         o = _lib.SpsgOutputs()
         _lib.check(self._l.mfr_spsg_get_outputs(self._h, ctypes.byref(o)))
         self._o = o
+
+    def load_state_dicts(self, sp_sd, sg_sd):
+        """Uploads new SuperPoint / SuperGlue weights (reference state_dict formats); a map of set_map is dropped."""
+        _lib.upload_weights(self._l, "spsg", self._h, prepare_weights(sp_sd, sg_sd), ctypes.c_void_p(self.stream.cuda_stream))
 
     def num_launches(self):
         return self._l.mfr_spsg_num_launches(self._h)
@@ -161,7 +165,7 @@ class SuperPointSuperGlue:
         return _lib.device_view(ptr, shape, dtype, self.device)
 
     # buffers stored in bf16 in bf16 mode: the SuperPoint activations, q|k|v, the attention message, the token shadow
-    BF16_TENSORS = ("x1a", "x4b", "qkv", "msg", "tokens_bf16")
+    BF16_TENSORS = ("x1a", "x4b", "cPa", "cDa", "qkv", "msg", "tokens_bf16")
 
     def debug_tensor(self, name, shape):
         """Named engine buffer as a device tensor view. fp32, except in bf16 mode (precision="bf16"), where the

@@ -97,8 +97,8 @@ def _mlp(x, sd, pre, n_layers):
 
 
 def normalize_keypoints(kpts, h, w):
-    """superglue.py:63-70."""
-    size = torch.tensor([[float(w), float(h)]])
+    """superglue.py:63-70 (on kpts' device, in its dtype)."""
+    size = kpts.new_tensor([[float(w), float(h)]])
     center = size / 2
     scaling = size.max(1, keepdim=True).values * 0.7
     return (kpts - center[:, None, :]) / scaling[:, None, :]
@@ -115,6 +115,17 @@ def _attention_layer(x, src, sd, pre):
     msg = torch.einsum("bhnm,bdhm->bdhn", prob, v).contiguous().view(b, 256, -1)
     msg = F.conv1d(msg, sd[f"{pre}.attn.merge.weight"], sd[f"{pre}.attn.merge.bias"])
     return _mlp(torch.cat([x, msg], dim=1), sd, f"{pre}.mlp", 2)
+
+
+def gnn(d0, d1, sd):
+    """AttentionalGNN.forward (superglue.py:130-138): 18 layers, ['self', 'cross'] * 9; both images are updated from the
+    previous layer's tokens."""
+    for i in range(18):
+        pre = f"gnn.layers.{i}"
+        s0, s1 = (d1, d0) if i % 2 == 1 else (d0, d1)       # ['self', 'cross'] * 9 (superglue.py:192)
+        delta0, delta1 = _attention_layer(d0, s0, sd, pre), _attention_layer(d1, s1, sd, pre)
+        d0, d1 = d0 + delta0, d1 + delta1
+    return d0, d1
 
 
 def log_optimal_transport(scores, alpha, iters):
@@ -146,11 +157,7 @@ def superglue(kpts0, sc0, desc0, kpts1, sc1, desc1, h, w, sd, cfg=None, return_s
     k1 = normalize_keypoints(kpts1[None], h, w)
     d0 = desc0[None] + _mlp(torch.cat([k0.transpose(1, 2), sc0[None, None]], 1), sd, "kenc.encoder", 5)
     d1 = desc1[None] + _mlp(torch.cat([k1.transpose(1, 2), sc1[None, None]], 1), sd, "kenc.encoder", 5)
-    for i in range(18):
-        pre = f"gnn.layers.{i}"
-        s0, s1 = (d1, d0) if i % 2 == 1 else (d0, d1)       # ['self', 'cross'] * 9 (superglue.py:192)
-        delta0, delta1 = _attention_layer(d0, s0, sd, pre), _attention_layer(d1, s1, sd, pre)
-        d0, d1 = d0 + delta0, d1 + delta1
+    d0, d1 = gnn(d0, d1, sd)
     m0 = F.conv1d(d0, sd["final_proj.weight"], sd["final_proj.bias"])
     m1 = F.conv1d(d1, sd["final_proj.weight"], sd["final_proj.bias"])
     scores = torch.einsum("bdn,bdm->bnm", m0, m1) / 256 ** 0.5

@@ -17,6 +17,31 @@ GOLD_H, GOLD_W = 720, 540
 GOLD_K = np.array([[600.0, 0, 269.5], [0, 600.0, 359.5], [0, 0, 1]])
 
 
+U32 = 2.0 ** -24    # fp32 unit roundoff
+
+
+def branch_err(x_in, x_out, ref_out, out_ulp=0.0):
+    """max |(out - in) - (ref - in)| / max |ref - in| in float64: the error of the layer's residual branch. ``out_ulp``
+    discounts the rounding of the residual sum itself, out_ulp |out| per element: when the branch is small next to the
+    input, that rounding alone exceeds the branch's own relative error."""
+    x_in = x_in.double()
+    ref_b = ref_out - x_in
+    d = (x_out.double() - x_in - ref_b).abs()
+    if out_ulp:
+        d = (d - out_ulp * x_out.double().abs()).clamp(min=0)
+    return (d.max() / ref_b.abs().max()).item()
+
+
+def dot_bound(a, w, c_op, bias=None):
+    """Per-element bound of an fp32-accumulated GEMM a @ w^T (+ bias) with operand rounding c_op: the accumulation of K
+    terms, the rounding of alpha / bias in the epilogue and the rounding of the result."""
+    K = a.shape[-1]
+    s = a.double().abs() @ w.double().abs().t()
+    if bias is not None:
+        s = s + bias.double().abs()
+    return (c_op + (K + 2) * U32) * s
+
+
 def pose_case(ci):
     seed, n, ratio, noise = POSE_CASES[ci]
     return synth.make_correspondences(seed, n=n, inlier_ratio=ratio, noise_px=noise, h=GOLD_H, w=GOLD_W, K=GOLD_K)

@@ -23,13 +23,12 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from helpers import fullres_inputs
+from helpers import U32, branch_err, dot_bound, fullres_inputs
 from oracle import loftr_oracle as lo
 
 pytestmark = pytest.mark.gpu
 
 PRECISIONS = ["tf32", "bf16", "fp32x3"]
-U32 = 2.0 ** -24
 C_OP = {"tf32": 2 * 2.0 ** -10, "bf16": 2 * 2.0 ** -10, "fp32x3": 2.0 ** -20}   # operand term of the fp32-input GEMMs
 # residual-branch bars of one encoder layer, as multiples of the unit roundoff (measured maxima in the test docstrings)
 COARSE_BAR = {"tf32": 4 * 2.0 ** -11, "bf16": 4 * 2.0 ** -8, "fp32x3": 32 * 2.0 ** -22}
@@ -101,23 +100,6 @@ def d64(sd):
 def bf16_view(eng, name, shape):
     """A bf16 debug buffer: ``shape`` in bf16 elements (the last axis even), read through the float32 view."""
     return eng.debug_tensor(name, (*shape[:-1], shape[-1] // 2)).view(torch.bfloat16)
-
-
-def branch_err(x_in, x_out, ref_out):
-    """max |(out - in) - (ref - in)| / max |ref - in| in float64: the error of the layer's residual branch."""
-    x_in = x_in.double()
-    ref_b = ref_out - x_in
-    return ((x_out.double() - x_in - ref_b).abs().max() / ref_b.abs().max()).item()
-
-
-def dot_bound(a, w, c_op, bias=None):
-    """Per-element bound of an fp32-accumulated GEMM a @ w^T (+ bias) with operand rounding c_op: the accumulation of K
-    terms, the rounding of alpha / bias in the epilogue and the rounding of the result."""
-    K = a.shape[-1]
-    s = a.double().abs() @ w.double().abs().t()
-    if bias is not None:
-        s = s + bias.double().abs()
-    return (c_op + (K + 2) * U32) * s
 
 
 def posenc(sd, h8, w8):

@@ -254,6 +254,17 @@ typedef struct mfr_pose_solver mfr_pose_solver;
 int mfr_pose_solver_create(int max_pairs, int max_pts_per_pair, int max_hypotheses,
                            mfr_pose_solver** out);
 void mfr_pose_solver_destroy(mfr_pose_solver* s);
+/* Named scratch buffers of the handle, for stage-wise parity tests; *words is the buffer's size in 4-byte words. They
+ * hold what the last call that wrote them left there:
+ *   "hyp_results" block winners [max_pairs][*] {double cost; int count, valid; double model[12]} (112 bytes), row
+ *                 stride = the blocks of that launch (E-mat: ceil(num_hyp / hypotheses per block); PnP: ceil(num_hyp / 128))
+ *   "lo_results"  E-mat LO candidates [max_pairs][4] {double cost, R[9], t[3]} (104 bytes)
+ *   "pts_norm"    float4 [max_pairs][max_pts_per_pair] normalised correspondences (x0, y0, x1, y1)
+ *   "Rd", "td"    double [max_pairs][9] / [max_pairs][3]: the final E-mat pose
+ *   "Xw", "uv", "vidx" PnP's compacted depth-valid points: double [max_pairs][max_pts_per_pair][3] (camera 0), float
+ *                 [..][2] (kpts1), int [..] (index within the pair)
+ *   "nvalid", "dmin" int [max_pairs] compacted count; float bits [max_pairs] of max(min(depth0), 0) */
+int mfr_pose_solver_debug_tensor(mfr_pose_solver* s, const char* name, void** ptr, long long* words);
 
 /* EssentialMatrixSolver.estimate_pose (pose_solver.py:29-61): cv.findEssentialMat(USAC_MAGSAC) +
  * cv.recoverPose. `num_hyp` 5-point hypotheses per pair (MSAC-scored). lo_enabled is a bit set:

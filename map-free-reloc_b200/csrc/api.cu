@@ -256,6 +256,10 @@ void mfr_pose_solver_destroy(mfr_pose_solver* s) {
   mfr::pose_solver_destroy(s->s);
   delete s;
 }
+int mfr_pose_solver_debug_tensor(mfr_pose_solver* s, const char* name, void** ptr, long long* words) {
+  if (!s) return MFR_ERR_ARG;
+  return mfr::pose_solver_debug_tensor(s->s, name, ptr, words);
+}
 int mfr_emat_ransac(mfr_pose_solver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
                     const float* K0, const float* K1, float pix_threshold, int num_hyp,
                     unsigned long long seed, int lo_enabled, float* R, float* t, int* n_inliers,

@@ -12,6 +12,8 @@
 #include "geometry.cuh"
 
 #include <algorithm>
+#include <cstddef>
+#include <cstring>
 
 #include "geometry_solvers.cuh"
 
@@ -29,6 +31,10 @@ struct HypResult {   // best hypothesis of one block
   int valid;
   double model[12];  // E[9] or R[9] t[3]
 };
+// the layout tests read through pose_solver_debug_tensor("hyp_results") as a numpy structured dtype
+static_assert(sizeof(HypResult) == 112 && offsetof(HypResult, cost) == 0 && offsetof(HypResult, count) == 8 &&
+                  offsetof(HypResult, valid) == 12 && offsetof(HypResult, model) == 16,
+              "HypResult layout is part of the debug interface");
 
 __device__ __forceinline__ unsigned long long splitmix64(unsigned long long& s) {
   s += 0x9E3779B97F4A7C15ull;
@@ -330,6 +336,9 @@ struct EmatShared {
 struct LoResult {
   double cost, R[9], t[3];
 };
+static_assert(sizeof(LoResult) == 104 && offsetof(LoResult, cost) == 0 && offsetof(LoResult, R) == 8 &&
+                  offsetof(LoResult, t) == 80,
+              "LoResult layout is part of the debug interface");
 
 // LM rounds on the Tukey-biweight M-estimator of the Sampson distance with cut-off sqrt(T2),
 // starting from (S.R, S.t); leaves the last accepted parameters there. All threads must call it.
@@ -1522,6 +1531,31 @@ void pose_solver_destroy(PoseSolver* s) {
 
 double* pose_solver_Rd(PoseSolver* s) { return s->Rd; }
 double* pose_solver_td(PoseSolver* s) { return s->td; }
+
+int pose_solver_debug_tensor(PoseSolver* s, const char* name, void** ptr, long long* words) {
+  if (!s || !name || !ptr || !words) return MFR_ERR_ARG;
+  const long long P = s->max_pairs, T = static_cast<long long>(s->total_pts);
+  const long long blocks = (s->max_hyp + 31) / 32;
+  const struct { const char* name; void* p; long long bytes; } bufs[] = {
+      {"hyp_results", s->results, static_cast<long long>(sizeof(HypResult)) * P * blocks},
+      {"lo_results", s->lo_out, static_cast<long long>(sizeof(LoResult)) * P * kLoTopK},
+      {"pts_norm", s->pts_norm, 16 * T},
+      {"Rd", s->Rd, 8 * 9 * P},
+      {"td", s->td, 8 * 3 * P},
+      {"Xw", s->Xw, 8 * 3 * T},
+      {"uv", s->uv, 4 * 2 * T},
+      {"vidx", s->vidx, 4 * T},
+      {"nvalid", s->nvalid, 4 * P},
+      {"dmin", s->dmin, 4 * P},
+  };
+  for (const auto& b : bufs)
+    if (strcmp(b.name, name) == 0) {
+      *ptr = b.p;
+      *words = b.bytes / 4;
+      return MFR_OK;
+    }
+  return MFR_ERR_ARG;
+}
 
 int emat_ransac(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
                 const float* K0, const float* K1, float pix_thr, int num_hyp, unsigned long long seed,

@@ -10,6 +10,8 @@ int pose_solver_create(int max_pairs, int max_pts, int max_hyp, PoseSolver** out
 void pose_solver_destroy(PoseSolver* s);
 double* pose_solver_Rd(PoseSolver* s);
 double* pose_solver_td(PoseSolver* s);
+// named scratch buffer of the handle (see mfr_pose_solver_debug_tensor); words = its size in 4-byte words
+int pose_solver_debug_tensor(PoseSolver* s, const char* name, void** ptr, long long* words);
 
 int emat_ransac(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
                 const float* K0, const float* K1, float pix_thr, int num_hyp, unsigned long long seed,

@@ -90,6 +90,7 @@ SIGNATURES = {
     "mfr_sift_profile": (c_int, [c_vp, c_vp, c_vp, c_vp]),
     "mfr_pose_solver_create": (c_int, [c_int, c_int, c_int, c_pp]),
     "mfr_pose_solver_destroy": (None, [c_vp]),
+    "mfr_pose_solver_debug_tensor": (c_int, [c_vp, ctypes.c_char_p, c_pp, ctypes.POINTER(c_ll)]),
     "mfr_emat_ransac": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_float, c_int,
                                 ctypes.c_ulonglong, c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "mfr_scale_from_depth": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp,
@@ -156,14 +157,14 @@ def cur_stream():
 
 
 def device_view(addr, shape, dtype, device):
-    """Zero-copy torch view (float32, int32 or bfloat16) of an engine-owned device buffer, valid while the engine
-    lives."""
+    """Zero-copy torch view (float32, float64, int32 or bfloat16) of an engine-owned device buffer, valid while the
+    engine lives."""
     import torch
 
     class _A:   # __cuda_array_interface__ carrier
         pass
     a = _A()
-    typestr = {torch.float32: "<f4", torch.int32: "<i4", torch.bfloat16: "<i2"}[dtype]
+    typestr = {torch.float32: "<f4", torch.float64: "<f8", torch.int32: "<i4", torch.bfloat16: "<i2"}[dtype]
     a.__cuda_array_interface__ = {"shape": (int(math.prod(shape)),), "typestr": typestr, "data": (int(addr), False),
                                   "version": 2}
     t = torch.as_tensor(a, device=device)
@@ -177,7 +178,7 @@ def debug_tensor(l, engine, h, name, shape, dtype, device):
     p, n = ctypes.c_void_p(), ctypes.c_longlong()
     check(getattr(l, f"mfr_{engine}_debug_tensor")(h, name.encode(), ctypes.byref(p), ctypes.byref(n)),
           f"debug tensor {name}")
-    assert math.prod(shape) * (2 if dtype == torch.bfloat16 else 4) <= 4 * n.value, (name, shape, n.value)
+    assert math.prod(shape) * torch.empty((), dtype=dtype).element_size() <= 4 * n.value, (name, shape, n.value)
     return device_view(p.value, shape, dtype, device)
 
 

@@ -136,6 +136,13 @@ class PoseBackend:
                                           _lib.ptr(R), _lib.ptr(t), _lib.ptr(n), _lib.cur_stream()), "mfr_icp_refine")
         return R, t, n
 
+    def debug_tensor(self, name, shape, dtype):
+        """Zero-copy view of a named scratch buffer of the handle (mfr_pose_solver_debug_tensor: "hyp_results",
+        "lo_results", "pts_norm", "Rd", "td", "Xw", "uv", "vidx", "nvalid", "dmin"), as torch ``dtype`` (float32,
+        float64 or int32) of ``shape``; it shows what the last call that wrote the buffer left there. The records
+        "hyp_results" and "lo_results" are read as raw words and reinterpreted on the host."""
+        return _lib.debug_tensor(self._l, "pose_solver", self._h, name, shape, dtype, self.device)
+
     def close(self):
         if getattr(self, "_h", None):
             self._l.mfr_pose_solver_destroy(self._h)

@@ -40,27 +40,78 @@ def test_pnp_matches_oracle(solvers, seed, n, ratio, noise):
     assert abs(ninl - no) <= max(3, 0.01 * no)
 
 
-@pytest.mark.parametrize("seed,n,ratio,noise", [(31, 1000, 0.6, 0.3), (32, 2000, 0.5, 0.5), (33, 600, 0.7, 0.2)])
-def test_scale_from_depth_exact_given_pose(solvers, seed, n, ratio, noise):
-    """Stage boundary: the oracle's own (R, t, mask) in -> identical consensus out."""
+def _scale_pairs(seed, n, ratio, noise):
+    """Inputs of one scale case: a list of (correspondences, K0, K1, the OpenCV oracle's R, t and mask). Seeds 31-33
+    are one pair each. Seed 34 is a batch of 16 pairs of n + 150 i correspondences (up to 3750, so the consensus runs
+    over several 1024-point chunks) with per-pair intrinsics (K1 != K0 in pair 2), a failed (NaN) pose in pair 5,
+    out-of-image inlier keypoints in pair 3 and zero depths at inlier pixels in pairs 7 (depth0) and 8 (depth1). Seed 35
+    is N = max_pts (8192) and N = 8300 > max_pts, of which the solver reads the first 8192."""
+    specs = {34: [n + 150 * i for i in range(16)], 35: [n, n + 108]}.get(seed, [n])
+    out = []
+    for i, ni in enumerate(specs):
+        f = 600.0 + (25.0 * i if seed == 34 else 0.0)
+        K = np.array([[f, 0, 269.5 - i], [0, f + 5.0 * (seed == 34), 359.5 + i], [0, 0, 1]])
+        c = synth.make_correspondences(seed * 100 + i if len(specs) > 1 else seed, n=ni, inlier_ratio=ratio,
+                                       noise_px=noise, K=K)
+        K0 = c["K_color0"]; K1 = c["K_color1"].copy()
+        if seed == 34 and i == 2:    # kpts1 re-expressed in another K1: the same normalised correspondences
+            K1 = np.array([[640.0, 0, 262.0], [0, 610.0, 350.0], [0, 0, 1]], np.float32)
+            x = (c["kpts1"].astype(np.float64) - K[:2, 2]) / np.diag(K)[:2]
+            c["kpts1"] = (x * np.diag(K1)[:2] + K1[:2, 2]).astype(np.float32)
+        Ro, to, _, mo = po.essential_matrix_solver(c["kpts0"], c["kpts1"], K0, K1, 2.0, 0.9999)
+        mo = mo.ravel() == 1
+        inl = np.nonzero(mo)[0]
+        if seed == 34 and i == 5:
+            Ro = np.full((3, 3), np.nan)
+        if seed == 34 and i == 3:
+            c["kpts0"][inl[0:40:4]] = (-1.5, 100.0); c["kpts0"][inl[1:40:4]] = (540.5, 200.0)
+            c["kpts1"][inl[2:40:4]] = (300.0, -1.25); c["kpts1"][inl[3:40:4]] = (10.0, 720.0)
+        if seed == 34 and i in (7, 8):
+            k = np.int32(c["kpts%d" % (i - 7)][inl[::3]])
+            c["depth%d" % (i - 7)][k[:, 1], k[:, 0]] = 0.0
+        out.append((c, K0, K1, Ro, np.ravel(to), mo))
+    return out
+
+
+@pytest.mark.parametrize("seed,n,ratio,noise", [(31, 1000, 0.6, 0.3), (32, 2000, 0.5, 0.5), (33, 600, 0.7, 0.2),
+                                                (34, 1500, 0.6, 0.3), (35, 8192, 0.5, 0.3)])
+def test_scale_from_depth_exact_given_pose(seed, n, ratio, noise):
+    """Stage boundary: the oracle's own (R, t, mask) in -> identical consensus out. Every pair's count is exact and its
+    pose equals the float32 rounding of the restatement (oracle/pose_stages_oracle.scale_consensus, which
+    tests/test_pose_stages_host.py pins to the reference's scale_from_depth); where the keypoints stay inside the images
+    that is the reference's scale_from_depth itself. A NaN pose fails its pair alone."""
     from mfr_b200 import pose_solver as ps
-    c = synth.make_correspondences(seed, n=n, inlier_ratio=ratio, noise_px=noise)
-    Ro, to, no, mo = po.essential_matrix_solver(c["kpts0"], c["kpts1"], c["K_color0"], c["K_color1"], 2.0, 0.9999)
-    Rm, tm, nm = po.scale_from_depth(Ro, to, mo, c["kpts0"], c["kpts1"], c["depth0"], c["depth1"],
-                                     c["K_color0"], c["K_color1"], 0.1)
-    be = solvers[1].backend
+    from oracle import pose_stages_oracle as so
+    pairs = _scale_pairs(seed, n, ratio, noise)
+    be = ps.PoseBackend(max_pairs=16, max_pts=8192, max_hyp=128)
     dev = be.device
-    k0 = torch.tensor(c["kpts0"], device=dev); k1 = torch.tensor(c["kpts1"], device=dev)
-    off = torch.tensor([0, n], dtype=torch.int32, device=dev)
-    K0 = torch.tensor(c["K_color0"], device=dev).reshape(1, 3, 3).contiguous()
-    Rd = torch.tensor(Ro, dtype=torch.float64, device=dev).reshape(1, 9).contiguous()
-    td = torch.tensor(np.asarray(to).ravel(), dtype=torch.float64, device=dev).reshape(1, 3).contiguous()
-    mk = torch.tensor(mo.ravel().astype(np.uint8), device=dev)
-    d0 = torch.tensor(c["depth0"], device=dev)[None]; d1 = torch.tensor(c["depth1"], device=dev)[None]
-    R, t, ninl = be.scale(k0, k1, off, K0, K0, mk, d0, d1, 0.1, Rd, td)
-    assert int(ninl.item()) == nm                                  # integer consensus count: exact
-    np.testing.assert_allclose(t[0].cpu().numpy(), np.float32(tm.ravel()), rtol=0, atol=1e-6)
-    np.testing.assert_allclose(R[0].cpu().numpy(), np.float32(Rm), rtol=0, atol=1e-6)
+    cat = lambda k: torch.tensor(np.concatenate([c[k] for c, *_ in pairs]), device=dev).contiguous()
+    st = lambda a: torch.tensor(np.stack(a), device=dev).contiguous()
+    off = torch.tensor(np.cumsum([0] + [len(c["kpts0"]) for c, *_ in pairs]), dtype=torch.int32, device=dev)
+    Rd = st([p[3].reshape(9) for p in pairs]).double(); td = st([p[4] for p in pairs]).double()
+    mk = torch.tensor(np.concatenate([p[5] for p in pairs]).astype(np.uint8), device=dev)
+    R, t, ninl = be.scale(cat("kpts0"), cat("kpts1"), off, st([p[1] for p in pairs]), st([p[2] for p in pairs]), mk,
+                          st([c["depth0"] for c, *_ in pairs]), st([c["depth1"] for c, *_ in pairs]), 0.1, Rd, td)
+    R, t, ninl = R.cpu().numpy(), t.cpu().numpy(), ninl.cpu().numpy()
+    be.close()
+    for i, (c, K0, K1, Ro, to, mo) in enumerate(pairs):
+        N = min(len(mo), 8192)
+        exp = so.scale_consensus(Ro, to, mo[:N], c["kpts0"][:N], c["kpts1"][:N], c["depth0"], c["depth1"], K0, K1, 0.1)
+        if exp is None:                                            # failed pair: NaN pose, 0 inliers
+            assert ninl[i] == 0 and np.isnan(R[i]).all() and np.isnan(t[i]).all()
+            continue
+        Rm, tm, nm = exp
+        inside = all((np.int32(c[k][:N][mo[:N]]) >= 0).all() and (np.int32(c[k][:N][mo[:N]]) < [540, 720]).all()
+                     for k in ("kpts0", "kpts1"))
+        if inside and N == len(mo):
+            _, tr, nr = po.scale_from_depth(Ro, to, mo.astype(np.uint8), c["kpts0"], c["kpts1"], c["depth0"],
+                                            c["depth1"], K0, K1, 0.1)
+            assert nr == nm and np.abs(tr.ravel() - tm).max() < 1e-12
+        assert int(ninl[i]) == nm                                  # integer consensus count: exact
+        np.testing.assert_allclose(t[i], np.float32(tm), rtol=0, atol=1e-6)
+        np.testing.assert_allclose(R[i], np.float32(Rm), rtol=0, atol=1e-6)
+    if seed == 34:
+        assert ninl[5] == 0 and (ninl[np.arange(16) != 5] > 0).all()
 
 
 @pytest.mark.parametrize("seed,n,ratio,noise", [(41, 1000, 0.6, 0.3), (42, 2000, 0.5, 0.5), (43, 800, 0.7, 0.2),

@@ -52,6 +52,17 @@ int mfr_conv2d_nhwc_bf16(const void* x, int N, int H, int W, int Cin, long long 
                          const void* residual, long long ldr, int act, float alpha, void* out,
                          long long ldo, int out_bf16, void* stream);
 
+/* Stage entry for tests: a token GEMM (Linear layer) with a device row count, the form of the LoFTR fine-level
+ * projections. n_img blocks of rows_cap token rows; block i computes rows r < *dyn_rows (read on the device at launch):
+ *   out[i][r][co] = act(sum_ci x[i][r][ci] * w[co][ci] + bias[co]), co < Cout
+ *   x   [n_img][rows_cap] rows of stride ldx elements, w [Cout] rows of stride ldw elements (0 = Cin); both bf16
+ *       (bf16 wgmma) when in_bf16 != 0, else fp32 (TF32 wgmma); fp32 accumulate; bias fp32 or NULL
+ *   out [n_img][rows_cap] rows of stride ldo elements, bf16 when out_bf16 != 0 (then Cout % 4 == 0), else fp32.
+ * Rows at or past *dyn_rows and elements past Cout of a row are not written. */
+int mfr_token_gemm_dyn_rows(const void* x, int n_img, int rows_cap, int Cin, long long ldx, const void* w,
+                            long long ldw, int in_bf16, int Cout, const float* bias, int act, void* out,
+                            long long ldo, int out_bf16, const int* dyn_rows, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * LoFTR matcher engine. Replaces LoFTR.forward of the reference
  * (etc/feature_matching_baselines/LoFTR/src/loftr/loftr.py:29-75) as driven by

@@ -71,6 +71,21 @@ int mfr_conv2d_nhwc_bf16(const void* x, int N, int H, int W, int Cin, long long 
   return mfr::conv_gemm_launch(p, static_cast<cudaStream_t>(stream));
 }
 
+int mfr_token_gemm_dyn_rows(const void* x, int n_img, int rows_cap, int Cin, long long ldx, const void* w, long long ldw,
+                            int in_bf16, int Cout, const float* bias, int act, void* out, long long ldo, int out_bf16,
+                            const int* dyn_rows, void* stream) {
+  if (dyn_rows == nullptr) return MFR_ERR_ARG;
+  mfr::ConvGemmDesc d{};
+  d.x = static_cast<const float*>(x); d.N = n_img; d.H = 1; d.W = rows_cap; d.Cin = Cin; d.ldx = ldx;
+  d.w = static_cast<const float*>(w); d.ldw = ldw; d.Cout = Cout; d.R = 1; d.S = 1; d.stride = 1; d.pad = 0;
+  d.bias = bias; d.act = act; d.alpha = 1.f; d.out = static_cast<float*>(out); d.ldo = ldo;
+  d.in_bf16 = in_bf16; d.out_bf16 = out_bf16; d.dyn_w = dyn_rows;
+  mfr::ConvGemmParams p;
+  int rc = mfr::conv_gemm_build(d, &p);
+  if (rc != MFR_OK) return rc;
+  return mfr::conv_gemm_launch(p, static_cast<cudaStream_t>(stream));
+}
+
 // ------------------------------------------------------------------------------------------ LoFTR
 struct mfr_loftr { mfr::LoftrEngine* e; };
 

@@ -70,16 +70,18 @@ constexpr uint64_t kDescHi = (1ull << 16) | (64ull << 32) | (1ull << 62);
 constexpr uint64_t kDescHi32 = (1ull << 16) | (16ull << 32) | (3ull << 62);
 
 // Epilogue kinds (ConvGemmParams::epi): bit 3 = bf16 output, bit 2 = residual, bits 0-1 = Act; kEpiAny = decided at
-// run time per element (token GEMMs with a dyn_w row count or act_cols, odd strides, the tf32 engine)
+// run time per element (act_cols, per-row B operands, odd strides, the other kinds of the tf32 operands)
 constexpr int kEpiAny = -1, kEpiOutBf16 = 8, kEpiResidual = 4;
 constexpr int epi_kind(bool out_bf16, bool residual, int act) {
   return (out_bf16 ? kEpiOutBf16 : 0) | (residual ? kEpiResidual : 0) | act;
 }
-// the kinds with their own (TMA-store) instantiations, at BN >= 128
+// the kinds with their own (TMA-store) instantiations, at BN >= 128: all five with bf16 operands, kF32 with tf32 ones
 constexpr int kBf = epi_kind(true, false, ACT_NONE), kBfRelu = epi_kind(true, false, ACT_RELU),
               kBfLeaky = epi_kind(true, false, ACT_LEAKY), kBfResRelu = epi_kind(true, true, ACT_RELU),
               kF32 = epi_kind(false, false, ACT_NONE);
-constexpr bool staged_kind(int k) { return k == kBf || k == kBfRelu || k == kBfLeaky || k == kBfResRelu || k == kF32; }
+__host__ __device__ constexpr bool staged_inst(int k, int BN, bool bf16) {
+  return BN >= 128 && (k == kF32 || (bf16 && (k == kBf || k == kBfRelu || k == kBfLeaky || k == kBfResRelu)));
+}
 
 // two neighbouring channels per store: every element offset even and the base pointers aligned accordingly
 __host__ __device__ __forceinline__ bool epilogue_vec2(const ConvGemmParams& p) {
@@ -272,12 +274,18 @@ __device__ __forceinline__ void epilogue_staged(const ConvGemmParams& p, const f
 
 // Store warp of the TMA-store epilogue: per pass of every tile it waits for the staging buffer, stores its boxes, and
 // once the stores have read it hands it back -- for the residual kind after loading the next tile's residual into it.
+// With a device row count (w_lim < Wo; H = 1, no residual) the output map still ends at Wo, so the one tile per image
+// that crosses w_lim is copied out by the warp itself, its live rows only: no row at or past w_lim is written.
 template <int BN_T, int MT_T, int EPI>
 __device__ __forceinline__ void store_warp(const ConvGemmParams& p, uint32_t stage, uint32_t st_empty, uint32_t st_full,
-                                           int total_tiles, int tiles_x, int tile_rows) {
+                                           int total_tiles, int tiles_x, int tile_rows, int w_lim) {
   constexpr bool kOutBf16 = (EPI & kEpiOutBf16) != 0, kRes = (EPI & kEpiResidual) != 0;
   constexpr int kNBox = stage_nbox(BN_T, kOutBf16), kCW = stage_cw(kOutBf16);
   constexpr int kPasses = (stage_place(BN_T, kOutBf16, MT_T * kNBox - 1) >> 16) + 1;
+  constexpr int kOsz = kOutBf16 ? 2 : 4;
+  // a device row count comes with H = 1, so MT = 1, and without a residual: only those instantiations handle it
+  constexpr bool kDynRows = MT_T == 1 && !kRes;
+  const int x_lim = kDynRows ? w_lim : p.Wo;
   struct Tile { int n0, x0, y0, img; };
   auto tile_of = [&](int item) {
     int mt, nt;
@@ -312,19 +320,45 @@ __device__ __forceinline__ void store_warp(const ConvGemmParams& p, uint32_t sta
   uint32_t parity = 0;
   for (int item = blockIdx.x; item < total_tiles; item += gridDim.x) {
     const Tile t = tile_of(item);
+    const bool part = kDynRows && x_lim < p.Wo && t.x0 + p.TW > x_lim;   // crosses the device row count
 #pragma unroll
     for (int pass = 0; pass < kPasses; ++pass) {
       mbar_wait_inl(st_full, parity, 8);
       parity ^= 1u;
-      if (elect_one_sync()) {
+      if (!part) {
+        if (elect_one_sync()) {
+#pragma unroll
+          for (int b = 0; b < MT_T * kNBox; ++b) {
+            const int m = b / kNBox, c = b % kNBox;
+            if ((stage_place(BN_T, kOutBf16, b) >> 16) != pass || t.y0 + m * p.TH >= p.Ho) continue;
+            tma_store_4d((c + 1) * kCW <= BN_T ? &p.tmO : &p.tmO2, stage + (stage_place(BN_T, kOutBf16, b) & 0xffff),
+                         t.n0 + c * kCW, t.x0, t.y0 + m * p.TH, t.img);
+          }
+          tma_store_commit();
+        }
+      } else if constexpr (kDynRows) {
+        // the live rows' channels below p.cout_tma, one 16-byte group per lane, un-swizzled from the staging buffer
+        static_assert(stage_narrow_row(BN_T, kOutBf16) % 16 == 0, "the narrow box holds whole 16-byte groups");
+        const int c_hi = min(p.cout_tma - t.n0, BN_T);
 #pragma unroll
         for (int b = 0; b < MT_T * kNBox; ++b) {
           const int m = b / kNBox, c = b % kNBox;
           if ((stage_place(BN_T, kOutBf16, b) >> 16) != pass || t.y0 + m * p.TH >= p.Ho) continue;
-          tma_store_4d((c + 1) * kCW <= BN_T ? &p.tmO : &p.tmO2, stage + (stage_place(BN_T, kOutBf16, b) & 0xffff),
-                       t.n0 + c * kCW, t.x0, t.y0 + m * p.TH, t.img);
+          const uint32_t box = stage + (stage_place(BN_T, kOutBf16, b) & 0xffff);
+          const bool full = (c + 1) * kCW <= BN_T;
+          const int groups = full ? 8 : stage_narrow_row(BN_T, kOutBf16) / 16;   // 16-byte groups per box row
+          for (int i = static_cast<int>(threadIdx.x & 31); i < p.TW * p.TH * groups; i += 32) {
+            const int row = i / groups, g = i - row * groups, cl = c * kCW + g * (16 / kOsz);
+            const int ly = row / p.TW, y = t.y0 + m * p.TH + ly, x = t.x0 + row - ly * p.TW;
+            if (cl >= c_hi || y >= p.Ho || x >= x_lim) continue;
+            const uint32_t addr = full ? box + static_cast<uint32_t>(row * 128 + ((g ^ (row & 7)) << 4))
+                                       : box + static_cast<uint32_t>(row * stage_narrow_row(BN_T, kOutBf16) + 16 * g);
+            uint4 v;
+            asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+            const long long o = t.img * p.out_img_stride + static_cast<long long>(y) * p.out_y_stride + static_cast<long long>(x) * p.ldo + t.n0 + cl;
+            *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(p.out) + o * kOsz) = v;
+          }
         }
-        tma_store_commit();
       }
       // TMA stores write whole 16-byte groups of channels: the output map ends at p.cout_tma (Cout rounded down to 16
       // bytes), and the warp copies the channels from there to Cout (196 = 192 + 4) with plain stores
@@ -333,7 +367,7 @@ __device__ __forceinline__ void store_warp(const ConvGemmParams& p, uint32_t sta
         for (int m = 0; m < MT_T; ++m)
           for (int row = static_cast<int>(threadIdx.x & 31); row < p.TW * p.TH; row += 32) {
             const int ly = row / p.TW, y = t.y0 + m * p.TH + ly, x = t.x0 + row - ly * p.TW;
-            if (y >= p.Ho || x >= p.Wo) continue;
+            if (y >= p.Ho || x >= x_lim) continue;
             const long long o = t.img * p.out_img_stride + static_cast<long long>(y) * p.out_y_stride + static_cast<long long>(x) * p.ldo + t.n0;
             for (int cl = c_lo; cl < c_hi; cl += 2) {
               const int c = cl / kCW, b = m * kNBox + c;
@@ -365,12 +399,13 @@ __device__ __forceinline__ void store_warp(const ConvGemmParams& p, uint32_t sta
 }
 
 // BN_T = N tile (wgmma N), MT_T = 128-pixel sub-tiles per CTA tile, BF16 = operand type, EPI = epilogue kind (kEpiAny:
-// the run-time generic epilogue); the host launches the instantiation equal to (p.BN, p.MT, p.in_bf16, p.epi) and
-// falls back to kEpiAny for an epilogue kind without its own instantiation. Between the wgmma instructions of a group
+// the run-time generic epilogue); the host launches the instantiation equal to (p.BN, p.MT, p.in_bf16, p.epi), and
+// conv_gemm_build only names a kind in p.epi that has one (staged_inst). Between the wgmma instructions of a group
 // there is no control flow (ptxas would otherwise serialise them): every k-block issues 4 k-steps, the channel tail of
 // a 128-byte k-block is zero-filled by TMA, and the 3 unused k-steps of a 32-byte tail group read the zero page.
 template <int BN_T, int MT_T, bool BF16, int EPI>
 __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
+  static_assert(EPI == kEpiAny || staged_inst(EPI, BN_T, BF16), "no TMA-store epilogue for this kind");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t s_bars[4 * kMaxSlots + 2];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -499,7 +534,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_gemm_kernel(const __grid_con
     }
   } else if (warp == 1) {
     // ------------------------------------------------------------------ TMA store warp
-    if constexpr (EPI != kEpiAny) store_warp<BN_T, MT_T, EPI>(p, stage, st_empty, st_full, total_tiles, tiles_x, tile_rows);
+    if constexpr (EPI != kEpiAny) store_warp<BN_T, MT_T, EPI>(p, stage, st_empty, st_full, total_tiles, tiles_x, tile_rows, w_lim);
   } else if (warp >= 4) {
     // ------------------------------------------------------------------ MMA + epilogue warpgroups
     const int wg = (warp - 4) >> 2;                   // rows 64 wg .. 64 wg + 63 of each sub-tile
@@ -810,14 +845,16 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
   p->out_img_stride = d.out_img_stride > 0 ? d.out_img_stride : static_cast<long long>(p->Ho) * p->Wo * d.ldo;
   p->b_xor = d.b_xor;
   p->res_img_stride = static_cast<long long>(p->Ho) * p->Wo * d.ldr;
-  // compile-time epilogue kind with TMA stores: bf16 operands, every column activated, no device row count, one B
-  // operand per image at most, and output / residual rows that tensor maps can address (16-byte strides and pointers)
+  // compile-time epilogue kind with TMA stores: a kind with an instantiation for the operand type (the N tile is
+  // checked once it is chosen), every column activated, no residual together with a device row count, one B operand
+  // per image at most, and output / residual rows that tensor maps can address (16-byte strides and pointers)
   p->epi = kEpiAny;
   {
     const int osz = d.out_bf16 ? 2 : 4;
     auto a16 = [](long long bytes) { return bytes % 16 == 0; };
     const int kind = epi_kind(d.out_bf16 != 0, d.residual != nullptr, d.act);
-    if (d.in_bf16 && d.dyn_w == nullptr && d.b_batched != 2 && p->act_cols >= p->Cout && staged_kind(kind) &&
+    if (staged_inst(kind, kMaxBN, d.in_bf16 != 0) && (d.dyn_w == nullptr || d.residual == nullptr) && d.b_batched != 2 &&
+        p->act_cols >= p->Cout &&
         epilogue_vec2(*p) && (reinterpret_cast<uintptr_t>(d.bias) & 7) == 0 && (reinterpret_cast<uintptr_t>(d.out) & 15) == 0 &&
         a16(p->ldo * osz) && a16(p->out_y_stride * osz) && a16(p->out_img_stride * osz) &&
         (d.residual == nullptr || ((reinterpret_cast<uintptr_t>(d.residual) & 15) == 0 && a16(p->ldr * osz))))
@@ -837,13 +874,8 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
   const int a_rows = p->halo ? p->MT * p->TH + 2 : p->MT * p->TH;   // pixel rows of the A box
   p->a_bytes = p->TW * a_rows * 128;
   p->b_bytes = p->BN * 128;                                           // multiple of 1 KB (BN % 8 == 0)
-  if (p->BN < 128) p->epi = kEpiAny;   // the narrow N tiles run the run-time generic epilogue
-  p->stage_bytes = staging_for(p->epi == kEpiAny ? -1 : (d.out_bf16 ? 1 : 0), p->MT, p->BN);
-  {
-    const RingCfg rc = ring_cfg(p->halo, p->kx_major != 0, p->MT, p->TW, p->TH, p->BN, kOperandBytes - p->stage_bytes);
-    p->a_slot_bytes = rc.a_slot_bytes; p->a_slots = rc.a_slots; p->b_slots = rc.b_slots;
-  }
-  if (p->a_slots < (p->halo && !p->kx_major ? 3 : 2) || p->b_slots < (p->halo ? 4 : 2)) return MFR_ERR_ARG;
+  // the narrow N tiles run the run-time generic epilogue: from here on p->epi names an instantiation
+  if (p->epi != kEpiAny && !staged_inst(p->epi, p->BN, d.in_bf16 != 0)) p->epi = kEpiAny;
   if (p->epi != kEpiAny) {   // output / residual: {Cout, Wo, Ho, N}; the bounds clip ragged tiles and channels >= Cout
     const int osz = d.out_bf16 ? 2 : 4, cw = stage_cw(d.out_bf16 != 0);
     const CUtensorMapDataType dt = d.out_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
@@ -866,8 +898,15 @@ int conv_gemm_build(const ConvGemmDesc& d, ConvGemmParams* p) {
     dims[0] = d.Cout;   // the residual is read up to Cout (channels beyond come back as zeros)
     if (ok && d.residual != nullptr)
       ok = encode(&p->tmR, &p->tmR2, d.residual, p->ldr, static_cast<long long>(p->Wo) * p->ldr, p->res_img_stride);
-    if (!ok) p->epi = kEpiAny;   // strides a tensor map cannot take: the run-time generic epilogue (the ring stays valid)
+    if (!ok) p->epi = kEpiAny;   // strides a tensor map cannot take: the run-time generic epilogue
   }
+  // the staging buffer and the rings follow the final p->epi
+  p->stage_bytes = staging_for(p->epi == kEpiAny ? -1 : (d.out_bf16 ? 1 : 0), p->MT, p->BN);
+  {
+    const RingCfg rc = ring_cfg(p->halo, p->kx_major != 0, p->MT, p->TW, p->TH, p->BN, kOperandBytes - p->stage_bytes);
+    p->a_slot_bytes = rc.a_slot_bytes; p->a_slots = rc.a_slots; p->b_slots = rc.b_slots;
+  }
+  if (p->a_slots < (p->halo && !p->kx_major ? 3 : 2) || p->b_slots < (p->halo ? 4 : 2)) return MFR_ERR_ARG;
 
   {  // activations: {C, W, H, N}
     cuuint64_t dims[4] = {(cuuint64_t)d.Cin, (cuuint64_t)d.W, (cuuint64_t)d.H, (cuuint64_t)d.N};
@@ -968,19 +1007,26 @@ int launch_one(const ConvGemmParams& p, int grid, cudaStream_t stream) {
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
 }
-template <int BN_T, int MT_T>
-int launch_inst(const ConvGemmParams& p, int grid, cudaStream_t stream) {
-  if (!p.in_bf16) return launch_one<BN_T, MT_T, false, kEpiAny>(p, grid, stream);
+template <int BN_T, int MT_T, bool BF16>
+int launch_typed(const ConvGemmParams& p, int grid, cudaStream_t stream) {
+  if (p.epi == kEpiAny) return launch_one<BN_T, MT_T, BF16, kEpiAny>(p, grid, stream);
   if constexpr (BN_T >= 128) {   // the compile-time epilogue kinds (TMA stores) have their own instantiations
     switch (p.epi) {
-      case kBf: return launch_one<BN_T, MT_T, true, kBf>(p, grid, stream);
-      case kBfRelu: return launch_one<BN_T, MT_T, true, kBfRelu>(p, grid, stream);
-      case kBfLeaky: return launch_one<BN_T, MT_T, true, kBfLeaky>(p, grid, stream);
-      case kBfResRelu: return launch_one<BN_T, MT_T, true, kBfResRelu>(p, grid, stream);
-      case kF32: return launch_one<BN_T, MT_T, true, kF32>(p, grid, stream);
+      case kF32: return launch_one<BN_T, MT_T, BF16, kF32>(p, grid, stream);
+      case kBf: if constexpr (BF16) return launch_one<BN_T, MT_T, true, kBf>(p, grid, stream); break;
+      case kBfRelu: if constexpr (BF16) return launch_one<BN_T, MT_T, true, kBfRelu>(p, grid, stream); break;
+      case kBfLeaky: if constexpr (BF16) return launch_one<BN_T, MT_T, true, kBfLeaky>(p, grid, stream); break;
+      case kBfResRelu: if constexpr (BF16) return launch_one<BN_T, MT_T, true, kBfResRelu>(p, grid, stream); break;
     }
   }
-  return launch_one<BN_T, MT_T, true, kEpiAny>(p, grid, stream);
+  // conv_gemm_build names only kinds with an instantiation (staged_inst): a params block that gets here is not its own
+  fprintf(stderr, "[mfr_b200] conv_gemm: no TMA-store kernel for epilogue kind %d at BN %d (%s operands)\n", p.epi, BN_T,
+          BF16 ? "bf16" : "tf32");
+  return MFR_ERR_UNSUPPORTED;
+}
+template <int BN_T, int MT_T>
+int launch_inst(const ConvGemmParams& p, int grid, cudaStream_t stream) {
+  return p.in_bf16 ? launch_typed<BN_T, MT_T, true>(p, grid, stream) : launch_typed<BN_T, MT_T, false>(p, grid, stream);
 }
 }  // namespace
 

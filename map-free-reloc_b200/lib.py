@@ -47,6 +47,8 @@ SIGNATURES = {
                                      c_vp, c_ll, c_vp]),
     "mfr_conv2d_nhwc_bf16": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_ll, c_vp, c_ll, c_int, c_int, c_int,
                                      c_int, c_int, c_vp, c_vp, c_ll, c_int, c_float, c_vp, c_ll, c_int, c_vp]),
+    "mfr_token_gemm_dyn_rows": (c_int, [c_vp, c_int, c_int, c_int, c_ll, c_vp, c_ll, c_int, c_int, c_vp, c_int, c_vp,
+                                        c_ll, c_int, c_vp, c_vp]),
     "mfr_loftr_create": (c_int, [c_int, c_int, c_int, c_float, c_int, c_float, c_int, c_int, c_pp]),
     "mfr_loftr_destroy": (None, [c_vp]),
     "mfr_loftr_num_weights": (c_int, [c_vp]),

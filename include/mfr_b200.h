@@ -131,6 +131,14 @@ int mfr_loftr_num_launches(const mfr_loftr* h); /* kernel launches per forward *
  * Returns the number of steps (or a negative MFR_ERR_*). */
 int mfr_loftr_profile(mfr_loftr* h, const float* img0, const float* img1, int src_h, int src_w,
                       void* stream, int max_steps, float* ms, double* flops, int* kinds, char* names);
+/* Stage-wise tests of buffers the forward overwrites later. mfr_loftr_step_name(h, i) is the name of step i of the
+ * paired forward list ("stem", a conv's weight name such as "layer2.0.down", "upsample", "split3", ...), NULL when i is
+ * out of range; the string lives as long as the engine. mfr_loftr_run_steps runs steps [begin, end) of that list
+ * eagerly on the engine's buffers as the previous calls left them (the staged images of the last forward), after
+ * rebuilding the derived weight copies as a forward does. MFR_ERR_ARG when the range is not within the list or a
+ * weight has not been uploaded. Neither is used by the forward or its CUDA graph. */
+const char* mfr_loftr_step_name(const mfr_loftr* h, int i);
+int mfr_loftr_run_steps(mfr_loftr* h, int begin, int end, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * SuperPoint + SuperGlue matcher engine. Replaces Matching.forward of the reference

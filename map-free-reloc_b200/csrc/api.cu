@@ -137,6 +137,14 @@ int mfr_loftr_profile(mfr_loftr* h, const float* img0, const float* img1, int sr
   return mfr::loftr_profile(h->e, img0, img1, src_h, src_w, static_cast<cudaStream_t>(stream), max_steps, ms, flops,
                             kinds, names);
 }
+const char* mfr_loftr_step_name(const mfr_loftr* h, int i) {
+  if (!h || i < 0 || i >= core(h).steps.size()) return nullptr;
+  return core(h).steps.steps[i].name.c_str();
+}
+int mfr_loftr_run_steps(mfr_loftr* h, int begin, int end, void* stream) {
+  if (!h) return MFR_ERR_ARG;
+  return mfr::loftr_run_steps(h->e, begin, end, static_cast<cudaStream_t>(stream));
+}
 
 // ------------------------------------------------------------------------------------------ SuperPoint + SuperGlue
 struct mfr_spsg { mfr::SpsgEngine* e; };

@@ -2,6 +2,7 @@
 // buffers with a debug registry, the fp32 weight table and the GEMM copies derived from it, launch lists and the CUDA
 // graphs they are replayed through.
 #pragma once
+#include <cstdint>
 #include <functional>
 #include <map>
 #include <string>
@@ -185,8 +186,8 @@ struct LaunchList {
     for (const auto& s : steps) n += s.launches;
     return n;
   }
-  int run(cudaStream_t st, size_t begin = 0) const {
-    for (size_t i = begin; i < steps.size(); ++i) {
+  int run(cudaStream_t st, size_t begin = 0, size_t end = SIZE_MAX) const {
+    for (size_t i = begin; i < steps.size() && i < end; ++i) {
       const int rc = steps[i].f(st);
       if (rc != MFR_OK) return rc;
     }

@@ -600,6 +600,14 @@ struct LoftrEngine : EngineCore {
     return shared_graph.launch(shared_steps, st, use_graph, "loftr");
   }
 
+  // Steps [begin, end) of the paired forward list, eagerly, on the buffers as earlier calls left them
+  int run_steps(int begin, int end, cudaStream_t st) {
+    if (begin < 0 || end < begin || end > steps.size() || !weights.complete()) return MFR_ERR_ARG;
+    const int r = derived.rebuild(weights, st);
+    if (r != MFR_OK) return r;
+    return steps.run(st, begin, end);
+  }
+
   // eager run with a CUDA event pair around every step; ms[i] = device time of step i
   int profile(const float* img0, const float* img1, int src_h, int src_w, cudaStream_t st, int max_steps,
               float* ms, double* flops, int* kinds, char* names) {
@@ -658,5 +666,6 @@ int loftr_profile(LoftrEngine* e, const float* img0, const float* img1, int src_
                   int max_steps, float* ms, double* flops, int* kinds, char* names) {
   return e->profile(img0, img1, src_h, src_w, st, max_steps, ms, flops, kinds, names);
 }
+int loftr_run_steps(LoftrEngine* e, int begin, int end, cudaStream_t st) { return e->run_steps(begin, end, st); }
 
 }  // namespace mfr

@@ -17,5 +17,6 @@ int loftr_forward_shared(LoftrEngine* e, const float* img1, int src_h, int src_w
 void loftr_outputs(LoftrEngine* e, mfr_loftr_outputs* o);
 int loftr_profile(LoftrEngine* e, const float* img0, const float* img1, int src_h, int src_w, cudaStream_t st,
                   int max_steps, float* ms, double* flops, int* kinds, char* names);
+int loftr_run_steps(LoftrEngine* e, int begin, int end, cudaStream_t st);
 
 }  // namespace mfr

@@ -64,6 +64,8 @@ SIGNATURES = {
     "mfr_loftr_num_kernels": (c_int, [c_vp]),
     "mfr_loftr_num_launches": (c_int, [c_vp]),
     "mfr_loftr_profile": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_vp]),
+    "mfr_loftr_step_name": (ctypes.c_char_p, [c_vp, c_int]),
+    "mfr_loftr_run_steps": (c_int, [c_vp, c_int, c_int, c_vp]),
     "mfr_spsg_create": (c_int, [c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_int, c_float, c_pp]),
     "mfr_spsg_create_ex": (c_int, [c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_int, c_float, c_int, c_pp]),
     "mfr_spsg_destroy": (None, [c_vp]),

@@ -338,6 +338,23 @@ class LoFTR:
         return [(raw[32 * i:32 * i + 32].split(b"\0")[0].decode(), int(kinds[i]), float(ms[i]), float(fl[i]))
                 for i in range(rc)]
 
+    def step_names(self):
+        """Names of the steps of the paired forward list, in launch order ("stem", "layer1.0.conv1", "upsample", ...)."""
+        names = []
+        while (n := self._l.mfr_loftr_step_name(self._h, len(names))) is not None:
+            names.append(n.decode())
+        return names
+
+    def run_steps(self, begin, end):
+        """Runs steps [begin, end) of the forward list eagerly on the engine's buffers as the last call left them (stage
+        tests: a forward stages the images first). Ordered after the current stream's work and before its later work."""
+        cur = torch.cuda.current_stream(self.device)
+        self.stream.wait_stream(cur)
+        with torch.cuda.stream(self.stream):
+            _lib.check(self._l.mfr_loftr_run_steps(self._h, int(begin), int(end), ctypes.c_void_p(self.stream.cuda_stream)),
+                       f"loftr run_steps [{begin}, {end})")
+        cur.wait_stream(self.stream)
+
     def _wrap(self, ptr, shape, dtype):
         return _lib.device_view(ptr, shape, dtype, self.device)
 

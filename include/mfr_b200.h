@@ -261,6 +261,38 @@ int mfr_sift_debug_tensor(mfr_sift* h, const char* name, float** ptr, long long*
  * selection, descriptors. */
 int mfr_sift_profile(mfr_sift* h, const unsigned char* imgs, float* ms, void* stream);
 
+/* SIFT pair engine for P pairs of uint8 gray images [H][W]: detection (mfr_sift_detect's engine and settings) and Lowe ratio
+ * matching (mfr_sift_match_pairs's) of both images of every pair, with the matches in engine-owned buffers in the pose
+ * back end's layout. Bit-identical to mfr_sift_detect on the pair-interleaved batch (image 2p = img0[p], 2p + 1 =
+ * img1[p]) followed by mfr_sift_match_pairs(ratio). Holds a B = 2P engine, a B = P engine for the queries of the shared
+ * map path and a B = 1 engine for the map image. */
+typedef struct mfr_sift_pairs mfr_sift_pairs;
+typedef struct {
+  const float* kpts0;         /* device float[capacity][2]: x, y of the matched keypoints of image 0, pair after pair */
+  const float* kpts1;         /* device float[capacity][2]: their nearest neighbours in image 1 */
+  const int* offsets;         /* device int[P + 1]: matches of pair p are rows offsets[p] .. offsets[p + 1] - 1 */
+  const int* overflow;        /* device int[P]: 1 when an image of pair p (or the map) had more refined extrema or oriented
+                                 keypoints than max_candidates; its matches are then incomplete */
+  int capacity;               /* = P * max_candidates */
+  int max_pts_per_pair;       /* = max_candidates: matches of one pair never exceed it */
+} mfr_sift_pair_outputs;
+int mfr_sift_pairs_create(int P, int H, int W, int nfeatures, int max_candidates, int root_sift, float ratio,
+                          mfr_sift_pairs** out);
+void mfr_sift_pairs_destroy(mfr_sift_pairs* h);
+void mfr_sift_pairs_set_graph(mfr_sift_pairs* h, int enabled);
+/* img0 / img1: device uint8 [P][H][W]. Two device copies stage them into the pair-interleaved input, then one launch list
+ * (detect, 2-NN, ratio test, offsets, ordered compaction, overflow flags) runs as one CUDA graph. No host synchronisation
+ * (after the first call, which captures the graph). Outputs are valid until the next forward on the handle. */
+int mfr_sift_forward_pairs(mfr_sift_pairs* h, const unsigned char* img0, const unsigned char* img1, void* stream);
+/* Detects and describes the map image img0 (device uint8 [H][W]) once, eagerly, into buffers of its own, valid until the
+ * next set_map; paired forwards in between leave them intact. */
+int mfr_sift_set_map(mfr_sift_pairs* h, const unsigned char* img0, void* stream);
+/* img1: device uint8 [P][H][W] query images, ratio-matched against the map of set_map (the map's descriptors are the
+ * knn query set, as image 0 of a pair is): the bits of mfr_sift_forward_pairs with the map repeated for every pair.
+ * One CUDA graph; MFR_ERR_ARG before the first set_map. */
+int mfr_sift_forward_shared(mfr_sift_pairs* h, const unsigned char* img1, void* stream);
+int mfr_sift_get_pair_outputs(mfr_sift_pairs* h, mfr_sift_pair_outputs* out);
+
 /* ---------------------------------------------------------------------------------------------
  * Pose back end (batched-hypothesis RANSAC). Replaces lib/models/matching/pose_solver.py.
  * Correspondences of P pairs are concatenated: kpts0/kpts1 device float[total][2] in pixels (x,y),

@@ -263,6 +263,36 @@ int mfr_sift_profile(mfr_sift* h, const unsigned char* imgs, float* ms, void* st
   return mfr::sift_profile(h->e, imgs, ms, static_cast<cudaStream_t>(stream));
 }
 
+struct mfr_sift_pairs { mfr::SiftPairs* e; };
+int mfr_sift_pairs_create(int P, int H, int W, int nfeatures, int max_candidates, int root_sift, float ratio,
+                          mfr_sift_pairs** out) {
+  if (!out) return MFR_ERR_ARG;
+  mfr::SiftPairs* e = nullptr;
+  int rc = mfr::sift_pairs_create(P, H, W, nfeatures, max_candidates, root_sift, ratio, &e);
+  if (rc != MFR_OK) return rc;
+  *out = new mfr_sift_pairs{e};
+  return MFR_OK;
+}
+void mfr_sift_pairs_destroy(mfr_sift_pairs* h) { if (h) { mfr::sift_pairs_destroy(h->e); delete h; } }
+void mfr_sift_pairs_set_graph(mfr_sift_pairs* h, int enabled) { if (h) core(h).use_graph = enabled != 0; }
+int mfr_sift_forward_pairs(mfr_sift_pairs* h, const unsigned char* img0, const unsigned char* img1, void* stream) {
+  if (!h) return MFR_ERR_ARG;
+  return mfr::sift_forward_pairs(h->e, img0, img1, static_cast<cudaStream_t>(stream));
+}
+int mfr_sift_set_map(mfr_sift_pairs* h, const unsigned char* img0, void* stream) {
+  if (!h) return MFR_ERR_ARG;
+  return mfr::sift_pairs_set_map(h->e, img0, static_cast<cudaStream_t>(stream));
+}
+int mfr_sift_forward_shared(mfr_sift_pairs* h, const unsigned char* img1, void* stream) {
+  if (!h) return MFR_ERR_ARG;
+  return mfr::sift_forward_shared(h->e, img1, static_cast<cudaStream_t>(stream));
+}
+int mfr_sift_get_pair_outputs(mfr_sift_pairs* h, mfr_sift_pair_outputs* out) {
+  if (!h || !out) return MFR_ERR_ARG;
+  mfr::sift_pair_outputs(h->e, out);
+  return MFR_OK;
+}
+
 // ------------------------------------------------------------------------------------------ pose back end
 struct mfr_pose_solver { mfr::PoseSolver* s; };
 

@@ -27,17 +27,19 @@ __device__ __forceinline__ void push(Best2& b, float d, int j) {
 
 // one block (128 threads) per query descriptor (grid-stride over queries); dim <= 256 and a multiple of 4.
 // blockIdx.y = pair p: its queries / train rows / outputs start p * q_stride / t_stride / o_stride rows in, and
-// with `counts` non-null the row counts are counts[2p] (queries) and counts[2p + 1] (train), read on the device.
+// with `qc` / `tc` non-null the row counts are qc[p * qc_stride] (queries) / tc[p * tc_stride] (train), read on the device.
 __global__ void __launch_bounds__(128, 8) knn2_kernel(const float* __restrict__ q, int nq,
                                                    const float* __restrict__ t, int nt, int dim,
                                                    int* __restrict__ idx1, float* __restrict__ dist1,
                                                    int* __restrict__ idx2, float* __restrict__ dist2,
                                                    long long q_stride, long long t_stride, long long o_stride,
-                                                   const int* __restrict__ counts) {
+                                                   const int* __restrict__ qc, int qc_stride,
+                                                   const int* __restrict__ tc, int tc_stride) {
   __shared__ __align__(16) float sq[256];
   __shared__ Best2 sb[4];
   const int p = blockIdx.y;
-  if (counts) { nq = counts[2 * p]; nt = counts[2 * p + 1]; }
+  if (qc) nq = qc[p * qc_stride];
+  if (tc) nt = tc[p * tc_stride];
   q += p * q_stride * dim; t += p * t_stride * dim;
   idx1 += p * o_stride; dist1 += p * o_stride; idx2 += p * o_stride; dist2 += p * o_stride;
   for (int qi = blockIdx.x; qi < nq; qi += gridDim.x) {
@@ -87,7 +89,7 @@ int knn2_l2(const float* q, int nq, const float* t, int nt, int dim, int* idx1, 
             float* dist2, cudaStream_t st) {
   if (nq <= 0) return MFR_OK;
   if (dim > 256 || (dim & 3) || nt < 0) return MFR_ERR_ARG;
-  knn2_kernel<<<nq, 128, 0, st>>>(q, nq, t, nt, dim, idx1, dist1, idx2, dist2, 0, 0, 0, nullptr);
+  knn2_kernel<<<nq, 128, 0, st>>>(q, nq, t, nt, dim, idx1, dist1, idx2, dist2, 0, 0, 0, nullptr, 0, nullptr, 0);
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
 }
@@ -98,7 +100,17 @@ int knn2_l2_pairs(const float* desc, const int* counts, int P, int cap, int dim,
   if (dim > 256 || (dim & 3)) return MFR_ERR_ARG;
   const dim3 grid(std::min(cap, 1024), P);
   knn2_kernel<<<grid, 128, 0, st>>>(desc, cap, desc + static_cast<size_t>(cap) * dim, cap, dim, idx1, dist1, idx2, dist2,
-                                    2LL * cap, 2LL * cap, cap, counts);
+                                    2LL * cap, 2LL * cap, cap, counts, 2, counts + 1, 2);
+  MFR_CUDA_CHECK(cudaGetLastError());
+  return MFR_OK;
+}
+
+int knn2_l2_shared(const float* q, const int* q_count, const float* t, const int* t_counts, int P, int cap, int dim,
+                   int* idx1, float* dist1, int* idx2, float* dist2, cudaStream_t st) {
+  if (P <= 0 || cap <= 0) return MFR_OK;
+  if (dim > 256 || (dim & 3)) return MFR_ERR_ARG;
+  const dim3 grid(std::min(cap, 1024), P);
+  knn2_kernel<<<grid, 128, 0, st>>>(q, cap, t, cap, dim, idx1, dist1, idx2, dist2, 0, cap, cap, q_count, 0, t_counts, 1);
   MFR_CUDA_CHECK(cudaGetLastError());
   return MFR_OK;
 }

@@ -536,11 +536,13 @@ __global__ void __launch_bounds__(kDescThreads) descriptor_kernel(Pyr pyr, const
 }
 
 // ---------------------------------------------------------------------------------------------------- ratio test
-// block per pair: good[q] = (train count >= 2) && d1 < ratio * d2; pair_n[p] = number of good queries
-__global__ void ratio_count_kernel(const int* __restrict__ counts, const float* __restrict__ d1, const float* __restrict__ d2,
-                                   int cap, float ratio, unsigned char* __restrict__ good, int* __restrict__ pair_n) {
+// block per pair: good[q] = (train count >= 2) && d1 < ratio * d2; pair_n[p] = number of good queries. Pair p's query /
+// train counts are qc[p * qs] / tc[p * ts].
+__global__ void ratio_count_kernel(const int* __restrict__ qc, int qs, const int* __restrict__ tc, int ts,
+                                   const float* __restrict__ d1, const float* __restrict__ d2, int cap, float ratio,
+                                   unsigned char* __restrict__ good, int* __restrict__ pair_n) {
   const int p = blockIdx.x;
-  const int nq = counts[2 * p], nt = counts[2 * p + 1];
+  const int nq = qc[p * qs], nt = tc[p * ts];
   __shared__ int s_n;
   if (threadIdx.x == 0) s_n = 0;
   __syncthreads();
@@ -563,15 +565,17 @@ __global__ void pair_offsets_kernel(const int* __restrict__ pair_n, int P, int* 
   offsets[P] = s;
 }
 
-// block per pair: ordered compaction of the good queries (query order, = np.where(good)) into the pose back end's layout
-__global__ void __launch_bounds__(256) compact_matches_kernel(const int* __restrict__ counts, const unsigned char* __restrict__ good,
-                                                              const int* __restrict__ i1, const float* __restrict__ kps, int cap,
+// block per pair: ordered compaction of the good queries (query order, = np.where(good)) into the pose back end's layout.
+// Pair p's query keypoints are image p * s0 of kp0 (qc[p * qs] of them), its train keypoints image p * s1 of kp1.
+__global__ void __launch_bounds__(256) compact_matches_kernel(const int* __restrict__ qc, int qs, const unsigned char* __restrict__ good,
+                                                              const int* __restrict__ i1, const float* __restrict__ kp0, int s0,
+                                                              const float* __restrict__ kp1, int s1, int cap,
                                                               const int* __restrict__ offsets, float* __restrict__ k0,
                                                               float* __restrict__ k1) {
   __shared__ int s_warp[8];
   __shared__ int s_base;
   const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int nq = counts[2 * p];
+  const int nq = qc[p * qs];
   if (tid == 0) s_base = offsets[p];
   __syncthreads();
   for (int c0 = 0; c0 < nq; c0 += 256) {
@@ -589,13 +593,23 @@ __global__ void __launch_bounds__(256) compact_matches_kernel(const int* __restr
     __syncthreads();
     if (g) {
       const int dst = s_warp[wid] + __popc(m & ((1u << lane) - 1u));
-      const float* a = kps + (static_cast<size_t>(2 * p) * cap + q) * 5;
-      const float* c = kps + (static_cast<size_t>(2 * p + 1) * cap + i1[o]) * 5;
+      const float* a = kp0 + (static_cast<size_t>(p) * s0 * cap + q) * 5;
+      const float* c = kp1 + (static_cast<size_t>(p) * s1 * cap + i1[o]) * 5;
       k0[2 * dst] = a[0]; k0[2 * dst + 1] = a[1];
       k1[2 * dst] = c[0]; k1[2 * dst + 1] = c[1];
     }
     __syncthreads();
   }
+}
+
+// flag[p] = 1 when image 0 (counters c0, B0 images, index p * s0 + o0) or image 1 (c1, B1, p * s1 + o1) of pair p found more
+// refined extrema or oriented keypoints than the capacity: its keypoints, and so the pair's matches, are then incomplete
+__global__ void overflow_kernel(const int* __restrict__ c0, int B0, int s0, int o0, const int* __restrict__ c1, int B1, int s1,
+                                int o1, int cap, int P, int* __restrict__ flag) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= P) return;
+  const int i0 = p * s0 + o0, i1 = p * s1 + o1;
+  flag[p] = c0[i0] > cap || c0[B0 + i0] > cap || c1[i1] > cap || c1[B1 + i1] > cap;
 }
 
 // getGaussianKernel(ksize, sigma, CV_32F): exp in double, rounded to float, normalised in double, rounded again
@@ -799,9 +813,10 @@ struct SiftEngine : EngineCore {
     int* cnt = counters + 2 * B;
     int r = knn2_l2_pairs(desc, cnt, P, cap, 128, m_i1, m_d1, m_i2, m_d2, st);
     if (r != MFR_OK) return r;
-    ratio_count_kernel<<<P, 256, 0, st>>>(cnt, m_d1, m_d2, cap, ratio, m_good, pair_n);
+    ratio_count_kernel<<<P, 256, 0, st>>>(cnt, 2, cnt + 1, 2, m_d1, m_d2, cap, ratio, m_good, pair_n);
     pair_offsets_kernel<<<1, 32, 0, st>>>(pair_n, P, offsets);
-    compact_matches_kernel<<<P, 256, 0, st>>>(cnt, m_good, m_i1, out_kp, cap, offsets, k0, k1);
+    compact_matches_kernel<<<P, 256, 0, st>>>(cnt, 2, m_good, m_i1, out_kp, 2, out_kp + static_cast<size_t>(cap) * 5, 2, cap,
+                                              offsets, k0, k1);
     MFR_CUDA_CHECK(cudaGetLastError());
     return MFR_OK;
   }
@@ -833,5 +848,119 @@ int sift_match_pairs(SiftEngine* e, float ratio, float* kpts0, float* kpts1, int
   return e->match_pairs(ratio, kpts0, kpts1, offsets, st);
 }
 int sift_profile(SiftEngine* e, const unsigned char* imgs, float* ms, cudaStream_t st) { return e->profile(imgs, ms, st); }
+
+// P pairs as a pair engine: detection of the 2P pair-interleaved images (image 2p = img0[p], 2p + 1 = img1[p]), 2-NN,
+// ratio test, offsets and the ordered compaction, in one launch list replayed as one CUDA graph, with no host
+// synchronisation. The kernels and their inputs are those of SiftEngine::detect + match_pairs, so the outputs are the
+// same bits. The shared-map path detects the map once (its own B = 1 engine, eagerly) and the P queries in a B = P
+// engine; per-image detection does not depend on the batch, so it gives the bits of the paired path with the map
+// repeated.
+struct SiftPairs : EngineCore {
+  int P = 0, cap = 0;
+  float ratio = 0.8f;
+  SiftEngine *pair = nullptr, *query = nullptr, *map = nullptr;
+  float *k0 = nullptr, *k1 = nullptr;
+  int *offsets = nullptr, *overflow = nullptr;
+  bool map_set = false;
+  LaunchList shared_steps;
+  GraphExec graph, shared_graph;
+
+  // the matching half: knn + ratio test + offsets + compaction + overflow flags, appended to a detection list
+  void push_match(LaunchList& list, const float* d0, const int* qc, int qs, const float* kp0, int s0, const float* d1,
+                  const int* tc, int ts, const float* kp1, int s1, bool shared, const int* c0, int B0, int cs0, int co0,
+                  const int* c1, int B1, int cs1, int co1) {
+    const int np = P, cp = cap;
+    const float rt = ratio;
+    int *i1 = pair->m_i1, *i2 = pair->m_i2, *pn = pair->pair_n, *off = offsets, *ov = overflow;
+    float *dd1 = pair->m_d1, *dd2 = pair->m_d2, *o0 = k0, *o1 = k1;
+    unsigned char* good = pair->m_good;
+    list.push([=](cudaStream_t st) {
+      return shared ? knn2_l2_shared(d0, qc, d1, tc, np, cp, 128, i1, dd1, i2, dd2, st)
+                    : knn2_l2_pairs(d0, qc, np, cp, 128, i1, dd1, i2, dd2, st);
+    }, "knn2");
+    list.push([=](cudaStream_t st) {
+      ratio_count_kernel<<<np, 256, 0, st>>>(qc, qs, tc, ts, dd1, dd2, cp, rt, good, pn);
+      pair_offsets_kernel<<<1, 32, 0, st>>>(pn, np, off);
+      compact_matches_kernel<<<np, 256, 0, st>>>(qc, qs, good, i1, kp0, s0, kp1, s1, cp, off, o0, o1);
+      overflow_kernel<<<(np + 127) / 128, 128, 0, st>>>(c0, B0, cs0, co0, c1, B1, cs1, co1, cp, np, ov);
+      MFR_CUDA_CHECK(cudaGetLastError());
+      return MFR_OK;
+    }, "ratio_compact", 4);
+  }
+
+  int build(int H, int W, int nfeat, int root) {
+    int r = sift_create(2 * P, H, W, nfeat, cap, root, &pair);
+    if (r == MFR_OK) r = sift_create(P, H, W, nfeat, cap, root, &query);
+    if (r == MFR_OK) r = sift_create(1, H, W, nfeat, cap, root, &map);
+    if (r != MFR_OK) return r;
+    const size_t pc = static_cast<size_t>(P) * cap;
+    k0 = mem.alloc<float>(pc * 2, "kpts0"); k1 = mem.alloc<float>(pc * 2, "kpts1");
+    offsets = mem.alloc<int>(P + 1, "offsets"); overflow = mem.alloc<int>(P, "overflow");
+    if (rc != MFR_OK) return rc;
+    // paired: image 0 of pair p is image 2p of the pair engine, image 1 is 2p + 1
+    steps.append(pair->steps, 0, pair->steps.size());
+    const int B2 = 2 * P;
+    const int* pc_sel = pair->counters + 2 * B2;
+    push_match(steps, pair->desc, pc_sel, 2, pair->out_kp, 2, pair->desc + static_cast<size_t>(cap) * 128, pc_sel + 1, 2,
+               pair->out_kp + static_cast<size_t>(cap) * 5, 2, false, pair->counters, B2, 2, 0, pair->counters, B2, 2, 1);
+    // shared: image 0 of every pair is the map image (stride 0), image 1 of pair p is query image p
+    shared_steps.append(query->steps, 0, query->steps.size());
+    const int* mc_sel = map->counters + 2;
+    const int* qc_sel = query->counters + 2 * P;
+    push_match(shared_steps, map->desc, mc_sel, 0, map->out_kp, 0, query->desc, qc_sel, 1, query->out_kp, 1, true,
+               map->counters, 1, 0, 0, query->counters, P, 1, 0);
+    return rc;
+  }
+
+  // img0 / img1: device uint8 [P][H][W], staged into the pair-interleaved input (the graph does not depend on their
+  // addresses)
+  int forward_pairs(const unsigned char* img0, const unsigned char* img1, cudaStream_t st) {
+    if (!img0 || !img1) return MFR_ERR_ARG;
+    const size_t hw = static_cast<size_t>(pair->H) * pair->W;
+    MFR_CUDA_CHECK(cudaMemcpy2DAsync(pair->img_u8, 2 * hw, img0, hw, hw, P, cudaMemcpyDeviceToDevice, st));
+    MFR_CUDA_CHECK(cudaMemcpy2DAsync(pair->img_u8 + hw, 2 * hw, img1, hw, hw, P, cudaMemcpyDeviceToDevice, st));
+    return graph.launch(steps, st, use_graph, "sift_pairs");
+  }
+  int set_map(const unsigned char* img0, cudaStream_t st) {
+    if (!img0) return MFR_ERR_ARG;
+    map_set = false;
+    MFR_CUDA_CHECK(cudaMemcpyAsync(map->img_u8, img0, static_cast<size_t>(map->H) * map->W, cudaMemcpyDeviceToDevice, st));
+    const int r = map->steps.run(st);
+    if (r != MFR_OK) return r;
+    map_set = true;
+    return MFR_OK;
+  }
+  int forward_shared(const unsigned char* img1, cudaStream_t st) {
+    if (!img1 || !map_set) return MFR_ERR_ARG;
+    MFR_CUDA_CHECK(cudaMemcpyAsync(query->img_u8, img1, static_cast<size_t>(P) * query->H * query->W, cudaMemcpyDeviceToDevice, st));
+    return shared_graph.launch(shared_steps, st, use_graph, "sift_pairs_shared");
+  }
+
+  ~SiftPairs() {
+    delete pair; delete query; delete map;
+  }
+};
+
+int sift_pairs_create(int P, int H, int W, int nfeatures, int max_candidates, int root_sift, float ratio, SiftPairs** out) {
+  if (!out || P < 1 || !(ratio > 0.f)) return MFR_ERR_ARG;
+  auto* e = new SiftPairs();
+  e->P = P; e->cap = max_candidates; e->ratio = ratio;
+  const int rc = e->build(H, W, nfeatures, root_sift);
+  if (rc != MFR_OK) { delete e; return rc; }
+  *out = e;
+  return MFR_OK;
+}
+void sift_pairs_destroy(SiftPairs* e) { delete e; }
+EngineCore& engine_core(SiftPairs* e) { return *e; }
+int sift_forward_pairs(SiftPairs* e, const unsigned char* img0, const unsigned char* img1, cudaStream_t st) {
+  return e->forward_pairs(img0, img1, st);
+}
+int sift_pairs_set_map(SiftPairs* e, const unsigned char* img0, cudaStream_t st) { return e->set_map(img0, st); }
+int sift_forward_shared(SiftPairs* e, const unsigned char* img1, cudaStream_t st) { return e->forward_shared(img1, st); }
+void sift_pair_outputs(SiftPairs* e, mfr_sift_pair_outputs* o) {
+  o->kpts0 = e->k0; o->kpts1 = e->k1; o->offsets = e->offsets; o->overflow = e->overflow;
+  o->capacity = e->P * e->cap; o->max_pts_per_pair = e->cap;
+}
+
 
 }  // namespace mfr

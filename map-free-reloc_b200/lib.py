@@ -36,6 +36,12 @@ class SiftOutputs(ctypes.Structure):
                 ("octaves", c_vp), ("descriptors", c_vp), ("capacity", c_int)]
 
 
+class SiftPairOutputs(ctypes.Structure):
+    """mfr_sift_pair_outputs of include/mfr_b200.h."""
+    _fields_ = [("kpts0", c_vp), ("kpts1", c_vp), ("offsets", c_vp), ("overflow", c_vp), ("capacity", c_int),
+                ("max_pts_per_pair", c_int)]
+
+
 c_pp = ctypes.POINTER(ctypes.c_void_p)
 
 # name -> (restype, argtypes); mirrors include/mfr_b200.h one to one
@@ -92,6 +98,13 @@ SIGNATURES = {
     "mfr_sift_match_pairs": (c_int, [c_vp, c_float, c_vp, c_vp, c_vp, c_vp]),
     "mfr_sift_debug_tensor": (c_int, [c_vp, ctypes.c_char_p, c_pp, ctypes.POINTER(c_ll)]),
     "mfr_sift_profile": (c_int, [c_vp, c_vp, c_vp, c_vp]),
+    "mfr_sift_pairs_create": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_pp]),
+    "mfr_sift_pairs_destroy": (None, [c_vp]),
+    "mfr_sift_pairs_set_graph": (None, [c_vp, c_int]),
+    "mfr_sift_forward_pairs": (c_int, [c_vp, c_vp, c_vp, c_vp]),
+    "mfr_sift_set_map": (c_int, [c_vp, c_vp, c_vp]),
+    "mfr_sift_forward_shared": (c_int, [c_vp, c_vp, c_vp]),
+    "mfr_sift_get_pair_outputs": (c_int, [c_vp, ctypes.POINTER(SiftPairOutputs)]),
     "mfr_pose_solver_create": (c_int, [c_int, c_int, c_int, c_pp]),
     "mfr_pose_solver_destroy": (None, [c_vp]),
     "mfr_pose_solver_debug_tensor": (c_int, [c_vp, ctypes.c_char_p, c_pp, ctypes.POINTER(c_ll)]),

@@ -276,6 +276,8 @@ def functional_state_dict(coarse_scale=200.0, fine_scale=30.0, ln_gain=40.0, noi
 class LoFTR:
     """CUDA LoFTR engine for ``batch`` pairs of [H, W] images (H, W multiples of 8)."""
 
+    input_dtype = torch.float32
+
     def __init__(self, state_dict, batch=1, height=720, width=544, cfg=None, device=0, graph=True,
                  precision="tf32", pipelined=False):
         if not torch.cuda.is_available():
@@ -305,6 +307,7 @@ class LoFTR:
         _lib.check(self._l.mfr_loftr_get_outputs(self._h, ctypes.byref(o)))
         self._o = o
         self.capacity = o.capacity
+        self.max_pts_per_pair = (self.H // 8) * (self.W // 8)   # one match per coarse cell of image 0 at most
         self._host_counts = torch.zeros(4 + self.B + 1, dtype=torch.int32).pin_memory()
 
     def load_state_dict(self, state_dict):
@@ -391,6 +394,12 @@ class LoFTR:
             "mkpts1_c": self._wrap(o.mkpts1_c, (cap, 2), torch.float32),
             "expec_f": self._wrap(o.expec_f, (cap, 3), torch.float32),
         }
+
+    def pose_inputs(self):
+        """(kpts0 [capacity, 2], kpts1 [capacity, 2], offsets [B + 1]): device views of the last forward's fine matches in
+        the pose back end's layout."""
+        d = self.device_outputs()
+        return d["mkpts0_f"], d["mkpts1_f"], d["m_offsets"]
 
     def set_map(self, img0):
         """Encodes the map image img0 (CUDA float32 [(1,)(1,)h,w], h <= H, w <= W) once, eagerly, on the engine stream.

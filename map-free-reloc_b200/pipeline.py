@@ -12,26 +12,87 @@ a *stream* of pairs they are overlapped:
 ``submit()`` enqueues a batch and returns the finished result of the batch submitted one call earlier
 (None on the first call); ``drain()`` returns the last one.
 
+The matcher is any pair engine: ``loftr.LoFTR``, ``spsg.SuperPointSuperGlue`` or ``sift.SIFTPairs``. The pipeline uses
+their common members: ``B``, ``device``, ``stream``, ``capacity`` (match rows of a batch), ``max_pts_per_pair``,
+``input_dtype`` (of the images), ``forward_async``, ``set_map``, ``forward_shared_async`` and ``pose_inputs()``. The
+solver is a pose stage (``EMatMetricStage``, ``EMatStage``, ``PnPStage``, ``ProcrustesStage``); ``from_cfg`` builds
+engine, back end and stage from one of the reference's method configs (config/matching/mapfree/*.yaml).
+
 Map-free scenes match every query against one map frame. ``set_map(g0, d0, K0)`` encodes that frame once on every
 engine; ``submit_host_queries`` / ``submit_device_queries`` then copy and match only the query side, with results
 bit-identical to submitting the map frame with every pair. Results are ``(R [B,3,3], t [B,3], inliers [B])``
 float32 / int32 tensors in pinned host memory, written by an asynchronous device->host copy that is
 complete when they are handed out.
 """
+import dataclasses
+import os
+
 import torch
 
+from . import lib as _lib
 from . import pose_solver as _ps
 
 
+# ------------------------------------------------------------------------------------------------ pose stages
+# Each runs on the solver stream: (be, kpts0, kpts1, offsets, K0, K1, depth0, depth1) -> R [B,3,3], t [B,3], inliers [B].
+# The stream runs one fixed hypothesis budget per batch: the CONFIDENCE escalation of the single-pair plugins
+# (pose_solver._SolverBase) needs the inlier ratio on the host, a round trip the stream does not make.
+class EMatMetricStage:
+    """EssentialMatrixMetricSolver: E-mat RANSAC, then the metric scale from depth at its inliers."""
+
+    def __init__(self, pix_thr, scale_thr, num_hyp=_ps.DEFAULT_NUM_HYP, seed=_ps.DEFAULT_SEED, lo=True):
+        self.pix_thr, self.scale_thr, self.num_hyp, self.seed, self.lo = float(pix_thr), float(scale_thr), int(num_hyp), seed, lo
+
+    def __call__(self, be, k0, k1, off, K0, K1, d0, d1):
+        return be.emat_metric(k0, k1, off, K0, K1, d0, d1, self.pix_thr, self.scale_thr, self.num_hyp, self.seed, self.lo)
+
+
+class EMatStage:
+    """EssentialMatrixSolver: the pose up to scale, t of unit norm."""
+
+    def __init__(self, pix_thr, num_hyp=_ps.DEFAULT_NUM_HYP, seed=_ps.DEFAULT_SEED, lo=True):
+        self.pix_thr, self.num_hyp, self.seed, self.lo = float(pix_thr), int(num_hyp), seed, lo
+
+    def __call__(self, be, k0, k1, off, K0, K1, d0, d1):
+        R, t, n, _ = be.emat(k0, k1, off, K0, K1, self.pix_thr, self.num_hyp, self.seed, self.lo)
+        return R, t, n
+
+
+class PnPStage:
+    """PnPSolver: 2D-3D RANSAC with the map frame's depth (depth1 is not read)."""
+
+    def __init__(self, reproj_thr, num_hyp=_ps.DEFAULT_NUM_HYP, seed=_ps.DEFAULT_SEED):
+        self.reproj_thr, self.num_hyp, self.seed = float(reproj_thr), int(num_hyp), seed
+
+    def __call__(self, be, k0, k1, off, K0, K1, d0, d1):
+        R, t, n, _ = be.pnp(k0, k1, off, K0, K1, d0, self.reproj_thr, self.num_hyp, self.seed)
+        return R, t, n
+
+
+class ProcrustesStage:
+    """ProcrustesSolver: 3D-3D RANSAC; with ``refine`` the ICP over the full depth clouds continues from its pose."""
+
+    def __init__(self, max_corr_dist, num_hyp=_ps.DEFAULT_NUM_HYP, seed=_ps.DEFAULT_SEED, refine=False):
+        self.max_corr_dist, self.num_hyp, self.seed, self.refine = float(max_corr_dist), int(num_hyp), seed, bool(refine)
+
+    def __call__(self, be, k0, k1, off, K0, K1, d0, d1):
+        R, t, n = be.procrustes(k0, k1, off, K0, K1, d0, d1, self.max_corr_dist, self.num_hyp, self.seed)
+        if self.refine:
+            R, t, n = be.icp(R, t, K0, K1, d0, d1, self.max_corr_dist)
+        return R, t, n
+
+
 class RelocPipeline:
-    def __init__(self, engine, backend, pix_thr, scale_thr, num_hyp=_ps.DEFAULT_NUM_HYP, depth_hw=None):
+    def __init__(self, engine, backend, pix_thr=None, scale_thr=None, num_hyp=_ps.DEFAULT_NUM_HYP, depth_hw=None,
+                 solver=None):
+        # solver=None: EMatMetricStage(pix_thr, scale_thr, num_hyp), i.e. emat_metric(..., lo=True)
         # `engine` may be a list of identical engines: consecutive batches then alternate between them, each on
         # its own stream, so that the HBM-bound kernels of one batch (attention, LayerNorm, dual softmax, token
         # GEMMs) share the SMs with the tensor-core-bound convolutions of the next.
         self.engines = list(engine) if isinstance(engine, (list, tuple)) else [engine]
         engine = self.engines[0]
         self.eng, self.be = engine, backend
-        self.pix_thr, self.scale_thr, self.num_hyp = float(pix_thr), float(scale_thr), int(num_hyp)
+        self.solver = EMatMetricStage(pix_thr, scale_thr, num_hyp) if solver is None else solver
         dev = engine.device
         self.dev = dev
         self.s_copy = torch.cuda.Stream(device=dev)
@@ -47,15 +108,21 @@ class RelocPipeline:
                 "ev_fwd": torch.cuda.Event(), "ev_solved": torch.cuda.Event(), "ev_in": torch.cuda.Event(),
                 "inputs": None, "busy": False,
             })
+        self.has_overflow = getattr(engine, "overflow", None) is not None   # SIFTPairs: per-pair capacity flags
+        if self.has_overflow:
+            for slot in self.slots:
+                slot["ovf"] = torch.zeros(B, dtype=torch.int32, device=dev)
+                slot["ovf_host"] = torch.zeros(B, dtype=torch.int32).pin_memory()
         self.stage = None
         if depth_hw is not None:                      # device staging for host inputs (two slots)
             h, w = depth_hw
-            self.stage = [{"g0": torch.empty(B, h, w, device=dev), "g1": torch.empty(B, h, w, device=dev),
+            gd = engine.input_dtype
+            self.stage = [{"g0": torch.empty(B, h, w, device=dev, dtype=gd), "g1": torch.empty(B, h, w, device=dev, dtype=gd),
                            "d0": torch.empty(B, h, w, device=dev), "d1": torch.empty(B, h, w, device=dev),
                            "K0": torch.empty(B, 3, 3, device=dev), "K1": torch.empty(B, 3, 3, device=dev)}
                           for _ in range(2)]
         self.i = 0
-        self._outs_all = [e.device_outputs() for e in self.engines]
+        self._outs_all = [e.pose_inputs() for e in self.engines]
         # shared map frame: its depth / intrinsics, a generation counter bumped by set_map, and per slot the [B,...]
         # copies the solver reads, refilled when the slot's generation is behind (the slot's last batch must be solved)
         self.map_gen, self.map_d0, self.map_K0 = 0, None, None
@@ -77,19 +144,22 @@ class RelocPipeline:
         else:
             eng.forward_async(g0, g1)
         with torch.cuda.stream(eng.stream):
-            slot["k0"].copy_(outs["mkpts0_f"], non_blocking=True)
-            slot["k1"].copy_(outs["mkpts1_f"], non_blocking=True)
-            slot["off"].copy_(outs["m_offsets"], non_blocking=True)
+            slot["k0"].copy_(outs[0], non_blocking=True)
+            slot["k1"].copy_(outs[1], non_blocking=True)
+            slot["off"].copy_(outs[2], non_blocking=True)
+            if self.has_overflow:
+                slot["ovf"].copy_(eng.overflow, non_blocking=True)
             slot["ev_fwd"].record(eng.stream)
         with torch.cuda.stream(self.s_solve):
             self.s_solve.wait_event(slot["ev_fwd"])
-            R, t, n = self.be.emat_metric(slot["k0"], slot["k1"], slot["off"], K0, K1, d0, d1, self.pix_thr,
-                                          self.scale_thr, self.num_hyp)
+            R, t, n = self.solver(self.be, slot["k0"], slot["k1"], slot["off"], K0, K1, d0, d1)
             B = eng.B
             slot["rec"][:, :9] = R.reshape(B, 9)
             slot["rec"][:, 9:12] = t.reshape(B, 3)
             slot["rec"][:, 12] = n.to(torch.float32)
             slot["rec_host"].copy_(slot["rec"], non_blocking=True)
+            if self.has_overflow:
+                slot["ovf_host"].copy_(slot["ovf"], non_blocking=True)
             slot["ev_solved"].record(self.s_solve)
         for x in (d0, d1, K0, K1):
             x.record_stream(self.s_solve)
@@ -101,6 +171,10 @@ class RelocPipeline:
         slot["ev_solved"].synchronize()
         rec = slot["rec_host"]
         B = self.eng.B
+        if self.has_overflow and bool(slot["ovf_host"].any()):
+            pairs = torch.nonzero(slot["ovf_host"]).flatten().tolist()
+            raise _lib.MfrError(f"batch {j}: pairs {pairs} had more SIFT candidates than the engine's max_candidates; "
+                                f"their matches are incomplete")
         return rec[:, :9].reshape(B, 3, 3).clone(), rec[:, 9:12].clone(), rec[:, 12].to(torch.int32)
 
     def _submit(self, g0, g1, d0, d1, K0, K1):
@@ -142,12 +216,12 @@ class RelocPipeline:
         return self._submit(g0, g1, d0, d1, K0, K0 if K1 is None else K1)
 
     def set_map(self, g0, d0, K0):
-        """Map frame of the batches submitted from now on: gray image g0 [(1,)h,w], depth d0 [(1,)h,w] and intrinsics
-        K0 [(1,)3,3], float32, on the host or the device. g0 is encoded once on every engine; batches already submitted
-        keep the map they were submitted with."""
+        """Map frame of the batches submitted from now on: gray image g0 [(1,)h,w] (of the engine's input_dtype), depth
+        d0 [(1,)h,w] and intrinsics K0 [(1,)3,3] float32, on the host or the device. g0 is encoded once on every engine;
+        batches already submitted keep the map they were submitted with."""
         cur = torch.cuda.current_stream(self.dev)
         h, w = g0.shape[-2:]
-        g0 = g0.reshape(h, w).to(self.dev, torch.float32)
+        g0 = g0.reshape(h, w).to(self.dev, self.eng.input_dtype)
         self.map_d0 = torch.empty(d0.shape[-2:], device=self.dev)
         self.map_d0.copy_(d0.reshape(self.map_d0.shape))
         self.map_K0 = torch.empty(3, 3, device=self.dev)
@@ -183,9 +257,9 @@ class RelocPipeline:
         return self._submit(None, st["g1"], d0, st["d1"], K0, st["K1"])
 
     def submit_host(self, g0, g1, d0, d1, K0, K1=None):
-        """Batch in pinned host memory ([B,h,w] float32 images / depths, [B,3,3] intrinsics of each frame; K1=None:
-        both frames share K0): the copy to the device runs on its own stream, overlapping the forward of the
-        previous batch."""
+        """Batch in pinned host memory ([B,h,w] images of the engine's input_dtype, float32 depths, [B,3,3] intrinsics of
+        each frame; K1=None: both frames share K0): the copy to the device runs on its own stream, overlapping the forward
+        of the previous batch."""
         assert self.stage is not None, "construct the pipeline with depth_hw=(h, w) to feed host batches"
         st, slot = self.stage[self.i % 2], self.slots[self.i % 2]
         with torch.cuda.stream(self.s_copy):
@@ -211,3 +285,123 @@ class RelocPipeline:
             slot["busy"] = False
             slot["inputs"] = None
         self.i = 0
+
+
+# ------------------------------------------------------------------------------------------------ method configs
+MATCHERS = ("LoFTR", "SG", "SIFT")      # etc/feature_matching_baselines/compute.py:10, the correspondences_<key>.npz names
+SOLVERS = ("EssentialMatrix", "EssentialMatrixMetric", "PNP", "Procrustes")   # lib/models/matching/model.py:18-27
+SIFT_NUM_FEATURES, SIFT_RATIO = 2048, 0.8                                     # matchers.py:145-146
+
+
+@dataclasses.dataclass(frozen=True)
+class MethodSpec:
+    """What one Map-free method config asks of the stream: the matcher, the solver with its thresholds, the RANSAC
+    settings (first budget only) and the engine frame."""
+    matcher: str                    # "LoFTR" | "SG" | "SIFT"
+    solver: str                     # "EssentialMatrix" | "EssentialMatrixMetric" | "PNP" | "Procrustes"
+    height: int                     # engine frame: DATASET.HEIGHT / WIDTH, padded as LoFTR_matcher pads for LoFTR
+    width: int
+    num_hyp: int
+    seed: int
+    lo: int                         # mfr_emat_ransac lo flags (E-mat solvers)
+    pix_thr: float = None           # EMAT_RANSAC.PIX_THRESHOLD
+    scale_thr: float = None         # EMAT_RANSAC.SCALE_THRESHOLD (metric solver)
+    reproj_thr: float = None        # PNP.REPROJECTION_INLIER_THRESHOLD
+    max_corr_dist: float = None     # PROCRUSTES.MAX_CORR_DIST [m]
+    refine: bool = False            # PROCRUSTES.REFINE
+    sift_features: int = None       # SIFT.NUM_FEATURES
+    sift_ratio: float = None        # SIFT.RATIO_THRESHOLD
+
+    def stage(self):
+        """The pose stage of this method."""
+        if self.solver == "EssentialMatrixMetric":
+            return EMatMetricStage(self.pix_thr, self.scale_thr, self.num_hyp, self.seed, self.lo)
+        if self.solver == "EssentialMatrix":
+            return EMatStage(self.pix_thr, self.num_hyp, self.seed, self.lo)
+        if self.solver == "PNP":
+            return PnPStage(self.reproj_thr, self.num_hyp, self.seed)
+        return ProcrustesStage(self.max_corr_dist, self.num_hyp, self.seed, self.refine)
+
+
+def _matcher_name(cfg):
+    path = _ps._cfg_get(cfg, "MATCHES_FILE_PATH")
+    fm = _ps._cfg_get(cfg, "FEATURE_MATCHING")
+    if fm == "Precomputed" or (fm is None and path):
+        base = os.path.basename(str(path or ""))
+        for m in MATCHERS:
+            if base == f"correspondences_{m}.npz":
+                return m
+        raise NotImplementedError(f"Invalid feature matching: no streaming matcher for MATCHES_FILE_PATH {path!r}")
+    if fm in ("LoFTR", "SIFT"):
+        return fm
+    raise NotImplementedError(f"Invalid feature matching {fm!r}")
+
+
+def resolve_method(cfg):
+    """Reference method config (a config.CfgNode or nested dict, e.g. config/mapfree.yaml + a
+    config/matching/mapfree/*.yaml) -> MethodSpec. Unknown matchers or solvers raise NotImplementedError as the
+    reference's FeatureMatchingModel does. Budget, seed and LO flags follow the single-pair plugins (pose_solver), with
+    their first hypothesis budget: the stream does not escalate on CONFIDENCE."""
+    g = lambda k, d=None: _ps._cfg_get(cfg, k, d)
+    matcher = _matcher_name(cfg)
+    solver = g("POSE_SOLVER")
+    if solver not in SOLVERS:
+        raise NotImplementedError(f"Invalid pose solver {solver!r}")
+    num_hyp, _, seed, lo = _ps.ransac_settings(cfg, _ps.pnp_default_hyp(cfg) if solver == "PNP" else _ps.DEFAULT_NUM_HYP)
+    h, w = int(g("DATASET.HEIGHT", 720)), int(g("DATASET.WIDTH", 540))   # Map-free's frame (config/mapfree.yaml)
+    if matcher == "LoFTR":                 # LoFTR_matcher's padding (matchers.py:41-46, loftr.pad_to_8): size % 8 more
+        h, w = h + h % 8, w + w % 8
+        if h % 8 or w % 8:
+            raise ValueError("LoFTR needs a resolution that the reference's padding turns into a multiple of 8")
+    f = lambda k: None if g(k) is None else float(g(k))
+    kw = {}
+    if solver.startswith("EssentialMatrix"):
+        kw["pix_thr"] = f("EMAT_RANSAC.PIX_THRESHOLD")
+        if solver == "EssentialMatrixMetric":
+            kw["scale_thr"] = f("EMAT_RANSAC.SCALE_THRESHOLD")
+    elif solver == "PNP":
+        kw["reproj_thr"] = f("PNP.REPROJECTION_INLIER_THRESHOLD")
+    else:
+        kw["max_corr_dist"] = f("PROCRUSTES.MAX_CORR_DIST")
+        kw["refine"] = bool(g("PROCRUSTES.REFINE", False))
+    if matcher == "SIFT":
+        kw["sift_features"] = int(g("SIFT.NUM_FEATURES", SIFT_NUM_FEATURES))
+        kw["sift_ratio"] = float(g("SIFT.RATIO_THRESHOLD", SIFT_RATIO))
+    return MethodSpec(matcher=matcher, solver=solver, height=h, width=w, num_hyp=num_hyp, seed=seed, lo=lo, **kw)
+
+
+def from_cfg(cfg, batch, weights=None, precision="tf32", depth_hw=None, outdoor=False, device=0, graph=True):
+    """Engine + PoseBackend + RelocPipeline for the method of ``cfg`` (see resolve_method), ``batch`` pairs per engine
+    call. ``weights``: LoFTR, a state dict (or a path to one); SG, a (superpoint, superglue) pair of state dicts or the
+    directory holding superpoint_v1.pth and superglue_{indoor,outdoor}.pth (indoor unless ``outdoor``); SIFT, none.
+    ``precision`` applies to LoFTR and SG. The method is at ``pipeline.method``."""
+    spec = resolve_method(cfg)
+    if spec.matcher == "LoFTR":
+        from . import loftr
+        if weights is None:
+            raise ValueError("LoFTR needs a state dict")
+        sd = torch.load(weights, map_location="cpu") if isinstance(weights, str) else weights
+        lc = {"thr": float(_ps._cfg_get(cfg, "LOFTR.THR", 0.2)), "border_rm": int(_ps._cfg_get(cfg, "LOFTR.BORDER_RM", 2)),
+              "temperature": float(_ps._cfg_get(cfg, "LOFTR.TEMPERATURE", 0.1))}
+        eng = loftr.LoFTR(sd, batch=batch, height=spec.height, width=spec.width, cfg=lc, device=device, graph=graph,
+                          precision=precision)
+    elif spec.matcher == "SG":
+        from . import spsg
+        if weights is None:
+            raise ValueError("SuperPoint + SuperGlue needs state dicts or their directory")
+        if isinstance(weights, str):
+            sp = torch.load(os.path.join(weights, "superpoint_v1.pth"), map_location="cpu")
+            sg = torch.load(os.path.join(weights, f"superglue_{'outdoor' if outdoor else 'indoor'}.pth"), map_location="cpu")
+        else:
+            sp, sg = weights
+        eng = spsg.SuperPointSuperGlue(sp, sg, batch=batch, height=spec.height, width=spec.width, device=device,
+                                       graph=graph, precision=precision)
+    else:
+        from . import sift
+        eng = sift.SIFTPairs(batch, spec.height, spec.width, nfeatures=spec.sift_features, ratio=spec.sift_ratio,
+                             root_sift=True, device=device, graph=graph)
+    be = _ps.PoseBackend(max_pairs=batch, max_pts=max(8, min(eng.max_pts_per_pair, _ps.MAX_PTS_LIMIT)),
+                         max_hyp=max(spec.num_hyp, 128), device=device)
+    pipe = RelocPipeline(eng, be, depth_hw=depth_hw, solver=spec.stage())
+    pipe.method = spec
+    return pipe

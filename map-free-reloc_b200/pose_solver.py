@@ -170,6 +170,27 @@ def required_hypotheses(confidence, inlier_ratio, sample_size):
     return int(min(2 ** 31 - 1, math.ceil(math.log(1.0 - c) / -w if w < 1e-8 else math.log(1.0 - c) / math.log1p(-w))))
 
 
+def ransac_settings(cfg, default_hyp=DEFAULT_NUM_HYP):
+    """GPU_RANSAC keys -> (first hypothesis budget, escalation cap, seed, lo flags of mfr_emat_ransac), as every solver
+    plugin reads them; ``default_hyp`` is the solver's budget when NUM_HYPOTHESES is unset."""
+    num_hyp = int(_cfg_get(cfg, "GPU_RANSAC.NUM_HYPOTHESES", default_hyp))
+    max_hyp = max(num_hyp, int(_cfg_get(cfg, "GPU_RANSAC.MAX_HYPOTHESES", 32768)))
+    seed = int(_cfg_get(cfg, "GPU_RANSAC.SEED", DEFAULT_SEED))
+    lo = bool(_cfg_get(cfg, "GPU_RANSAC.LOCAL_OPTIMISATION", True))
+    refit = str(_cfg_get(cfg, "GPU_RANSAC.FINAL_REFIT", DEFAULT_FINAL_REFIT)).lower()
+    if refit not in ("lsq", "tukey"):
+        raise ValueError("GPU_RANSAC.FINAL_REFIT must be 'lsq' or 'tukey'")
+    return num_hyp, max_hyp, seed, (LO_LSQ if refit == "lsq" else LO_TUKEY) if lo else 0
+
+
+def pnp_default_hyp(cfg):
+    """PnPSolver's budget when GPU_RANSAC.NUM_HYPOTHESES is unset: PNP.RANSAC_ITER (the reference's iteration cap of
+    cv2.solvePnPRansac) rounded up to a multiple of 128, at least 128."""
+    iters = _cfg_get(cfg, "PNP.RANSAC_ITER")
+    iters = int(iters) if iters else DEFAULT_NUM_HYP
+    return max(128, (iters + 127) // 128 * 128)
+
+
 class _SolverBase:
     """The GPU solvers run a fixed hypothesis budget per launch instead of OpenCV's sequential loop with an early
     exit. The reference's `CONFIDENCE` is honoured as an escalation rule: when the inlier ratio a launch found says
@@ -178,14 +199,7 @@ class _SolverBase:
     SAMPLE_SIZE = 5
 
     def __init__(self, cfg, default_hyp=DEFAULT_NUM_HYP):
-        self.num_hyp = int(_cfg_get(cfg, "GPU_RANSAC.NUM_HYPOTHESES", default_hyp))
-        self.max_hyp = max(self.num_hyp, int(_cfg_get(cfg, "GPU_RANSAC.MAX_HYPOTHESES", 32768)))
-        self.seed = int(_cfg_get(cfg, "GPU_RANSAC.SEED", DEFAULT_SEED))
-        lo = bool(_cfg_get(cfg, "GPU_RANSAC.LOCAL_OPTIMISATION", True))
-        refit = str(_cfg_get(cfg, "GPU_RANSAC.FINAL_REFIT", DEFAULT_FINAL_REFIT)).lower()
-        if refit not in ("lsq", "tukey"):
-            raise ValueError("GPU_RANSAC.FINAL_REFIT must be 'lsq' or 'tukey'")
-        self.lo = (LO_LSQ if refit == "lsq" else LO_TUKEY) if lo else 0
+        self.num_hyp, self.max_hyp, self.seed, self.lo = ransac_settings(cfg, default_hyp)
         self.backend = PoseBackend(max_pairs=1, max_hyp=max(self.max_hyp, 128))
         self.dev = self.backend.device
         self.last_num_hyp = 0       # budget of the launch whose result was returned
@@ -279,8 +293,7 @@ class PnPSolver(_SolverBase):
         # PNP.RANSAC_ITER (reference: the iteration cap of cv2.solvePnPRansac) is the first launch's hypothesis
         # budget unless GPU_RANSAC.NUM_HYPOTHESES overrides it; PNP.CONFIDENCE escalates it (see _SolverBase)
         self.ransac_iterations = _cfg_get(cfg, "PNP.RANSAC_ITER")
-        iters = int(self.ransac_iterations) if self.ransac_iterations else DEFAULT_NUM_HYP
-        super().__init__(cfg, default_hyp=max(128, (iters + 127) // 128 * 128))
+        super().__init__(cfg, default_hyp=pnp_default_hyp(cfg))
         self.reprojection_inlier_threshold = float(_cfg_get(cfg, "PNP.REPROJECTION_INLIER_THRESHOLD"))
         self.confidence = _cfg_get(cfg, "PNP.CONFIDENCE")
 

@@ -1,8 +1,9 @@
 """Host side of the CUDA SIFT engine: ``SIFT(batch, height, width)`` detects, describes and ratio-matches keypoints
 of uint8 gray images on the device, as cv2.SIFT_create(nfeatures).detectAndCompute + exact 2-NN + Lowe's ratio test
 do on the host in the reference's SIFT plugins (lib/models/matching/feature_matching.py:53-118,
-etc/feature_matching_baselines/matchers.py:123-188). All arithmetic runs in libmfr_b200.so; torch is used for
-device memory and streams only. No CPU fallback."""
+etc/feature_matching_baselines/matchers.py:123-188). ``SIFTPairs(batch, height, width)`` is the same engine as a pair
+engine for ``pipeline.RelocPipeline``. All arithmetic runs in libmfr_b200.so; torch is used for device memory and
+streams only. No CPU fallback."""
 import ctypes
 
 import numpy as np
@@ -90,6 +91,85 @@ class SIFT:
         if getattr(self, "h", None):
             torch.cuda.synchronize()
             self.l.mfr_sift_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class SIFTPairs:
+    """Pair engine for ``batch`` pairs of ``height`` x ``width`` uint8 gray images (the bytes the reference's SIFT_matcher
+    hands to cv2: ``imread(path, 0)`` then ``cv2.resize`` on uint8): detection, 2-NN and the ratio test of both images of
+    every pair in one CUDA graph with no host synchronisation, matches in engine-owned buffers. Bit-identical to
+    ``SIFT(2 * batch, ...).detect(interleaved)`` + ``match_pairs(ratio)``. ``root_sift=True`` is what the reference's
+    SIFT plugins match on. When an image has more than ``max_candidates`` refined extrema or oriented keypoints, the
+    pair's flag in ``overflow`` is set on the device (nothing is read on the host here)."""
+
+    input_dtype = torch.uint8
+
+    def __init__(self, batch, height, width, nfeatures=2048, ratio=0.8, root_sift=True, max_candidates=32768, device=0,
+                 graph=True):
+        if not torch.cuda.is_available():
+            raise _lib.MfrError("SIFT pair engine needs a CUDA device (there is no CPU fallback)")
+        self.l = _lib.load()
+        self.B, self.H, self.W = int(batch), int(height), int(width)
+        self.device = torch.device("cuda", device)
+        torch.cuda.set_device(self.device)
+        self.stream = torch.cuda.Stream(device=self.device)
+        h = ctypes.c_void_p()
+        _lib.check(self.l.mfr_sift_pairs_create(self.B, self.H, self.W, int(nfeatures), int(max_candidates),
+                                                int(bool(root_sift)), float(ratio), ctypes.byref(h)),
+                   "mfr_sift_pairs_create")
+        self.h = h
+        self.l.mfr_sift_pairs_set_graph(self.h, int(bool(graph)))
+        o = _lib.SiftPairOutputs()
+        _lib.check(self.l.mfr_sift_get_pair_outputs(self.h, ctypes.byref(o)), "mfr_sift_get_pair_outputs")
+        self.capacity, self.max_pts_per_pair = o.capacity, o.max_pts_per_pair
+        view = lambda a, shape, dt: _lib.device_view(a, shape, dt, self.device)
+        self._k0 = view(o.kpts0, (self.capacity, 2), torch.float32)
+        self._k1 = view(o.kpts1, (self.capacity, 2), torch.float32)
+        self._off = view(o.offsets, (self.B + 1,), torch.int32)
+        self.overflow = view(o.overflow, (self.B,), torch.int32)
+
+    def _images(self, imgs, n):
+        imgs = imgs.reshape(n, self.H, self.W).contiguous()
+        if imgs.dtype != torch.uint8 or not imgs.is_cuda:
+            raise ValueError(f"expected uint8 CUDA images of shape [{n}, {self.H}, {self.W}]")
+        return imgs
+
+    def _run(self, fn, name, *imgs):
+        self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(self.stream):
+            _lib.check(fn(self.h, *[_lib.ptr(x) for x in imgs], ctypes.c_void_p(self.stream.cuda_stream)), name)
+        for x in imgs:
+            x.record_stream(self.stream)
+
+    def forward_async(self, img0, img1):
+        """Enqueues one batch of pairs (uint8 CUDA [B,(1,)H,W] each) on the engine stream."""
+        self._run(self.l.mfr_sift_forward_pairs, "mfr_sift_forward_pairs", self._images(img0, self.B),
+                  self._images(img1, self.B))
+
+    def set_map(self, img0):
+        """Detects and describes the map image img0 (uint8 CUDA [(1,)(1,)H,W]) once, eagerly, on the engine stream. Until
+        the next set_map, ``forward_shared_async(img1)`` gives the bits ``forward_async`` gives with img0 repeated for every
+        pair; a paired forward in between does not disturb the map."""
+        self._run(self.l.mfr_sift_set_map, "mfr_sift_set_map", self._images(img0, 1))
+
+    def forward_shared_async(self, img1):
+        """Enqueues one batch of B query images (uint8 CUDA [B,(1,)H,W]) against the map of ``set_map``."""
+        self._run(self.l.mfr_sift_forward_shared, "mfr_sift_forward_shared", self._images(img1, self.B))
+
+    def pose_inputs(self):
+        """(kpts0 [capacity, 2], kpts1 [capacity, 2], offsets [B + 1]): device views of the last forward's matches."""
+        return self._k0, self._k1, self._off
+
+    def close(self):
+        if getattr(self, "h", None):
+            torch.cuda.synchronize()
+            self.l.mfr_sift_pairs_destroy(self.h)
             self.h = None
 
     def __del__(self):

@@ -131,12 +131,15 @@ def synthetic_state_dicts(seed=0):
 class SuperPointSuperGlue:
     """CUDA SuperPoint+SuperGlue engine for ``batch`` pairs of [H, W] gray images."""
 
+    input_dtype = torch.float32
+
     def __init__(self, sp_sd, sg_sd, batch=1, height=720, width=540, cfg=None, device=0, graph=True, precision="tf32"):
         if not torch.cuda.is_available():
             raise _lib.MfrError("mfr_b200.SuperPointSuperGlue needs a CUDA device (no CPU fallback)")
         self._l = _lib.load()
         self.cfg = {**DEFAULTS, **(cfg or {})}
         self.B, self.H, self.W, self.K = int(batch), int(height), int(width), int(self.cfg["max_keypoints"])
+        self.capacity, self.max_pts_per_pair = self.B * self.K, self.K
         self.device = torch.device("cuda", device)
         torch.cuda.set_device(self.device)
         self.stream = torch.cuda.Stream(device=self.device)
@@ -186,6 +189,13 @@ class SuperPointSuperGlue:
                 "m_offsets": self._wrap(o.m_offsets, (B + 1,), torch.int32),
                 "mkpts0": self._wrap(o.mkpts0, (B * K, 2), torch.float32),
                 "mkpts1": self._wrap(o.mkpts1, (B * K, 2), torch.float32)}
+
+    def pose_inputs(self):
+        """(kpts0 [capacity, 2], kpts1 [capacity, 2], offsets [B + 1]): device views of the last forward's matches in the
+        pose back end's layout."""
+        o = self._o
+        return (self._wrap(o.mkpts0, (self.capacity, 2), torch.float32), self._wrap(o.mkpts1, (self.capacity, 2), torch.float32),
+                self._wrap(o.m_offsets, (self.B + 1,), torch.int32))
 
     def forward_async(self, img0, img1):
         img0 = img0.reshape(self.B, self.H, self.W).contiguous()

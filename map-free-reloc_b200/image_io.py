@@ -3,6 +3,7 @@ resize + normalise steps as CUDA kernels (libmfr_b200.so: mfr_jpeg_decode, mfr_r
 
   read_image(path, resize, resize_float)   = SuperGlue/models/utils.py:263-285 (gray, cv2.resize, / 255) -> CUDA [h, w]
   read_color_image(path, resize)           = lib/datasets/utils.py:58-75 (RGB, uint8 cv2.resize, / 255)   -> CUDA [3, h, w]
+  PairMatcher                              = match / match_scene / match_arrays of the LoFTR and SuperGlue plugins
 
 JPEG files are decoded on the GPU (luma plane = OpenCV's IMREAD_GRAYSCALE of a JPEG, up to the +-1 level differences
 between two IDCT implementations); other formats are decoded by OpenCV on the host and uploaded as uint8. The resize
@@ -85,6 +86,42 @@ def read_image(path, resize, resize_float=True, device=None):
     if im is None:
         return None
     return resize_linear(im, resize, MODE_U8_AS_F32 if resize_float else MODE_U8_FIXED, 1.0 / 255.0)
+
+
+class PairMatcher:
+    """Body of the image-pair matcher plugins (loftr.LoFTR_matcher, spsg.SuperGlue_matcher) over a batch-1 pair engine:
+    images read with ``read_image(path, resize, True)`` on the engine's device, results as the reference's plugins give
+    them, float [N, 4] (x0, y0, x1, y1) or ``np.full((1, 4), nan)``. A subclass builds the engine and reads the matched
+    keypoints of an engine output in ``_matches(out) -> (kpts0, kpts1)``."""
+
+    def __init__(self, resize, engine):
+        self.resize, self.engine = resize, engine
+
+    def match(self, pair_path):
+        """matchers.py:24-59 / 93-120; images decoded (JPEG: nvJPEG) and resized on the GPU."""
+        return self._result(self.engine.forward(self._read(pair_path[0]), self._read(pair_path[1])))
+
+    def match_scene(self, ref_path, query_paths):
+        """``[self.match((ref_path, q)) for q in query_paths]``, array for array, with the reference image decoded and
+        encoded once (Map-free: every pair of a scene shares its first image)."""
+        self.engine.set_map(self._read(ref_path))
+        return [self._result(self.engine.forward_shared(self._read(q))) for q in query_paths]
+
+    def match_arrays(self, im0, im1):
+        """``match`` on two gray float [h, w] arrays in [0, 1]."""
+        dev = self.engine.device
+        t0 = torch.from_numpy(np.ascontiguousarray(im0, dtype=np.float32))[None].to(dev)
+        t1 = torch.from_numpy(np.ascontiguousarray(im1, dtype=np.float32))[None].to(dev)
+        return self._result(self.engine.forward(t0, t1))
+
+    def _read(self, path):
+        return read_image(path, self.resize, True, self.engine.device)[None]
+
+    def _result(self, out):
+        kpts0, kpts1 = self._matches(out)
+        if len(kpts0) > 0:
+            return torch.cat([kpts0, kpts1], 1).cpu().numpy()
+        return np.full((1, 4), np.nan)
 
 
 def read_color_image(path, resize=(640, 480), device=None):

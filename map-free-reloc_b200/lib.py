@@ -1,8 +1,10 @@
-"""ctypes binding of libmfr_b200.so. There is NO CPU fallback: if the library is missing or a
-CUDA device is absent, compute entry points raise."""
+"""ctypes binding of libmfr_b200.so, and ``Engine``, the host side that every engine class shares. There is NO CPU
+fallback: if the library is missing or a CUDA device is absent, compute entry points raise."""
 import ctypes
 import math
 import os
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libmfr_b200.so")
@@ -169,46 +171,103 @@ def ptr(t):
 
 
 def cur_stream():
-    import torch
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-def device_view(addr, shape, dtype, device):
-    """Zero-copy torch view (float32, float64, int32 or bfloat16) of an engine-owned device buffer, valid while the
-    engine lives."""
-    import torch
+class Engine:
+    """Host side of one engine handle of the library (its ``mfr_<name>_*`` functions): the handle, the device and, for
+    the pair engines, the stream the engine runs on. ``close`` (also run by ``__del__``) waits for the engine's work and
+    destroys the handle."""
 
-    class _A:   # __cuda_array_interface__ carrier
-        pass
-    a = _A()
-    typestr = {torch.float32: "<f4", torch.float64: "<f8", torch.int32: "<i4", torch.bfloat16: "<i2"}[dtype]
-    a.__cuda_array_interface__ = {"shape": (int(math.prod(shape)),), "typestr": typestr, "data": (int(addr), False),
-                                  "version": 2}
-    t = torch.as_tensor(a, device=device)
-    return (t.view(torch.bfloat16) if dtype == torch.bfloat16 else t).view(*shape)
+    def __init__(self, name, create, args, device=None, stream=True):
+        """Creates the handle with ``create(*args, &handle)`` (the name of an mfr_* function) on cuda:``device`` (None:
+        the current device). ``stream``: whether the engine runs on a stream of its own (``_call``) rather than on the
+        caller's current stream."""
+        if not torch.cuda.is_available():
+            raise MfrError(f"{type(self).__name__} needs a CUDA device (there is no CPU fallback)")
+        self._l, self._name = load(), name
+        self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
+        torch.cuda.set_device(self.device)
+        self.stream = torch.cuda.Stream(device=self.device) if stream else None
+        h = ctypes.c_void_p()
+        check(getattr(self._l, create)(*args, ctypes.byref(h)), create)
+        self._h = h
 
+    def _get_outputs(self, fn, struct):
+        """The engine's table of output buffers: ``fn`` is its mfr_*_get_outputs function, ``struct`` the table's type."""
+        o = struct()
+        check(fn(self._h, ctypes.byref(o)), fn.__name__)
+        return o
 
-def debug_tensor(l, engine, h, name, shape, dtype, device):
-    """View of the named buffer of engine handle ``h`` (mfr_<engine>_debug_tensor, which reports its size in 4-byte
-    words); ``shape`` must fit in it."""
-    import torch
-    p, n = ctypes.c_void_p(), ctypes.c_longlong()
-    check(getattr(l, f"mfr_{engine}_debug_tensor")(h, name.encode(), ctypes.byref(p), ctypes.byref(n)),
-          f"debug tensor {name}")
-    assert math.prod(shape) * torch.empty((), dtype=dtype).element_size() <= 4 * n.value, (name, shape, n.value)
-    return device_view(p.value, shape, dtype, device)
+    def _upload_weights(self, weights):
+        """Uploads ``weights`` ({name: float32 ndarray}) on the engine stream in the engine's order; a tensor the engine
+        expects that is missing or of another size raises MfrError naming it."""
+        l, h, stream = self._l, self._h, ctypes.c_void_p(self.stream.cuda_stream)
+        for i in range(getattr(l, f"mfr_{self._name}_num_weights")(h)):
+            name = getattr(l, f"mfr_{self._name}_weight_name")(h, i).decode()
+            numel = getattr(l, f"mfr_{self._name}_weight_numel")(h, i)
+            if name not in weights:
+                raise MfrError(f"missing weight tensor {name}")
+            a = weights[name].reshape(-1)
+            if a.size != numel:
+                raise MfrError(f"weight {name}: {a.size} elements, engine expects {numel}")
+            check(getattr(l, f"mfr_{self._name}_set_weight")(h, i, a.ctypes.data_as(ctypes.c_void_p), numel, stream),
+                  f"set_weight {name}")
 
+    def _images(self, imgs, *shape):
+        """``imgs`` as a contiguous tensor of ``shape``; ValueError unless it is a CUDA tensor of the engine's
+        ``input_dtype``."""
+        if not imgs.is_cuda or imgs.dtype != self.input_dtype:
+            raise ValueError(f"expected {self.input_dtype} CUDA images of shape {list(shape)}")
+        return imgs.reshape(shape).contiguous()
 
-def upload_weights(l, engine, h, weights, stream):
-    """Uploads ``weights`` ({name: float32 ndarray}) into engine handle ``h`` in the engine's order; a tensor the
-    engine expects that is missing or of another size raises MfrError naming it."""
-    for i in range(getattr(l, f"mfr_{engine}_num_weights")(h)):
-        name = getattr(l, f"mfr_{engine}_weight_name")(h, i).decode()
-        numel = getattr(l, f"mfr_{engine}_weight_numel")(h, i)
-        if name not in weights:
-            raise MfrError(f"missing weight tensor {name}")
-        a = weights[name].reshape(-1)
-        if a.size != numel:
-            raise MfrError(f"weight {name}: {a.size} elements, engine expects {numel}")
-        check(getattr(l, f"mfr_{engine}_set_weight")(h, i, a.ctypes.data_as(ctypes.c_void_p), numel, stream),
-              f"set_weight {name}")
+    def _call(self, fn, *args):
+        """Runs ``fn(handle, *args, engine stream)`` on the engine stream, after the work queued so far on the caller's
+        current stream. Tensor arguments are passed as pointers and kept alive until the engine stream is done with
+        them."""
+        self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(self.stream):
+            check(fn(self._h, *[ptr(a) if isinstance(a, torch.Tensor) else a for a in args],
+                     ctypes.c_void_p(self.stream.cuda_stream)), fn.__name__)
+        for a in args:
+            if isinstance(a, torch.Tensor):
+                a.record_stream(self.stream)
+
+    def view(self, addr, shape, dtype):
+        """Zero-copy torch view (float32, float64, int32 or bfloat16) of an engine-owned device buffer, valid while the
+        engine lives."""
+        class _A:   # __cuda_array_interface__ carrier
+            pass
+        a = _A()
+        typestr = {torch.float32: "<f4", torch.float64: "<f8", torch.int32: "<i4", torch.bfloat16: "<i2"}[dtype]
+        a.__cuda_array_interface__ = {"shape": (int(math.prod(shape)),), "typestr": typestr, "data": (int(addr), False),
+                                      "version": 2}
+        t = torch.as_tensor(a, device=self.device)
+        return (t.view(torch.bfloat16) if dtype == torch.bfloat16 else t).view(*shape)
+
+    def debug_tensor(self, name, shape, dtype=torch.float32):
+        """View of the engine's named intermediate buffer (listed at mfr_<name>_debug_tensor in include/mfr_b200.h, which
+        reports its size in 4-byte words); ``shape`` must fit in it. It shows what the last call that wrote the buffer
+        left there."""
+        p, n = ctypes.c_void_p(), ctypes.c_longlong()
+        fn = getattr(self._l, f"mfr_{self._name}_debug_tensor")
+        check(fn(self._h, name.encode(), ctypes.byref(p), ctypes.byref(n)), f"debug tensor {name}")
+        assert math.prod(shape) * torch.empty((), dtype=dtype).element_size() <= 4 * n.value, (name, shape, n.value)
+        return self.view(p.value, shape, dtype)
+
+    def close(self):
+        """Waits for the engine's work (its stream's, or the device's for an engine without one), then destroys the
+        handle. Later calls do nothing."""
+        if getattr(self, "_h", None):
+            if self.stream is None:
+                torch.cuda.synchronize(self.device)
+            else:
+                self.stream.synchronize()
+            getattr(self._l, f"mfr_{self._name}_destroy")(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

@@ -12,6 +12,8 @@ import numpy as np
 import torch
 
 from . import lib as _lib
+from .image_io import PairMatcher
+from .pose_solver import _cfg_get
 
 DEFAULT_CFG = {"thr": 0.2, "border_rm": 2, "temperature": 0.1}  # cvpr_ds_config.py:31-35
 
@@ -273,22 +275,15 @@ def functional_state_dict(coarse_scale=200.0, fine_scale=30.0, ln_gain=40.0, noi
     return {k: v.float().contiguous() for k, v in sd.items()}
 
 
-class LoFTR:
+class LoFTR(_lib.Engine):
     """CUDA LoFTR engine for ``batch`` pairs of [H, W] images (H, W multiples of 8)."""
 
     input_dtype = torch.float32
 
     def __init__(self, state_dict, batch=1, height=720, width=544, cfg=None, device=0, graph=True,
                  precision="tf32", pipelined=False):
-        if not torch.cuda.is_available():
-            raise _lib.MfrError("mfr_b200.LoFTR needs a CUDA device (no CPU fallback)")
-        self._l = _lib.load()
         self.cfg = {**DEFAULT_CFG, **(cfg or {})}
         self.B, self.H, self.W = int(batch), int(height), int(width)
-        self.device = torch.device("cuda", device)
-        torch.cuda.set_device(self.device)
-        self.stream = torch.cuda.Stream(device=self.device)
-        h = ctypes.c_void_p()
         # tf32: fp32 storage, TF32 tensor-core inputs; bf16: bf16 storage + kind::f16 MMAs (backbone, token GEMMs,
         # correlation, attention); fp32x3: fp32 storage, every GEMM as a 3xTF32 split product (fp32-faithful)
         self.precision = {"tf32": 0, "bf16": 1, "fp32x3": 2, "fp32": 2}[precision]
@@ -297,22 +292,18 @@ class LoFTR:
         # with the first layers of this batch's matcher: those launches then leave 8 SMs to it (reserved_sms of
         # mfr_loftr_create; measured +0.8 % pairs/s in the pipeline, -0.6 % for a matcher running alone)
         reserved_sms = 8 if pipelined else 0
-        _lib.check(self._l.mfr_loftr_create(self.B, self.H, self.W, float(self.cfg["thr"]),
-                                            int(self.cfg["border_rm"]), float(self.cfg["temperature"]),
-                                            self.precision, reserved_sms, ctypes.byref(h)), "mfr_loftr_create")
-        self._h = h
+        super().__init__("loftr", "mfr_loftr_create", (self.B, self.H, self.W, float(self.cfg["thr"]),
+                                                       int(self.cfg["border_rm"]), float(self.cfg["temperature"]),
+                                                       self.precision, reserved_sms), device)
         self._l.mfr_loftr_set_graph(self._h, int(bool(graph)))
         self.load_state_dict(state_dict)
-        o = _lib.LoftrOutputs()
-        _lib.check(self._l.mfr_loftr_get_outputs(self._h, ctypes.byref(o)))
-        self._o = o
-        self.capacity = o.capacity
+        self._o = self._get_outputs(self._l.mfr_loftr_get_outputs, _lib.LoftrOutputs)
+        self.capacity = self._o.capacity
         self.max_pts_per_pair = (self.H // 8) * (self.W // 8)   # one match per coarse cell of image 0 at most
         self._host_counts = torch.zeros(4 + self.B + 1, dtype=torch.int32).pin_memory()
 
     def load_state_dict(self, state_dict):
-        _lib.upload_weights(self._l, "loftr", self._h, prepare_weights(state_dict, self.H // 8, self.W // 8),
-                            ctypes.c_void_p(self.stream.cuda_stream))
+        self._upload_weights(prepare_weights(state_dict, self.H // 8, self.W // 8))
 
     def num_kernels(self):
         return self._l.mfr_loftr_num_kernels(self._h)
@@ -322,19 +313,16 @@ class LoFTR:
         return self._l.mfr_loftr_num_launches(self._h)
 
     def profile(self, img0, img1):
-        """Per-step device times of one eager forward: list of (name, kind, ms, flops)."""
+        """Per-step device times of one eager forward: list of (name, kind, ms, flops). Returns when it is done."""
         h, w = img0.shape[-2:]
-        img0 = img0.reshape(self.B, h, w).contiguous()
-        img1 = img1.reshape(self.B, h, w).contiguous()
+        img0, img1 = self._images(img0, self.B, h, w), self._images(img1, self.B, h, w)
         n = self.num_kernels()
         ms = np.zeros(n, np.float32); fl = np.zeros(n, np.float64); kinds = np.zeros(n, np.int32)
         names = ctypes.create_string_buffer(32 * n)
-        self.stream.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(self.stream):
-            rc = self._l.mfr_loftr_profile(self._h, _lib.ptr(img0), _lib.ptr(img1), int(h), int(w),
-                                           ctypes.c_void_p(self.stream.cuda_stream), n,
-                                           ms.ctypes.data_as(ctypes.c_void_p), fl.ctypes.data_as(ctypes.c_void_p),
-                                           kinds.ctypes.data_as(ctypes.c_void_p), names)
+        torch.cuda.current_stream(self.device).synchronize()     # the images are written; the engine stream orders the rest
+        rc = self._l.mfr_loftr_profile(self._h, _lib.ptr(img0), _lib.ptr(img1), h, w,
+                                       ctypes.c_void_p(self.stream.cuda_stream), n, ms.ctypes.data_as(ctypes.c_void_p),
+                                       fl.ctypes.data_as(ctypes.c_void_p), kinds.ctypes.data_as(ctypes.c_void_p), names)
         if rc < 0:
             raise _lib.MfrError(f"mfr_loftr_profile failed rc={rc}")
         raw = names.raw
@@ -350,49 +338,31 @@ class LoFTR:
 
     def run_steps(self, begin, end):
         """Runs steps [begin, end) of the forward list eagerly on the engine's buffers as the last call left them (stage
-        tests: a forward stages the images first). Ordered after the current stream's work and before its later work."""
-        cur = torch.cuda.current_stream(self.device)
-        self.stream.wait_stream(cur)
-        with torch.cuda.stream(self.stream):
-            _lib.check(self._l.mfr_loftr_run_steps(self._h, int(begin), int(end), ctypes.c_void_p(self.stream.cuda_stream)),
-                       f"loftr run_steps [{begin}, {end})")
-        cur.wait_stream(self.stream)
-
-    def _wrap(self, ptr, shape, dtype):
-        return _lib.device_view(ptr, shape, dtype, self.device)
-
-    def debug_tensor(self, name, shape):
-        return _lib.debug_tensor(self._l, "loftr", self._h, name, shape, torch.float32, self.device)
+        tests: a forward stages the images first). Ordered after the current stream's work; returns when it is done."""
+        self._call(self._l.mfr_loftr_run_steps, int(begin), int(end))
+        self.stream.synchronize()
 
     def forward_async(self, img0, img1):
         """Enqueues one batch on the engine stream. img0/img1: CUDA float32 [B,(1,)h,w] with h <= H,
         w <= W; the engine zero-pads to its [H, W] frame (the reference's pad-to-8)."""
         h, w = img0.shape[-2:]
-        img0 = img0.reshape(self.B, h, w).contiguous()
-        img1 = img1.reshape(self.B, h, w).contiguous()
-        assert img0.is_cuda and img0.dtype == torch.float32
-        self.stream.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(self.stream):
-            _lib.check(self._l.mfr_loftr_forward(self._h, _lib.ptr(img0), _lib.ptr(img1), int(h), int(w),
-                                                 ctypes.c_void_p(self.stream.cuda_stream)), "loftr forward")
-        img0.record_stream(self.stream)
-        img1.record_stream(self.stream)
+        self._call(self._l.mfr_loftr_forward, self._images(img0, self.B, h, w), self._images(img1, self.B, h, w), h, w)
 
     def device_outputs(self):
         """Views of the engine's output buffers (valid until the next forward)."""
         cap = self.capacity
         o = self._o
         return {
-            "m_total": self._wrap(o.m_total, (4,), torch.int32),
-            "m_offsets": self._wrap(o.m_offsets, (self.B + 1,), torch.int32),
-            "b_ids": self._wrap(o.b_ids, (cap,), torch.int32),
-            "i_ids": self._wrap(o.i_ids, (cap,), torch.int32),
-            "j_ids": self._wrap(o.j_ids, (cap,), torch.int32),
-            "mconf": self._wrap(o.mconf, (cap,), torch.float32),
-            "mkpts0_f": self._wrap(o.mkpts0_f, (cap, 2), torch.float32),
-            "mkpts1_f": self._wrap(o.mkpts1_f, (cap, 2), torch.float32),
-            "mkpts1_c": self._wrap(o.mkpts1_c, (cap, 2), torch.float32),
-            "expec_f": self._wrap(o.expec_f, (cap, 3), torch.float32),
+            "m_total": self.view(o.m_total, (4,), torch.int32),
+            "m_offsets": self.view(o.m_offsets, (self.B + 1,), torch.int32),
+            "b_ids": self.view(o.b_ids, (cap,), torch.int32),
+            "i_ids": self.view(o.i_ids, (cap,), torch.int32),
+            "j_ids": self.view(o.j_ids, (cap,), torch.int32),
+            "mconf": self.view(o.mconf, (cap,), torch.float32),
+            "mkpts0_f": self.view(o.mkpts0_f, (cap, 2), torch.float32),
+            "mkpts1_f": self.view(o.mkpts1_f, (cap, 2), torch.float32),
+            "mkpts1_c": self.view(o.mkpts1_c, (cap, 2), torch.float32),
+            "expec_f": self.view(o.expec_f, (cap, 3), torch.float32),
         }
 
     def pose_inputs(self):
@@ -406,24 +376,12 @@ class LoFTR:
         Until the next set_map or weight upload, ``forward_shared[_async](img1)`` gives the bits ``forward[_async]`` gives
         with img0 repeated for every pair; a paired forward in between does not disturb the map."""
         h, w = img0.shape[-2:]
-        img0 = img0.reshape(h, w).contiguous()
-        assert img0.is_cuda and img0.dtype == torch.float32
-        self.stream.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(self.stream):
-            _lib.check(self._l.mfr_loftr_set_map(self._h, _lib.ptr(img0), int(h), int(w),
-                                                 ctypes.c_void_p(self.stream.cuda_stream)), "loftr set_map")
-        img0.record_stream(self.stream)
+        self._call(self._l.mfr_loftr_set_map, self._images(img0, h, w), h, w)
 
     def forward_shared_async(self, img1):
         """Enqueues one batch of B query images [B,(1,)h,w] against the map of ``set_map`` (same h, w; else MfrError)."""
         h, w = img1.shape[-2:]
-        img1 = img1.reshape(self.B, h, w).contiguous()
-        assert img1.is_cuda and img1.dtype == torch.float32
-        self.stream.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(self.stream):
-            _lib.check(self._l.mfr_loftr_forward_shared(self._h, _lib.ptr(img1), int(h), int(w),
-                                                        ctypes.c_void_p(self.stream.cuda_stream)), "loftr forward_shared")
-        img1.record_stream(self.stream)
+        self._call(self._l.mfr_loftr_forward_shared, self._images(img1, self.B, h, w), h, w)
 
     def forward_shared(self, img1):
         """forward_shared_async + the live matches, as ``forward`` returns them."""
@@ -447,17 +405,6 @@ class LoFTR:
         out["M"] = m
         return out
 
-    def close(self):
-        if getattr(self, "_h", None) is not None and self._h:
-            self._l.mfr_loftr_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 def read_image_gray(path, resize):
     """Reference image loader (SuperGlue/models/utils.py:263-285 with resize_float=True):
@@ -479,48 +426,37 @@ def pad_to_8(img):
     return torch.nn.functional.pad(img, (0, pad_right, 0, pad_bottom), value=0.0)
 
 
-class LoFTR_matcher:
-    """Drop-in for the reference's offline matcher plugin (matchers.py:12-59). ``weights`` is a
-    reference-format state_dict or a checkpoint path ({'state_dict': ...}); the reference reads
-    LoFTR/weights/{indoor,outdoor}_ot.ckpt, which are not distributed with it."""
+def engine_frame(h, w):
+    """The engine frame (H, W) for h x w images: what ``pad_to_8`` makes of them, which must be a multiple of 8."""
+    hp, wp = h + h % 8, w + w % 8
+    if hp % 8 or wp % 8:
+        raise ValueError(f"LoFTR needs a resolution that the reference's padding turns into a multiple of 8, got {h}x{w}")
+    return hp, wp
+
+
+def load_weights(w):
+    """The reference-format LoFTR state dict in ``w``: a state dict, a Lightning checkpoint ({'state_dict': ...}), or
+    the path of a file holding either."""
+    if isinstance(w, str):
+        w = torch.load(w, map_location="cpu")
+    return w.get("state_dict", w)
+
+
+def engine_cfg(cfg):
+    """The engine's ``cfg`` from a method config's LOFTR.{THR, BORDER_RM, TEMPERATURE} keys, DEFAULT_CFG where unset."""
+    return {k: type(v)(_cfg_get(cfg, "LOFTR." + k.upper(), v)) for k, v in DEFAULT_CFG.items()}
+
+
+class LoFTR_matcher(PairMatcher):
+    """Drop-in for the reference's offline matcher plugin (matchers.py:12-59). ``weights``: anything ``load_weights``
+    takes; the reference reads LoFTR/weights/{indoor,outdoor}_ot.ckpt, which are not distributed with it."""
 
     def __init__(self, resize, outdoor=False, weights=None, cfg=None):
         if weights is None:
             weights = "LoFTR/weights/outdoor_ot.ckpt" if outdoor else "LoFTR/weights/indoor_ot.ckpt"
-        if isinstance(weights, str):
-            weights = torch.load(weights, map_location="cpu")["state_dict"]
-        self.resize = resize
-        w, h = int(resize[0]), int(resize[1])
-        self.hp, self.wp = h + h % 8, w + w % 8
-        if self.hp % 8 or self.wp % 8:
-            raise ValueError("LoFTR needs a resolution that the reference's padding turns into a multiple of 8")
-        self.engine = LoFTR(weights, batch=1, height=self.hp, width=self.wp, cfg=cfg)
-
-    def match(self, pair_path):
-        """matchers.py:24-59: both images through read_image(path, device, resize, 0, True) — here decoded (JPEG: nvJPEG)
-        and resized on the GPU (mfr_b200.image_io)."""
-        from . import image_io
-        im0 = image_io.read_image(pair_path[0], self.resize, True, self.engine.device)
-        im1 = image_io.read_image(pair_path[1], self.resize, True, self.engine.device)
-        return self._result(self.engine.forward(im0[None], im1[None]))
-
-    def match_scene(self, ref_path, query_paths):
-        """``[self.match((ref_path, q)) for q in query_paths]``, array for array, with the reference image decoded and
-        encoded once (Map-free: every pair of a scene shares its first image)."""
-        from . import image_io
-        dev = self.engine.device
-        self.engine.set_map(image_io.read_image(ref_path, self.resize, True, dev)[None])
-        return [self._result(self.engine.forward_shared(image_io.read_image(q, self.resize, True, dev)[None]))
-                for q in query_paths]
+        h, w = engine_frame(int(resize[1]), int(resize[0]))
+        super().__init__(resize, LoFTR(load_weights(weights), batch=1, height=h, width=w, cfg=cfg))
 
     @staticmethod
-    def _result(out):
-        if out["M"] > 0:
-            return torch.cat([out["mkpts0_f"], out["mkpts1_f"]], 1).cpu().numpy()
-        return np.full((1, 4), np.nan)
-
-    def match_arrays(self, im0, im1):
-        dev = self.engine.device
-        t0 = torch.from_numpy(np.ascontiguousarray(im0, dtype=np.float32))[None].to(dev)
-        t1 = torch.from_numpy(np.ascontiguousarray(im1, dtype=np.float32))[None].to(dev)
-        return self._result(self.engine.forward(t0, t1))     # padding to the engine frame happens on the device
+    def _matches(out):
+        return out["mkpts0_f"], out["mkpts1_f"]

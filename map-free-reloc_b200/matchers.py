@@ -6,7 +6,7 @@ packs a scene's pairs into the NaN-padded [Npairs, maxN, 4] float64 array the on
 import numpy as np
 
 from .loftr import LoFTR_matcher
-from .model import knn2_gpu, root_sift
+from .model import sift_matches_gpu, sift_matches_host
 from .spsg import SuperGlue_matcher
 
 
@@ -29,31 +29,18 @@ class SIFT_matcher:
         return self.match_arrays(sift, img0, img1)
 
     def match_arrays_gpu(self, img0, img1, ratio=0.8):
-        import torch
-        from . import sift
-        key = img0.shape
-        if key not in self.engines:
-            self.engines[key] = sift.SIFT(2, key[0], key[1], nfeatures=2048, root_sift=True)
-        eng = self.engines[key]
-        eng.detect(torch.from_numpy(np.stack([img0, img1])).to(eng.device))
-        k0, k1, _ = eng.match_pairs(ratio)
-        if k0.shape[0] == 0:
-            return np.full((1, 4), np.nan)
-        return torch.cat([k0, k1], 1).cpu().numpy()
+        return _rows(*sift_matches_gpu(self.engines, img0, img1, 2048, ratio))
 
     @staticmethod
     def match_arrays(sift, img0, img1, ratio=0.8):
-        kp0, des0 = sift.detectAndCompute(img0, None)
-        kp1, des1 = sift.detectAndCompute(img1, None)
-        if des0 is None or des1 is None or len(des1) < 2:
-            return np.full((1, 4), np.nan)
-        i1, d1, _, d2 = knn2_gpu(root_sift(des0), root_sift(des1))
-        good = d1 < ratio * d2
-        if not good.any():
-            return np.full((1, 4), np.nan)
-        pts1 = np.float32([kp0[i].pt for i in np.where(good)[0]]).reshape(-1, 2)
-        pts2 = np.float32([kp1[j].pt for j in i1[good]]).reshape(-1, 2)
-        return np.concatenate([pts1, pts2], axis=1)
+        return _rows(*sift_matches_host(sift, img0, img1, ratio))
+
+
+def _rows(pts0, pts1):
+    """The plugins' result: [N, 4] rows (x0, y0, x1, y1), or np.full((1, 4), nan) when there is no match."""
+    if len(pts0) == 0:
+        return np.full((1, 4), np.nan)
+    return np.concatenate([pts0, pts1], axis=1)
 
 
 MATCHERS = {"LoFTR": LoFTR_matcher, "SG": SuperGlue_matcher, "SIFT": SIFT_matcher}

@@ -65,6 +65,32 @@ def knn2_gpu(des0, des1):
     return i1.cpu().numpy(), d1.cpu().numpy(), i2.cpu().numpy(), d2.cpu().numpy()
 
 
+def sift_matches_host(sift, img0, img1, ratio):
+    """Matches of two uint8 gray images with OpenCV's detector ``sift`` (a cv2.SIFT), RootSIFT, the exact 2-NN on the GPU
+    and Lowe's ratio test (feature_matching.py:75-118) -> (pts0, pts1) float32 [N, 2]."""
+    kp0, des0 = sift.detectAndCompute(img0, None)
+    kp1, des1 = sift.detectAndCompute(img1, None)
+    if des0 is None or des1 is None or len(des1) < 2:
+        return np.zeros((0, 2), np.float32), np.zeros((0, 2), np.float32)
+    i1, d1, _, d2 = knn2_gpu(root_sift(des0), root_sift(des1))
+    good = d1 < ratio * d2          # Lowe's ratio test (feature_matching.py:97-99)
+    pts0 = np.float32([kp0[i].pt for i in np.where(good)[0]]).reshape(-1, 2)
+    pts1 = np.float32([kp1[j].pt for j in i1[good]]).reshape(-1, 2)
+    return pts0, pts1
+
+
+def sift_matches_gpu(engines, img0, img1, nfeatures, ratio):
+    """The same with detection, description and matching on the CUDA SIFT engine (mfr_b200.sift); ``engines`` caches
+    one engine per frame shape. img0 and img1 have the same shape."""
+    from . import sift
+    if img0.shape not in engines:
+        engines[img0.shape] = sift.SIFT(2, img0.shape[0], img0.shape[1], nfeatures=nfeatures, root_sift=True)
+    eng = engines[img0.shape]
+    eng.detect(torch.from_numpy(np.stack([img0, img1])).to(eng.device))
+    k0, k1, _ = eng.match_pairs(ratio)
+    return k0.cpu().numpy(), k1.cpu().numpy()
+
+
 class SIFTMatching:
     """SIFT + RootSIFT + 2-NN ratio test (feature_matching.py:53-118). By default detection/description
     stays on OpenCV's CPU SIFT exactly as in the reference; with SIFT.GPU_DETECTOR the CUDA SIFT engine
@@ -86,31 +112,12 @@ class SIFTMatching:
         img = torch.as_tensor(img).permute(1, 2, 0).numpy()
         return self.cv.cvtColor((255 * img).astype(np.uint8), self.cv.COLOR_RGB2GRAY)
 
-    def _gpu_correspondences(self, img0, img1):
-        from . import sift
-        key = img0.shape
-        if key not in self.engines:
-            self.engines[key] = sift.SIFT(2, key[0], key[1], nfeatures=self.num_features, root_sift=True)
-        eng = self.engines[key]
-        eng.detect(torch.from_numpy(np.stack([img0, img1])).to(eng.device))
-        k0, k1, _ = eng.match_pairs(self.ratio_threshold)
-        return k0.cpu().numpy().reshape(-1, 2), k1.cpu().numpy().reshape(-1, 2)
-
     def get_correspondences(self, data):
         img0 = self.transform_grayscale(torch.as_tensor(data["image0"]).squeeze(0))
         img1 = self.transform_grayscale(torch.as_tensor(data["image1"]).squeeze(0))
         if self.gpu_detector and img0.shape == img1.shape:
-            return self._gpu_correspondences(img0, img1)
-        kp0, des0 = self.sift.detectAndCompute(img0, None)
-        kp1, des1 = self.sift.detectAndCompute(img1, None)
-        if des0 is None or des1 is None or len(des1) < 2:
-            return np.zeros((0, 2), np.float32), np.zeros((0, 2), np.float32)
-        des0, des1 = root_sift(des0), root_sift(des1)
-        i1, d1, _, d2 = knn2_gpu(des0, des1)
-        good = d1 < self.ratio_threshold * d2          # Lowe's ratio test (feature_matching.py:97-99)
-        pts1 = np.float32([kp0[i].pt for i in np.where(good)[0]]).reshape(-1, 2)
-        pts2 = np.float32([kp1[j].pt for j in i1[good]]).reshape(-1, 2)
-        return pts1, pts2
+            return sift_matches_gpu(self.engines, img0, img1, self.num_features, self.ratio_threshold)
+        return sift_matches_host(self.sift, img0, img1, self.ratio_threshold)
 
 
 class LoFTRMatching:
@@ -121,14 +128,9 @@ class LoFTRMatching:
     def __init__(self, cfg):
         from . import loftr, synth
         self._gray = synth.rgb_to_gray_u8
-        w = cfg.LOFTR.WEIGHTS
-        if isinstance(w, str):
-            w = torch.load(w, map_location="cpu")
-            w = w.get("state_dict", w)
-        self.engine = loftr.LoFTR(w, batch=1, height=int(cfg.DATASET.HEIGHT) + int(cfg.DATASET.HEIGHT) % 8,
-                                  width=int(cfg.DATASET.WIDTH) + int(cfg.DATASET.WIDTH) % 8,
-                                  cfg={"thr": cfg.LOFTR.THR, "border_rm": cfg.LOFTR.BORDER_RM,
-                                       "temperature": cfg.LOFTR.TEMPERATURE})
+        h, w = loftr.engine_frame(int(cfg.DATASET.HEIGHT), int(cfg.DATASET.WIDTH))
+        self.engine = loftr.LoFTR(loftr.load_weights(cfg.LOFTR.WEIGHTS), batch=1, height=h, width=w,
+                                  cfg=loftr.engine_cfg(cfg))
 
     def get_correspondences(self, data):
         g0 = self._gray(torch.as_tensor(data["image0"]).squeeze(0).numpy()).astype(np.float32) / 255.0

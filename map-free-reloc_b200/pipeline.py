@@ -30,6 +30,7 @@ import os
 import torch
 
 from . import lib as _lib
+from . import loftr, sift, spsg
 from . import pose_solver as _ps
 
 
@@ -299,7 +300,7 @@ class MethodSpec:
     settings (first budget only) and the engine frame."""
     matcher: str                    # "LoFTR" | "SG" | "SIFT"
     solver: str                     # "EssentialMatrix" | "EssentialMatrixMetric" | "PNP" | "Procrustes"
-    height: int                     # engine frame: DATASET.HEIGHT / WIDTH, padded as LoFTR_matcher pads for LoFTR
+    height: int                     # engine frame: DATASET.HEIGHT / WIDTH, for LoFTR padded by loftr.engine_frame
     width: int
     num_hyp: int
     seed: int
@@ -349,10 +350,8 @@ def resolve_method(cfg):
         raise NotImplementedError(f"Invalid pose solver {solver!r}")
     num_hyp, _, seed, lo = _ps.ransac_settings(cfg, _ps.pnp_default_hyp(cfg) if solver == "PNP" else _ps.DEFAULT_NUM_HYP)
     h, w = int(g("DATASET.HEIGHT", 720)), int(g("DATASET.WIDTH", 540))   # Map-free's frame (config/mapfree.yaml)
-    if matcher == "LoFTR":                 # LoFTR_matcher's padding (matchers.py:41-46, loftr.pad_to_8): size % 8 more
-        h, w = h + h % 8, w + w % 8
-        if h % 8 or w % 8:
-            raise ValueError("LoFTR needs a resolution that the reference's padding turns into a multiple of 8")
+    if matcher == "LoFTR":
+        h, w = loftr.engine_frame(h, w)
     f = lambda k: None if g(k) is None else float(g(k))
     kw = {}
     if solver.startswith("EssentialMatrix"):
@@ -372,32 +371,23 @@ def resolve_method(cfg):
 
 def from_cfg(cfg, batch, weights=None, precision="tf32", depth_hw=None, outdoor=False, device=0, graph=True):
     """Engine + PoseBackend + RelocPipeline for the method of ``cfg`` (see resolve_method), ``batch`` pairs per engine
-    call. ``weights``: LoFTR, a state dict (or a path to one); SG, a (superpoint, superglue) pair of state dicts or the
-    directory holding superpoint_v1.pth and superglue_{indoor,outdoor}.pth (indoor unless ``outdoor``); SIFT, none.
+    call. ``weights``: LoFTR, what loftr.load_weights takes (a state dict, a {'state_dict': ...} checkpoint or a path to
+    either); SG, what spsg.load_weights takes (a (superpoint, superglue) pair of state dicts or the directory holding
+    superpoint_v1.pth and superglue_{indoor,outdoor}.pth, indoor unless ``outdoor``); SIFT, none.
     ``precision`` applies to LoFTR and SG. The method is at ``pipeline.method``."""
     spec = resolve_method(cfg)
     if spec.matcher == "LoFTR":
-        from . import loftr
         if weights is None:
             raise ValueError("LoFTR needs a state dict")
-        sd = torch.load(weights, map_location="cpu") if isinstance(weights, str) else weights
-        lc = {"thr": float(_ps._cfg_get(cfg, "LOFTR.THR", 0.2)), "border_rm": int(_ps._cfg_get(cfg, "LOFTR.BORDER_RM", 2)),
-              "temperature": float(_ps._cfg_get(cfg, "LOFTR.TEMPERATURE", 0.1))}
-        eng = loftr.LoFTR(sd, batch=batch, height=spec.height, width=spec.width, cfg=lc, device=device, graph=graph,
-                          precision=precision)
+        eng = loftr.LoFTR(loftr.load_weights(weights), batch=batch, height=spec.height, width=spec.width,
+                          cfg=loftr.engine_cfg(cfg), device=device, graph=graph, precision=precision)
     elif spec.matcher == "SG":
-        from . import spsg
         if weights is None:
             raise ValueError("SuperPoint + SuperGlue needs state dicts or their directory")
-        if isinstance(weights, str):
-            sp = torch.load(os.path.join(weights, "superpoint_v1.pth"), map_location="cpu")
-            sg = torch.load(os.path.join(weights, f"superglue_{'outdoor' if outdoor else 'indoor'}.pth"), map_location="cpu")
-        else:
-            sp, sg = weights
+        sp, sg = spsg.load_weights(weights, outdoor)
         eng = spsg.SuperPointSuperGlue(sp, sg, batch=batch, height=spec.height, width=spec.width, device=device,
                                        graph=graph, precision=precision)
     else:
-        from . import sift
         eng = sift.SIFTPairs(batch, spec.height, spec.width, nfeatures=spec.sift_features, ratio=spec.sift_ratio,
                              root_sift=True, device=device, graph=graph)
     be = _ps.PoseBackend(max_pairs=batch, max_pts=max(8, min(eng.max_pts_per_pair, _ps.MAX_PTS_LIMIT)),

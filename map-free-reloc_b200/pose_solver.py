@@ -30,22 +30,15 @@ def _cfg_get(cfg, path, default=None):
     return default if cur is None else cur
 
 
-class PoseBackend:
-    """Batched GPU pose solver for up to ``max_pairs`` pairs per call."""
+class PoseBackend(_lib.Engine):
+    """Batched GPU pose solver for up to ``max_pairs`` pairs per call, on the caller's current stream."""
 
     def __init__(self, max_pairs=1, max_pts=8192, max_hyp=8192, device=0):
-        if not torch.cuda.is_available():
-            raise _lib.MfrError("mfr_b200.PoseBackend needs a CUDA device (no CPU fallback)")
-        self._l = _lib.load()
-        self.device = torch.device("cuda", device)
-        torch.cuda.set_device(self.device)
         if not 8 <= int(max_pts) <= MAX_PTS_LIMIT:
             raise ValueError(f"PoseBackend: max_pts must be in [8, {MAX_PTS_LIMIT}] (correspondences of a pair are staged "
                              f"in shared memory), got {max_pts}")
-        h = ctypes.c_void_p()
-        _lib.check(self._l.mfr_pose_solver_create(int(max_pairs), int(max_pts), int(max_hyp), ctypes.byref(h)),
-                   "mfr_pose_solver_create")
-        self._h = h
+        super().__init__("pose_solver", "mfr_pose_solver_create", (int(max_pairs), int(max_pts), int(max_hyp)), device,
+                         stream=False)
         self.max_pairs, self.max_pts, self.max_hyp = int(max_pairs), int(max_pts), int(max_hyp)
 
     def _outs(self, P, total):
@@ -135,24 +128,6 @@ class PoseBackend:
                                           float(max_corr_dist), int(max_iter), float(rel_fitness), float(rel_rmse),
                                           _lib.ptr(R), _lib.ptr(t), _lib.ptr(n), _lib.cur_stream()), "mfr_icp_refine")
         return R, t, n
-
-    def debug_tensor(self, name, shape, dtype):
-        """Zero-copy view of a named scratch buffer of the handle (mfr_pose_solver_debug_tensor: "hyp_results",
-        "lo_results", "pts_norm", "Rd", "td", "Xw", "uv", "vidx", "nvalid", "dmin"), as torch ``dtype`` (float32,
-        float64 or int32) of ``shape``; it shows what the last call that wrote the buffer left there. The records
-        "hyp_results" and "lo_results" are read as raw words and reinterpreted on the host."""
-        return _lib.debug_tensor(self._l, "pose_solver", self._h, name, shape, dtype, self.device)
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._l.mfr_pose_solver_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 # ------------------------------------------------------------------------------------------------

@@ -12,38 +12,33 @@ import torch
 from . import lib as _lib
 
 
-class SIFT:
-    """Engine for ``batch`` images of ``height`` x ``width``. ``nfeatures`` = 0 keeps every keypoint; otherwise
-    OpenCV's retainBest (all keypoints whose response is >= the N-th largest). ``root_sift`` makes the descriptors
-    RootSIFT rows. ``max_candidates`` bounds the refined extrema and the oriented keypoints per image; ``detect``
-    raises when an image has more."""
+class SIFT(_lib.Engine):
+    """Engine for ``batch`` images of ``height`` x ``width`` on the current device, running on the caller's stream.
+    ``nfeatures`` = 0 keeps every keypoint; otherwise OpenCV's retainBest (all keypoints whose response is >= the N-th
+    largest). ``root_sift`` makes the descriptors RootSIFT rows. ``max_candidates`` bounds the refined extrema and the
+    oriented keypoints per image; ``detect`` raises when an image has more."""
 
     def __init__(self, batch, height, width, nfeatures=2048, root_sift=False, max_candidates=32768, graph=True):
-        if not torch.cuda.is_available():
-            raise _lib.MfrError("SIFT engine needs a CUDA device (there is no CPU fallback)")
-        self.l = _lib.load()
         self.B, self.H, self.W = int(batch), int(height), int(width)
-        self.device = torch.device("cuda", torch.cuda.current_device())
-        h = ctypes.c_void_p()
-        _lib.check(self.l.mfr_sift_create(self.B, self.H, self.W, int(nfeatures), int(max_candidates), int(bool(root_sift)),
-                                          ctypes.byref(h)), "mfr_sift_create")
-        self.h = h
-        self.l.mfr_sift_set_graph(self.h, int(bool(graph)))
-        o = _lib.SiftOutputs()
-        _lib.check(self.l.mfr_sift_get_outputs(self.h, ctypes.byref(o)), "mfr_sift_get_outputs")
+        super().__init__("sift", "mfr_sift_create", (self.B, self.H, self.W, int(nfeatures), int(max_candidates),
+                                                     int(bool(root_sift))), stream=False)
+        self._l.mfr_sift_set_graph(self._h, int(bool(graph)))
+        o = self._get_outputs(self._l.mfr_sift_get_outputs, _lib.SiftOutputs)
         self.cap = o.capacity
         B, cap = self.B, self.cap
-        self._counts = self._wrap(o.extrema_counts, (3, B), torch.int32)   # rows: extrema, oriented, selected
-        self._kp = self._wrap(o.keypoints, (B, cap, 5), torch.float32)
-        self._oct = self._wrap(o.octaves, (B, cap), torch.int32)
-        self._desc = self._wrap(o.descriptors, (B, cap, 128), torch.float32)
+        self._counts = self.view(o.extrema_counts, (3, B), torch.int32)   # rows: extrema, oriented, selected
+        self._kp = self.view(o.keypoints, (B, cap, 5), torch.float32)
+        self._oct = self.view(o.octaves, (B, cap), torch.int32)
+        self._desc = self.view(o.descriptors, (B, cap, 128), torch.float32)
 
-    def _wrap(self, addr, shape, dtype):
-        return _lib.device_view(addr, shape, dtype, self.device)
+    @property
+    def l(self):
+        """The library, with ``h`` the handle: for calling mfr_sift_* directly, e.g. with caller-owned buffers."""
+        return self._l
 
-    def debug_tensor(self, name, shape, dtype=torch.float32):
-        """Named intermediate buffer (see mfr_sift_debug_tensor): "gauss_<o>", "dog_<o>", "kp_pre", "kp_pre_octave"."""
-        return _lib.debug_tensor(self.l, "sift", self.h, name, shape, dtype, self.device)
+    @property
+    def h(self):
+        return self._h
 
     def octave_shapes(self):
         """(h, w) of every octave's levels, octave 0 = the doubled image."""
@@ -60,7 +55,7 @@ class SIFT:
         if imgs.dtype != torch.uint8 or tuple(imgs.shape) != (self.B, self.H, self.W) or not imgs.is_cuda:
             raise ValueError(f"expected a uint8 CUDA tensor of shape {(self.B, self.H, self.W)}")
         imgs = imgs.contiguous()
-        _lib.check(self.l.mfr_sift_detect(self.h, _lib.ptr(imgs), _lib.cur_stream()), "mfr_sift_detect")
+        _lib.check(self._l.mfr_sift_detect(self._h, _lib.ptr(imgs), _lib.cur_stream()), "mfr_sift_detect")
         c = self._counts.cpu()
         if int(c[:2].max()) > self.cap:
             raise _lib.MfrError(f"SIFT candidates exceed max_candidates={self.cap}: extrema {c[0].tolist()}, "
@@ -76,31 +71,20 @@ class SIFT:
             raise ValueError("match_pairs needs an even batch (pairs of images 2p, 2p + 1)")
         k0 = torch.empty(P * self.cap, 2, device=self.device); k1 = torch.empty_like(k0)
         off = torch.empty(P + 1, dtype=torch.int32, device=self.device)
-        _lib.check(self.l.mfr_sift_match_pairs(self.h, float(ratio), _lib.ptr(k0), _lib.ptr(k1), _lib.ptr(off),
-                                               _lib.cur_stream()), "mfr_sift_match_pairs")
+        _lib.check(self._l.mfr_sift_match_pairs(self._h, float(ratio), _lib.ptr(k0), _lib.ptr(k1), _lib.ptr(off),
+                                                _lib.cur_stream()), "mfr_sift_match_pairs")
         n = int(off[-1])
         return k0[:n], k1[:n], off
 
     def profile(self, imgs):
         """Eager detect with events between the stages -> dict of milliseconds."""
         ms = (ctypes.c_float * 5)()
-        _lib.check(self.l.mfr_sift_profile(self.h, _lib.ptr(imgs.contiguous()), ms, _lib.cur_stream()), "mfr_sift_profile")
+        _lib.check(self._l.mfr_sift_profile(self._h, _lib.ptr(imgs.contiguous()), ms, _lib.cur_stream()),
+                   "mfr_sift_profile")
         return dict(zip(("pyramid", "extrema", "orientation", "selection", "descriptors"), list(ms)))
 
-    def close(self):
-        if getattr(self, "h", None):
-            torch.cuda.synchronize()
-            self.l.mfr_sift_destroy(self.h)
-            self.h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class SIFTPairs:
+class SIFTPairs(_lib.Engine):
     """Pair engine for ``batch`` pairs of ``height`` x ``width`` uint8 gray images (the bytes the reference's SIFT_matcher
     hands to cv2: ``imread(path, 0)`` then ``cv2.resize`` on uint8): detection, 2-NN and the ratio test of both images of
     every pair in one CUDA graph with no host synchronisation, matches in engine-owned buffers. Bit-identical to
@@ -112,68 +96,33 @@ class SIFTPairs:
 
     def __init__(self, batch, height, width, nfeatures=2048, ratio=0.8, root_sift=True, max_candidates=32768, device=0,
                  graph=True):
-        if not torch.cuda.is_available():
-            raise _lib.MfrError("SIFT pair engine needs a CUDA device (there is no CPU fallback)")
-        self.l = _lib.load()
         self.B, self.H, self.W = int(batch), int(height), int(width)
-        self.device = torch.device("cuda", device)
-        torch.cuda.set_device(self.device)
-        self.stream = torch.cuda.Stream(device=self.device)
-        h = ctypes.c_void_p()
-        _lib.check(self.l.mfr_sift_pairs_create(self.B, self.H, self.W, int(nfeatures), int(max_candidates),
-                                                int(bool(root_sift)), float(ratio), ctypes.byref(h)),
-                   "mfr_sift_pairs_create")
-        self.h = h
-        self.l.mfr_sift_pairs_set_graph(self.h, int(bool(graph)))
-        o = _lib.SiftPairOutputs()
-        _lib.check(self.l.mfr_sift_get_pair_outputs(self.h, ctypes.byref(o)), "mfr_sift_get_pair_outputs")
+        super().__init__("sift_pairs", "mfr_sift_pairs_create",
+                         (self.B, self.H, self.W, int(nfeatures), int(max_candidates), int(bool(root_sift)), float(ratio)),
+                         device)
+        self._l.mfr_sift_pairs_set_graph(self._h, int(bool(graph)))
+        o = self._get_outputs(self._l.mfr_sift_get_pair_outputs, _lib.SiftPairOutputs)
         self.capacity, self.max_pts_per_pair = o.capacity, o.max_pts_per_pair
-        view = lambda a, shape, dt: _lib.device_view(a, shape, dt, self.device)
-        self._k0 = view(o.kpts0, (self.capacity, 2), torch.float32)
-        self._k1 = view(o.kpts1, (self.capacity, 2), torch.float32)
-        self._off = view(o.offsets, (self.B + 1,), torch.int32)
-        self.overflow = view(o.overflow, (self.B,), torch.int32)
-
-    def _images(self, imgs, n):
-        imgs = imgs.reshape(n, self.H, self.W).contiguous()
-        if imgs.dtype != torch.uint8 or not imgs.is_cuda:
-            raise ValueError(f"expected uint8 CUDA images of shape [{n}, {self.H}, {self.W}]")
-        return imgs
-
-    def _run(self, fn, name, *imgs):
-        self.stream.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(self.stream):
-            _lib.check(fn(self.h, *[_lib.ptr(x) for x in imgs], ctypes.c_void_p(self.stream.cuda_stream)), name)
-        for x in imgs:
-            x.record_stream(self.stream)
+        self._k0 = self.view(o.kpts0, (self.capacity, 2), torch.float32)
+        self._k1 = self.view(o.kpts1, (self.capacity, 2), torch.float32)
+        self._off = self.view(o.offsets, (self.B + 1,), torch.int32)
+        self.overflow = self.view(o.overflow, (self.B,), torch.int32)
 
     def forward_async(self, img0, img1):
         """Enqueues one batch of pairs (uint8 CUDA [B,(1,)H,W] each) on the engine stream."""
-        self._run(self.l.mfr_sift_forward_pairs, "mfr_sift_forward_pairs", self._images(img0, self.B),
-                  self._images(img1, self.B))
+        self._call(self._l.mfr_sift_forward_pairs, self._images(img0, self.B, self.H, self.W),
+                   self._images(img1, self.B, self.H, self.W))
 
     def set_map(self, img0):
         """Detects and describes the map image img0 (uint8 CUDA [(1,)(1,)H,W]) once, eagerly, on the engine stream. Until
         the next set_map, ``forward_shared_async(img1)`` gives the bits ``forward_async`` gives with img0 repeated for every
         pair; a paired forward in between does not disturb the map."""
-        self._run(self.l.mfr_sift_set_map, "mfr_sift_set_map", self._images(img0, 1))
+        self._call(self._l.mfr_sift_set_map, self._images(img0, self.H, self.W))
 
     def forward_shared_async(self, img1):
         """Enqueues one batch of B query images (uint8 CUDA [B,(1,)H,W]) against the map of ``set_map``."""
-        self._run(self.l.mfr_sift_forward_shared, "mfr_sift_forward_shared", self._images(img1, self.B))
+        self._call(self._l.mfr_sift_forward_shared, self._images(img1, self.B, self.H, self.W))
 
     def pose_inputs(self):
         """(kpts0 [capacity, 2], kpts1 [capacity, 2], offsets [B + 1]): device views of the last forward's matches."""
         return self._k0, self._k1, self._off
-
-    def close(self):
-        if getattr(self, "h", None):
-            torch.cuda.synchronize()
-            self.l.mfr_sift_pairs_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass

@@ -9,6 +9,7 @@ import numpy as np
 import torch
 
 from . import lib as _lib
+from .image_io import PairMatcher
 
 DEFAULTS = {"nms_radius": 4, "keypoint_threshold": 0.005, "max_keypoints": 1024, "remove_borders": 4,
             "sinkhorn_iterations": 20, "match_threshold": 0.2}          # matchers.py:65-71
@@ -128,44 +129,40 @@ def synthetic_state_dicts(seed=0):
     return sp, sg
 
 
-class SuperPointSuperGlue:
+def load_weights(w, outdoor):
+    """(superpoint, superglue) state dicts from ``w``: such a pair, or the directory holding superpoint_v1.pth and
+    superglue_{indoor,outdoor}.pth (SuperGlue/models/weights in the reference tree)."""
+    if not isinstance(w, str):
+        sp, sg = w
+        return sp, sg
+    return (torch.load(os.path.join(w, "superpoint_v1.pth"), map_location="cpu"),
+            torch.load(os.path.join(w, f"superglue_{'outdoor' if outdoor else 'indoor'}.pth"), map_location="cpu"))
+
+
+class SuperPointSuperGlue(_lib.Engine):
     """CUDA SuperPoint+SuperGlue engine for ``batch`` pairs of [H, W] gray images."""
 
     input_dtype = torch.float32
 
     def __init__(self, sp_sd, sg_sd, batch=1, height=720, width=540, cfg=None, device=0, graph=True, precision="tf32"):
-        if not torch.cuda.is_available():
-            raise _lib.MfrError("mfr_b200.SuperPointSuperGlue needs a CUDA device (no CPU fallback)")
-        self._l = _lib.load()
-        self.cfg = {**DEFAULTS, **(cfg or {})}
+        self.cfg = c = {**DEFAULTS, **(cfg or {})}
         self.B, self.H, self.W, self.K = int(batch), int(height), int(width), int(self.cfg["max_keypoints"])
         self.capacity, self.max_pts_per_pair = self.B * self.K, self.K
-        self.device = torch.device("cuda", device)
-        torch.cuda.set_device(self.device)
-        self.stream = torch.cuda.Stream(device=self.device)
-        h = ctypes.c_void_p()
-        c = self.cfg
         self.precision = {"tf32": 0, "bf16": 1, "fp32x3": 2, "fp32": 2}[precision]
-        _lib.check(self._l.mfr_spsg_create_ex(self.B, self.H, self.W, self.K, int(c["nms_radius"]),
-                                              float(c["keypoint_threshold"]), int(c["remove_borders"]),
-                                              int(c["sinkhorn_iterations"]), float(c["match_threshold"]),
-                                              self.precision, ctypes.byref(h)), "mfr_spsg_create_ex")
-        self._h = h
+        super().__init__("spsg", "mfr_spsg_create_ex", (self.B, self.H, self.W, self.K, int(c["nms_radius"]),
+                                                        float(c["keypoint_threshold"]), int(c["remove_borders"]),
+                                                        int(c["sinkhorn_iterations"]), float(c["match_threshold"]),
+                                                        self.precision), device)
         self._l.mfr_spsg_set_graph(self._h, int(bool(graph)))
         self.load_state_dicts(sp_sd, sg_sd)
-        o = _lib.SpsgOutputs()
-        _lib.check(self._l.mfr_spsg_get_outputs(self._h, ctypes.byref(o)))
-        self._o = o
+        self._o = self._get_outputs(self._l.mfr_spsg_get_outputs, _lib.SpsgOutputs)
 
     def load_state_dicts(self, sp_sd, sg_sd):
         """Uploads new SuperPoint / SuperGlue weights (reference state_dict formats); a map of set_map is dropped."""
-        _lib.upload_weights(self._l, "spsg", self._h, prepare_weights(sp_sd, sg_sd), ctypes.c_void_p(self.stream.cuda_stream))
+        self._upload_weights(prepare_weights(sp_sd, sg_sd))
 
     def num_launches(self):
         return self._l.mfr_spsg_num_launches(self._h)
-
-    def _wrap(self, ptr, shape, dtype):
-        return _lib.device_view(ptr, shape, dtype, self.device)
 
     # buffers stored in bf16 in bf16 mode: the SuperPoint activations, q|k|v, the attention message, the token shadow
     BF16_TENSORS = ("x1a", "x4b", "cPa", "cDa", "qkv", "msg", "tokens_bf16")
@@ -175,60 +172,41 @@ class SuperPointSuperGlue:
         buffers named in BF16_TENSORS ("qkv" [2B][K][768], "msg" [2B][K][256], ...) are torch.bfloat16 views, and
         "attn_scores" / "attn_vt" do not exist (the fused attention never stores them)."""
         bf = self.precision == 1 and name in self.BF16_TENSORS
-        return _lib.debug_tensor(self._l, "spsg", self._h, name, shape, torch.bfloat16 if bf else torch.float32,
-                                 self.device)
+        return super().debug_tensor(name, shape, torch.bfloat16 if bf else torch.float32)
 
     def device_outputs(self):
         o, B, K = self._o, self.B, self.K
-        return {"counts": self._wrap(o.counts, (2 * B,), torch.int32),
-                "keypoints": self._wrap(o.keypoints, (2 * B, K, 2), torch.float32),
-                "scores": self._wrap(o.scores, (2 * B, K), torch.float32),
-                "descriptors": self._wrap(o.descriptors, (2 * B, K, o.desc_ld), torch.float32),
-                "matches0": self._wrap(o.matches0, (B, K), torch.int32),
-                "matching_scores0": self._wrap(o.matching_scores0, (B, K), torch.float32),
-                "m_offsets": self._wrap(o.m_offsets, (B + 1,), torch.int32),
-                "mkpts0": self._wrap(o.mkpts0, (B * K, 2), torch.float32),
-                "mkpts1": self._wrap(o.mkpts1, (B * K, 2), torch.float32)}
+        return {"counts": self.view(o.counts, (2 * B,), torch.int32),
+                "keypoints": self.view(o.keypoints, (2 * B, K, 2), torch.float32),
+                "scores": self.view(o.scores, (2 * B, K), torch.float32),
+                "descriptors": self.view(o.descriptors, (2 * B, K, o.desc_ld), torch.float32),
+                "matches0": self.view(o.matches0, (B, K), torch.int32),
+                "matching_scores0": self.view(o.matching_scores0, (B, K), torch.float32),
+                "m_offsets": self.view(o.m_offsets, (B + 1,), torch.int32),
+                "mkpts0": self.view(o.mkpts0, (B * K, 2), torch.float32),
+                "mkpts1": self.view(o.mkpts1, (B * K, 2), torch.float32)}
 
     def pose_inputs(self):
         """(kpts0 [capacity, 2], kpts1 [capacity, 2], offsets [B + 1]): device views of the last forward's matches in the
         pose back end's layout."""
         o = self._o
-        return (self._wrap(o.mkpts0, (self.capacity, 2), torch.float32), self._wrap(o.mkpts1, (self.capacity, 2), torch.float32),
-                self._wrap(o.m_offsets, (self.B + 1,), torch.int32))
+        return (self.view(o.mkpts0, (self.capacity, 2), torch.float32), self.view(o.mkpts1, (self.capacity, 2), torch.float32),
+                self.view(o.m_offsets, (self.B + 1,), torch.int32))
 
     def forward_async(self, img0, img1):
-        img0 = img0.reshape(self.B, self.H, self.W).contiguous()
-        img1 = img1.reshape(self.B, self.H, self.W).contiguous()
-        assert img0.is_cuda and img0.dtype == torch.float32
-        self.stream.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(self.stream):
-            _lib.check(self._l.mfr_spsg_forward(self._h, _lib.ptr(img0), _lib.ptr(img1),
-                                                ctypes.c_void_p(self.stream.cuda_stream)), "spsg forward")
-        img0.record_stream(self.stream)
-        img1.record_stream(self.stream)
+        """Enqueues one batch of pairs (CUDA float32 [B,(1,)H,W] each) on the engine stream."""
+        self._call(self._l.mfr_spsg_forward, self._images(img0, self.B, self.H, self.W),
+                   self._images(img1, self.B, self.H, self.W))
 
     def set_map(self, img0):
         """Runs SuperPoint once, eagerly on the engine stream, on the map image img0 (CUDA float32 [(1,)(1,)H,W]). Until
         the next set_map, ``forward_shared[_async](img1)`` gives the bits ``forward[_async]`` gives with img0 repeated for
         every pair; a paired forward in between does not disturb the map."""
-        img0 = img0.reshape(self.H, self.W).contiguous()
-        assert img0.is_cuda and img0.dtype == torch.float32
-        self.stream.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(self.stream):
-            _lib.check(self._l.mfr_spsg_set_map(self._h, _lib.ptr(img0), ctypes.c_void_p(self.stream.cuda_stream)),
-                       "spsg set_map")
-        img0.record_stream(self.stream)
+        self._call(self._l.mfr_spsg_set_map, self._images(img0, self.H, self.W))
 
     def forward_shared_async(self, img1):
         """Enqueues one batch of B query images [B,(1,)H,W] against the map of ``set_map``."""
-        img1 = img1.reshape(self.B, self.H, self.W).contiguous()
-        assert img1.is_cuda and img1.dtype == torch.float32
-        self.stream.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(self.stream):
-            _lib.check(self._l.mfr_spsg_forward_shared(self._h, _lib.ptr(img1), ctypes.c_void_p(self.stream.cuda_stream)),
-                       "spsg forward_shared")
-        img1.record_stream(self.stream)
+        self._call(self._l.mfr_spsg_forward_shared, self._images(img1, self.B, self.H, self.W))
 
     def forward_shared(self, img1):
         self.forward_shared_async(img1)
@@ -242,9 +220,7 @@ class SuperPointSuperGlue:
         s_ = np.ascontiguousarray(scores, dtype=np.float32); d = np.ascontiguousarray(desc, dtype=np.float32)
         assert k.shape == (2 * self.B, self.K, 2) and d.shape == (2 * self.B, self.K, 256)
         P = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-        with torch.cuda.stream(self.stream):
-            _lib.check(self._l.mfr_spsg_forward_superglue(self._h, P(c), P(k), P(s_), P(d),
-                                                          ctypes.c_void_p(self.stream.cuda_stream)), "superglue")
+        self._call(self._l.mfr_spsg_forward_superglue, P(c), P(k), P(s_), P(d))
         self.stream.synchronize()
         return self.device_outputs()
 
@@ -253,57 +229,19 @@ class SuperPointSuperGlue:
         self.stream.synchronize()
         return self.device_outputs()
 
-    def close(self):
-        if getattr(self, "_h", None):
-            self._l.mfr_spsg_destroy(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class SuperGlue_matcher:
-    """Drop-in for the reference's offline matcher plugin (matchers.py:62-120). ``weights_dir``
-    holds superpoint_v1.pth and superglue_{indoor,outdoor}.pth (SuperGlue/models/weights in the
-    reference tree)."""
+class SuperGlue_matcher(PairMatcher):
+    """Drop-in for the reference's offline matcher plugin (matchers.py:62-120). ``weights_dir`` holds superpoint_v1.pth
+    and superglue_{indoor,outdoor}.pth (SuperGlue/models/weights in the reference tree); ``state_dicts``, a (superpoint,
+    superglue) pair, replaces it."""
 
     def __init__(self, resize, outdoor=False, weights_dir="SuperGlue/models/weights", state_dicts=None, precision="tf32"):
-        if state_dicts is None:
-            sp = torch.load(os.path.join(weights_dir, "superpoint_v1.pth"), map_location="cpu")
-            sg = torch.load(os.path.join(weights_dir, f"superglue_{'outdoor' if outdoor else 'indoor'}.pth"), map_location="cpu")
-        else:
-            sp, sg = state_dicts
-        self.resize = resize
+        sp, sg = load_weights(weights_dir if state_dicts is None else state_dicts, outdoor)
         # precision: "tf32" (default), "bf16" (throughput mode, see include/mfr_b200.h) or "fp32x3"
-        self.engine = SuperPointSuperGlue(sp, sg, batch=1, height=int(resize[1]), width=int(resize[0]), precision=precision)
-
-    def match(self, pair_path):
-        """matchers.py:93-120; images decoded (JPEG: nvJPEG) and resized on the GPU (mfr_b200.image_io)."""
-        from . import image_io
-        dev = self.engine.device
-        return self._result(self.engine.forward(image_io.read_image(pair_path[0], self.resize, True, dev)[None],
-                                                image_io.read_image(pair_path[1], self.resize, True, dev)[None]))
-
-    def match_scene(self, ref_path, query_paths):
-        """``[self.match((ref_path, q)) for q in query_paths]``, array for array, with the reference image decoded and
-        run through SuperPoint once (Map-free: every pair of a scene shares its first image)."""
-        from . import image_io
-        dev = self.engine.device
-        self.engine.set_map(image_io.read_image(ref_path, self.resize, True, dev)[None])
-        return [self._result(self.engine.forward_shared(image_io.read_image(q, self.resize, True, dev)[None]))
-                for q in query_paths]
-
-    def match_arrays(self, im0, im1):
-        dev = self.engine.device
-        return self._result(self.engine.forward(torch.from_numpy(np.ascontiguousarray(im0, dtype=np.float32))[None].to(dev),
-                                                torch.from_numpy(np.ascontiguousarray(im1, dtype=np.float32))[None].to(dev)))
+        super().__init__(resize, SuperPointSuperGlue(sp, sg, batch=1, height=int(resize[1]), width=int(resize[0]),
+                                                     precision=precision))
 
     @staticmethod
-    def _result(o):
+    def _matches(o):
         m = int(o["m_offsets"][1].item())
-        if m > 0:
-            return torch.cat([o["mkpts0"][:m], o["mkpts1"][:m]], 1).cpu().numpy()
-        return np.full((1, 4), np.nan)
+        return o["mkpts0"][:m], o["mkpts1"][:m]

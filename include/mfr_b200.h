@@ -350,6 +350,33 @@ int mfr_pnp_ransac(mfr_pose_solver* s, const float* kpts0, const float* kpts1, c
                    int num_hyp, float reproj_threshold, unsigned long long seed, float* R, float* t,
                    int* n_inliers, unsigned char* mask, void* stream);
 
+/* mfr_emat_ransac / mfr_pnp_ransac with the CONFIDENCE escalation of the solver plugins (pose_solver._SolverBase:
+ * EMAT_RANSAC.CONFIDENCE / PNP.CONFIDENCE up to GPU_RANSAC.MAX_HYPOTHESES), per pair, on the device:
+ *   budgets  h0 = num_hyp, then min(max_hyp, 4 h_prev) while h_prev < max_hyp. Every round is enqueued up front; a round
+ *            is the fixed-budget call at its budget (same seed, same block partition) restricted to the pairs still
+ *            active, and a pair that is done skips the later rounds' blocks. No host synchronisation: the call can be
+ *            captured in a CUDA graph.
+ *   rule     after the round at h, a pair stops iff h >= required(confidence, n / N, s) with N = min(offsets[p+1] -
+ *            offsets[p], max_pts_per_pair), n its inliers at h, s = 5 (E-mat) or 4 (PnP), required = the number of
+ *            samples after which an all-inlier sample has been drawn with probability confidence (capped at 2^31 - 1).
+ *            n <= 0 stops only at max_hyp (the NaN pose stands). A pair with N < s is done after round 0 with budget 0.
+ *   result   pair p's outputs (R, t, n_inliers, its mask rows; for E-mat also the fp64 pose kept for
+ *            mfr_scale_from_depth) equal bit for bit those of the fixed-budget call on the same batch at num_hyp =
+ *            budgets_out[p], the budget at which it stopped (max_hyp if it never did).
+ * budgets_out: device int[P], or NULL. confidence <= 0: one round at num_hyp. num_hyp < 1, max_hyp < num_hyp or max_hyp
+ * above the handle's max_hypotheses: MFR_ERR_ARG (nothing is clipped).
+ * The rule is evaluated with the device's fp64 log / log1p / pow, which may differ from the host libm's in the last bit:
+ * a decision can differ from the plugins' only where the required count lies within ~1e-15 (relative) of a budget. */
+int mfr_emat_ransac_escalate(mfr_pose_solver* s, const float* kpts0, const float* kpts1, const int* offsets,
+                             int P, const float* K0, const float* K1, float pix_threshold, int num_hyp,
+                             unsigned long long seed, int lo_enabled, float* R, float* t, int* n_inliers,
+                             unsigned char* mask, double confidence, int max_hyp, int* budgets_out, void* stream);
+int mfr_pnp_ransac_escalate(mfr_pose_solver* s, const float* kpts0, const float* kpts1, const int* offsets,
+                            int P, const float* K0, const float* K1, const float* depth0, int H, int W,
+                            int num_hyp, float reproj_threshold, unsigned long long seed, float* R, float* t,
+                            int* n_inliers, unsigned char* mask, double confidence, int max_hyp, int* budgets_out,
+                            void* stream);
+
 /* ProcrustesSolver.estimate_pose with REFINE = False (pose_solver.py:247-320): lift both keypoint sets
  * through their depth maps (valid iff depth > depth.min() on both sides), RANSAC over 3-point Kabsch
  * alignments with inlier distance max_corr_dist (metres), refit on the inliers. The reference calls
@@ -365,11 +392,15 @@ int mfr_procrustes_ransac(mfr_pose_solver* s, const float* kpts0, const float* k
  * They are NOT a CPU fallback: no product entry point calls them.
  *   five_point : x0, x1 double[5][2] normalised points, E_out double[10][9]; returns #solutions
  *   p3p        : X double[3][3] points, f double[3][3] unit bearings, R_out [4][9], t_out [4][3]
- *   poly roots : coef[0..deg] ascending, deg <= 10; returns #real roots (ascending)          */
+ *   poly roots : coef[0..deg] ascending, deg <= 10; returns #real roots (ascending)
+ *   ransac_satisfied : 1 iff the escalation stops after a round at `budget` that found n_inliers of n_points
+ *                (the rule of mfr_emat_ransac_escalate, cap max_budget, minimal sample sample_size), else 0    */
 int mfr_host_five_point(const double* x0, const double* x1, double* E_out);
 int mfr_host_p3p(const double* X, const double* f, double* R_out, double* t_out);
 int mfr_host_poly_real_roots(const double* coef, int deg, double* roots);
 int mfr_host_decompose_essential(const double* E, double* R1, double* R2, double* t);
+int mfr_host_ransac_satisfied(double confidence, int n_inliers, int n_points, int budget, int max_budget,
+                              int sample_size);
 
 /* Debug probe (microbenchmark used by scripts/, not part of the product path): microseconds per
  * launch of a prebuilt conv/GEMM op launched back to back.

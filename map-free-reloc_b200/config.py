@@ -83,7 +83,8 @@ def get_default_cfg():
         # additive
         "LOFTR": {"WEIGHTS": None, "THR": 0.2, "BORDER_RM": 2, "TEMPERATURE": 0.1, "BATCH": 1},
         # NUM_HYPOTHESES None = the solver's default (E-mat 2048; PnP: PNP.RANSAC_ITER rounded up to 128);
-        # MAX_HYPOTHESES bounds the CONFIDENCE-driven escalation (pose_solver._SolverBase)
+        # MAX_HYPOTHESES bounds the CONFIDENCE-driven escalation of the solver plugins (pose_solver._SolverBase) and of
+        # the stream when it is asked to escalate (pipeline.from_cfg(..., escalate=True), decided per pair on the device)
         "GPU_RANSAC": {"NUM_HYPOTHESES": None, "MAX_HYPOTHESES": 32768, "SEED": 0x5EED, "LOCAL_OPTIMISATION": True,
                        "FINAL_REFIT": "lsq"},
     })

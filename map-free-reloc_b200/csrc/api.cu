@@ -334,6 +334,22 @@ int mfr_pnp_ransac(mfr_pose_solver* s, const float* kpts0, const float* kpts1, c
   return mfr::pnp_ransac(s->s, kpts0, kpts1, offsets, P, K0, K1, depth0, H, W, num_hyp, reproj_threshold, seed,
                          R, t, n_inliers, mask, static_cast<cudaStream_t>(stream));
 }
+int mfr_emat_ransac_escalate(mfr_pose_solver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
+                             const float* K0, const float* K1, float pix_threshold, int num_hyp,
+                             unsigned long long seed, int lo_enabled, float* R, float* t, int* n_inliers,
+                             unsigned char* mask, double confidence, int max_hyp, int* budgets_out, void* stream) {
+  if (!s) return MFR_ERR_ARG;
+  return mfr::emat_ransac_escalate(s->s, kpts0, kpts1, offsets, P, K0, K1, pix_threshold, num_hyp, seed, lo_enabled, R,
+                                   t, n_inliers, mask, confidence, max_hyp, budgets_out, static_cast<cudaStream_t>(stream));
+}
+int mfr_pnp_ransac_escalate(mfr_pose_solver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
+                            const float* K0, const float* K1, const float* depth0, int H, int W, int num_hyp,
+                            float reproj_threshold, unsigned long long seed, float* R, float* t, int* n_inliers,
+                            unsigned char* mask, double confidence, int max_hyp, int* budgets_out, void* stream) {
+  if (!s) return MFR_ERR_ARG;
+  return mfr::pnp_ransac_escalate(s->s, kpts0, kpts1, offsets, P, K0, K1, depth0, H, W, num_hyp, reproj_threshold, seed,
+                                  R, t, n_inliers, mask, confidence, max_hyp, budgets_out, static_cast<cudaStream_t>(stream));
+}
 
 int mfr_procrustes_ransac(mfr_pose_solver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
                           const float* K0, const float* K1, const float* depth0, const float* depth1, int H, int W,
@@ -359,6 +375,9 @@ int mfr_host_poly_real_roots(const double* coef, int deg, double* roots) {
 int mfr_host_decompose_essential(const double* E, double* R1, double* R2, double* t) {
   mfr::geo::decompose_essential(E, R1, R2, t);
   return MFR_OK;
+}
+int mfr_host_ransac_satisfied(double confidence, int n_inliers, int n_points, int budget, int max_budget, int sample_size) {
+  return mfr::geo::ransac_satisfied(confidence, n_inliers, n_points, budget, max_budget, sample_size) ? 1 : 0;
 }
 
 // ------------------------------------------------------------------------------------------ debug probes

@@ -139,9 +139,10 @@ __global__ void __launch_bounds__(256) emat_normalise_kernel(const float* __rest
 __global__ void __maxnreg__(160) emat_hyp_kernel(   // launched with <= kHypPerBlock threads
     const float4* __restrict__ pts_all, const int* __restrict__ offsets,
     const float* __restrict__ K0s, const float* __restrict__ K1s, float pix_thr, int num_hyp,
-    unsigned long long seed, int max_pts, HypResult* __restrict__ results) {
+    unsigned long long seed, int max_pts, HypResult* __restrict__ results, const int* __restrict__ active) {
   __shared__ double s_cost[kHypPerBlock / 32];
   const int pair = blockIdx.y;
+  if (active && !active[pair]) return;
   const int n0 = offsets[pair];
   const int N = min(offsets[pair + 1] - n0, max_pts);
   HypResult* out = results + static_cast<size_t>(pair) * gridDim.x + blockIdx.x;
@@ -495,10 +496,12 @@ constexpr int kLoMaxPts = 1024;    // correspondences used by the candidate LO r
 __global__ void __launch_bounds__(kLoThreads) emat_lo_kernel(
     const float* __restrict__ kpts0, const float* __restrict__ kpts1, const int* __restrict__ offsets,
     const float* __restrict__ K0s, const float* __restrict__ K1s, float pix_thr, int blocks_per_pair,
-    int max_pts, const HypResult* __restrict__ results, LoResult* __restrict__ lo_out, int lo_enabled) {
+    int max_pts, const HypResult* __restrict__ results, LoResult* __restrict__ lo_out, int lo_enabled,
+    const int* __restrict__ active) {
   extern __shared__ float4 s_pts[];
   __shared__ EmatShared S;
   const int pair = blockIdx.x, c = blockIdx.y;
+  if (active && !active[pair]) return;
   LoResult* out = lo_out + static_cast<size_t>(pair) * kLoTopK + c;
   const float* K0 = K0s + 9 * pair;
   const float* K1 = K1s + 9 * pair;
@@ -534,10 +537,11 @@ __global__ void __launch_bounds__(kLoThreads) emat_final_kernel(
     int max_pts, const HypResult* __restrict__ results, const LoResult* __restrict__ lo_out,
     double* __restrict__ Rd, double* __restrict__ td,
     float* __restrict__ Rf, float* __restrict__ tf, int* __restrict__ n_inl,
-    unsigned char* __restrict__ mask, int lo_enabled) {
+    unsigned char* __restrict__ mask, int lo_enabled, const int* __restrict__ active) {
   extern __shared__ float4 s_pts[];
   __shared__ EmatShared S;
   const int pair = blockIdx.x;
+  if (active && !active[pair]) return;   // a finished pair keeps R, t, n, mask, Rd and td of its last round
   const int n0 = offsets[pair];
   const int Nall = offsets[pair + 1] - n0;
   auto fail = [&]() {
@@ -814,10 +818,11 @@ struct PnpPt { float X, Y, Z, u, v; };
 __global__ void __launch_bounds__(kHypPerBlock) pnp_hyp_kernel(
     const double* __restrict__ Xw, const float* __restrict__ uv, const int* __restrict__ offsets,
     const int* __restrict__ nvalid, const float* __restrict__ K1s, float reproj_thr, int num_hyp,
-    unsigned long long seed, int max_pts, HypResult* __restrict__ results) {
+    unsigned long long seed, int max_pts, HypResult* __restrict__ results, const int* __restrict__ active) {
   extern __shared__ float s_raw[];
   __shared__ HypResult s_best[kHypPerBlock / 32];
   const int pair = blockIdx.y;
+  if (active && !active[pair]) return;
   const int s0 = pair * max_pts;   // scratch rows of this pair (compacted, at most max_pts)
   const int N = nvalid[pair];
   HypResult* out = results + static_cast<size_t>(pair) * gridDim.x + blockIdx.x;
@@ -927,12 +932,13 @@ __global__ void __launch_bounds__(256) pnp_final_kernel(
     const double* __restrict__ Xw, const float* __restrict__ uv, const int* __restrict__ vidx,
     const int* __restrict__ offsets, const int* __restrict__ nvalid, const float* __restrict__ K1s,
     float reproj_thr, int blocks_per_pair, int max_pts, const HypResult* __restrict__ results, float* __restrict__ Rf,
-    float* __restrict__ tf, int* __restrict__ n_inl, unsigned char* __restrict__ mask) {
+    float* __restrict__ tf, int* __restrict__ n_inl, unsigned char* __restrict__ mask, const int* __restrict__ active) {
   __shared__ double sh_red[8 * 28];
   __shared__ double s_R[9], s_t[3], s_R0[9], s_t0[3], s_prevR[9], s_prevt[3], s_H[36], s_g[6];
   __shared__ double s_prev_cost, s_lambda;
   __shared__ int s_flag, s_n;
   const int pair = blockIdx.x;
+  if (active && !active[pair]) return;   // a finished pair keeps R, t, n and mask of its last round
   const int n0 = offsets[pair];
   const int Nall = offsets[pair + 1] - n0;
   const int s0 = pair * max_pts;
@@ -1471,6 +1477,26 @@ __global__ void icp_finish_kernel(const double* __restrict__ state, int P, float
   n_inl[pair] = static_cast<int>(st[12] * st[17]);                // pose_solver.py:319: int(fitness * len(pcl_1.points))
 }
 
+// ================================================================================================
+// CONFIDENCE escalation (pose_solver._SolverBase on the device): after the round at `budget`, every pair still active
+// records that budget (its outputs now hold that round's result) and stays active iff the stopping rule asks for more.
+// Round 0 runs every pair (first_round); a pair with fewer correspondences than a minimal sample leaves with budget 0.
+// ================================================================================================
+__global__ void ransac_escalate_kernel(const int* __restrict__ offsets, const int* __restrict__ n_inl, int P, int max_pts,
+                                       double confidence, int budget, int max_budget, int sample_size, int first_round,
+                                       int* __restrict__ active, int* __restrict__ budgets) {
+  const int pair = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pair >= P || (!first_round && !active[pair])) return;
+  const int N = min(offsets[pair + 1] - offsets[pair], max_pts);
+  if (N < sample_size) {
+    active[pair] = 0;
+    budgets[pair] = 0;
+    return;
+  }
+  budgets[pair] = budget;
+  active[pair] = ransac_satisfied(confidence, n_inl[pair], N, budget, max_budget, sample_size) ? 0 : 1;
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -1484,6 +1510,7 @@ struct PoseSolver {
   double *Rd = nullptr, *td = nullptr, *Xw = nullptr, *X1w = nullptr;
   float* uv = nullptr;
   int *vidx = nullptr, *nvalid = nullptr;
+  int *active = nullptr, *budgets = nullptr;   // CONFIDENCE escalation: pair still solving / budget of its outputs
   unsigned int *dmin = nullptr, *dmin1 = nullptr;
   double* icp_state = nullptr;   // ICP refinement scratch (allocated on first use)
   size_t total_pts;
@@ -1507,6 +1534,8 @@ int pose_solver_create(int max_pairs, int max_pts, int max_hyp, PoseSolver** out
   ok &= cudaMalloc(&s->uv, sizeof(float) * 2 * s->total_pts) == cudaSuccess;
   ok &= cudaMalloc(&s->vidx, sizeof(int) * s->total_pts) == cudaSuccess;
   ok &= cudaMalloc(&s->nvalid, sizeof(int) * max_pairs) == cudaSuccess;
+  ok &= cudaMalloc(&s->active, sizeof(int) * max_pairs) == cudaSuccess;
+  ok &= cudaMalloc(&s->budgets, sizeof(int) * max_pairs) == cudaSuccess;
   ok &= cudaMalloc(&s->dmin, sizeof(unsigned int) * max_pairs) == cudaSuccess;
   ok &= cudaMalloc(&s->dmin1, sizeof(unsigned int) * max_pairs) == cudaSuccess;
   if (!ok) { pose_solver_destroy(s); return MFR_ERR_CUDA; }
@@ -1525,7 +1554,7 @@ int pose_solver_create(int max_pairs, int max_pts, int max_hyp, PoseSolver** out
 void pose_solver_destroy(PoseSolver* s) {
   if (!s) return;
   cudaFree(s->results); cudaFree(s->lo_out); cudaFree(s->pts_norm); cudaFree(s->Rd); cudaFree(s->td); cudaFree(s->Xw); cudaFree(s->uv);
-  cudaFree(s->vidx); cudaFree(s->nvalid); cudaFree(s->dmin); cudaFree(s->dmin1); cudaFree(s->X1w); cudaFree(s->icp_state);
+  cudaFree(s->vidx); cudaFree(s->nvalid); cudaFree(s->active); cudaFree(s->budgets); cudaFree(s->dmin); cudaFree(s->dmin1); cudaFree(s->X1w); cudaFree(s->icp_state);
   delete s;
 }
 
@@ -1557,28 +1586,101 @@ int pose_solver_debug_tensor(PoseSolver* s, const char* name, void** ptr, long l
   return MFR_ERR_ARG;
 }
 
-int emat_ransac(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
-                const float* K0, const float* K1, float pix_thr, int num_hyp, unsigned long long seed,
-                int lo_enabled, float* R, float* t, int* n_inl, unsigned char* mask, cudaStream_t st) {
-  if (P < 1 || P > s->max_pairs || num_hyp < 1) return MFR_ERR_ARG;
-  num_hyp = std::min(num_hyp, s->max_hyp);
-  // hypotheses per block: 128 when that already gives >= 2 blocks per SM, else down to one warp per block
-  // (enough pairs: full 128-thread blocks, one per SM beside the matcher's GEMM CTAs — see emat_hyp_kernel)
-  int hpb = kHypPerBlock;
-  while (hpb > 32 && static_cast<long long>(P) * ((num_hyp + hpb - 1) / hpb) < sm_count() / 2) hpb /= 2;
-  const int blocks = (num_hyp + hpb - 1) / hpb;
+namespace {
+
+// The hypothesis budgets of one solve: one entry for a fixed-budget call, h0, min(cap, 4 h0), ... up to the cap for an
+// escalating one (at most 17 entries: the cap is an int).
+struct BudgetSeq {
+  int h[17];
+  int n = 0;
+  double confidence = 0.0;
+  int cap = 0;
+  int* budgets_out = nullptr;   // device int[P] or nullptr
+};
+
+BudgetSeq fixed_budget(const PoseSolver* s, int num_hyp) {
+  BudgetSeq b;
+  b.h[0] = b.cap = std::min(num_hyp, s->max_hyp);
+  b.n = 1;
+  return b;
+}
+
+int escalation_budgets(const PoseSolver* s, int num_hyp, double confidence, int max_hyp, int* budgets_out, BudgetSeq* b) {
+  if (num_hyp < 1 || max_hyp < num_hyp || max_hyp > s->max_hyp) return MFR_ERR_ARG;
+  b->h[0] = num_hyp;
+  b->n = 1;
+  if (confidence > 0.0)
+    for (long long h = num_hyp; h < max_hyp;) {
+      h = std::min<long long>(max_hyp, 4 * h);
+      b->h[b->n++] = static_cast<int>(h);
+    }
+  b->confidence = confidence;
+  b->cap = max_hyp;
+  b->budgets_out = budgets_out;
+  return MFR_OK;
+}
+
+// Runs round(h, active) for every budget h of `b`: round 0 on every pair (active = nullptr), each later round on the
+// pairs the stopping rule kept active. All rounds are enqueued up front; no host synchronisation.
+template <class Round>
+int run_rounds(PoseSolver* s, const BudgetSeq& b, const int* offsets, int P, const int* n_inl, int sample_size,
+               cudaStream_t st, Round round) {
+  int* budgets = b.budgets_out ? b.budgets_out : s->budgets;
+  for (int k = 0; k < b.n; ++k) {
+    round(b.h[k], k == 0 ? nullptr : s->active);
+    if (b.n > 1 || b.budgets_out)
+      ransac_escalate_kernel<<<(P + 255) / 256, 256, 0, st>>>(offsets, n_inl, P, s->max_pts, b.confidence, b.h[k], b.cap,
+                                                             sample_size, k == 0, s->active, budgets);
+  }
+  MFR_CUDA_CHECK(cudaGetLastError());
+  return MFR_OK;
+}
+
+}  // namespace
+
+static int emat_solve(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P, const float* K0,
+                      const float* K1, float pix_thr, const BudgetSeq& b, unsigned long long seed, int lo_enabled,
+                      float* R, float* t, int* n_inl, unsigned char* mask, cudaStream_t st) {
+  if (P < 1 || P > s->max_pairs) return MFR_ERR_ARG;
   const size_t smem = static_cast<size_t>(s->max_pts) * 16;
   emat_normalise_kernel<<<dim3((s->max_pts + 255) / 256, P), 256, 0, st>>>(kpts0, kpts1, offsets, K0, K1, s->max_pts,
                                                                           static_cast<float4*>(s->pts_norm));
-  emat_hyp_kernel<<<dim3(blocks, P), hpb, 0, st>>>(static_cast<const float4*>(s->pts_norm), offsets, K0, K1, pix_thr, num_hyp,
-                                                   seed, s->max_pts, s->results);
-  emat_lo_kernel<<<dim3(P, kLoTopK), kLoThreads, smem, st>>>(kpts0, kpts1, offsets, K0, K1, pix_thr, blocks, s->max_pts,
-                                                      s->results, static_cast<LoResult*>(s->lo_out), lo_enabled);
-  emat_final_kernel<<<P, kLoThreads, smem, st>>>(kpts0, kpts1, offsets, K0, K1, pix_thr, blocks, s->max_pts,
-                                          s->results, static_cast<const LoResult*>(s->lo_out), s->Rd, s->td, R, t,
-                                          n_inl, mask, lo_enabled);
-  MFR_CUDA_CHECK(cudaGetLastError());
-  return MFR_OK;
+  // a round at budget h is the fixed-budget solve at h: the same hypotheses per block (so the same block partition
+  // and LO candidates) and the same seed
+  auto round = [&](int num_hyp, const int* active) {
+    // hypotheses per block: 128 when that already gives >= 2 blocks per SM, else down to one warp per block
+    // (enough pairs: full 128-thread blocks, one per SM beside the matcher's GEMM CTAs — see emat_hyp_kernel)
+    int hpb = kHypPerBlock;
+    while (hpb > 32 && static_cast<long long>(P) * ((num_hyp + hpb - 1) / hpb) < sm_count() / 2) hpb /= 2;
+    const int blocks = (num_hyp + hpb - 1) / hpb;
+    emat_hyp_kernel<<<dim3(blocks, P), hpb, 0, st>>>(static_cast<const float4*>(s->pts_norm), offsets, K0, K1, pix_thr,
+                                                     num_hyp, seed, s->max_pts, s->results, active);
+    emat_lo_kernel<<<dim3(P, kLoTopK), kLoThreads, smem, st>>>(kpts0, kpts1, offsets, K0, K1, pix_thr, blocks, s->max_pts,
+                                                               s->results, static_cast<LoResult*>(s->lo_out), lo_enabled,
+                                                               active);
+    emat_final_kernel<<<P, kLoThreads, smem, st>>>(kpts0, kpts1, offsets, K0, K1, pix_thr, blocks, s->max_pts, s->results,
+                                                   static_cast<const LoResult*>(s->lo_out), s->Rd, s->td, R, t, n_inl, mask,
+                                                   lo_enabled, active);
+  };
+  return run_rounds(s, b, offsets, P, n_inl, 5, st, round);
+}
+
+int emat_ransac(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
+                const float* K0, const float* K1, float pix_thr, int num_hyp, unsigned long long seed,
+                int lo_enabled, float* R, float* t, int* n_inl, unsigned char* mask, cudaStream_t st) {
+  if (num_hyp < 1) return MFR_ERR_ARG;
+  return emat_solve(s, kpts0, kpts1, offsets, P, K0, K1, pix_thr, fixed_budget(s, num_hyp), seed, lo_enabled, R, t, n_inl,
+                    mask, st);
+}
+
+int emat_ransac_escalate(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
+                         const float* K0, const float* K1, float pix_thr, int num_hyp, unsigned long long seed,
+                         int lo_enabled, float* R, float* t, int* n_inl, unsigned char* mask, double confidence,
+                         int max_hyp, int* budgets_out, cudaStream_t st) {
+  BudgetSeq b;
+  const int rc = escalation_budgets(s, num_hyp, confidence, max_hyp, budgets_out, &b);
+  if (rc != MFR_OK) return rc;
+  return emat_solve(s, kpts0, kpts1, offsets, P, K0, K1, pix_thr, b, seed, lo_enabled, R, t, n_inl, mask, st);
 }
 
 int scale_from_depth(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
@@ -1595,23 +1697,41 @@ int scale_from_depth(PoseSolver* s, const float* kpts0, const float* kpts1, cons
   return MFR_OK;
 }
 
-int pnp_ransac(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
-               const float* K0, const float* K1, const float* depth0, int H, int W, int num_hyp,
-               float reproj_thr, unsigned long long seed, float* R, float* t, int* n_inl,
-               unsigned char* mask, cudaStream_t st) {
-  if (P < 1 || P > s->max_pairs || num_hyp < 1) return MFR_ERR_ARG;
-  num_hyp = std::min(num_hyp, s->max_hyp);
-  const int blocks = (num_hyp + kHypPerBlock - 1) / kHypPerBlock;
+static int pnp_solve(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P, const float* K0,
+                     const float* K1, const float* depth0, int H, int W, const BudgetSeq& b, float reproj_thr,
+                     unsigned long long seed, float* R, float* t, int* n_inl, unsigned char* mask, cudaStream_t st) {
+  if (P < 1 || P > s->max_pairs) return MFR_ERR_ARG;
   MFR_CUDA_CHECK(cudaMemsetAsync(s->dmin, 0x7f, sizeof(unsigned int) * P, st));
   depth_min_kernel<<<dim3(64, P), 256, 0, st>>>(depth0, static_cast<long long>(H) * W, s->dmin);
   pnp_prepare_kernel<<<P, 1024, 0, st>>>(kpts0, kpts1, offsets, K0, depth0, H, W, s->dmin, s->max_pts, s->Xw,
                                          s->uv, s->vidx, s->nvalid);
-  pnp_hyp_kernel<<<dim3(blocks, P), kHypPerBlock, static_cast<size_t>(s->max_pts) * 20, st>>>(
-      s->Xw, s->uv, offsets, s->nvalid, K1, reproj_thr, num_hyp, seed, s->max_pts, s->results);
-  pnp_final_kernel<<<P, 256, 0, st>>>(s->Xw, s->uv, s->vidx, offsets, s->nvalid, K1, reproj_thr, blocks,
-                                      s->max_pts, s->results, R, t, n_inl, mask);
-  MFR_CUDA_CHECK(cudaGetLastError());
-  return MFR_OK;
+  auto round = [&](int num_hyp, const int* active) {
+    const int blocks = (num_hyp + kHypPerBlock - 1) / kHypPerBlock;
+    pnp_hyp_kernel<<<dim3(blocks, P), kHypPerBlock, static_cast<size_t>(s->max_pts) * 20, st>>>(
+        s->Xw, s->uv, offsets, s->nvalid, K1, reproj_thr, num_hyp, seed, s->max_pts, s->results, active);
+    pnp_final_kernel<<<P, 256, 0, st>>>(s->Xw, s->uv, s->vidx, offsets, s->nvalid, K1, reproj_thr, blocks,
+                                        s->max_pts, s->results, R, t, n_inl, mask, active);
+  };
+  return run_rounds(s, b, offsets, P, n_inl, 4, st, round);
+}
+
+int pnp_ransac(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
+               const float* K0, const float* K1, const float* depth0, int H, int W, int num_hyp,
+               float reproj_thr, unsigned long long seed, float* R, float* t, int* n_inl,
+               unsigned char* mask, cudaStream_t st) {
+  if (num_hyp < 1) return MFR_ERR_ARG;
+  return pnp_solve(s, kpts0, kpts1, offsets, P, K0, K1, depth0, H, W, fixed_budget(s, num_hyp), reproj_thr, seed, R, t,
+                   n_inl, mask, st);
+}
+
+int pnp_ransac_escalate(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
+                        const float* K0, const float* K1, const float* depth0, int H, int W, int num_hyp,
+                        float reproj_thr, unsigned long long seed, float* R, float* t, int* n_inl,
+                        unsigned char* mask, double confidence, int max_hyp, int* budgets_out, cudaStream_t st) {
+  BudgetSeq b;
+  const int rc = escalation_budgets(s, num_hyp, confidence, max_hyp, budgets_out, &b);
+  if (rc != MFR_OK) return rc;
+  return pnp_solve(s, kpts0, kpts1, offsets, P, K0, K1, depth0, H, W, b, reproj_thr, seed, R, t, n_inl, mask, st);
 }
 
 int procrustes_ransac(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,

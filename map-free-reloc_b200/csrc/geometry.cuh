@@ -16,6 +16,12 @@ int pose_solver_debug_tensor(PoseSolver* s, const char* name, void** ptr, long l
 int emat_ransac(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
                 const float* K0, const float* K1, float pix_thr, int num_hyp, unsigned long long seed,
                 int lo_enabled, float* R, float* t, int* n_inl, unsigned char* mask, cudaStream_t st);
+// the same solve repeated at h0, min(max_hyp, 4 h0), ... for the pairs whose CONFIDENCE stopping rule asks for more
+// (mfr_emat_ransac_escalate); budgets_out: device int[P] or nullptr
+int emat_ransac_escalate(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
+                         const float* K0, const float* K1, float pix_thr, int num_hyp, unsigned long long seed,
+                         int lo_enabled, float* R, float* t, int* n_inl, unsigned char* mask, double confidence,
+                         int max_hyp, int* budgets_out, cudaStream_t st);
 int scale_from_depth(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
                      const float* K0, const float* K1, const unsigned char* mask, const double* Rd,
                      const double* td, const float* depth0, const float* depth1, int H, int W,
@@ -24,6 +30,10 @@ int pnp_ransac(PoseSolver* s, const float* kpts0, const float* kpts1, const int*
                const float* K0, const float* K1, const float* depth0, int H, int W, int num_hyp,
                float reproj_thr, unsigned long long seed, float* R, float* t, int* n_inl,
                unsigned char* mask, cudaStream_t st);
+int pnp_ransac_escalate(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
+                        const float* K0, const float* K1, const float* depth0, int H, int W, int num_hyp,
+                        float reproj_thr, unsigned long long seed, float* R, float* t, int* n_inl,
+                        unsigned char* mask, double confidence, int max_hyp, int* budgets_out, cudaStream_t st);
 
 int procrustes_ransac(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
                       const float* K0, const float* K1, const float* depth0, const float* depth1, int H, int W,

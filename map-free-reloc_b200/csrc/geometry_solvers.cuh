@@ -530,5 +530,27 @@ MFR_HD double sampson_sq(const double* E, double x0, double y0, double x1, doubl
   return num * num / den;
 }
 
+// ------------------------------------------------------------------------------------------------
+// RANSAC stopping rule of the solver plugins (pose_solver.required_hypotheses and _SolverBase._satisfied), branch for
+// branch in fp64: the number of minimal samples after which an all-inlier sample has been drawn with probability
+// `confidence`, given the inlier ratio found, capped at 2^31 - 1.
+// ------------------------------------------------------------------------------------------------
+MFR_HD long long ransac_required_hypotheses(double confidence, double inlier_ratio, int sample_size) {
+  const double w = pow(fmin(fmax(inlier_ratio, 0.0), 1.0), static_cast<double>(sample_size));
+  if (w >= 1.0 - 1e-12) return 1;
+  const double c = fmin(fmax(confidence, 0.0), 1.0 - 1e-12);
+  if (w < 1e-15) return 2147483647LL;   // no consensus at all: no finite budget reaches the confidence
+  const double k = w < 1e-8 ? log(1.0 - c) / -w : log(1.0 - c) / log1p(-w);
+  return static_cast<long long>(fmin(2147483647.0, ceil(k)));
+}
+
+// Whether a solve at `budget` hypotheses that found n_inliers of n_points stops the escalation. Nothing found
+// (n <= 0) stops it only at the cap `max_budget` (the NaN pose stands then).
+MFR_HD bool ransac_satisfied(double confidence, int n_inliers, int n_points, int budget, int max_budget,
+                             int sample_size) {
+  if (n_points <= 0 || n_inliers <= 0) return n_points <= 0 || budget >= max_budget;
+  return budget >= ransac_required_hypotheses(confidence, static_cast<double>(n_inliers) / n_points, sample_size);
+}
+
 }  // namespace geo
 }  // namespace mfr

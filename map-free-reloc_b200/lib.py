@@ -116,6 +116,10 @@ SIGNATURES = {
                                      c_vp, c_vp, c_int, c_int, c_float, c_vp, c_vp, c_vp, c_vp]),
     "mfr_pnp_ransac": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_int,
                                c_float, ctypes.c_ulonglong, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "mfr_emat_ransac_escalate": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_float, c_int, ctypes.c_ulonglong,
+                                         c_int, c_vp, c_vp, c_vp, c_vp, ctypes.c_double, c_int, c_vp, c_vp]),
+    "mfr_pnp_ransac_escalate": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_float,
+                                        ctypes.c_ulonglong, c_vp, c_vp, c_vp, c_vp, ctypes.c_double, c_int, c_vp, c_vp]),
     "mfr_linear_attention": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
     "mfr_superglue_attention": (c_int, [c_vp, c_ll, c_vp, c_int, c_int, c_int, c_vp, c_ll, c_vp]),
     "mfr_stem_conv7x7": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
@@ -133,6 +137,7 @@ SIGNATURES = {
     "mfr_host_p3p": (c_int, [c_vp, c_vp, c_vp, c_vp]),
     "mfr_host_poly_real_roots": (c_int, [c_vp, c_int, c_vp]),
     "mfr_host_decompose_essential": (c_int, [c_vp, c_vp, c_vp, c_vp]),
+    "mfr_host_ransac_satisfied": (c_int, [ctypes.c_double, c_int, c_int, c_int, c_int, c_int]),
 }
 
 

@@ -36,37 +36,46 @@ from . import pose_solver as _ps
 
 # ------------------------------------------------------------------------------------------------ pose stages
 # Each runs on the solver stream: (be, kpts0, kpts1, offsets, K0, K1, depth0, depth1) -> R [B,3,3], t [B,3], inliers [B].
-# The stream runs one fixed hypothesis budget per batch: the CONFIDENCE escalation of the single-pair plugins
-# (pose_solver._SolverBase) needs the inlier ratio on the host, a round trip the stream does not make.
+# By default a stage runs one fixed hypothesis budget per batch. With ``confidence`` (EMAT_RANSAC.CONFIDENCE /
+# PNP.CONFIDENCE) and ``max_hyp`` (GPU_RANSAC.MAX_HYPOTHESES) the E-mat and PnP stages escalate each pair's budget as
+# the single-pair plugins (pose_solver._SolverBase) do, x4 per round up to max_hyp, decided per pair on the device
+# with no host round trip; each pair's result is then that of the fixed-budget call at the budget where it stopped.
 class EMatMetricStage:
     """EssentialMatrixMetricSolver: E-mat RANSAC, then the metric scale from depth at its inliers."""
 
-    def __init__(self, pix_thr, scale_thr, num_hyp=_ps.DEFAULT_NUM_HYP, seed=_ps.DEFAULT_SEED, lo=True):
+    def __init__(self, pix_thr, scale_thr, num_hyp=_ps.DEFAULT_NUM_HYP, seed=_ps.DEFAULT_SEED, lo=True, confidence=None,
+                 max_hyp=None):
         self.pix_thr, self.scale_thr, self.num_hyp, self.seed, self.lo = float(pix_thr), float(scale_thr), int(num_hyp), seed, lo
+        self.confidence, self.max_hyp = confidence, max_hyp
 
     def __call__(self, be, k0, k1, off, K0, K1, d0, d1):
-        return be.emat_metric(k0, k1, off, K0, K1, d0, d1, self.pix_thr, self.scale_thr, self.num_hyp, self.seed, self.lo)
+        return be.emat_metric(k0, k1, off, K0, K1, d0, d1, self.pix_thr, self.scale_thr, self.num_hyp, self.seed, self.lo,
+                              confidence=self.confidence, max_hyp=self.max_hyp)
 
 
 class EMatStage:
     """EssentialMatrixSolver: the pose up to scale, t of unit norm."""
 
-    def __init__(self, pix_thr, num_hyp=_ps.DEFAULT_NUM_HYP, seed=_ps.DEFAULT_SEED, lo=True):
+    def __init__(self, pix_thr, num_hyp=_ps.DEFAULT_NUM_HYP, seed=_ps.DEFAULT_SEED, lo=True, confidence=None, max_hyp=None):
         self.pix_thr, self.num_hyp, self.seed, self.lo = float(pix_thr), int(num_hyp), seed, lo
+        self.confidence, self.max_hyp = confidence, max_hyp
 
     def __call__(self, be, k0, k1, off, K0, K1, d0, d1):
-        R, t, n, _ = be.emat(k0, k1, off, K0, K1, self.pix_thr, self.num_hyp, self.seed, self.lo)
+        R, t, n, _ = be.emat(k0, k1, off, K0, K1, self.pix_thr, self.num_hyp, self.seed, self.lo,
+                             confidence=self.confidence, max_hyp=self.max_hyp)
         return R, t, n
 
 
 class PnPStage:
     """PnPSolver: 2D-3D RANSAC with the map frame's depth (depth1 is not read)."""
 
-    def __init__(self, reproj_thr, num_hyp=_ps.DEFAULT_NUM_HYP, seed=_ps.DEFAULT_SEED):
+    def __init__(self, reproj_thr, num_hyp=_ps.DEFAULT_NUM_HYP, seed=_ps.DEFAULT_SEED, confidence=None, max_hyp=None):
         self.reproj_thr, self.num_hyp, self.seed = float(reproj_thr), int(num_hyp), seed
+        self.confidence, self.max_hyp = confidence, max_hyp
 
     def __call__(self, be, k0, k1, off, K0, K1, d0, d1):
-        R, t, n, _ = be.pnp(k0, k1, off, K0, K1, d0, self.reproj_thr, self.num_hyp, self.seed)
+        R, t, n, _ = be.pnp(k0, k1, off, K0, K1, d0, self.reproj_thr, self.num_hyp, self.seed,
+                            confidence=self.confidence, max_hyp=self.max_hyp)
         return R, t, n
 
 
@@ -297,7 +306,7 @@ SIFT_NUM_FEATURES, SIFT_RATIO = 2048, 0.8                                     # 
 @dataclasses.dataclass(frozen=True)
 class MethodSpec:
     """What one Map-free method config asks of the stream: the matcher, the solver with its thresholds, the RANSAC
-    settings (first budget only) and the engine frame."""
+    settings and the engine frame."""
     matcher: str                    # "LoFTR" | "SG" | "SIFT"
     solver: str                     # "EssentialMatrix" | "EssentialMatrixMetric" | "PNP" | "Procrustes"
     height: int                     # engine frame: DATASET.HEIGHT / WIDTH, for LoFTR padded by loftr.engine_frame
@@ -312,15 +321,19 @@ class MethodSpec:
     refine: bool = False            # PROCRUSTES.REFINE
     sift_features: int = None       # SIFT.NUM_FEATURES
     sift_ratio: float = None        # SIFT.RATIO_THRESHOLD
+    confidence: float = None        # EMAT_RANSAC.CONFIDENCE / PNP.CONFIDENCE (None: Procrustes, or the key unset)
+    max_hyp: int = None             # GPU_RANSAC.MAX_HYPOTHESES, at least num_hyp: the escalation's cap
 
-    def stage(self):
-        """The pose stage of this method."""
+    def stage(self, escalate=False):
+        """The pose stage of this method: the first hypothesis budget only, or with ``escalate`` the CONFIDENCE
+        escalation up to max_hyp (E-mat and PnP; the Procrustes plugin does not escalate)."""
+        esc = {"confidence": self.confidence, "max_hyp": self.max_hyp} if escalate else {}
         if self.solver == "EssentialMatrixMetric":
-            return EMatMetricStage(self.pix_thr, self.scale_thr, self.num_hyp, self.seed, self.lo)
+            return EMatMetricStage(self.pix_thr, self.scale_thr, self.num_hyp, self.seed, self.lo, **esc)
         if self.solver == "EssentialMatrix":
-            return EMatStage(self.pix_thr, self.num_hyp, self.seed, self.lo)
+            return EMatStage(self.pix_thr, self.num_hyp, self.seed, self.lo, **esc)
         if self.solver == "PNP":
-            return PnPStage(self.reproj_thr, self.num_hyp, self.seed)
+            return PnPStage(self.reproj_thr, self.num_hyp, self.seed, **esc)
         return ProcrustesStage(self.max_corr_dist, self.num_hyp, self.seed, self.refine)
 
 
@@ -341,14 +354,14 @@ def _matcher_name(cfg):
 def resolve_method(cfg):
     """Reference method config (a config.CfgNode or nested dict, e.g. config/mapfree.yaml + a
     config/matching/mapfree/*.yaml) -> MethodSpec. Unknown matchers or solvers raise NotImplementedError as the
-    reference's FeatureMatchingModel does. Budget, seed and LO flags follow the single-pair plugins (pose_solver), with
-    their first hypothesis budget: the stream does not escalate on CONFIDENCE."""
+    reference's FeatureMatchingModel does. Budget, escalation cap, confidence, seed and LO flags follow the single-pair
+    plugins (pose_solver); the stage escalates on the confidence only when asked to (``MethodSpec.stage``)."""
     g = lambda k, d=None: _ps._cfg_get(cfg, k, d)
     matcher = _matcher_name(cfg)
     solver = g("POSE_SOLVER")
     if solver not in SOLVERS:
         raise NotImplementedError(f"Invalid pose solver {solver!r}")
-    num_hyp, _, seed, lo = _ps.ransac_settings(cfg, _ps.pnp_default_hyp(cfg) if solver == "PNP" else _ps.DEFAULT_NUM_HYP)
+    num_hyp, max_hyp, seed, lo = _ps.ransac_settings(cfg, _ps.pnp_default_hyp(cfg) if solver == "PNP" else _ps.DEFAULT_NUM_HYP)
     h, w = int(g("DATASET.HEIGHT", 720)), int(g("DATASET.WIDTH", 540))   # Map-free's frame (config/mapfree.yaml)
     if matcher == "LoFTR":
         h, w = loftr.engine_frame(h, w)
@@ -356,25 +369,31 @@ def resolve_method(cfg):
     kw = {}
     if solver.startswith("EssentialMatrix"):
         kw["pix_thr"] = f("EMAT_RANSAC.PIX_THRESHOLD")
+        kw["confidence"] = f("EMAT_RANSAC.CONFIDENCE")
         if solver == "EssentialMatrixMetric":
             kw["scale_thr"] = f("EMAT_RANSAC.SCALE_THRESHOLD")
     elif solver == "PNP":
         kw["reproj_thr"] = f("PNP.REPROJECTION_INLIER_THRESHOLD")
+        kw["confidence"] = f("PNP.CONFIDENCE")
     else:
         kw["max_corr_dist"] = f("PROCRUSTES.MAX_CORR_DIST")
         kw["refine"] = bool(g("PROCRUSTES.REFINE", False))
     if matcher == "SIFT":
         kw["sift_features"] = int(g("SIFT.NUM_FEATURES", SIFT_NUM_FEATURES))
         kw["sift_ratio"] = float(g("SIFT.RATIO_THRESHOLD", SIFT_RATIO))
-    return MethodSpec(matcher=matcher, solver=solver, height=h, width=w, num_hyp=num_hyp, seed=seed, lo=lo, **kw)
+    return MethodSpec(matcher=matcher, solver=solver, height=h, width=w, num_hyp=num_hyp, seed=seed, lo=lo,
+                      max_hyp=max_hyp, **kw)
 
 
-def from_cfg(cfg, batch, weights=None, precision="tf32", depth_hw=None, outdoor=False, device=0, graph=True):
+def from_cfg(cfg, batch, weights=None, precision="tf32", depth_hw=None, outdoor=False, device=0, graph=True,
+             escalate=False):
     """Engine + PoseBackend + RelocPipeline for the method of ``cfg`` (see resolve_method), ``batch`` pairs per engine
     call. ``weights``: LoFTR, what loftr.load_weights takes (a state dict, a {'state_dict': ...} checkpoint or a path to
     either); SG, what spsg.load_weights takes (a (superpoint, superglue) pair of state dicts or the directory holding
     superpoint_v1.pth and superglue_{indoor,outdoor}.pth, indoor unless ``outdoor``); SIFT, none.
-    ``precision`` applies to LoFTR and SG. The method is at ``pipeline.method``."""
+    ``precision`` applies to LoFTR and SG. ``escalate``: the E-mat / PnP stage escalates on the config's CONFIDENCE up
+    to GPU_RANSAC.MAX_HYPOTHESES, as the single-pair plugins do (default: the first budget only). The method is at
+    ``pipeline.method``."""
     spec = resolve_method(cfg)
     if spec.matcher == "LoFTR":
         if weights is None:
@@ -391,7 +410,7 @@ def from_cfg(cfg, batch, weights=None, precision="tf32", depth_hw=None, outdoor=
         eng = sift.SIFTPairs(batch, spec.height, spec.width, nfeatures=spec.sift_features, ratio=spec.sift_ratio,
                              root_sift=True, device=device, graph=graph)
     be = _ps.PoseBackend(max_pairs=batch, max_pts=max(8, min(eng.max_pts_per_pair, _ps.MAX_PTS_LIMIT)),
-                         max_hyp=max(spec.num_hyp, 128), device=device)
-    pipe = RelocPipeline(eng, be, depth_hw=depth_hw, solver=spec.stage())
+                         max_hyp=max(spec.max_hyp if escalate else spec.num_hyp, 128), device=device)
+    pipe = RelocPipeline(eng, be, depth_hw=depth_hw, solver=spec.stage(escalate))
     pipe.method = spec
     return pipe

@@ -55,18 +55,34 @@ class PoseBackend(_lib.Engine):
         assert K1.is_cuda and K1.dtype == torch.float32 and K1.is_contiguous()
         return offsets.numel() - 1
 
+    def _escalation(self, P, num_hyp, max_hyp, budgets):
+        """(cap, budgets pointer) of an escalating call: the cap defaults to the handle's max_hyp."""
+        cap = self.max_hyp if max_hyp is None else int(max_hyp)
+        if cap < int(num_hyp):
+            raise ValueError(f"max_hyp {cap} is below the first budget {num_hyp}")
+        if budgets is not None:
+            assert budgets.is_cuda and budgets.dtype == torch.int32 and budgets.is_contiguous() and budgets.numel() >= P
+        return cap, _lib.ptr(budgets)
+
     def emat(self, kpts0, kpts1, offsets, K0, K1, pix_thr, num_hyp=DEFAULT_NUM_HYP, seed=DEFAULT_SEED,
-             lo=True, total=None):
+             lo=True, total=None, confidence=None, max_hyp=None, budgets=None):
         """EssentialMatrixSolver for P pairs. Returns R [P,3,3], t [P,3] (unit), n [P], mask [total].
         lo: False / 0 = raw RANSAC winner; True / 1 = local optimisation (LO_TUKEY); 3 = LO + the final truncated
-        least-squares refit on the model's own inlier set (LO_LSQ, the reference-equivalent optimum)."""
+        least-squares refit on the model's own inlier set (LO_LSQ, the reference-equivalent optimum).
+        confidence: None = one solve at num_hyp; else EMAT_RANSAC.CONFIDENCE, escalated per pair on the device as the
+        plugins do (x4 per round up to max_hyp, default the handle's max_hyp; mfr_emat_ransac_escalate). budgets: optional
+        int32 [P] CUDA tensor that receives the budget each pair's result comes from (0: fewer than 5 correspondences)."""
         P = self._prep(kpts0, kpts1, offsets, K0, K1)
         total = kpts0.shape[0] if total is None else total
         R, t, n, mask = self._outs(P, total)
-        _lib.check(self._l.mfr_emat_ransac(self._h, _lib.ptr(kpts0), _lib.ptr(kpts1), _lib.ptr(offsets), P,
-                                           _lib.ptr(K0), _lib.ptr(K1), float(pix_thr), int(num_hyp),
-                                           ctypes.c_ulonglong(seed), int(lo), _lib.ptr(R), _lib.ptr(t),
-                                           _lib.ptr(n), _lib.ptr(mask), _lib.cur_stream()), "mfr_emat_ransac")
+        args = (self._h, _lib.ptr(kpts0), _lib.ptr(kpts1), _lib.ptr(offsets), P, _lib.ptr(K0), _lib.ptr(K1), float(pix_thr),
+                int(num_hyp), ctypes.c_ulonglong(seed), int(lo), _lib.ptr(R), _lib.ptr(t), _lib.ptr(n), _lib.ptr(mask))
+        if confidence is None:
+            _lib.check(self._l.mfr_emat_ransac(*args, _lib.cur_stream()), "mfr_emat_ransac")
+        else:
+            cap, b = self._escalation(P, num_hyp, max_hyp, budgets)
+            _lib.check(self._l.mfr_emat_ransac_escalate(*args, float(confidence), cap, b, _lib.cur_stream()),
+                       "mfr_emat_ransac_escalate")
         return R, t, n, mask
 
     def scale(self, kpts0, kpts1, offsets, K0, K1, mask, depth0, depth1, scale_thr, Rd=None, td=None):
@@ -85,22 +101,31 @@ class PoseBackend(_lib.Engine):
         return R, t, n
 
     def emat_metric(self, kpts0, kpts1, offsets, K0, K1, depth0, depth1, pix_thr, scale_thr,
-                    num_hyp=DEFAULT_NUM_HYP, seed=DEFAULT_SEED, lo=True):
-        """EssentialMatrixMetricSolver for P pairs: R [P,3,3], t [P,3] metres, inliers [P]."""
-        _, _, _, mask = self.emat(kpts0, kpts1, offsets, K0, K1, pix_thr, num_hyp, seed, lo)
+                    num_hyp=DEFAULT_NUM_HYP, seed=DEFAULT_SEED, lo=True, confidence=None, max_hyp=None, budgets=None):
+        """EssentialMatrixMetricSolver for P pairs: R [P,3,3], t [P,3] metres, inliers [P]. confidence / max_hyp /
+        budgets: the E-mat escalation of ``emat`` (driven by the E-mat inlier count); the scale runs once, on the
+        final pose."""
+        _, _, _, mask = self.emat(kpts0, kpts1, offsets, K0, K1, pix_thr, num_hyp, seed, lo, confidence=confidence,
+                                  max_hyp=max_hyp, budgets=budgets)
         return self.scale(kpts0, kpts1, offsets, K0, K1, mask, depth0, depth1, scale_thr)
 
     def pnp(self, kpts0, kpts1, offsets, K0, K1, depth0, reproj_thr, num_hyp=DEFAULT_NUM_HYP,
-            seed=DEFAULT_SEED):
-        """PnPSolver for P pairs: R [P,3,3], t [P,3], inliers [P], mask [total]."""
+            seed=DEFAULT_SEED, confidence=None, max_hyp=None, budgets=None):
+        """PnPSolver for P pairs: R [P,3,3], t [P,3], inliers [P], mask [total]. confidence / max_hyp / budgets: the
+        PNP.CONFIDENCE escalation, as in ``emat`` (budget 0: fewer than 4 correspondences)."""
         P = self._prep(kpts0, kpts1, offsets, K0, K1)
         H, W = depth0.shape[-2:]
         R, t, n, mask = self._outs(P, kpts0.shape[0])
-        _lib.check(self._l.mfr_pnp_ransac(self._h, _lib.ptr(kpts0), _lib.ptr(kpts1), _lib.ptr(offsets), P,
-                                          _lib.ptr(K0), _lib.ptr(K1), _lib.ptr(depth0.contiguous()), int(H),
-                                          int(W), int(num_hyp), float(reproj_thr), ctypes.c_ulonglong(seed),
-                                          _lib.ptr(R), _lib.ptr(t), _lib.ptr(n), _lib.ptr(mask),
-                                          _lib.cur_stream()), "mfr_pnp_ransac")
+        depth0 = depth0.contiguous()
+        args = (self._h, _lib.ptr(kpts0), _lib.ptr(kpts1), _lib.ptr(offsets), P, _lib.ptr(K0), _lib.ptr(K1),
+                _lib.ptr(depth0), int(H), int(W), int(num_hyp), float(reproj_thr), ctypes.c_ulonglong(seed),
+                _lib.ptr(R), _lib.ptr(t), _lib.ptr(n), _lib.ptr(mask))
+        if confidence is None:
+            _lib.check(self._l.mfr_pnp_ransac(*args, _lib.cur_stream()), "mfr_pnp_ransac")
+        else:
+            cap, b = self._escalation(P, num_hyp, max_hyp, budgets)
+            _lib.check(self._l.mfr_pnp_ransac_escalate(*args, float(confidence), cap, b, _lib.cur_stream()),
+                       "mfr_pnp_ransac_escalate")
         return R, t, n, mask
 
     def procrustes(self, kpts0, kpts1, offsets, K0, K1, depth0, depth1, max_corr_dist,

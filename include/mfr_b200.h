@@ -377,6 +377,26 @@ int mfr_pnp_ransac_escalate(mfr_pose_solver* s, const float* kpts0, const float*
                             int* n_inliers, unsigned char* mask, double confidence, int max_hyp, int* budgets_out,
                             void* stream);
 
+/* mfr_emat_ransac_escalate with the estimator of the reference's cv.USAC_MAGSAC: MAGSAC++ (Barath et al., CVPR 2020)
+ * in place of MSAC and its LO. Same arguments without lo_enabled.
+ *   loss     rho of the Sampson distance r (normalised coordinates) for nu = 4 degrees of freedom, sigma_max = the
+ *            normalised threshold pix_threshold / mean(K0.fx, K1.fy, K0.fy, K1.fx), cut-off k sigma_max with k = 3.64
+ *            (mfr_host_magsac_loss evaluates it).
+ *   scoring  each 5-point hypothesis scores sum rho (fp32 per point); the inlier count at the threshold is unchanged.
+ *   LO       sigma-consensus++ (IRLS / LM on sum rho in fp64, MAGSAC++ weights) from each of the 4 cheapest block
+ *            winners, at most 10 passes over a strided subsample of <= 1024 correspondences; the candidate with the
+ *            lowest sum rho over all correspondences is polished the same way on all of them, at most 30 passes.
+ *            Both stop once sum rho drops by <= 1e-10 (relative). No noise-adaptive tightening, no least-squares refit.
+ *   outputs  as mfr_emat_ransac: mask = Sampson^2 < threshold^2 under the final E, filtered by recoverPose's
+ *            cheirality vote; the fp64 pose is kept for mfr_scale_from_depth. "hyp_results" / "lo_results" hold sum rho
+ *            as their costs.
+ * confidence <= 0: one round at num_hyp (max_hyp must still be >= num_hyp); otherwise the escalation contract of
+ * mfr_emat_ransac_escalate, with the same budget sequence, rule and bit-for-bit result. Capturable in a CUDA graph. */
+int mfr_emat_magsac(mfr_pose_solver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
+                    const float* K0, const float* K1, float pix_threshold, int num_hyp, unsigned long long seed,
+                    float* R, float* t, int* n_inliers, unsigned char* mask, double confidence, int max_hyp,
+                    int* budgets_out, void* stream);
+
 /* ProcrustesSolver.estimate_pose with REFINE = False (pose_solver.py:247-320): lift both keypoint sets
  * through their depth maps (valid iff depth > depth.min() on both sides), RANSAC over 3-point Kabsch
  * alignments with inlier distance max_corr_dist (metres), refit on the inliers. The reference calls
@@ -394,13 +414,16 @@ int mfr_procrustes_ransac(mfr_pose_solver* s, const float* kpts0, const float* k
  *   p3p        : X double[3][3] points, f double[3][3] unit bearings, R_out [4][9], t_out [4][3]
  *   poly roots : coef[0..deg] ascending, deg <= 10; returns #real roots (ascending)
  *   ransac_satisfied : 1 iff the escalation stops after a round at `budget` that found n_inliers of n_points
- *                (the rule of mfr_emat_ransac_escalate, cap max_budget, minimal sample sample_size), else 0    */
+ *                (the rule of mfr_emat_ransac_escalate, cap max_budget, minimal sample sample_size), else 0
+ *   magsac_loss : MAGSAC++ rho(r) and w(r) = rho'(r) / r of mfr_emat_magsac (the fp64 version of its LO / polish) for
+ *                a Sampson distance r and sigma_max > 0 (else MFR_ERR_ARG)                                      */
 int mfr_host_five_point(const double* x0, const double* x1, double* E_out);
 int mfr_host_p3p(const double* X, const double* f, double* R_out, double* t_out);
 int mfr_host_poly_real_roots(const double* coef, int deg, double* roots);
 int mfr_host_decompose_essential(const double* E, double* R1, double* R2, double* t);
 int mfr_host_ransac_satisfied(double confidence, int n_inliers, int n_points, int budget, int max_budget,
                               int sample_size);
+int mfr_host_magsac_loss(double r, double sigma_max, double* rho, double* w);
 
 /* Debug probe (microbenchmark used by scripts/, not part of the product path): microseconds per
  * launch of a prebuilt conv/GEMM op launched back to back.

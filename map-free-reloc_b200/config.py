@@ -6,7 +6,7 @@ pre-declared keys may be set. The reference's yaml files load unchanged.
 
 Additive keys (not in the reference): FEATURE_MATCHING may also be 'LoFTR' (fused on-GPU matcher),
 LOFTR.{WEIGHTS, THR, BORDER_RM, TEMPERATURE, BATCH}, GPU_RANSAC.{NUM_HYPOTHESES, MAX_HYPOTHESES, SEED,
-LOCAL_OPTIMISATION, FINAL_REFIT}, SIFT.GPU_DETECTOR (False: OpenCV's host SIFT as in the reference; True: the CUDA
+LOCAL_OPTIMISATION, FINAL_REFIT, SCORING}, SIFT.GPU_DETECTOR (False: OpenCV's host SIFT as in the reference; True: the CUDA
 SIFT engine detects, describes and ratio-matches on the device).
 """
 import copy
@@ -85,8 +85,11 @@ def get_default_cfg():
         # NUM_HYPOTHESES None = the solver's default (E-mat 2048; PnP: PNP.RANSAC_ITER rounded up to 128);
         # MAX_HYPOTHESES bounds the CONFIDENCE-driven escalation of the solver plugins (pose_solver._SolverBase) and of
         # the stream when it is asked to escalate (pipeline.from_cfg(..., escalate=True), decided per pair on the device)
+        # SCORING: objective of the E-mat RANSAC, 'msac' (MSAC + Tukey LO, as LOCAL_OPTIMISATION / FINAL_REFIT say) or
+        # 'magsac' (MAGSAC++ scoring with sigma-consensus++, the estimator of the reference's USAC_MAGSAC; LO keys at
+        # their defaults)
         "GPU_RANSAC": {"NUM_HYPOTHESES": None, "MAX_HYPOTHESES": 32768, "SEED": 0x5EED, "LOCAL_OPTIMISATION": True,
-                       "FINAL_REFIT": "lsq"},
+                       "FINAL_REFIT": "lsq", "SCORING": "msac"},
     })
 
 

@@ -342,6 +342,14 @@ int mfr_emat_ransac_escalate(mfr_pose_solver* s, const float* kpts0, const float
   return mfr::emat_ransac_escalate(s->s, kpts0, kpts1, offsets, P, K0, K1, pix_threshold, num_hyp, seed, lo_enabled, R,
                                    t, n_inliers, mask, confidence, max_hyp, budgets_out, static_cast<cudaStream_t>(stream));
 }
+int mfr_emat_magsac(mfr_pose_solver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
+                    const float* K0, const float* K1, float pix_threshold, int num_hyp, unsigned long long seed, float* R,
+                    float* t, int* n_inliers, unsigned char* mask, double confidence, int max_hyp, int* budgets_out,
+                    void* stream) {
+  if (!s) return MFR_ERR_ARG;
+  return mfr::emat_magsac(s->s, kpts0, kpts1, offsets, P, K0, K1, pix_threshold, num_hyp, seed, R, t, n_inliers, mask,
+                          confidence, max_hyp, budgets_out, static_cast<cudaStream_t>(stream));
+}
 int mfr_pnp_ransac_escalate(mfr_pose_solver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
                             const float* K0, const float* K1, const float* depth0, int H, int W, int num_hyp,
                             float reproj_threshold, unsigned long long seed, float* R, float* t, int* n_inliers,
@@ -378,6 +386,11 @@ int mfr_host_decompose_essential(const double* E, double* R1, double* R2, double
 }
 int mfr_host_ransac_satisfied(double confidence, int n_inliers, int n_points, int budget, int max_budget, int sample_size) {
   return mfr::geo::ransac_satisfied(confidence, n_inliers, n_points, budget, max_budget, sample_size) ? 1 : 0;
+}
+int mfr_host_magsac_loss(double r, double sigma_max, double* rho, double* w) {
+  if (!(sigma_max > 0.0) || !rho || !w) return MFR_ERR_ARG;
+  mfr::geo::magsac_loss_sq(r * r, sigma_max, rho, w);
+  return MFR_OK;
 }
 
 // ------------------------------------------------------------------------------------------ debug probes

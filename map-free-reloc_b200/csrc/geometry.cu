@@ -25,8 +25,15 @@ using namespace geo;
 
 constexpr int kHypPerBlock = 128;  // 4 warps x 32 lanes
 
+// Scoring rule of the E-mat RANSAC, a compile-time policy of its three kernels:
+//   kMsac   sum min(d^2, thr^2) ranks the hypotheses; LO = LM on a Tukey M-estimator + noise-adaptive tightening (+ the
+//           truncated least-squares refit), as lo_enabled asks (mfr_emat_ransac)
+//   kMagsac sum rho, the MAGSAC++ loss with sigma_max = thr (geometry_solvers.cuh), ranks the hypotheses; LO and the
+//           final polish are sigma-consensus++, i.e. IRLS / LM on sum rho (mfr_emat_magsac)
+enum class Scoring { kMsac, kMagsac };
+
 struct HypResult {   // best hypothesis of one block
-  double cost;       // MSAC cost (emat) or -inlier count (pnp): lower is better
+  double cost;       // MSAC cost or sum of MAGSAC++ rho (emat), -inlier count (pnp): lower is better
   int count;
   int valid;
   double model[12];  // E[9] or R[9] t[3]
@@ -136,6 +143,7 @@ __global__ void __launch_bounds__(256) emat_normalise_kernel(const float* __rest
 // memory and all but ~21 K of its registers. It therefore keeps out of shared memory (the points come through L1 / L2,
 // 32 bytes of block-reduction scratch) and under 160 registers, so that one of its blocks fits NEXT to a GEMM CTA
 // instead of making that CTA (and, with static tile assignment, the whole GEMM kernel) wait for it.
+template <Scoring kScore>
 __global__ void __maxnreg__(160) emat_hyp_kernel(   // launched with <= kHypPerBlock threads
     const float4* __restrict__ pts_all, const int* __restrict__ offsets,
     const float* __restrict__ K0s, const float* __restrict__ K1s, float pix_thr, int num_hyp,
@@ -155,6 +163,7 @@ __global__ void __maxnreg__(160) emat_hyp_kernel(   // launched with <= kHypPerB
   const float4* s_pts = pts_all + static_cast<size_t>(pair) * max_pts;
   const float thr = emat_threshold(pix_thr, K0, K1);
   const float thr2 = thr * thr;
+  const float inv2s2 = 0.5f / thr2;   // MAGSAC++: x = d^2 / (2 sigma_max^2); the scores are sums of rho / (C 2^1.5 thr)
 
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int h = blockIdx.x * blockDim.x + threadIdx.x;   // 32..128 hypotheses per block (host picks, to fill the SMs)
@@ -193,11 +202,14 @@ __global__ void __maxnreg__(160) emat_hyp_kernel(   // launched with <= kHypPerB
           if (i < N) {
             d2 = sampson_sq_f(E, __ldg(s_pts + i));
             ok = d2 < thr2;
-            cost += fminf(d2, thr2);
+            if constexpr (kScore == Scoring::kMsac)
+              cost += fminf(d2, thr2);
+            else
+              cost += magsac_rho_unit_f(d2 * inv2s2);
           }
           inl += __popc(__ballot_sync(0xffffffffu, ok));
         }
-        // MSAC cost only grows: give up on this model once it cannot beat the best so far
+        // the cost (MSAC or MAGSAC++: rho >= 0) only grows: give up on this model once it cannot beat the best so far
         const float partial = warp_sum_f(cost);
         if (partial >= best_cost) { dead = true; break; }
       }
@@ -212,6 +224,7 @@ __global__ void __maxnreg__(160) emat_hyp_kernel(   // launched with <= kHypPerB
     }
   }
   // block winner = the warp with the lowest cost (first one on ties); that warp writes the record itself
+  if constexpr (kScore == Scoring::kMagsac) best_cost *= static_cast<float>(kMagsacC2) * thr;   // sum rho
   if (lane == 0) s_cost[warp] = best_src >= 0 ? static_cast<double>(best_cost) : 1e300;
   __syncthreads();
   int bw = 0;
@@ -333,7 +346,7 @@ struct EmatShared {
   int ncand, cnt, done;
 };
 
-// one locally-optimised candidate: MSAC cost at the RANSAC threshold and its pose
+// one locally-optimised candidate: MSAC cost at the RANSAC threshold (MAGSAC++: sum rho, in fp64) and its pose
 struct LoResult {
   double cost, R[9], t[3];
 };
@@ -345,8 +358,13 @@ static_assert(sizeof(LoResult) == 104 && offsetof(LoResult, cost) == 0 && offset
 // starting from (S.R, S.t); leaves the last accepted parameters there. All threads must call it.
 // hard = true: truncated least squares instead (weight 1 inside the cut-off, cost sum min(r^2, T2) / T2 = the MSAC cost):
 // its fixed point is the least-squares optimum of the model's own inlier set.
+// kScore = kMagsac: sigma-consensus++ instead, with sigma_max = sqrt(T2) (hard is ignored): the weights are the MAGSAC++
+// w(r) of the current model, H = sum w J J^T, g = sum w J r (the gradient of sum rho) and the cost is sum rho, so every
+// pass is one IRLS step, damped by LM. It stops after max_it passes or once sum rho drops by <= 1e-10 (relative).
+template <Scoring kScore = Scoring::kMsac>
 __device__ void emat_lm_round(EmatShared& S, const float4* pts, int N, double T2, int step = 1, bool hard = false,
                               int max_it = kLoInner) {
+  const double sigma = kScore == Scoring::kMagsac ? sqrt(T2) : 0.0;
   if (threadIdx.x == 0) { S.lambda = 1e-6; S.prev_cost = 1e300; S.done = 0; }
   __syncthreads();
   for (int it = 0; it <= max_it; ++it) {
@@ -360,6 +378,18 @@ __device__ void emat_lm_round(EmatShared& S, const float4* pts, int N, double T2
     for (int i = threadIdx.x * step; i < N; i += blockDim.x * step) {   // step > 1: every step-th correspondence
       double J[5];
       const double r = sampson_res_jac(R, t, b1, b2, pts[i], J);
+      if constexpr (kScore == Scoring::kMagsac) {
+        double rho, w;
+        magsac_loss_sq(r * r, sigma, &rho, &w);
+        if (w > 0.0) {
+          int qq = 0;
+          for (int a = 0; a < 5; ++a)
+            for (int b = a; b < 5; ++b) acc[qq++] += w * J[a] * J[b];
+          for (int a = 0; a < 5; ++a) acc[15 + a] += w * J[a] * r;
+        }
+        acc[20] += rho;
+        continue;
+      }
       const double q = r * r / T2;
       if (q < 1.0) {
         const double u = 1.0 - q, w = hard ? 1.0 : u * u;
@@ -458,6 +488,25 @@ __device__ double emat_msac(EmatShared& S, const float4* pts, int N, double thr2
   return r;
 }
 
+// sum of the MAGSAC++ rho (sigma_max = sigma) of the model (S.R, S.t); result broadcast to all threads
+__device__ double emat_sum_rho(EmatShared& S, const float4* pts, int N, double sigma) {
+  double E[9];
+  essential_from_rt(S.R, S.t, E);
+  double c[1] = {0.0};
+  for (int i = threadIdx.x; i < N; i += blockDim.x) {
+    const float4 p = pts[i];
+    double rho, w;
+    magsac_loss_sq(sampson_sq(E, p.x, p.y, p.z, p.w), sigma, &rho, &w);
+    c[0] += rho;
+  }
+  block_sum_256<1>(c, S.red);
+  if (threadIdx.x == 0) S.prev_cost = c[0];
+  __syncthreads();
+  const double r = S.prev_cost;
+  __syncthreads();
+  return r;
+}
+
 // Shared prologue of the two kernels below: points of the pair into shared memory, the kLoTopK
 // cheapest block winners (cheapest first) into S.cand. Returns N (0 = nothing to do).
 __device__ int emat_stage_in(EmatShared& S, float4* s_pts, const float* kpts0, const float* kpts1, const int* offsets,
@@ -492,7 +541,11 @@ __device__ int emat_stage_in(EmatShared& S, float4* s_pts, const float* kpts0, c
 constexpr int kLoThreads = 512;    // the LM passes are fp64-latency bound: more warps per pair
 constexpr int kLoMaxPts = 1024;    // correspondences used by the candidate LO rounds (strided subsample beyond that);
                                    // the final tightening rounds and every cost / mask evaluation use all of them
+// MAGSAC++ iteration caps (IRLS / LM passes; each stops earlier once sum rho drops by <= 1e-10 relative): the
+// sigma-consensus++ of each candidate on the LO subsample, then the final polish of the winner on all correspondences
+constexpr int kMagsacLoIters = 10, kMagsacFinalIters = 30;
 
+template <Scoring kScore>
 __global__ void __launch_bounds__(kLoThreads) emat_lo_kernel(
     const float* __restrict__ kpts0, const float* __restrict__ kpts1, const int* __restrict__ offsets,
     const float* __restrict__ K0s, const float* __restrict__ K1s, float pix_thr, int blocks_per_pair,
@@ -517,13 +570,15 @@ __global__ void __launch_bounds__(kLoThreads) emat_lo_kernel(
     for (int k = 0; k < 9; ++k) S.E[k] = res[S.cand[c]].model[k];
   __syncthreads();
   emat_choose_pose(S, s_pts, N, thr2);
-  if (lo_enabled) {
+  if constexpr (kScore == Scoring::kMagsac) {
+    emat_lm_round<Scoring::kMagsac>(S, s_pts, N, thr2, (N + kLoMaxPts - 1) / kLoMaxPts, false, kMagsacLoIters);
+  } else if (lo_enabled) {
     // cut-off shrinking from 3x to 1x the RANSAC threshold
     const double sched[kLoRounds] = {3.0, 2.0, 1.5, 1.0, 1.0, 1.0};
     const int step = (N + kLoMaxPts - 1) / kLoMaxPts;
     for (int r = 0; r < kLoRounds; ++r) emat_lm_round(S, s_pts, N, sched[r] * sched[r] * thr2, step);
   }
-  const double cost = emat_msac(S, s_pts, N, thr2);
+  const double cost = kScore == Scoring::kMagsac ? emat_sum_rho(S, s_pts, N, thr) : emat_msac(S, s_pts, N, thr2);
   if (threadIdx.x == 0) {
     out->cost = cost;
     for (int k = 0; k < 9; ++k) out->R[k] = S.R[k];
@@ -531,6 +586,7 @@ __global__ void __launch_bounds__(kLoThreads) emat_lo_kernel(
   }
 }
 
+template <Scoring kScore>
 __global__ void __launch_bounds__(kLoThreads) emat_final_kernel(
     const float* __restrict__ kpts0, const float* __restrict__ kpts1, const int* __restrict__ offsets,
     const float* __restrict__ K0s, const float* __restrict__ K1s, float pix_thr, int blocks_per_pair,
@@ -574,7 +630,10 @@ __global__ void __launch_bounds__(kLoThreads) emat_final_kernel(
     for (int k = 0; k < 3; ++k) S.t[k] = S.bestt[k];
   }
   __syncthreads();
-  if (lo_enabled) {
+  if constexpr (kScore == Scoring::kMagsac) {
+    // sigma-consensus++ polish on all correspondences; no tightening, no refit
+    emat_lm_round<Scoring::kMagsac>(S, s_pts, N, thr2, 1, false, kMagsacFinalIters);
+  } else if (lo_enabled) {
     // noise-adaptive tightening: robust scale of the inlier residuals (1.4826 * median |r|), cut-off
     // = clamp(3 sigma, ., thr). With clean data this discards chance near-threshold outliers that a
     // fixed cut-off keeps (the sigma-consensus idea of MAGSAC++).
@@ -1541,8 +1600,10 @@ int pose_solver_create(int max_pairs, int max_pts, int max_hyp, PoseSolver** out
   if (!ok) { pose_solver_destroy(s); return MFR_ERR_CUDA; }
   static bool attr_seen[64] = {};
   if (first_call_on_device(attr_seen)) {
-    cudaFuncSetAttribute(emat_final_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16);
-    cudaFuncSetAttribute(emat_lo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16);
+    cudaFuncSetAttribute(emat_final_kernel<Scoring::kMsac>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16);
+    cudaFuncSetAttribute(emat_lo_kernel<Scoring::kMsac>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16);
+    cudaFuncSetAttribute(emat_final_kernel<Scoring::kMagsac>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16);
+    cudaFuncSetAttribute(emat_lo_kernel<Scoring::kMagsac>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16);
     cudaFuncSetAttribute(scale_consensus_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 8);
     cudaFuncSetAttribute(pnp_hyp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 20);
     cudaFuncSetAttribute(procrustes_hyp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 24);
@@ -1638,6 +1699,8 @@ int run_rounds(PoseSolver* s, const BudgetSeq& b, const int* offsets, int P, con
 
 }  // namespace
 
+// kScore = kMagsac runs with lo_enabled = 1 (sigma-consensus++ from every LO candidate)
+template <Scoring kScore>
 static int emat_solve(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P, const float* K0,
                       const float* K1, float pix_thr, const BudgetSeq& b, unsigned long long seed, int lo_enabled,
                       float* R, float* t, int* n_inl, unsigned char* mask, cudaStream_t st) {
@@ -1653,12 +1716,12 @@ static int emat_solve(PoseSolver* s, const float* kpts0, const float* kpts1, con
     int hpb = kHypPerBlock;
     while (hpb > 32 && static_cast<long long>(P) * ((num_hyp + hpb - 1) / hpb) < sm_count() / 2) hpb /= 2;
     const int blocks = (num_hyp + hpb - 1) / hpb;
-    emat_hyp_kernel<<<dim3(blocks, P), hpb, 0, st>>>(static_cast<const float4*>(s->pts_norm), offsets, K0, K1, pix_thr,
+    emat_hyp_kernel<kScore><<<dim3(blocks, P), hpb, 0, st>>>(static_cast<const float4*>(s->pts_norm), offsets, K0, K1, pix_thr,
                                                      num_hyp, seed, s->max_pts, s->results, active);
-    emat_lo_kernel<<<dim3(P, kLoTopK), kLoThreads, smem, st>>>(kpts0, kpts1, offsets, K0, K1, pix_thr, blocks, s->max_pts,
+    emat_lo_kernel<kScore><<<dim3(P, kLoTopK), kLoThreads, smem, st>>>(kpts0, kpts1, offsets, K0, K1, pix_thr, blocks, s->max_pts,
                                                                s->results, static_cast<LoResult*>(s->lo_out), lo_enabled,
                                                                active);
-    emat_final_kernel<<<P, kLoThreads, smem, st>>>(kpts0, kpts1, offsets, K0, K1, pix_thr, blocks, s->max_pts, s->results,
+    emat_final_kernel<kScore><<<P, kLoThreads, smem, st>>>(kpts0, kpts1, offsets, K0, K1, pix_thr, blocks, s->max_pts, s->results,
                                                    static_cast<const LoResult*>(s->lo_out), s->Rd, s->td, R, t, n_inl, mask,
                                                    lo_enabled, active);
   };
@@ -1669,8 +1732,8 @@ int emat_ransac(PoseSolver* s, const float* kpts0, const float* kpts1, const int
                 const float* K0, const float* K1, float pix_thr, int num_hyp, unsigned long long seed,
                 int lo_enabled, float* R, float* t, int* n_inl, unsigned char* mask, cudaStream_t st) {
   if (num_hyp < 1) return MFR_ERR_ARG;
-  return emat_solve(s, kpts0, kpts1, offsets, P, K0, K1, pix_thr, fixed_budget(s, num_hyp), seed, lo_enabled, R, t, n_inl,
-                    mask, st);
+  return emat_solve<Scoring::kMsac>(s, kpts0, kpts1, offsets, P, K0, K1, pix_thr, fixed_budget(s, num_hyp), seed,
+                                    lo_enabled, R, t, n_inl, mask, st);
 }
 
 int emat_ransac_escalate(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
@@ -1680,7 +1743,17 @@ int emat_ransac_escalate(PoseSolver* s, const float* kpts0, const float* kpts1, 
   BudgetSeq b;
   const int rc = escalation_budgets(s, num_hyp, confidence, max_hyp, budgets_out, &b);
   if (rc != MFR_OK) return rc;
-  return emat_solve(s, kpts0, kpts1, offsets, P, K0, K1, pix_thr, b, seed, lo_enabled, R, t, n_inl, mask, st);
+  return emat_solve<Scoring::kMsac>(s, kpts0, kpts1, offsets, P, K0, K1, pix_thr, b, seed, lo_enabled, R, t, n_inl, mask,
+                                    st);
+}
+
+int emat_magsac(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P, const float* K0,
+                const float* K1, float pix_thr, int num_hyp, unsigned long long seed, float* R, float* t, int* n_inl,
+                unsigned char* mask, double confidence, int max_hyp, int* budgets_out, cudaStream_t st) {
+  BudgetSeq b;
+  const int rc = escalation_budgets(s, num_hyp, confidence, max_hyp, budgets_out, &b);
+  if (rc != MFR_OK) return rc;
+  return emat_solve<Scoring::kMagsac>(s, kpts0, kpts1, offsets, P, K0, K1, pix_thr, b, seed, 1, R, t, n_inl, mask, st);
 }
 
 int scale_from_depth(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,

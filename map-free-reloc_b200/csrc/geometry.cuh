@@ -22,6 +22,10 @@ int emat_ransac_escalate(PoseSolver* s, const float* kpts0, const float* kpts1, 
                          const float* K0, const float* K1, float pix_thr, int num_hyp, unsigned long long seed,
                          int lo_enabled, float* R, float* t, int* n_inl, unsigned char* mask, double confidence,
                          int max_hyp, int* budgets_out, cudaStream_t st);
+// emat_ransac_escalate with MAGSAC++ scoring and sigma-consensus++ in place of MSAC and its LO (mfr_emat_magsac)
+int emat_magsac(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P, const float* K0,
+                const float* K1, float pix_thr, int num_hyp, unsigned long long seed, float* R, float* t, int* n_inl,
+                unsigned char* mask, double confidence, int max_hyp, int* budgets_out, cudaStream_t st);
 int scale_from_depth(PoseSolver* s, const float* kpts0, const float* kpts1, const int* offsets, int P,
                      const float* K0, const float* K1, const unsigned char* mask, const double* Rd,
                      const double* td, const float* depth0, const float* depth1, int H, int W,

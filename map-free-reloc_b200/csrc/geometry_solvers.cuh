@@ -531,6 +531,61 @@ MFR_HD double sampson_sq(const double* E, double x0, double y0, double x1, doubl
 }
 
 // ------------------------------------------------------------------------------------------------
+// MAGSAC++ loss (Barath et al., CVPR 2020; the objective of cv.findEssentialMat(USAC_MAGSAC)) of a residual with
+// nu = 4 degrees of freedom, the Sampson distance r in normalised coordinates, with sigma = sigma_max (the normalised
+// RANSAC threshold). With x = r^2 / (2 sigma^2), x_k = k^2 / 2, G_k = Gamma(1.5, x_k) and C = 1 / (2^(nu/2) Gamma(nu/2)):
+//   rho(r) = (C 2^2.5 / sigma) [sigma^2 / 2 gamma(2.5, x) + r^2 / 4 (Gamma(1.5, x) - G_k)]
+//          = C 2^1.5 sigma [gamma(2.5, x) + x (Gamma(1.5, x) - G_k)]                 for r < k sigma, rho(k sigma) beyond
+//   w(r)   = rho'(r) / r = (C 2^1.5 / sigma) (Gamma(1.5, x) - G_k)                  for r < k sigma, 0 beyond
+// Closed forms: Gamma(1.5, x) = sqrt(x) e^-x + sqrt(pi)/2 erfc(sqrt(x)),
+//               gamma(2.5, x) = 3 sqrt(pi)/4 erf(sqrt(x)) - sqrt(x) e^-x (x + 1.5).
+// ------------------------------------------------------------------------------------------------
+constexpr double kMagsacK = 3.64;                          // 0.99 quantile of chi_4 (3.6437), as OpenCV's USAC has it
+constexpr double kMagsacXk = 0.5 * kMagsacK * kMagsacK;    // 6.6248
+constexpr double kMagsacGk = 0.0036572608340910780;        // Gamma(1.5, x_k)
+constexpr double kMagsacG25k = 1.3012265540498873;         // gamma(2.5, x_k)
+constexpr double kMagsacC2 = 0.70710678118654752;          // C 2^1.5 with C = 0.25
+constexpr double kHalfSqrtPi = 0.88622692545275801;        // sqrt(pi) / 2 = Gamma(1.5)
+constexpr double kThreeQuarterSqrtPi = 1.3293403881791370; // 3 sqrt(pi) / 4 = Gamma(2.5)
+
+// fp64 rho and w of a residual given as r^2. gamma(2.5, x) comes from its power series below x = 1, where the closed
+// form loses digits to cancellation (x^2.5 against 1.5 sqrt(x)).
+MFR_HD void magsac_loss_sq(double r2, double sigma, double* rho, double* w) {
+  const double x = r2 / (2.0 * sigma * sigma);
+  if (!(x < kMagsacXk)) {
+    *rho = kMagsacC2 * sigma * kMagsacG25k;
+    *w = 0.0;
+    return;
+  }
+  const double sx = sqrt(x), e = exp(-x);
+  const double G15 = sx * e + kHalfSqrtPi * erfc(sx);
+  double g25;
+  if (x < 1.0) {   // gamma(a, x) = x^a e^-x sum_n x^n / (a (a + 1) ... (a + n)); 18 terms reach 1e-17 at x < 1
+    double term = 1.0 / 2.5, sum = term;
+    for (int n = 1; n < 18; ++n) {
+      term *= x / (2.5 + n);
+      sum += term;
+    }
+    g25 = x * x * sx * e * sum;
+  } else {
+    g25 = kThreeQuarterSqrtPi * erf(sx) - sx * e * (x + 1.5);
+  }
+  *rho = kMagsacC2 * sigma * (g25 + x * (G15 - kMagsacGk));
+  *w = kMagsacC2 / sigma * (G15 - kMagsacGk);
+}
+
+// fp32 rho / (C 2^1.5 sigma) of a residual at x = r^2 / (2 sigma^2), for the hypothesis scoring: one erfc and one exp
+// per point. With erf = 1 - erfc the two closed forms combine to
+//   gamma(2.5, x) + x (Gamma(1.5, x) - G_k) = 3 sqrt(pi)/4 (1 - erfc) - 1.5 sqrt(x) e^-x + x (sqrt(pi)/2 erfc - G_k).
+MFR_HD float magsac_rho_unit_f(float x) {
+  if (!(x < static_cast<float>(kMagsacXk))) return static_cast<float>(kMagsacG25k);
+  const float sx = sqrtf(x), ec = erfcf(sx);
+  const float e = expf(-x);
+  return fmaf(x, fmaf(static_cast<float>(kHalfSqrtPi), ec, -static_cast<float>(kMagsacGk)),
+              fmaf(static_cast<float>(kThreeQuarterSqrtPi), 1.0f - ec, -1.5f * sx * e));
+}
+
+// ------------------------------------------------------------------------------------------------
 // RANSAC stopping rule of the solver plugins (pose_solver.required_hypotheses and _SolverBase._satisfied), branch for
 // branch in fp64: the number of minimal samples after which an all-inlier sample has been drawn with probability
 // `confidence`, given the inlier ratio found, capped at 2^31 - 1.

@@ -118,6 +118,8 @@ SIGNATURES = {
                                c_float, ctypes.c_ulonglong, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "mfr_emat_ransac_escalate": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_float, c_int, ctypes.c_ulonglong,
                                          c_int, c_vp, c_vp, c_vp, c_vp, ctypes.c_double, c_int, c_vp, c_vp]),
+    "mfr_emat_magsac": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_float, c_int, ctypes.c_ulonglong, c_vp, c_vp,
+                                c_vp, c_vp, ctypes.c_double, c_int, c_vp, c_vp]),
     "mfr_pnp_ransac_escalate": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_float,
                                         ctypes.c_ulonglong, c_vp, c_vp, c_vp, c_vp, ctypes.c_double, c_int, c_vp, c_vp]),
     "mfr_linear_attention": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
@@ -138,6 +140,7 @@ SIGNATURES = {
     "mfr_host_poly_real_roots": (c_int, [c_vp, c_int, c_vp]),
     "mfr_host_decompose_essential": (c_int, [c_vp, c_vp, c_vp, c_vp]),
     "mfr_host_ransac_satisfied": (c_int, [ctypes.c_double, c_int, c_int, c_int, c_int, c_int]),
+    "mfr_host_magsac_loss": (c_int, [ctypes.c_double, ctypes.c_double, c_vp, c_vp]),
 }
 
 

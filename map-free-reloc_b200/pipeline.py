@@ -40,29 +40,32 @@ from . import pose_solver as _ps
 # PNP.CONFIDENCE) and ``max_hyp`` (GPU_RANSAC.MAX_HYPOTHESES) the E-mat and PnP stages escalate each pair's budget as
 # the single-pair plugins (pose_solver._SolverBase) do, x4 per round up to max_hyp, decided per pair on the device
 # with no host round trip; each pair's result is then that of the fixed-budget call at the budget where it stopped.
+# The E-mat stages take ``scoring`` (GPU_RANSAC.SCORING): "msac", or "magsac" for the MAGSAC++ estimator of the
+# reference's USAC_MAGSAC (PoseBackend.emat), which leaves ``lo`` at its default.
 class EMatMetricStage:
     """EssentialMatrixMetricSolver: E-mat RANSAC, then the metric scale from depth at its inliers."""
 
     def __init__(self, pix_thr, scale_thr, num_hyp=_ps.DEFAULT_NUM_HYP, seed=_ps.DEFAULT_SEED, lo=True, confidence=None,
-                 max_hyp=None):
+                 max_hyp=None, scoring="msac"):
         self.pix_thr, self.scale_thr, self.num_hyp, self.seed, self.lo = float(pix_thr), float(scale_thr), int(num_hyp), seed, lo
-        self.confidence, self.max_hyp = confidence, max_hyp
+        self.confidence, self.max_hyp, self.scoring = confidence, max_hyp, scoring
 
     def __call__(self, be, k0, k1, off, K0, K1, d0, d1):
         return be.emat_metric(k0, k1, off, K0, K1, d0, d1, self.pix_thr, self.scale_thr, self.num_hyp, self.seed, self.lo,
-                              confidence=self.confidence, max_hyp=self.max_hyp)
+                              confidence=self.confidence, max_hyp=self.max_hyp, scoring=self.scoring)
 
 
 class EMatStage:
     """EssentialMatrixSolver: the pose up to scale, t of unit norm."""
 
-    def __init__(self, pix_thr, num_hyp=_ps.DEFAULT_NUM_HYP, seed=_ps.DEFAULT_SEED, lo=True, confidence=None, max_hyp=None):
+    def __init__(self, pix_thr, num_hyp=_ps.DEFAULT_NUM_HYP, seed=_ps.DEFAULT_SEED, lo=True, confidence=None, max_hyp=None,
+                 scoring="msac"):
         self.pix_thr, self.num_hyp, self.seed, self.lo = float(pix_thr), int(num_hyp), seed, lo
-        self.confidence, self.max_hyp = confidence, max_hyp
+        self.confidence, self.max_hyp, self.scoring = confidence, max_hyp, scoring
 
     def __call__(self, be, k0, k1, off, K0, K1, d0, d1):
         R, t, n, _ = be.emat(k0, k1, off, K0, K1, self.pix_thr, self.num_hyp, self.seed, self.lo,
-                             confidence=self.confidence, max_hyp=self.max_hyp)
+                             confidence=self.confidence, max_hyp=self.max_hyp, scoring=self.scoring)
         return R, t, n
 
 
@@ -313,7 +316,7 @@ class MethodSpec:
     width: int
     num_hyp: int
     seed: int
-    lo: int                         # mfr_emat_ransac lo flags (E-mat solvers)
+    lo: int                         # mfr_emat_ransac lo flags (E-mat solvers with MSAC scoring)
     pix_thr: float = None           # EMAT_RANSAC.PIX_THRESHOLD
     scale_thr: float = None         # EMAT_RANSAC.SCALE_THRESHOLD (metric solver)
     reproj_thr: float = None        # PNP.REPROJECTION_INLIER_THRESHOLD
@@ -323,15 +326,20 @@ class MethodSpec:
     sift_ratio: float = None        # SIFT.RATIO_THRESHOLD
     confidence: float = None        # EMAT_RANSAC.CONFIDENCE / PNP.CONFIDENCE (None: Procrustes, or the key unset)
     max_hyp: int = None             # GPU_RANSAC.MAX_HYPOTHESES, at least num_hyp: the escalation's cap
+    scoring: str = "msac"           # GPU_RANSAC.SCORING: E-mat objective, "msac" or "magsac" (MAGSAC++)
 
     def stage(self, escalate=False):
         """The pose stage of this method: the first hypothesis budget only, or with ``escalate`` the CONFIDENCE
-        escalation up to max_hyp (E-mat and PnP; the Procrustes plugin does not escalate)."""
+        escalation up to max_hyp (E-mat and PnP; the Procrustes plugin does not escalate). The E-mat stages score with
+        ``scoring``; MAGSAC++ brings its own LO, so ``lo`` is not passed to it."""
         esc = {"confidence": self.confidence, "max_hyp": self.max_hyp} if escalate else {}
+        if self.solver.startswith("EssentialMatrix"):
+            esc["scoring"] = self.scoring
+            lo = True if self.scoring == "magsac" else self.lo
         if self.solver == "EssentialMatrixMetric":
-            return EMatMetricStage(self.pix_thr, self.scale_thr, self.num_hyp, self.seed, self.lo, **esc)
+            return EMatMetricStage(self.pix_thr, self.scale_thr, self.num_hyp, self.seed, lo, **esc)
         if self.solver == "EssentialMatrix":
-            return EMatStage(self.pix_thr, self.num_hyp, self.seed, self.lo, **esc)
+            return EMatStage(self.pix_thr, self.num_hyp, self.seed, lo, **esc)
         if self.solver == "PNP":
             return PnPStage(self.reproj_thr, self.num_hyp, self.seed, **esc)
         return ProcrustesStage(self.max_corr_dist, self.num_hyp, self.seed, self.refine)
@@ -354,8 +362,9 @@ def _matcher_name(cfg):
 def resolve_method(cfg):
     """Reference method config (a config.CfgNode or nested dict, e.g. config/mapfree.yaml + a
     config/matching/mapfree/*.yaml) -> MethodSpec. Unknown matchers or solvers raise NotImplementedError as the
-    reference's FeatureMatchingModel does. Budget, escalation cap, confidence, seed and LO flags follow the single-pair
-    plugins (pose_solver); the stage escalates on the confidence only when asked to (``MethodSpec.stage``)."""
+    reference's FeatureMatchingModel does. Budget, escalation cap, confidence, seed, LO flags and the E-mat scoring
+    follow the single-pair plugins (pose_solver); the stage escalates on the confidence only when asked to
+    (``MethodSpec.stage``)."""
     g = lambda k, d=None: _ps._cfg_get(cfg, k, d)
     matcher = _matcher_name(cfg)
     solver = g("POSE_SOLVER")
@@ -368,6 +377,7 @@ def resolve_method(cfg):
     f = lambda k: None if g(k) is None else float(g(k))
     kw = {}
     if solver.startswith("EssentialMatrix"):
+        kw["scoring"] = _ps.ransac_scoring(cfg)
         kw["pix_thr"] = f("EMAT_RANSAC.PIX_THRESHOLD")
         kw["confidence"] = f("EMAT_RANSAC.CONFIDENCE")
         if solver == "EssentialMatrixMetric":

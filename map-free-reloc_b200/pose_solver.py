@@ -17,6 +17,7 @@ DEFAULT_NUM_HYP = 2048
 DEFAULT_SEED = 0x5EED
 LO_TUKEY, LO_LSQ = 1, 3       # mfr_emat_ransac lo_enabled flags: bit 0 local optimisation, bit 1 final least-squares refit
 DEFAULT_FINAL_REFIT = "lsq"
+SCORINGS = ("msac", "magsac")  # GPU_RANSAC.SCORING: E-mat RANSAC objective (mfr_emat_ransac* / mfr_emat_magsac)
 MAX_PTS_LIMIT = 8192          # correspondences per pair the RANSAC kernels can hold (shared memory)
 
 
@@ -65,18 +66,31 @@ class PoseBackend(_lib.Engine):
         return cap, _lib.ptr(budgets)
 
     def emat(self, kpts0, kpts1, offsets, K0, K1, pix_thr, num_hyp=DEFAULT_NUM_HYP, seed=DEFAULT_SEED,
-             lo=True, total=None, confidence=None, max_hyp=None, budgets=None):
+             lo=True, total=None, confidence=None, max_hyp=None, budgets=None, scoring="msac"):
         """EssentialMatrixSolver for P pairs. Returns R [P,3,3], t [P,3] (unit), n [P], mask [total].
         lo: False / 0 = raw RANSAC winner; True / 1 = local optimisation (LO_TUKEY); 3 = LO + the final truncated
         least-squares refit on the model's own inlier set (LO_LSQ, the reference-equivalent optimum).
         confidence: None = one solve at num_hyp; else EMAT_RANSAC.CONFIDENCE, escalated per pair on the device as the
         plugins do (x4 per round up to max_hyp, default the handle's max_hyp; mfr_emat_ransac_escalate). budgets: optional
-        int32 [P] CUDA tensor that receives the budget each pair's result comes from (0: fewer than 5 correspondences)."""
+        int32 [P] CUDA tensor that receives the budget each pair's result comes from (0: fewer than 5 correspondences).
+        scoring: "msac" (the above) or "magsac", the estimator of the reference's cv.USAC_MAGSAC (mfr_emat_magsac:
+        MAGSAC++ scoring, sigma-consensus++ LO and polish); ``lo`` must then stay at its default."""
+        if scoring not in SCORINGS:
+            raise ValueError(f"scoring must be one of {SCORINGS}, got {scoring!r}")
+        if scoring == "magsac" and lo is not True:
+            raise ValueError("scoring='magsac' has its own local optimisation: leave lo at its default")
         P = self._prep(kpts0, kpts1, offsets, K0, K1)
         total = kpts0.shape[0] if total is None else total
         R, t, n, mask = self._outs(P, total)
-        args = (self._h, _lib.ptr(kpts0), _lib.ptr(kpts1), _lib.ptr(offsets), P, _lib.ptr(K0), _lib.ptr(K1), float(pix_thr),
-                int(num_hyp), ctypes.c_ulonglong(seed), int(lo), _lib.ptr(R), _lib.ptr(t), _lib.ptr(n), _lib.ptr(mask))
+        head = (self._h, _lib.ptr(kpts0), _lib.ptr(kpts1), _lib.ptr(offsets), P, _lib.ptr(K0), _lib.ptr(K1), float(pix_thr),
+                int(num_hyp), ctypes.c_ulonglong(seed))
+        outs = (_lib.ptr(R), _lib.ptr(t), _lib.ptr(n), _lib.ptr(mask))
+        if scoring == "magsac":
+            cap, b = (int(num_hyp), _lib.ptr(budgets)) if confidence is None else self._escalation(P, num_hyp, max_hyp, budgets)
+            _lib.check(self._l.mfr_emat_magsac(*head, *outs, 0.0 if confidence is None else float(confidence), cap, b,
+                                               _lib.cur_stream()), "mfr_emat_magsac")
+            return R, t, n, mask
+        args = (*head, int(lo), *outs)
         if confidence is None:
             _lib.check(self._l.mfr_emat_ransac(*args, _lib.cur_stream()), "mfr_emat_ransac")
         else:
@@ -101,12 +115,13 @@ class PoseBackend(_lib.Engine):
         return R, t, n
 
     def emat_metric(self, kpts0, kpts1, offsets, K0, K1, depth0, depth1, pix_thr, scale_thr,
-                    num_hyp=DEFAULT_NUM_HYP, seed=DEFAULT_SEED, lo=True, confidence=None, max_hyp=None, budgets=None):
+                    num_hyp=DEFAULT_NUM_HYP, seed=DEFAULT_SEED, lo=True, confidence=None, max_hyp=None, budgets=None,
+                    scoring="msac"):
         """EssentialMatrixMetricSolver for P pairs: R [P,3,3], t [P,3] metres, inliers [P]. confidence / max_hyp /
-        budgets: the E-mat escalation of ``emat`` (driven by the E-mat inlier count); the scale runs once, on the
-        final pose."""
+        budgets / scoring: the E-mat escalation and objective of ``emat`` (the escalation is driven by the E-mat inlier
+        count); the scale runs once, on the final pose."""
         _, _, _, mask = self.emat(kpts0, kpts1, offsets, K0, K1, pix_thr, num_hyp, seed, lo, confidence=confidence,
-                                  max_hyp=max_hyp, budgets=budgets)
+                                  max_hyp=max_hyp, budgets=budgets, scoring=scoring)
         return self.scale(kpts0, kpts1, offsets, K0, K1, mask, depth0, depth1, scale_thr)
 
     def pnp(self, kpts0, kpts1, offsets, K0, K1, depth0, reproj_thr, num_hyp=DEFAULT_NUM_HYP,
@@ -183,6 +198,20 @@ def ransac_settings(cfg, default_hyp=DEFAULT_NUM_HYP):
     return num_hyp, max_hyp, seed, (LO_LSQ if refit == "lsq" else LO_TUKEY) if lo else 0
 
 
+def ransac_scoring(cfg):
+    """GPU_RANSAC.SCORING -> "msac" (the default) or "magsac" (the MAGSAC++ estimator of the reference's USAC_MAGSAC).
+    Anything else raises ValueError, and so does "magsac" with a non-default GPU_RANSAC.LOCAL_OPTIMISATION or FINAL_REFIT:
+    MAGSAC++ has its own LO, so those keys would be ignored."""
+    scoring = str(_cfg_get(cfg, "GPU_RANSAC.SCORING", "msac")).lower()
+    if scoring not in SCORINGS:
+        raise ValueError("GPU_RANSAC.SCORING must be 'msac' or 'magsac'")
+    if scoring == "magsac" and (_cfg_get(cfg, "GPU_RANSAC.LOCAL_OPTIMISATION", True) is not True or
+                                str(_cfg_get(cfg, "GPU_RANSAC.FINAL_REFIT", DEFAULT_FINAL_REFIT)).lower() != DEFAULT_FINAL_REFIT):
+        raise ValueError("GPU_RANSAC.SCORING 'magsac' has its own local optimisation: leave GPU_RANSAC.LOCAL_OPTIMISATION "
+                         "and GPU_RANSAC.FINAL_REFIT at their defaults")
+    return scoring
+
+
 def pnp_default_hyp(cfg):
     """PnPSolver's budget when GPU_RANSAC.NUM_HYPOTHESES is unset: PNP.RANSAC_ITER (the reference's iteration cap of
     cv2.solvePnPRansac) rounded up to a multiple of 128, at least 128."""
@@ -243,6 +272,7 @@ class EssentialMatrixSolver(_SolverBase):
         super().__init__(cfg)
         self.ransac_pix_threshold = float(_cfg_get(cfg, "EMAT_RANSAC.PIX_THRESHOLD"))
         self.ransac_confidence = _cfg_get(cfg, "EMAT_RANSAC.CONFIDENCE")  # escalation rule, see _SolverBase
+        self.scoring = ransac_scoring(cfg)
         self.mask = None
 
     def estimate_pose(self, kpts0, kpts1, data):
@@ -250,8 +280,12 @@ class EssentialMatrixSolver(_SolverBase):
             return self._nan()
         k0, k1, off, K0, K1 = self._upload(kpts0, kpts1, data)
         for budget in self._budgets(self.ransac_confidence):
-            R, t, n, mask = self.backend.emat(k0, k1, off, K0, K1, self.ransac_pix_threshold, budget,
-                                              self.seed, self.lo)
+            if self.scoring == "magsac":
+                R, t, n, mask = self.backend.emat(k0, k1, off, K0, K1, self.ransac_pix_threshold, budget, self.seed,
+                                                  scoring="magsac")
+            else:
+                R, t, n, mask = self.backend.emat(k0, k1, off, K0, K1, self.ransac_pix_threshold, budget,
+                                                  self.seed, self.lo)
             n = int(n.item())
             self.last_num_hyp = budget
             if self._satisfied(self.ransac_confidence, n, k0.shape[0], budget):

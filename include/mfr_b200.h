@@ -416,7 +416,9 @@ int mfr_procrustes_ransac(mfr_pose_solver* s, const float* kpts0, const float* k
  *   ransac_satisfied : 1 iff the escalation stops after a round at `budget` that found n_inliers of n_points
  *                (the rule of mfr_emat_ransac_escalate, cap max_budget, minimal sample sample_size), else 0
  *   magsac_loss : MAGSAC++ rho(r) and w(r) = rho'(r) / r of mfr_emat_magsac (the fp64 version of its LO / polish) for
- *                a Sampson distance r and sigma_max > 0 (else MFR_ERR_ARG)                                      */
+ *                a Sampson distance r and sigma_max > 0 (else MFR_ERR_ARG)
+ *   jpeg_decode : mfr_jpeg_decode's arithmetic run serially on the CPU; data and dst in HOST memory, dst sized
+ *                width x height (x 3 when rgb), the oriented size; returns the file's status                      */
 int mfr_host_five_point(const double* x0, const double* x1, double* E_out);
 int mfr_host_p3p(const double* X, const double* f, double* R_out, double* t_out);
 int mfr_host_poly_real_roots(const double* coef, int deg, double* roots);
@@ -424,6 +426,7 @@ int mfr_host_decompose_essential(const double* E, double* R1, double* R2, double
 int mfr_host_ransac_satisfied(double confidence, int n_inliers, int n_points, int budget, int max_budget,
                               int sample_size);
 int mfr_host_magsac_loss(double r, double sigma_max, double* rho, double* w);
+int mfr_host_jpeg_decode(const unsigned char* data, long long length, int rgb, unsigned char* dst, int width, int height);
 
 /* Debug probe (microbenchmark used by scripts/, not part of the product path): microseconds per
  * launch of a prebuilt conv/GEMM op launched back to back.
@@ -465,16 +468,45 @@ int mfr_icp_refine(mfr_pose_solver* s, const float* depth0, const float* depth1,
                    const float* K1, const float* R_in, const float* t_in, float max_corr_dist, int max_iterations,
                    float relative_fitness, float relative_rmse, float* R, float* t, int* n_inliers, void* stream);
 
-/* Input path on the GPU (SURVEY §8(f) rank 1). mfr_jpeg_info / mfr_jpeg_decode: nvJPEG decode of a JPEG held in HOST
- * memory into a DEVICE uint8 image — rgb = 0: the luma plane [h][w] (cv2.imread(IMREAD_GRAYSCALE) of a JPEG,
- * SuperGlue/models/utils.py:264), rgb = 1: interleaved RGB [h][w][3] (lib/datasets/utils.py:67 imread).
+/* Input path on the GPU (SURVEY §8(f) rank 1): JPEG decode with cv2.imread's exact pixels, and cv2.resize.
+ *
+ * JPEG decode (csrc/jpeg.cuh, csrc/image_io.cu): libjpeg(-turbo)'s decompression arithmetic as CUDA kernels (ISLOW IDCT,
+ * fancy upsampling, its YCbCr -> RGB tables) plus the Exif Orientation that cv2.imread applies. Output in DEVICE memory:
+ * rgb = 0: gray [h][w], the Y plane as coded (cv2.imread(IMREAD_GRAYSCALE), SuperGlue/models/utils.py:264); rgb = 1:
+ * interleaved RGB [h][w][3] (cv2.imread(IMREAD_COLOR) in RGB order, lib/datasets/utils.py:67); h, w after the
+ * orientation (5-8 swap them). Supported: SOF0 / SOF1 8-bit Huffman, one interleaved scan, gray or YCbCr with luma
+ * sampling 1x1 / 2x1 / 2x2 and chroma 1x1, any size, DRI / RSTn, 8- or 16-bit quantisation tables. A valid file outside
+ * that set gives MFR_ERR_UNSUPPORTED (progressive, arithmetic, lossless, 12-bit, 4:4:0, 4:1:1, CMYK, RGB-coded,
+ * multi-scan); malformed headers give MFR_ERR_ARG; entropy-coded data with an invalid code, or that ends before its
+ * last block, gives MFR_ERR_ARG once decoded (libjpeg decodes such data with warnings: cv2 is the answer for it).
+ *   mfr_jpeg_info: parses one file (HOST bytes): oriented width / height and component count, or the file's error code.
+ *   mfr_jpeg_decode: one file through a process-wide decoder per device (created on first use, grown when a file does
+ *     not fit, guarded by a mutex); width / height must be mfr_jpeg_info's. Returns once the image is decoded, with its
+ *     status.
+ *   mfr_jpeg_decoder_create: a decoder for batches of up to max_images files holding up to max_bytes of entropy-coded
+ *     data and max_pixels pixels in all, each image counted at its size rounded up to multiples of 16 (what its
+ *     coefficient planes need). It owns pinned staging, device buffers and two events; not thread-safe.
+ *   mfr_jpeg_batch_info: per file (HOST arrays) the oriented width / height (0 unless supported) and status MFR_OK,
+ *     MFR_ERR_UNSUPPORTED or MFR_ERR_ARG, from the headers alone.
+ *   mfr_jpeg_decode_batch: decodes n files (HOST byte pointers and lengths) into dst[i] (DEVICE pointers, sized from
+ *     mfr_jpeg_batch_info; ignored for files that are not MFR_OK there) asynchronously on `stream`: it returns once the
+ *     work is enqueued, the bytes having been copied into the decoder's staging. status: DEVICE int[n], written on the
+ *     stream: the header status of each file, then MFR_ERR_ARG where its entropy-coded data fails. The call returns
+ *     MFR_ERR_ARG when the batch exceeds the decoder's capacity (nothing is enqueued). Successive calls on one decoder
+ *     may use different streams: each waits on the device for the previous call's kernels.
  * mfr_resize_linear: cv2.resize(INTER_LINEAR) + scale on the device, dst fp32 [dst_h][dst_w][channels] (chw = 0) or
  * [channels][dst_h][dst_w] (chw = 1) = resized * out_scale. mode 0: float source, float arithmetic; mode 1: uint8 source
  * converted to float first (read_image with resize_float = True, utils.py:272-273: the FMB matcher plugins);
  * mode 2: uint8 source, OpenCV's 11-bit fixed-point uint8 path, rounded to uint8 before the scale (utils.py:275,
  * lib/datasets/utils.py:68). src_row_stride in elements. */
+typedef struct mfr_jpeg_decoder mfr_jpeg_decoder;
 int mfr_jpeg_info(const unsigned char* data, long long length, int* width, int* height, int* components);
 int mfr_jpeg_decode(const unsigned char* data, long long length, int rgb, unsigned char* dst, int width, int height, void* stream);
+int mfr_jpeg_decoder_create(int max_images, long long max_bytes, long long max_pixels, mfr_jpeg_decoder** out);
+void mfr_jpeg_decoder_destroy(mfr_jpeg_decoder* dec);
+int mfr_jpeg_batch_info(const unsigned char* const* data, const long long* lengths, int n, int* width, int* height, int* status);
+int mfr_jpeg_decode_batch(mfr_jpeg_decoder* dec, const unsigned char* const* data, const long long* lengths, int n, int rgb,
+                          unsigned char* const* dst, int* status, void* stream);
 int mfr_resize_linear(const void* src, int src_is_u8, int src_w, int src_h, long long src_row_stride, int channels, float* dst,
                       int dst_w, int dst_h, int mode, float out_scale, int chw, void* stream);
 

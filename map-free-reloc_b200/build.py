@@ -57,7 +57,7 @@ def build(force=False, verbose=True):
                     print(os.path.basename(src), line.strip())
     if not ok:
         raise RuntimeError("nvcc failed")
-    cmd = [NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", OUT, *objs, "-lcudart", "-lnvjpeg"]
+    cmd = [NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", OUT, *objs, "-lcudart"]
     subprocess.check_call(cmd)
     return OUT
 

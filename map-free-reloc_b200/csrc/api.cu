@@ -21,7 +21,17 @@ int resize_linear(const void* src, int src_is_u8, int sw, int sh, long long src_
                   int mode, float out_scale, int chw, cudaStream_t st);
 int jpeg_info(const unsigned char* data, size_t length, int* width, int* height, int* components);
 int jpeg_decode(const unsigned char* data, size_t length, int rgb, unsigned char* dst, int width, int height, cudaStream_t st);
+struct JpegDecoder;
+int jpeg_decoder_create(int max_images, long long max_bytes, long long max_pixels, JpegDecoder** out);
+void jpeg_decoder_destroy(JpegDecoder* dec);
+int jpeg_decode_batch(JpegDecoder* dec, const unsigned char* const* data, const long long* lengths, int n, int rgb,
+                      unsigned char* const* dst, int* status, cudaStream_t st);
+void jpeg_batch_info(const unsigned char* const* data, const long long* lengths, int n, int* width, int* height, int* status);
+int jpeg_host_decode(const unsigned char* data, size_t length, int rgb, unsigned char* dst, int width, int height);
 }
+struct mfr_jpeg_decoder {
+  mfr::JpegDecoder* d;
+};
 namespace mfr {   // metrics.cu
 int pose_metrics(const double* q_gt, const double* t_gt, const double* q_est, const double* t_est, const double* K, int W, int H,
                  int n, double* trans_err, double* rot_err, double* reproj_err, cudaStream_t st);
@@ -392,6 +402,10 @@ int mfr_host_magsac_loss(double r, double sigma_max, double* rho, double* w) {
   mfr::geo::magsac_loss_sq(r * r, sigma_max, rho, w);
   return MFR_OK;
 }
+int mfr_host_jpeg_decode(const unsigned char* data, long long length, int rgb, unsigned char* dst, int width, int height) {
+  if (!data || length <= 0 || !dst) return MFR_ERR_ARG;
+  return mfr::jpeg_host_decode(data, static_cast<size_t>(length), rgb, dst, width, height);
+}
 
 // ------------------------------------------------------------------------------------------ debug probes
 float mfr_debug_time_conv(const float* x, int N, int H, int W, int Cin, const float* w, int Cout, int R,
@@ -468,6 +482,30 @@ int mfr_jpeg_info(const unsigned char* data, long long length, int* width, int* 
 int mfr_jpeg_decode(const unsigned char* data, long long length, int rgb, unsigned char* dst, int width, int height, void* stream) {
   if (!data || length <= 0 || !dst) return MFR_ERR_ARG;
   return mfr::jpeg_decode(data, static_cast<size_t>(length), rgb, dst, width, height, static_cast<cudaStream_t>(stream));
+}
+int mfr_jpeg_decoder_create(int max_images, long long max_bytes, long long max_pixels, mfr_jpeg_decoder** out) {
+  if (!out) return MFR_ERR_ARG;
+  *out = nullptr;
+  mfr::JpegDecoder* d = nullptr;
+  const int rc = mfr::jpeg_decoder_create(max_images, max_bytes, max_pixels, &d);
+  if (rc != MFR_OK) return rc;
+  *out = new mfr_jpeg_decoder{d};
+  return MFR_OK;
+}
+void mfr_jpeg_decoder_destroy(mfr_jpeg_decoder* dec) {
+  if (!dec) return;
+  mfr::jpeg_decoder_destroy(dec->d);
+  delete dec;
+}
+int mfr_jpeg_batch_info(const unsigned char* const* data, const long long* lengths, int n, int* width, int* height, int* status) {
+  if (n < 0 || (n > 0 && (!data || !lengths || !width || !height || !status))) return MFR_ERR_ARG;
+  mfr::jpeg_batch_info(data, lengths, n, width, height, status);
+  return MFR_OK;
+}
+int mfr_jpeg_decode_batch(mfr_jpeg_decoder* dec, const unsigned char* const* data, const long long* lengths, int n, int rgb,
+                          unsigned char* const* dst, int* status, void* stream) {
+  if (!dec) return MFR_ERR_ARG;
+  return mfr::jpeg_decode_batch(dec->d, data, lengths, n, rgb, dst, status, static_cast<cudaStream_t>(stream));
 }
 
 int mfr_pose_metrics(const double* q_gt, const double* t_gt, const double* q_est, const double* t_est, const double* K, int W,

@@ -1,14 +1,16 @@
-"""Input path of the matcher plugins on the GPU (SURVEY §8(f) rank 1): JPEG decode with nvJPEG and the reference's
-resize + normalise steps as CUDA kernels (libmfr_b200.so: mfr_jpeg_decode, mfr_resize_linear).
+"""Input path of the matcher plugins on the GPU (SURVEY §8(f) rank 1): JPEG decode and the reference's resize +
+normalise steps as CUDA kernels (libmfr_b200.so: mfr_jpeg_decode_batch / mfr_jpeg_decode, mfr_resize_linear).
 
+  decode_jpegs(items, rgb)                 = [cv2.imread(p, GRAYSCALE or COLOR) for p in items], one batched GPU decode
   read_image(path, resize, resize_float)   = SuperGlue/models/utils.py:263-285 (gray, cv2.resize, / 255) -> CUDA [h, w]
   read_color_image(path, resize)           = lib/datasets/utils.py:58-75 (RGB, uint8 cv2.resize, / 255)   -> CUDA [3, h, w]
   PairMatcher                              = match / match_scene / match_arrays of the LoFTR and SuperGlue plugins
 
-JPEG files are decoded on the GPU (luma plane = OpenCV's IMREAD_GRAYSCALE of a JPEG, up to the +-1 level differences
-between two IDCT implementations); other formats are decoded by OpenCV on the host and uploaded as uint8. The resize
-kernels restate cv2.resize(INTER_LINEAR) for both of its arithmetic paths (tests/test_image_io_gpu.py: float path
-within 1e-6 of cv2, uint8 path bit-exact)."""
+JPEG files are decoded on the GPU with libjpeg's arithmetic (csrc/jpeg.cuh): the bytes equal cv2.imread's (Exif
+orientation included) for baseline / extended-sequential Huffman files, gray or YCbCr 4:4:4 / 4:2:2 / 4:2:0. Other files
+(progressive, 4:1:1, CMYK, ... and other formats) are decoded by OpenCV on the host and uploaded as uint8, so every
+loader returns cv2's pixels. The resize kernels restate cv2.resize(INTER_LINEAR) for both of its arithmetic paths
+(tests/test_image_io_gpu.py: float path within 1e-6 of cv2, uint8 path bit-exact)."""
 import ctypes
 import os
 
@@ -28,21 +30,114 @@ def _device(device):
     return torch.device("cuda", torch.cuda.current_device() if device is None else int(device))
 
 
+def _bytes(item):
+    if isinstance(item, (bytes, bytearray, memoryview)):
+        return bytes(item)
+    with open(item, "rb") as f:
+        return f.read()
+
+
 def decode_jpeg(data, rgb=False, device=None):
-    """JPEG bytes (or a path) -> CUDA uint8 tensor [h, w] (luma) or [h, w, 3] (RGB)."""
+    """JPEG bytes (or a path) -> CUDA uint8 tensor [h, w] (gray) or [h, w, 3] (RGB): cv2.imread's pixels. Raises
+    MfrError for a file the GPU decoder does not take (mfr_jpeg_info's status) or whose data fails to decode."""
     dev = _device(device)
-    if not isinstance(data, (bytes, bytearray)):
-        with open(data, "rb") as f:
-            data = f.read()
+    data = _bytes(data)
     l = _lib.load()
-    buf = (ctypes.c_ubyte * len(data)).from_buffer_copy(data)
     w, h, c = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-    _lib.check(l.mfr_jpeg_info(buf, len(data), ctypes.byref(w), ctypes.byref(h), ctypes.byref(c)), "mfr_jpeg_info")
+    _lib.check(l.mfr_jpeg_info(data, len(data), ctypes.byref(w), ctypes.byref(h), ctypes.byref(c)), "mfr_jpeg_info")
     out = torch.empty((h.value, w.value, 3) if rgb else (h.value, w.value), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(l.mfr_jpeg_decode(buf, len(data), int(rgb), _lib.ptr(out), w.value, h.value, _lib.cur_stream()), "mfr_jpeg_decode")
-        torch.cuda.current_stream().synchronize()          # `buf` (host) must outlive the decode
+    with torch.cuda.device(dev):     # returns once decoded: the bytes need not outlive the call
+        _lib.check(l.mfr_jpeg_decode(data, len(data), int(rgb), _lib.ptr(out), w.value, h.value, _lib.cur_stream()), "mfr_jpeg_decode")
     return out
+
+
+class _JpegDecoder:
+    """A batch decoder handle (mfr_jpeg_decoder_create) and its capacity; one per device, grown on demand."""
+
+    def __init__(self, images, nbytes, pixels):
+        self.caps = (images, nbytes, pixels)
+        h = ctypes.c_void_p()
+        _lib.check(_lib.load().mfr_jpeg_decoder_create(images, nbytes, pixels, ctypes.byref(h)), "mfr_jpeg_decoder_create")
+        self.h = h
+
+    def fits(self, images, nbytes, pixels):
+        return all(a <= b for a, b in zip((images, nbytes, pixels), self.caps))
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None):
+                _lib.load().mfr_jpeg_decoder_destroy(self.h)  # waits for the decoder's last batch
+                self.h = None
+        except Exception:
+            pass                                          # interpreter shutdown: the module may be gone
+
+
+_DECODERS = {}
+
+
+def _decoder(dev, images, nbytes, pixels):
+    d = _DECODERS.get(dev.index)
+    if d is None or not d.fits(images, nbytes, pixels):
+        old = d.caps if d is not None else (0, 0, 0)
+        _DECODERS.pop(dev.index, None)
+        with torch.cuda.device(dev):
+            d = _DECODERS[dev.index] = _JpegDecoder(max(images, old[0], 16), max(nbytes, old[1], 1 << 22),
+                                                    max(pixels, old[2], 1 << 22))
+    return d
+
+
+def _host_decode(item, rgb, dev):
+    """cv2's decode of a file or bytes, uploaded (None if OpenCV cannot read it)."""
+    import cv2
+    flag = cv2.IMREAD_COLOR if rgb else cv2.IMREAD_GRAYSCALE
+    if isinstance(item, (bytes, bytearray, memoryview)):
+        im = cv2.imdecode(np.frombuffer(bytes(item), np.uint8), flag)
+    else:
+        im = cv2.imread(str(item), flag)
+    if im is None:
+        return None
+    if rgb:
+        im = np.ascontiguousarray(im[:, :, ::-1])    # lib/datasets/utils.py:7-17: BGR -> RGB
+    return torch.from_numpy(im).to(dev)
+
+
+def decode_jpegs(items, rgb=False, device=None):
+    """JPEG files (bytes or paths) -> list of CUDA uint8 tensors [h, w] / [h, w, 3], cv2.imread's pixels, in one decoder
+    call on the current stream. Files the GPU decoder does not take, or whose data it rejects, are decoded by OpenCV on
+    the host in their place in the list (None where OpenCV cannot read them either). The per-image statuses are read
+    back once for the batch."""
+    dev = _device(device)
+    datas = [_bytes(x) for x in items]
+    n = len(datas)
+    if n == 0:
+        return []
+    l = _lib.load()
+    ptrs = (ctypes.c_char_p * n)(*datas)
+    lens = (ctypes.c_longlong * n)(*[len(d) for d in datas])
+    w, h, st = (ctypes.c_int * n)(), (ctypes.c_int * n)(), (ctypes.c_int * n)()
+    _lib.check(l.mfr_jpeg_batch_info(ptrs, lens, n, w, h, st), "mfr_jpeg_batch_info")
+    outs = [None] * n
+    dst = (ctypes.c_void_p * n)()
+    nbytes = pixels = 0
+    for i in range(n):
+        if st[i] == 0:
+            outs[i] = torch.empty((h[i], w[i], 3) if rgb else (h[i], w[i]), dtype=torch.uint8, device=dev)
+            dst[i] = outs[i].data_ptr()
+            nbytes += len(datas[i])
+            pixels += -(-w[i] // 16) * 16 * (-(-h[i] // 16) * 16)
+    if nbytes:
+        status = torch.empty(n, dtype=torch.int32, device=dev)
+        dec = _decoder(dev, n, nbytes, pixels)
+        with torch.cuda.device(dev):
+            _lib.check(l.mfr_jpeg_decode_batch(dec.h, ptrs, lens, n, int(rgb), dst, _lib.ptr(status), _lib.cur_stream()),
+                       "mfr_jpeg_decode_batch")
+        ok = status.cpu().tolist()
+    else:
+        ok = [1] * n
+    for i in range(n):
+        if ok[i] != 0:
+            outs[i] = _host_decode(items[i], rgb, dev)
+    return outs
 
 
 def resize_linear(img, size, mode, out_scale=1.0, chw=False):
@@ -61,31 +156,43 @@ def resize_linear(img, size, mode, out_scale=1.0, chw=False):
     return out
 
 
+def _is_jpeg(path):
+    return str(path).lower().endswith((".jpg", ".jpeg"))
+
+
 def _load_u8(path, rgb, device):
     p = str(path)
     if not os.path.isfile(p):
         return None                                  # cv2.imread's convention for unreadable files (utils.py:265-266)
-    if p.lower().endswith((".jpg", ".jpeg")):
+    if _is_jpeg(p):
         try:
             return decode_jpeg(p, rgb=rgb, device=device)
         except _lib.MfrError:
-            pass                                     # e.g. progressive / CMYK files nvJPEG's simple API rejects: decode on the host
-    import cv2
-    im = cv2.imread(p, cv2.IMREAD_COLOR if rgb else cv2.IMREAD_GRAYSCALE)
+            pass                                     # a file the GPU decoder does not take: OpenCV on the host
+    return _host_decode(p, rgb, _device(device))
+
+
+def _load_u8_many(paths, rgb, device):
+    """[_load_u8(p, rgb, device) for p in paths] with every existing JPEG decoded in one decode_jpegs call."""
+    out = [None] * len(paths)
+    jpg = [i for i, p in enumerate(paths) if _is_jpeg(p) and os.path.isfile(str(p))]
+    for i, im in zip(jpg, decode_jpegs([str(paths[i]) for i in jpg], rgb, device)):
+        out[i] = im
+    for i in set(range(len(paths))) - set(jpg):
+        out[i] = _load_u8(paths[i], rgb, device)
+    return out
+
+
+def _gray_input(im, resize, resize_float):
     if im is None:
         return None
-    if rgb:
-        im = np.ascontiguousarray(im[:, :, ::-1])    # lib/datasets/utils.py:7-17: BGR -> RGB
-    return torch.from_numpy(im).to(_device(device))
+    return resize_linear(im, resize, MODE_U8_AS_F32 if resize_float else MODE_U8_FIXED, 1.0 / 255.0)
 
 
 def read_image(path, resize, resize_float=True, device=None):
     """Gray image, resized to resize = (w, h), in [0, 1]: CUDA float32 [h, w]; None if the file cannot be read
     (SuperGlue/models/utils.py:263-285 with rotation 0; `resize` given as the two-element form the FMB plugins use)."""
-    im = _load_u8(path, False, device)
-    if im is None:
-        return None
-    return resize_linear(im, resize, MODE_U8_AS_F32 if resize_float else MODE_U8_FIXED, 1.0 / 255.0)
+    return _gray_input(_load_u8(path, False, device), resize, resize_float)
 
 
 class PairMatcher:
@@ -98,14 +205,15 @@ class PairMatcher:
         self.resize, self.engine = resize, engine
 
     def match(self, pair_path):
-        """matchers.py:24-59 / 93-120; images decoded (JPEG: nvJPEG) and resized on the GPU."""
+        """matchers.py:24-59 / 93-120; images decoded and resized on the GPU."""
         return self._result(self.engine.forward(self._read(pair_path[0]), self._read(pair_path[1])))
 
     def match_scene(self, ref_path, query_paths):
         """``[self.match((ref_path, q)) for q in query_paths]``, array for array, with the reference image decoded and
-        encoded once (Map-free: every pair of a scene shares its first image)."""
+        encoded once (Map-free: every pair of a scene shares its first image) and the query JPEGs decoded in one batch."""
         self.engine.set_map(self._read(ref_path))
-        return [self._result(self.engine.forward_shared(self._read(q))) for q in query_paths]
+        ims = _load_u8_many(list(query_paths), False, self.engine.device)
+        return [self._result(self.engine.forward_shared(_gray_input(im, self.resize, True)[None])) for im in ims]
 
     def match_arrays(self, im0, im1):
         """``match`` on two gray float [h, w] arrays in [0, 1]."""
@@ -130,3 +238,15 @@ def read_color_image(path, resize=(640, 480), device=None):
     if im is None:
         return None
     return resize_linear(im, resize, MODE_U8_FIXED, 1.0 / 255.0, chw=True)
+
+
+def jpeg_size(path):
+    """(width, height) cv2.imread would return for a JPEG file the GPU decoder takes (orientation applied), else None."""
+    try:
+        data = _bytes(path)
+    except OSError:
+        return None
+    w, h, c = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    if _lib.load().mfr_jpeg_info(data, len(data), ctypes.byref(w), ctypes.byref(h), ctypes.byref(c)) != 0:
+        return None
+    return w.value, h.value

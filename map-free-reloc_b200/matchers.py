@@ -5,6 +5,7 @@ packs a scene's pairs into the NaN-padded [Npairs, maxN, 4] float64 array the on
 ``PrecomputedMatching`` plugin reads (etc/feature_matching_baselines/utils.py:59-69)."""
 import numpy as np
 
+from . import image_io
 from .loftr import LoFTR_matcher
 from .model import sift_matches_gpu, sift_matches_host
 from .spsg import SuperGlue_matcher
@@ -12,7 +13,8 @@ from .spsg import SuperGlue_matcher
 
 class SIFT_matcher:
     """matchers.py:123-188: 2048 SIFT features, RootSIFT, 2-NN + ratio 0.8 (exact NN on the GPU).
-    gpu_detector=True: detection, description and matching run on the CUDA SIFT engine (mfr_b200.sift)."""
+    gpu_detector=True: detection, description and matching run on the CUDA SIFT engine (mfr_b200.sift); JPEG frames whose
+    size equals ``resize`` are also decoded on the GPU (image_io.decode_jpegs, cv2.imread's pixels)."""
 
     def __init__(self, resize, outdoor=False, gpu_detector=False):
         self.resize = resize
@@ -21,6 +23,12 @@ class SIFT_matcher:
 
     def match(self, pair_path):
         import cv2
+        if self.gpu_detector and all(image_io.jpeg_size(p) == tuple(self.resize) for p in pair_path):
+            # resize = the image size (Map-free frames: cv2.resize is a copy): decode on the GPU, cv2's exact pixels;
+            # other sizes keep cv2.resize on the host, whose dispatched uint8 path the GPU resize does not restate
+            img0, img1 = image_io.decode_jpegs(list(pair_path))
+            if img0 is not None and img1 is not None:
+                return self.match_arrays_gpu(img0, img1)
         img0 = cv2.resize(cv2.imread(pair_path[0], 0), self.resize)
         img1 = cv2.resize(cv2.imread(pair_path[1], 0), self.resize)
         if self.gpu_detector and img0.shape == img1.shape:

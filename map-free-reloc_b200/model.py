@@ -81,12 +81,13 @@ def sift_matches_host(sift, img0, img1, ratio):
 
 def sift_matches_gpu(engines, img0, img1, nfeatures, ratio):
     """The same with detection, description and matching on the CUDA SIFT engine (mfr_b200.sift); ``engines`` caches
-    one engine per frame shape. img0 and img1 have the same shape."""
+    one engine per frame shape. img0 and img1 (uint8 arrays or tensors) have the same shape."""
     from . import sift
     if img0.shape not in engines:
         engines[img0.shape] = sift.SIFT(2, img0.shape[0], img0.shape[1], nfeatures=nfeatures, root_sift=True)
     eng = engines[img0.shape]
-    eng.detect(torch.from_numpy(np.stack([img0, img1])).to(eng.device))
+    imgs = torch.stack([img0, img1]) if isinstance(img0, torch.Tensor) else torch.from_numpy(np.stack([img0, img1]))
+    eng.detect(imgs.to(eng.device))
     k0, k1, _ = eng.match_pairs(ratio)
     return k0.cpu().numpy(), k1.cpu().numpy()
 

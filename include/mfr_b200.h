@@ -418,7 +418,10 @@ int mfr_procrustes_ransac(mfr_pose_solver* s, const float* kpts0, const float* k
  *   magsac_loss : MAGSAC++ rho(r) and w(r) = rho'(r) / r of mfr_emat_magsac (the fp64 version of its LO / polish) for
  *                a Sampson distance r and sigma_max > 0 (else MFR_ERR_ARG)
  *   jpeg_decode : mfr_jpeg_decode's arithmetic run serially on the CPU; data and dst in HOST memory, dst sized
- *                width x height (x 3 when rgb), the oriented size; returns the file's status                      */
+ *                width x height (x 3 when rgb), the oriented size; returns the file's status
+ *   png_decode : mfr_png_decode_batch's arithmetic for one file run serially on the CPU; data and dst in HOST memory,
+ *                dst sized width x height samples of the out_kind's type (mfr_png_info's size); returns the file's
+ *                status                                                                                         */
 int mfr_host_five_point(const double* x0, const double* x1, double* E_out);
 int mfr_host_p3p(const double* X, const double* f, double* R_out, double* t_out);
 int mfr_host_poly_real_roots(const double* coef, int deg, double* roots);
@@ -427,6 +430,12 @@ int mfr_host_ransac_satisfied(double confidence, int n_inliers, int n_points, in
                               int sample_size);
 int mfr_host_magsac_loss(double r, double sigma_max, double* rho, double* w);
 int mfr_host_jpeg_decode(const unsigned char* data, long long length, int rgb, unsigned char* dst, int width, int height);
+int mfr_host_png_decode(const unsigned char* data, long long length, int out_kind, void* dst, int width, int height);
+
+/* Debug probe (scripts/png_decode_bench.py): milliseconds of the CRC, inflate and unfilter kernels (ms[0..2], CUDA
+ * events) of the decoder's last mfr_png_decode_batch call; waits for that call's kernels. */
+typedef struct mfr_png_decoder mfr_png_decoder;
+int mfr_debug_png_kernel_ms(mfr_png_decoder* dec, float* ms);
 
 /* Debug probe (microbenchmark used by scripts/, not part of the product path): microseconds per
  * launch of a prebuilt conv/GEMM op launched back to back.
@@ -507,6 +516,34 @@ void mfr_jpeg_decoder_destroy(mfr_jpeg_decoder* dec);
 int mfr_jpeg_batch_info(const unsigned char* const* data, const long long* lengths, int n, int* width, int* height, int* status);
 int mfr_jpeg_decode_batch(mfr_jpeg_decoder* dec, const unsigned char* const* data, const long long* lengths, int n, int rgb,
                           unsigned char* const* dst, int* status, void* stream);
+
+/* 16-bit depth PNG decode on the GPU (lib/datasets/utils.py:77-81, read_depth_image: cv2.imread(path, IMREAD_UNCHANGED)
+ * / 1000, then .float()). Supported: non-interlaced gray PNGs (colour type 0) of bit depth 8 or 16, any size within
+ * libpng's default limits and OpenCV's, any IDAT chunking and any deflate content, with only tEXt / zTXt / iTXt / tIME /
+ * pHYs besides the critical chunks. A valid file outside that set gives MFR_ERR_UNSUPPORTED (other colour types and
+ * depths, Adam7, PLTE / tRNS / sBIT / gAMA / iCCP / eXIf / APNG and unknown chunks); malformed structure gives
+ * MFR_ERR_ARG (signature, chunk lengths, IHDR fields, chunk order, a missing IEND, the zlib header, the CRC of IHDR or
+ * IEND). On the device, a file whose IDAT CRC, deflate data, Adler-32 or row filter types fail gets MFR_ERR_ARG: libpng
+ * refuses such files, so a caller that falls back to cv2 for it gets cv2's answer.
+ *   mfr_png_info: parses one file (HOST bytes): width, height, bit depth, or the file's error code.
+ *   mfr_png_decoder_create: a decoder for batches of up to max_images files holding up to max_bytes of zlib data and
+ *     max_pixels pixels in all. It owns pinned staging, device buffers and two events; not thread-safe.
+ *   mfr_png_batch_info: per file (HOST arrays) width / height / bit depth (0 unless supported) and status MFR_OK,
+ *     MFR_ERR_UNSUPPORTED or MFR_ERR_ARG, from the chunk structure alone.
+ *   mfr_png_decode_batch: decodes n files (HOST byte pointers and lengths) into dst[i] (DEVICE pointers; ignored for
+ *     files that are not MFR_OK in mfr_png_batch_info) asynchronously on `stream`; the bytes are copied into the
+ *     decoder's staging before it returns. out_kind 0: the samples as stored, uint8 or uint16 (native order) [h][w] =
+ *     cv2.imread(IMREAD_UNCHANGED); out_kind 1: float32 [h][w] = (float)((double)v / 1000). status: DEVICE int[n],
+ *     written on the stream: the header status of each file, then MFR_ERR_ARG where its data fails a device check.
+ *     MFR_ERR_ARG when the batch exceeds the decoder's capacity (nothing is enqueued). Successive calls on one decoder
+ *     may use different streams: each waits on the device for the previous call's kernels. */
+int mfr_png_info(const unsigned char* data, long long length, int* width, int* height, int* bit_depth);
+int mfr_png_decoder_create(int max_images, long long max_bytes, long long max_pixels, mfr_png_decoder** out);
+void mfr_png_decoder_destroy(mfr_png_decoder* dec);
+int mfr_png_batch_info(const unsigned char* const* data, const long long* lengths, int n, int* width, int* height, int* bit_depth,
+                       int* status);
+int mfr_png_decode_batch(mfr_png_decoder* dec, const unsigned char* const* data, const long long* lengths, int n, int out_kind,
+                         void* const* dst, int* status, void* stream);
 int mfr_resize_linear(const void* src, int src_is_u8, int src_w, int src_h, long long src_row_stride, int channels, float* dst,
                       int dst_w, int dst_h, int mode, float out_scale, int chw, void* stream);
 

@@ -28,9 +28,22 @@ int jpeg_decode_batch(JpegDecoder* dec, const unsigned char* const* data, const 
                       unsigned char* const* dst, int* status, cudaStream_t st);
 void jpeg_batch_info(const unsigned char* const* data, const long long* lengths, int n, int* width, int* height, int* status);
 int jpeg_host_decode(const unsigned char* data, size_t length, int rgb, unsigned char* dst, int width, int height);
+struct PngDecoder;
+int png_info(const unsigned char* data, size_t length, int* width, int* height, int* bit_depth);
+int png_decoder_create(int max_images, long long max_bytes, long long max_pixels, PngDecoder** out);
+void png_decoder_destroy(PngDecoder* dec);
+void png_batch_info(const unsigned char* const* data, const long long* lengths, int n, int* width, int* height, int* bit_depth,
+                    int* status);
+int png_decode_batch(PngDecoder* dec, const unsigned char* const* data, const long long* lengths, int n, int out_kind,
+                     void* const* dst, int* status, cudaStream_t st);
+int png_host_decode(const unsigned char* data, size_t length, int out_kind, void* dst, int width, int height);
+int png_decoder_kernel_ms(PngDecoder* dec, float* ms);
 }
 struct mfr_jpeg_decoder {
   mfr::JpegDecoder* d;
+};
+struct mfr_png_decoder {
+  mfr::PngDecoder* d;
 };
 namespace mfr {   // metrics.cu
 int pose_metrics(const double* q_gt, const double* t_gt, const double* q_est, const double* t_est, const double* K, int W, int H,
@@ -406,8 +419,17 @@ int mfr_host_jpeg_decode(const unsigned char* data, long long length, int rgb, u
   if (!data || length <= 0 || !dst) return MFR_ERR_ARG;
   return mfr::jpeg_host_decode(data, static_cast<size_t>(length), rgb, dst, width, height);
 }
+// lib/datasets/utils.py:77-81 (read_depth_image), serially on the CPU
+int mfr_host_png_decode(const unsigned char* data, long long length, int out_kind, void* dst, int width, int height) {
+  if (!data || length <= 0 || !dst) return MFR_ERR_ARG;
+  return mfr::png_host_decode(data, static_cast<size_t>(length), out_kind, dst, width, height);
+}
 
 // ------------------------------------------------------------------------------------------ debug probes
+int mfr_debug_png_kernel_ms(mfr_png_decoder* dec, float* ms) {
+  if (!dec || !ms) return MFR_ERR_ARG;
+  return mfr::png_decoder_kernel_ms(dec->d, ms);
+}
 float mfr_debug_time_conv(const float* x, int N, int H, int W, int Cin, const float* w, int Cout, int R,
                           int stride, float* out, int iters, int flags, const float* residual) {
   mfr::ConvGemmDesc d{};
@@ -506,6 +528,39 @@ int mfr_jpeg_decode_batch(mfr_jpeg_decoder* dec, const unsigned char* const* dat
                           unsigned char* const* dst, int* status, void* stream) {
   if (!dec) return MFR_ERR_ARG;
   return mfr::jpeg_decode_batch(dec->d, data, lengths, n, rgb, dst, status, static_cast<cudaStream_t>(stream));
+}
+// lib/datasets/utils.py:77-81: read_depth_image's cv2.imread(path, IMREAD_UNCHANGED) of a 16-bit depth PNG
+int mfr_png_info(const unsigned char* data, long long length, int* width, int* height, int* bit_depth) {
+  if (!data || length <= 0 || !width || !height || !bit_depth) return MFR_ERR_ARG;
+  return mfr::png_info(data, static_cast<size_t>(length), width, height, bit_depth);
+}
+// lib/datasets/utils.py:77-81
+int mfr_png_decoder_create(int max_images, long long max_bytes, long long max_pixels, mfr_png_decoder** out) {
+  if (!out) return MFR_ERR_ARG;
+  *out = nullptr;
+  mfr::PngDecoder* d = nullptr;
+  const int rc = mfr::png_decoder_create(max_images, max_bytes, max_pixels, &d);
+  if (rc != MFR_OK) return rc;
+  *out = new mfr_png_decoder{d};
+  return MFR_OK;
+}
+void mfr_png_decoder_destroy(mfr_png_decoder* dec) {
+  if (!dec) return;
+  mfr::png_decoder_destroy(dec->d);
+  delete dec;
+}
+// lib/datasets/utils.py:77-81
+int mfr_png_batch_info(const unsigned char* const* data, const long long* lengths, int n, int* width, int* height, int* bit_depth,
+                       int* status) {
+  if (n < 0 || (n > 0 && (!data || !lengths || !width || !height || !bit_depth || !status))) return MFR_ERR_ARG;
+  mfr::png_batch_info(data, lengths, n, width, height, bit_depth, status);
+  return MFR_OK;
+}
+// lib/datasets/utils.py:77-81: out_kind 0 = cv2.imread(IMREAD_UNCHANGED), 1 = that / 1000 as float32
+int mfr_png_decode_batch(mfr_png_decoder* dec, const unsigned char* const* data, const long long* lengths, int n, int out_kind,
+                         void* const* dst, int* status, void* stream) {
+  if (!dec) return MFR_ERR_ARG;
+  return mfr::png_decode_batch(dec->d, data, lengths, n, out_kind, dst, status, static_cast<cudaStream_t>(stream));
 }
 
 int mfr_pose_metrics(const double* q_gt, const double* t_gt, const double* q_est, const double* t_est, const double* K, int W,

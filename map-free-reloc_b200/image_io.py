@@ -1,7 +1,11 @@
 """Input path of the matcher plugins on the GPU (SURVEY §8(f) rank 1): JPEG decode and the reference's resize +
-normalise steps as CUDA kernels (libmfr_b200.so: mfr_jpeg_decode_batch / mfr_jpeg_decode, mfr_resize_linear).
+normalise steps as CUDA kernels (libmfr_b200.so: mfr_jpeg_decode_batch / mfr_jpeg_decode, mfr_png_decode_batch,
+mfr_resize_linear).
 
   decode_jpegs(items, rgb)                 = [cv2.imread(p, GRAYSCALE or COLOR) for p in items], one batched GPU decode
+  decode_pngs(items)                       = [cv2.imread(p, IMREAD_UNCHANGED) for p in items], one batched GPU decode
+  read_depth_image(path) / read_depth_images(paths)
+                                           = lib/datasets/utils.py:77-81 (IMREAD_UNCHANGED / 1000, .float()) -> CUDA [h, w] / [B, h, w]
   read_image(path, resize, resize_float)   = SuperGlue/models/utils.py:263-285 (gray, cv2.resize, / 255) -> CUDA [h, w]
   read_color_image(path, resize)           = lib/datasets/utils.py:58-75 (RGB, uint8 cv2.resize, / 255)   -> CUDA [3, h, w]
   PairMatcher                              = match / match_scene / match_arrays of the LoFTR and SuperGlue plugins
@@ -9,7 +13,9 @@ normalise steps as CUDA kernels (libmfr_b200.so: mfr_jpeg_decode_batch / mfr_jpe
 JPEG files are decoded on the GPU with libjpeg's arithmetic (csrc/jpeg.cuh): the bytes equal cv2.imread's (Exif
 orientation included) for baseline / extended-sequential Huffman files, gray or YCbCr 4:4:4 / 4:2:2 / 4:2:0. Other files
 (progressive, 4:1:1, CMYK, ... and other formats) are decoded by OpenCV on the host and uploaded as uint8, so every
-loader returns cv2's pixels. The resize kernels restate cv2.resize(INTER_LINEAR) for both of its arithmetic paths
+loader returns cv2's pixels. Gray 8- / 16-bit PNGs (the depth maps) are inflated, unfiltered and converted on the GPU
+(csrc/png.cuh); other PNGs, and files the device rejects (bad CRC, deflate data or Adler-32), go to OpenCV on the host.
+The resize kernels restate cv2.resize(INTER_LINEAR) for both of its arithmetic paths
 (tests/test_image_io_gpu.py: float path within 1e-6 of cv2, uint8 path bit-exact)."""
 import ctypes
 import os
@@ -51,13 +57,14 @@ def decode_jpeg(data, rgb=False, device=None):
     return out
 
 
-class _JpegDecoder:
-    """A batch decoder handle (mfr_jpeg_decoder_create) and its capacity; one per device, grown on demand."""
+class _Decoder:
+    """A batch decoder handle (mfr_jpeg_decoder_create / mfr_png_decoder_create) and its capacity."""
 
-    def __init__(self, images, nbytes, pixels):
-        self.caps = (images, nbytes, pixels)
+    def __init__(self, fmt, images, nbytes, pixels):
+        self.fmt, self.caps = fmt, (images, nbytes, pixels)
         h = ctypes.c_void_p()
-        _lib.check(_lib.load().mfr_jpeg_decoder_create(images, nbytes, pixels, ctypes.byref(h)), "mfr_jpeg_decoder_create")
+        _lib.check(getattr(_lib.load(), f"mfr_{fmt}_decoder_create")(images, nbytes, pixels, ctypes.byref(h)),
+                   f"mfr_{fmt}_decoder_create")
         self.h = h
 
     def fits(self, images, nbytes, pixels):
@@ -66,7 +73,7 @@ class _JpegDecoder:
     def __del__(self):
         try:
             if getattr(self, "h", None):
-                _lib.load().mfr_jpeg_decoder_destroy(self.h)  # waits for the decoder's last batch
+                getattr(_lib.load(), f"mfr_{self.fmt}_decoder_destroy")(self.h)  # waits for the decoder's last batch
                 self.h = None
         except Exception:
             pass                                          # interpreter shutdown: the module may be gone
@@ -75,14 +82,16 @@ class _JpegDecoder:
 _DECODERS = {}
 
 
-def _decoder(dev, images, nbytes, pixels):
-    d = _DECODERS.get(dev.index)
+def _decoder(fmt, dev, images, nbytes, pixels):
+    """The decoder of format `fmt` ("jpeg" or "png") on `dev`, one per (format, device), grown on demand."""
+    key = (fmt, dev.index)
+    d = _DECODERS.get(key)
     if d is None or not d.fits(images, nbytes, pixels):
         old = d.caps if d is not None else (0, 0, 0)
-        _DECODERS.pop(dev.index, None)
+        _DECODERS.pop(key, None)
         with torch.cuda.device(dev):
-            d = _DECODERS[dev.index] = _JpegDecoder(max(images, old[0], 16), max(nbytes, old[1], 1 << 22),
-                                                    max(pixels, old[2], 1 << 22))
+            d = _DECODERS[key] = _Decoder(fmt, max(images, old[0], 16), max(nbytes, old[1], 1 << 22),
+                                          max(pixels, old[2], 1 << 22))
     return d
 
 
@@ -127,7 +136,7 @@ def decode_jpegs(items, rgb=False, device=None):
             pixels += -(-w[i] // 16) * 16 * (-(-h[i] // 16) * 16)
     if nbytes:
         status = torch.empty(n, dtype=torch.int32, device=dev)
-        dec = _decoder(dev, n, nbytes, pixels)
+        dec = _decoder("jpeg", dev, n, nbytes, pixels)
         with torch.cuda.device(dev):
             _lib.check(l.mfr_jpeg_decode_batch(dec.h, ptrs, lens, n, int(rgb), dst, _lib.ptr(status), _lib.cur_stream()),
                        "mfr_jpeg_decode_batch")
@@ -138,6 +147,126 @@ def decode_jpegs(items, rgb=False, device=None):
         if ok[i] != 0:
             outs[i] = _host_decode(items[i], rgb, dev)
     return outs
+
+
+def _png_batch(datas, kind, dev, dst_of):
+    """One mfr_png_decode_batch call over the files `datas` (bytes). dst_of(i, w, h, depth) returns the CUDA tensor file
+    i is decoded into (or None to skip it). Returns (tensors, per-file status: 0 where the GPU decoded the file)."""
+    n = len(datas)
+    l = _lib.load()
+    ptrs = (ctypes.c_char_p * n)(*datas)
+    lens = (ctypes.c_longlong * n)(*[len(d) for d in datas])
+    w, h, bd, st = (ctypes.c_int * n)(), (ctypes.c_int * n)(), (ctypes.c_int * n)(), (ctypes.c_int * n)()
+    _lib.check(l.mfr_png_batch_info(ptrs, lens, n, w, h, bd, st), "mfr_png_batch_info")
+    outs = [None] * n
+    dst = (ctypes.c_void_p * n)()
+    nbytes = pixels = 0
+    for i in range(n):
+        if st[i] == 0:
+            outs[i] = dst_of(i, w[i], h[i], bd[i])
+        if outs[i] is not None:
+            dst[i] = outs[i].data_ptr()
+            nbytes += len(datas[i])
+            pixels += w[i] * h[i]
+        else:
+            st[i] = 1
+    if not nbytes:
+        return outs, [1] * n
+    status = torch.empty(n, dtype=torch.int32, device=dev)
+    dec = _decoder("png", dev, n, nbytes, pixels)
+    with torch.cuda.device(dev):
+        _lib.check(l.mfr_png_decode_batch(dec.h, ptrs, lens, n, kind, dst, _lib.ptr(status), _lib.cur_stream()),
+                   "mfr_png_decode_batch")
+    return outs, status.cpu().tolist()
+
+
+def _host_png(item, dev, depth_kind):
+    """cv2.imread(IMREAD_UNCHANGED) of a file or bytes, uploaded (None if OpenCV cannot read it); with depth_kind,
+    read_depth_image's float32 v / 1000."""
+    import cv2
+    if isinstance(item, (bytes, bytearray, memoryview)):
+        im = cv2.imdecode(np.frombuffer(bytes(item), np.uint8), cv2.IMREAD_UNCHANGED)
+    else:
+        im = cv2.imread(str(item), cv2.IMREAD_UNCHANGED)
+    if im is None:
+        return None
+    t = torch.from_numpy(im / 1000).float() if depth_kind else torch.from_numpy(np.ascontiguousarray(im))
+    return t.to(dev)
+
+
+def _readable(items):
+    """(bytes or None per item): a path that does not exist reads as None, as cv2.imread returns None for it."""
+    out = []
+    for x in items:
+        try:
+            out.append(_bytes(x))
+        except OSError:
+            out.append(None)
+    return out
+
+
+def decode_pngs(items, device=None):
+    """PNG files (bytes or paths) -> list of CUDA tensors, each cv2.imread(p, IMREAD_UNCHANGED) (torch.uint16 or uint8
+    [h, w] for the gray 8- / 16-bit files the GPU decoder takes), from one decoder call on the current stream. Other
+    files, and files the device rejects, are decoded by OpenCV on the host in their place in the list (None where
+    OpenCV cannot read them either)."""
+    dev = _device(device)
+    datas = _readable(items)
+    ok_idx = [i for i, d in enumerate(datas) if d]
+    outs = [None] * len(items)
+    if ok_idx:
+        def alloc(i, w, h, depth):
+            return torch.empty((h, w), dtype=torch.uint16 if depth == 16 else torch.uint8, device=dev)
+        got, st = _png_batch([datas[i] for i in ok_idx], 0, dev, alloc)
+        for i, g, s in zip(ok_idx, got, st):
+            outs[i] = g if s == 0 else None
+    for i in range(len(items)):
+        if outs[i] is None and datas[i]:
+            outs[i] = _host_png(datas[i], dev, False)
+    return outs
+
+
+def read_depth_image(path, device=None):
+    """lib/datasets/utils.py:77-81: torch.from_numpy(cv2.imread(path, IMREAD_UNCHANGED) / 1000).float() as a CUDA
+    float32 [h, w], bit for bit, or None if the file cannot be read. Gray 8- / 16-bit PNGs decode on the GPU; other
+    files, and files the device rejects, are read by OpenCV on the host with that same expression."""
+    out = read_depth_images([path], device)
+    return None if out is None else out[0]
+
+
+def read_depth_images(paths, device=None):
+    """[read_depth_image(p) for p in paths] stacked into one CUDA float32 [B, h, w], from one decoder call whose kernels
+    write each map straight into its slice (the form RelocPipeline.set_map / submit_device_queries take). The maps
+    must share one size; None if any file cannot be read."""
+    dev = _device(device)
+    datas = _readable(paths)
+    if not datas or any(d is None for d in datas):
+        return None
+    l = _lib.load()
+    shapes = []
+    for d in datas:
+        w, h, bd = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+        rc = l.mfr_png_info(d, len(d), ctypes.byref(w), ctypes.byref(h), ctypes.byref(bd))
+        shapes.append((h.value, w.value) if rc == 0 else None)
+    known = [s for s in shapes if s]
+    out = None
+    if known:
+        hw = known[0]
+        out = torch.empty((len(datas), *hw), dtype=torch.float32, device=dev)
+        _, st = _png_batch(datas, 1, dev, lambda i, w, h, depth: out[i] if (h, w) == hw else None)
+    else:
+        st = [1] * len(datas)
+    for i, s in enumerate(st):
+        if s != 0:
+            im = _host_png(datas[i], dev, True)
+            if im is None:
+                return None
+            if out is None:
+                out = torch.empty((len(datas), *im.shape), dtype=torch.float32, device=dev)
+            if tuple(im.shape) != tuple(out.shape[1:]):
+                raise ValueError(f"read_depth_images: depth map {i} is {tuple(im.shape)}, not {tuple(out.shape[1:])}")
+            out[i] = im
+    return out
 
 
 def resize_linear(img, size, mode, out_scale=1.0, chw=False):

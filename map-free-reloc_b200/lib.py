@@ -133,6 +133,12 @@ SIGNATURES = {
     "mfr_jpeg_decoder_destroy": (None, [c_vp]),
     "mfr_jpeg_batch_info": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp]),
     "mfr_jpeg_decode_batch": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp]),
+    "mfr_png_info": (c_int, [c_vp, c_ll, c_vp, c_vp, c_vp]),
+    "mfr_png_decoder_create": (c_int, [c_int, c_ll, c_ll, c_pp]),
+    "mfr_png_decoder_destroy": (None, [c_vp]),
+    "mfr_png_batch_info": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp]),
+    "mfr_debug_png_kernel_ms": (c_int, [c_vp, c_vp]),
+    "mfr_png_decode_batch": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_vp, c_vp]),
     "mfr_resize_linear": (c_int, [c_vp, c_int, c_int, c_int, c_ll, c_int, c_vp, c_int, c_int, c_int, c_float, c_int, c_vp]),
     "mfr_pose_metrics": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp]),
     "mfr_encoder_tail": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_ll, c_vp, c_int, c_vp]),
@@ -146,6 +152,7 @@ SIGNATURES = {
     "mfr_host_ransac_satisfied": (c_int, [ctypes.c_double, c_int, c_int, c_int, c_int, c_int]),
     "mfr_host_magsac_loss": (c_int, [ctypes.c_double, ctypes.c_double, c_vp, c_vp]),
     "mfr_host_jpeg_decode": (c_int, [c_vp, c_ll, c_int, c_vp, c_int, c_int]),
+    "mfr_host_png_decode": (c_int, [c_vp, c_ll, c_int, c_vp, c_int, c_int]),
 }
 
 

@@ -314,7 +314,13 @@ void mfr_pose_solver_destroy(mfr_pose_solver* s);
  *   "Rd", "td"    double [max_pairs][9] / [max_pairs][3]: the final E-mat pose
  *   "Xw", "uv", "vidx" PnP's compacted depth-valid points: double [max_pairs][max_pts_per_pair][3] (camera 0), float
  *                 [..][2] (kpts1), int [..] (index within the pair)
- *   "nvalid", "dmin" int [max_pairs] compacted count; float bits [max_pairs] of max(min(depth0), 0) */
+ *   "nvalid", "dmin" int [max_pairs] compacted count; float bits [max_pairs] of max(min(depth0), 0)
+ *   "X1w", "dmin1" Procrustes: the compacted points lifted through depth1, double [max_pairs][max_pts_per_pair][3]
+ *                 (camera 1; "Xw" holds their camera-0 partners); float bits [max_pairs] of max(min(depth1), 0)
+ *   "icp_state"   double [max_pairs][18] of the last mfr_icp_refine: R [9], t [3] (source -> target), fitness, rmse,
+ *                 stopped flag, correspondences of the last association, valid source / target points. A call with
+ *                 max_iterations = k leaves the pose after k updates (fewer if it converged) and the association at
+ *                 that pose. Exists after the first mfr_icp_refine call (MFR_ERR_ARG before). */
 int mfr_pose_solver_debug_tensor(mfr_pose_solver* s, const char* name, void** ptr, long long* words);
 
 /* EssentialMatrixSolver.estimate_pose (pose_solver.py:29-61): cv.findEssentialMat(USAC_MAGSAC) +
@@ -412,6 +418,9 @@ int mfr_procrustes_ransac(mfr_pose_solver* s, const float* kpts0, const float* k
  * They are NOT a CPU fallback: no product entry point calls them.
  *   five_point : x0, x1 double[5][2] normalised points, E_out double[10][9]; returns #solutions
  *   p3p        : X double[3][3] points, f double[3][3] unit bearings, R_out [4][9], t_out [4][3]
+ *   kabsch     : the least-squares rigid transform of the Procrustes / ICP kernels (q ~ R p + t) from the moment sums
+ *                n, sum_p [3], sum_q [3], sum_pq [9] (row-major sum p q^T); R_out [9], t_out [3]; returns 1, or 0 when
+ *                n < 3 or the points are coincident or collinear
  *   poly roots : coef[0..deg] ascending, deg <= 10; returns #real roots (ascending)
  *   ransac_satisfied : 1 iff the escalation stops after a round at `budget` that found n_inliers of n_points
  *                (the rule of mfr_emat_ransac_escalate, cap max_budget, minimal sample sample_size), else 0
@@ -424,6 +433,8 @@ int mfr_procrustes_ransac(mfr_pose_solver* s, const float* kpts0, const float* k
  *                status                                                                                         */
 int mfr_host_five_point(const double* x0, const double* x1, double* E_out);
 int mfr_host_p3p(const double* X, const double* f, double* R_out, double* t_out);
+int mfr_host_kabsch(double n, const double* sum_p, const double* sum_q, const double* sum_pq, double* R_out,
+                    double* t_out);
 int mfr_host_poly_real_roots(const double* coef, int deg, double* roots);
 int mfr_host_decompose_essential(const double* E, double* R1, double* R2, double* t);
 int mfr_host_ransac_satisfied(double confidence, int n_inliers, int n_points, int budget, int max_budget,
@@ -471,8 +482,12 @@ int mfr_stem_conv7x7(const float* img, const float* w, const float* bias, void* 
 /* ProcrustesSolver's ICP refinement (PROCRUSTES.REFINE, pose_solver.py:289-315: Open3D registration_icp, point-to-point,
  * correspondence radius max_corr_dist, criteria relative_fitness / relative_rmse / max_iterations = 1e-4 / 1e-4 / 30 in the
  * reference) of the poses (R_in, t_in) [P][9] / [P][3] over the FULL clouds of both depth maps (every pixel with depth > 0),
- * device float [P][H][W]. Nearest neighbours are exact within the radius (bounded window search in the organised target
- * cloud). n_inliers = int(fitness * valid target points), the reference's return value (pose_solver.py:319). */
+ * device float [P][H][W]. Nearest neighbours are exact within the radius (window search in the organised target cloud,
+ * clamped to 96 pixels and widened when a nearer point could lie beyond the clamp) for every target point at least
+ * 2 max_corr_dist + 1 mm in front of camera 1. The per-pass sums are added in a fixed order over chunks of the frame, so a
+ * pair's result is bit for bit the same alone, in any batch, on any GPU and in a graph replay. The first call at a
+ * larger H x W allocates scratch: make it before capturing the call in a CUDA graph.
+ * n_inliers = int(fitness * valid target points), the reference's return value (pose_solver.py:319). */
 int mfr_icp_refine(mfr_pose_solver* s, const float* depth0, const float* depth1, int H, int W, int P, const float* K0,
                    const float* K1, const float* R_in, const float* t_in, float max_corr_dist, int max_iterations,
                    float relative_fitness, float relative_rmse, float* R, float* t, int* n_inliers, void* stream);

@@ -399,6 +399,9 @@ int mfr_host_p3p(const double* X, const double* f, double* R_out, double* t_out)
   return mfr::geo::p3p(reinterpret_cast<const double(*)[3]>(X), reinterpret_cast<const double(*)[3]>(f),
                        reinterpret_cast<double(*)[9]>(R_out), reinterpret_cast<double(*)[3]>(t_out));
 }
+int mfr_host_kabsch(double n, const double* sum_p, const double* sum_q, const double* sum_pq, double* R, double* t) {
+  return mfr::geo::kabsch_from_sums(n, sum_p, sum_q, sum_pq, R, t) ? 1 : 0;
+}
 int mfr_host_poly_real_roots(const double* coef, int deg, double* roots) {
   if (deg < 1 || deg > mfr::geo::kMaxDeg) return -1;
   return mfr::geo::poly_real_roots(coef, deg, roots);

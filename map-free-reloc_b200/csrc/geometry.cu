@@ -1131,45 +1131,7 @@ __global__ void __launch_bounds__(256) pnp_final_kernel(
 // RANSAC over 3-point Kabsch alignments, refit on the inliers. (The reference delegates this to
 // Open3D's registration_ransac_based_on_correspondence.)
 // ================================================================================================
-// R, t minimising sum |R p + t - q|^2 from the moment sums (n, sum p, sum q, sum p q^T)
-__device__ inline bool kabsch_from_sums(double n, const double* sp, const double* sq, const double* spq,
-                                        double* R, double* t) {
-  if (n < 3.0) return false;
-  double pb[3], qb[3], Hm[9];
-  for (int k = 0; k < 3; ++k) { pb[k] = sp[k] / n; qb[k] = sq[k] / n; }
-  for (int a = 0; a < 3; ++a)
-    for (int b = 0; b < 3; ++b) Hm[3 * a + b] = spq[3 * a + b] - n * pb[a] * qb[b];
-  double M[9], V[9], w[3];
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) M[3 * i + j] = Hm[i] * Hm[j] + Hm[3 + i] * Hm[3 + j] + Hm[6 + i] * Hm[6 + j];  // H^T H
-  jacobi_eig3(M, V, w);
-  int o[3] = {0, 1, 2};
-  for (int a = 0; a < 2; ++a)
-    for (int b = a + 1; b < 3; ++b)
-      if (w[o[b]] > w[o[a]]) { const int tmp = o[a]; o[a] = o[b]; o[b] = tmp; }
-  double v0[3], v1[3], v2[3], u0[3], u1[3], u2[3];
-  for (int k = 0; k < 3; ++k) { v0[k] = V[3 * k + o[0]]; v1[k] = V[3 * k + o[1]]; }
-  cross3(v0, v1, v2);
-  mat3_vec(Hm, v0, u0);
-  mat3_vec(Hm, v1, u1);
-  const double n0 = norm3(u0);
-  if (!(n0 > 1e-12)) return false;
-  for (int k = 0; k < 3; ++k) u0[k] /= n0;
-  const double d01 = dot3(u0, u1);
-  for (int k = 0; k < 3; ++k) u1[k] -= d01 * u0[k];
-  const double n1 = norm3(u1);
-  if (!(n1 > 1e-12 * n0)) return false;     // collinear sample
-  for (int k = 0; k < 3; ++k) u1[k] /= n1;
-  cross3(u0, u1, u2);
-  // H = U S V^T  with U's columns u_i, V's columns v_i (both right-handed)  =>  R = V U^T
-  for (int a = 0; a < 3; ++a)
-    for (int b = 0; b < 3; ++b) R[3 * a + b] = v0[a] * u0[b] + v1[a] * u1[b] + v2[a] * u2[b];
-  double Rp[3];
-  mat3_vec(R, pb, Rp);
-  for (int k = 0; k < 3; ++k) t[k] = qb[k] - Rp[k];
-  return true;
-}
-
+// kabsch_from_sums (geometry_solvers.cuh, host hook mfr_host_kabsch): R, t from the moment sums of the inliers
 __global__ void __launch_bounds__(1024) procrustes_prepare_kernel(
     const float* __restrict__ kpts0, const float* __restrict__ kpts1, const int* __restrict__ offsets,
     const float* __restrict__ K0s, const float* __restrict__ K1s, const float* __restrict__ depth0,
@@ -1390,11 +1352,18 @@ __global__ void __launch_bounds__(256) procrustes_final_kernel(
 // ICP refinement of the Procrustes pose over the FULL depth clouds (pose_solver.py:289-315: Open3D registration_icp,
 // point-to-point, max correspondence distance = PROCRUSTES.MAX_CORR_DIST, <= 30 iterations, relative fitness / rmse 1e-4).
 // Both clouds are organised (one 3-D point per valid depth pixel), so the nearest neighbour of a transformed source point
-// inside the correspondence radius D is found EXACTLY by a bounded window search around its projection into image 1: a
-// target point within D of the query lies within ceil(D (f + |u - c|) / (z - D)) pixels of it on each axis. No k-d tree.
+// P inside the correspondence radius D is found EXACTLY by a window search around its projection into image 1: a target
+// point within D of P lies within r = ceil(D (f + |u - c|) / (z - D)) + 1 pixels of it on each axis (the + 1 covers the
+// rounding of the projection to a pixel and the float32 inverse of K). The window is clamped to kIcpMaxRadius; when the
+// clamp cuts it, a point outside the clamped window is at least delta* = m z / (f + |u - c| + m), m = kIcpMaxRadius - 1,
+// away from P (the same inequality solved for the distance), so the unclamped window is scanned only when no match
+// closer than delta* was found. Source points with z <= D + 1 mm in camera 1 are not associated: exact as long as no
+// target point is nearer than 2 D + 1 mm to camera 1. No k-d tree.
 // State per pair (double[kIcpState]): [0..8] R, [9..11] t (current source -> target transform), [12] fitness, [13] rmse,
 // [14] converged flag, [15] correspondences, [16] valid source points, [17] valid target points.
-// Accumulator per pair (double[17]): n, sum p [3], sum q [3], sum p q^T [9], sum |p - q|^2  (p = transformed source point).
+// Partial sums per pair and chunk of kIcpChunk source pixels (double[17]): n, sum p [3], sum q [3], sum p q^T [9],
+// sum |p - q|^2 (p = transformed source point). The chunks depend on H W only, and icp_update_kernel adds them in chunk
+// order, so a pair's result does not depend on the batch it runs in or on the GPU's SM count.
 // ================================================================================================
 __global__ void f32_to_f64_kernel(const float* __restrict__ a, double* __restrict__ b, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1403,6 +1372,7 @@ __global__ void f32_to_f64_kernel(const float* __restrict__ a, double* __restric
 
 constexpr int kIcpState = 18;
 constexpr int kIcpMaxRadius = 96;
+constexpr int kIcpChunk = 512;        // source pixels per association block (2 per thread)
 
 __global__ void icp_count_kernel(const float* __restrict__ depth0, const float* __restrict__ depth1, int hw,
                                  const double* __restrict__ Rd, const double* __restrict__ td, double* __restrict__ state) {
@@ -1419,7 +1389,7 @@ __global__ void icp_count_kernel(const float* __restrict__ depth0, const float* 
   if (threadIdx.x == 0) {
     int a = 0, b = 0;
     for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) { a += s0[w]; b += s1[w]; }
-    atomicAdd(state + pair * kIcpState + 16, static_cast<double>(a));
+    atomicAdd(state + pair * kIcpState + 16, static_cast<double>(a));   // integer-valued: exact in any order
     atomicAdd(state + pair * kIcpState + 17, static_cast<double>(b));
     if (blockIdx.x == 0) {
       for (int k = 0; k < 9; ++k) state[pair * kIcpState + k] = Rd[9 * pair + k];
@@ -1428,9 +1398,26 @@ __global__ void icp_count_kernel(const float* __restrict__ depth0, const float* 
   }
 }
 
+// nearest target point to P with squared distance < best over pixels [u_lo, u_hi] x [v_lo, v_hi] of depth1 (row-major
+// order, first on ties); z1 outside (zlo, zhi) (which also holds invalid depth 0) cannot be within D
+__device__ __forceinline__ void icp_scan(const float* __restrict__ d1, int W, const float* Ki1, const double* P, float zlo,
+                                         float zhi, int u_lo, int u_hi, int v_lo, int v_hi, double& best, double* Q) {
+  for (int v = v_lo; v <= v_hi; ++v)
+    for (int u = u_lo; u <= u_hi; ++u) {
+      const float z1 = d1[v * W + u];
+      if (!(z1 > zlo && z1 < zhi)) continue;
+      double Y[3];
+      backproject(Ki1, u, v, z1, Y);
+      const double dx = Y[0] - P[0], dy = Y[1] - P[1], dz = Y[2] - P[2];
+      const double dd = dx * dx + dy * dy + dz * dz;
+      if (dd < best) { best = dd; Q[0] = Y[0]; Q[1] = Y[1]; Q[2] = Y[2]; }
+    }
+}
+
 __global__ void __launch_bounds__(256) icp_assoc_kernel(const float* __restrict__ depth0, const float* __restrict__ depth1,
                                                         int H, int W, const float* __restrict__ K0s, const float* __restrict__ K1s,
-                                                        float max_dist, const double* __restrict__ state, double* __restrict__ acc) {
+                                                        float max_dist, const double* __restrict__ state,
+                                                        double* __restrict__ partial) {
   const int pair = blockIdx.y;
   const double* st = state + pair * kIcpState;
   if (st[14] != 0.0 || !(st[0] == st[0])) return;                 // converged (or no initial pose): nothing to do
@@ -1449,36 +1436,44 @@ __global__ void __launch_bounds__(256) icp_assoc_kernel(const float* __restrict_
   const float* d1 = depth1 + static_cast<size_t>(pair) * H * W;
   const double D = max_dist, D2 = D * D;
   const double fx = s_K1[0], fy = s_K1[4], cx = s_K1[2], cy = s_K1[5];
+  const double rmax = static_cast<double>(W + H);                  // a radius that covers the whole image
   double a[17];
   for (int k = 0; k < 17; ++k) a[k] = 0.0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < H * W; i += gridDim.x * blockDim.x) {
+  const int i_end = min(H * W, (blockIdx.x + 1) * kIcpChunk);
+  for (int i = blockIdx.x * kIcpChunk + threadIdx.x; i < i_end; i += blockDim.x) {
     const float z0 = d0[i];
     if (!(z0 > 0.f)) continue;
     double X[3], P[3];
     backproject(s_Ki0, i % W, i / W, z0, X);
     mat3_vec(R, X, P);
     for (int k = 0; k < 3; ++k) P[k] += t[k];
-    if (!(P[2] > D + 1e-3)) continue;                              // behind / too close to camera 1: no target point can be within D
+    if (!(P[2] > D + 1e-3)) continue;                              // behind / too close to camera 1 (see above)
     const double up = fx * P[0] / P[2] + cx, vp = fy * P[1] / P[2] + cy;
     const double zr = 1.0 / (P[2] - D);
-    const int ru = min(kIcpMaxRadius, static_cast<int>(ceil(D * (fx + fabs(up - cx)) * zr)) + 1);
-    const int rv = min(kIcpMaxRadius, static_cast<int>(ceil(D * (fy + fabs(vp - cy)) * zr)) + 1);
-    const int uc = static_cast<int>(floor(up + 0.5)), vc = static_cast<int>(floor(vp + 0.5));
-    const int u_lo = max(0, uc - ru), u_hi = min(W - 1, uc + ru), v_lo = max(0, vc - rv), v_hi = min(H - 1, vc + rv);
+    const double au = fabs(up - cx), av = fabs(vp - cy);
+    const double ru_full = fmin(rmax, ceil(D * (fx + au) * zr) + 1.0);
+    const double rv_full = fmin(rmax, ceil(D * (fy + av) * zr) + 1.0);
+    const int ru = min(kIcpMaxRadius, static_cast<int>(ru_full)), rv = min(kIcpMaxRadius, static_cast<int>(rv_full));
+    // far outside the image the window is empty either way: clamp before the conversion to int
+    const int uc = static_cast<int>(floor(fmin(fmax(up, -rmax - 2.0), W + rmax + 2.0) + 0.5));
+    const int vc = static_cast<int>(floor(fmin(fmax(vp, -rmax - 2.0), H + rmax + 2.0) + 0.5));
     double best = D2, Q[3] = {0, 0, 0};
-    bool found = false;
-    const float zlo = static_cast<float>(P[2] - D), zhi = static_cast<float>(P[2] + D);
-    for (int v = v_lo; v <= v_hi; ++v)
-      for (int u = u_lo; u <= u_hi; ++u) {
-        const float z1 = d1[v * W + u];
-        if (!(z1 > zlo && z1 < zhi)) continue;                     // also skips invalid (0) depth
-        double Y[3];
-        backproject(s_Ki1, u, v, z1, Y);
-        const double dx = Y[0] - P[0], dy = Y[1] - P[1], dz = Y[2] - P[2];
-        const double dd = dx * dx + dy * dy + dz * dz;
-        if (dd < best) { best = dd; Q[0] = Y[0]; Q[1] = Y[1]; Q[2] = Y[2]; found = true; }
+    // conservative float32 bounds of the depth band (P.z - D, P.z + D)
+    const float zlo = __double2float_rd(P[2] - D), zhi = __double2float_ru(P[2] + D);
+    icp_scan(d1, W, s_Ki1, P, zlo, zhi, max(0, uc - ru), min(W - 1, uc + ru), max(0, vc - rv), min(H - 1, vc + rv), best, Q);
+    if (ru < ru_full || rv < rv_full) {
+      constexpr double m = kIcpMaxRadius - 1;
+      double dstar = D;
+      if (ru < ru_full) dstar = fmin(dstar, m * P[2] / (fx + au + m));
+      if (rv < rv_full) dstar = fmin(dstar, m * P[2] / (fy + av + m));
+      dstar *= 1.0 - 1e-12;
+      if (!(best < dstar * dstar)) {
+        const int RU = static_cast<int>(ru_full), RV = static_cast<int>(rv_full);
+        icp_scan(d1, W, s_Ki1, P, zlo, zhi, max(0, uc - RU), min(W - 1, uc + RU), max(0, vc - RV), min(H - 1, vc + RV),
+                 best, Q);
       }
-    if (found) {
+    }
+    if (best < D2) {
       a[0] += 1.0;
       for (int r = 0; r < 3; ++r) {
         a[1 + r] += P[r]; a[4 + r] += Q[r];
@@ -1488,18 +1483,29 @@ __global__ void __launch_bounds__(256) icp_assoc_kernel(const float* __restrict_
     }
   }
   block_sum_256<17>(a, sh_red);
-  if (threadIdx.x == 0 && a[0] > 0.0)
-    for (int k = 0; k < 17; ++k) atomicAdd(acc + pair * 17 + k, a[k]);
+  if (threadIdx.x == 0) {
+    double* out = partial + (static_cast<size_t>(pair) * gridDim.x + blockIdx.x) * 17;
+    for (int k = 0; k < 17; ++k) out[k] = a[k];
+  }
 }
 
-// one thread per pair: fitness / rmse of the association just computed, convergence test against the previous one
-// (Open3D RegistrationICP: |d fitness| < rel_fitness and |d rmse| < rel_rmse), Kabsch update composed onto the transform
-__global__ void icp_update_kernel(double* __restrict__ state, double* __restrict__ acc, int P, int iter, double rel_fit, double rel_rmse) {
-  const int pair = blockIdx.x * blockDim.x + threadIdx.x;
+// one warp per pair: the association's sums (chunk partials added in a fixed order), its fitness / rmse, the convergence
+// test against the previous association (Open3D RegistrationICP: |d fitness| < rel_fitness and |d rmse| < rel_rmse),
+// the Kabsch update composed onto the transform
+__global__ void __launch_bounds__(64) icp_update_kernel(double* __restrict__ state, const double* __restrict__ partial,
+                                                        int chunks, int P, int iter, double rel_fit, double rel_rmse) {
+  const int pair = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (pair >= P) return;
   double* st = state + pair * kIcpState;
-  double* a = acc + pair * 17;
   if (st[14] != 0.0 || !(st[0] == st[0])) return;
+  double a[17];
+  for (int k = 0; k < 17; ++k) a[k] = 0.0;
+  const double* pp = partial + static_cast<size_t>(pair) * chunks * 17;
+  for (int c = lane; c < chunks; c += 32)
+    for (int k = 0; k < 17; ++k) a[k] += pp[static_cast<size_t>(c) * 17 + k];
+  for (int k = 0; k < 17; ++k)
+    for (int o = 16; o > 0; o >>= 1) a[k] += __shfl_down_sync(0xffffffffu, a[k], o);
+  if (lane != 0) return;
   const double n = a[0];
   const double fit = st[16] > 0.0 ? n / st[16] : 0.0, rmse = n > 0.0 ? sqrt(a[16] / n) : 0.0;
   const bool conv = iter > 0 && fabs(st[12] - fit) < rel_fit && fabs(st[13] - rmse) < rel_rmse;
@@ -1517,7 +1523,6 @@ __global__ void icp_update_kernel(double* __restrict__ state, double* __restrict
       st[14] = 1.0;
     }
   }
-  for (int k = 0; k < 17; ++k) a[k] = 0.0;
 }
 
 __global__ void icp_finish_kernel(const double* __restrict__ state, int P, float* __restrict__ Rf, float* __restrict__ tf,
@@ -1572,6 +1577,8 @@ struct PoseSolver {
   int *active = nullptr, *budgets = nullptr;   // CONFIDENCE escalation: pair still solving / budget of its outputs
   unsigned int *dmin = nullptr, *dmin1 = nullptr;
   double* icp_state = nullptr;   // ICP refinement scratch (allocated on first use)
+  double* icp_partial = nullptr; // ICP chunk partial sums [max_pairs][icp_chunks][17] (allocated / grown on use)
+  int icp_chunks = 0;
   size_t total_pts;
 };
 
@@ -1616,6 +1623,7 @@ void pose_solver_destroy(PoseSolver* s) {
   if (!s) return;
   cudaFree(s->results); cudaFree(s->lo_out); cudaFree(s->pts_norm); cudaFree(s->Rd); cudaFree(s->td); cudaFree(s->Xw); cudaFree(s->uv);
   cudaFree(s->vidx); cudaFree(s->nvalid); cudaFree(s->active); cudaFree(s->budgets); cudaFree(s->dmin); cudaFree(s->dmin1); cudaFree(s->X1w); cudaFree(s->icp_state);
+  cudaFree(s->icp_partial);
   delete s;
 }
 
@@ -1637,9 +1645,13 @@ int pose_solver_debug_tensor(PoseSolver* s, const char* name, void** ptr, long l
       {"vidx", s->vidx, 4 * T},
       {"nvalid", s->nvalid, 4 * P},
       {"dmin", s->dmin, 4 * P},
+      {"X1w", s->X1w, 8 * 3 * T},
+      {"dmin1", s->dmin1, 4 * P},
+      {"icp_state", s->icp_state, 8 * kIcpState * P},
   };
   for (const auto& b : bufs)
     if (strcmp(b.name, name) == 0) {
+      if (!b.p) return MFR_ERR_ARG;     // icp_state: no mfr_icp_refine call yet
       *ptr = b.p;
       *words = b.bytes / 4;
       return MFR_OK;
@@ -1831,24 +1843,31 @@ int procrustes_ransac(PoseSolver* s, const float* kpts0, const float* kpts1, con
 int icp_refine(PoseSolver* s, const float* depth0, const float* depth1, int H, int W, int P, const float* K0, const float* K1,
                const float* R_in, const float* t_in, float max_corr_dist, int max_iter, float rel_fitness, float rel_rmse,
                float* R, float* t, int* n_inl, cudaStream_t st) {
-  if (P < 1 || P > s->max_pairs || max_iter < 1) return MFR_ERR_ARG;
+  if (P < 1 || P > s->max_pairs || max_iter < 1 || H < 1 || W < 1) return MFR_ERR_ARG;
+  const int chunks = static_cast<int>((static_cast<long long>(H) * W + kIcpChunk - 1) / kIcpChunk);
   if (!s->icp_state) {
-    if (cudaMalloc(&s->icp_state, sizeof(double) * (kIcpState + 17 + 12) * s->max_pairs) != cudaSuccess) return MFR_ERR_CUDA;
+    if (cudaMalloc(&s->icp_state, sizeof(double) * (kIcpState + 12) * s->max_pairs) != cudaSuccess) return MFR_ERR_CUDA;
+  }
+  if (chunks > s->icp_chunks) {     // first call at a larger frame (not inside a graph capture: warm up at that size first)
+    cudaFree(s->icp_partial);
+    s->icp_partial = nullptr;
+    s->icp_chunks = 0;
+    if (cudaMalloc(&s->icp_partial, sizeof(double) * 17 * chunks * s->max_pairs) != cudaSuccess) return MFR_ERR_CUDA;
+    s->icp_chunks = chunks;
   }
   double* state = s->icp_state;
-  double* acc = state + static_cast<size_t>(kIcpState) * s->max_pairs;
-  double* Rd = acc + static_cast<size_t>(17) * s->max_pairs;      // initial pose in double: R [P][9] then t [P][3]
+  double* Rd = state + static_cast<size_t>(kIcpState) * s->max_pairs;      // initial pose in double: R [P][9] then t [P][3]
   double* td = Rd + static_cast<size_t>(9) * s->max_pairs;
-  MFR_CUDA_CHECK(cudaMemsetAsync(state, 0, sizeof(double) * (kIcpState + 17) * s->max_pairs, st));
+  MFR_CUDA_CHECK(cudaMemsetAsync(state, 0, sizeof(double) * kIcpState * s->max_pairs, st));
   f32_to_f64_kernel<<<(9 * P + 255) / 256, 256, 0, st>>>(R_in, Rd, 9 * P);
   f32_to_f64_kernel<<<(3 * P + 255) / 256, 256, 0, st>>>(t_in, td, 3 * P);
   icp_count_kernel<<<dim3(64, P), 256, 0, st>>>(depth0, depth1, H * W, Rd, td, state);
-  const int blocks = std::max(1, std::min((H * W + 255) / 256, 4 * sm_count() / P + 1));
   for (int it = 0; it <= max_iter; ++it) {
     // association under the current transform; the update kernel evaluates it (fitness, rmse), tests convergence against the
     // previous association and applies the Kabsch step. The last pass (it == max_iter) only evaluates.
-    icp_assoc_kernel<<<dim3(blocks, P), 256, 0, st>>>(depth0, depth1, H, W, K0, K1, max_corr_dist, state, acc);
-    icp_update_kernel<<<(P + 63) / 64, 64, 0, st>>>(state, acc, P, it, it == max_iter ? 1e300 : rel_fitness, it == max_iter ? 1e300 : rel_rmse);
+    icp_assoc_kernel<<<dim3(chunks, P), 256, 0, st>>>(depth0, depth1, H, W, K0, K1, max_corr_dist, state, s->icp_partial);
+    icp_update_kernel<<<(P + 1) / 2, 64, 0, st>>>(state, s->icp_partial, chunks, P, it, it == max_iter ? 1e300 : rel_fitness,
+                                                 it == max_iter ? 1e300 : rel_rmse);
   }
   icp_finish_kernel<<<(P + 63) / 64, 64, 0, st>>>(state, P, R, t, n_inl);
   MFR_CUDA_CHECK(cudaGetLastError());

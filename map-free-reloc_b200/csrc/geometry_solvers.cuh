@@ -143,6 +143,67 @@ MFR_HD void decompose_essential(const double* E, double* R1, double* R2, double*
   for (int k = 0; k < 3; ++k) t[k] = u2[k];
 }
 
+// Least-squares rigid transform (Kabsch): R, t minimising sum |R p + t - q|^2 from the moment sums n, sum p, sum q,
+// sum p q^T (row-major). H = sum (p - pb)(q - qb)^T = U S V^T by one-sided Jacobi on H's columns (accurate relative to
+// the smaller singular values, unlike an eigen-decomposition of H^T H, which squares H's condition: near-collinear point
+// sets lose the rotation about their line there); U, V right-handed, so R = V U^T is a rotation (for a reflection
+// optimum, the rotation that flips the weakest direction, as SVD-based Kabsch does with its sign correction). false:
+// n < 3, or H of rank < 2 (coincident or collinear points) above the rounding noise of the sums, 1e-13 of their scale.
+MFR_HD bool kabsch_from_sums(double n, const double* sp, const double* sq, const double* spq, double* R, double* t) {
+  if (n < 3.0) return false;
+  double pb[3], qb[3], B[9], V[9];
+  for (int k = 0; k < 3; ++k) { pb[k] = sp[k] / n; qb[k] = sq[k] / n; }
+  for (int a = 0; a < 3; ++a)
+    for (int b = 0; b < 3; ++b) B[3 * a + b] = spq[3 * a + b] - n * pb[a] * qb[b];
+  const double noise = 1e-13 * (n * norm3(pb) * norm3(qb) + sqrt(dot3(spq, spq) + dot3(spq + 3, spq + 3) +
+                                                                   dot3(spq + 6, spq + 6)));
+  for (int i = 0; i < 9; ++i) V[i] = (i % 4 == 0) ? 1.0 : 0.0;
+  // B <- H V with orthogonal columns (fixed sweep count)
+  for (int sweep = 0; sweep < 8; ++sweep)
+    for (int p = 0; p < 2; ++p)
+      for (int q = p + 1; q < 3; ++q) {
+        double al = 0.0, be = 0.0, ga = 0.0;
+        for (int k = 0; k < 3; ++k) {
+          al += B[3 * k + p] * B[3 * k + p]; be += B[3 * k + q] * B[3 * k + q]; ga += B[3 * k + p] * B[3 * k + q];
+        }
+        if (fabs(ga) < 1e-300) continue;
+        const double ze = (be - al) / (2.0 * ga);
+        const double tt = (ze >= 0 ? 1.0 : -1.0) / (fabs(ze) + sqrt(ze * ze + 1.0));
+        const double c = 1.0 / sqrt(tt * tt + 1.0), s = tt * c;
+        for (int k = 0; k < 3; ++k) {
+          const double bp = B[3 * k + p], bq = B[3 * k + q];
+          B[3 * k + p] = c * bp - s * bq; B[3 * k + q] = s * bp + c * bq;
+          const double vp = V[3 * k + p], vq = V[3 * k + q];
+          V[3 * k + p] = c * vp - s * vq; V[3 * k + q] = s * vp + c * vq;
+        }
+      }
+  double w[3];
+  for (int j = 0; j < 3; ++j) w[j] = B[j] * B[j] + B[3 + j] * B[3 + j] + B[6 + j] * B[6 + j];   // singular values^2
+  int o[3] = {0, 1, 2};
+  for (int a = 0; a < 2; ++a)
+    for (int b = a + 1; b < 3; ++b)
+      if (w[o[b]] > w[o[a]]) { const int tmp = o[a]; o[a] = o[b]; o[b] = tmp; }
+  double v0[3], v1[3], v2[3], u0[3], u1[3], u2[3];
+  for (int k = 0; k < 3; ++k) { v0[k] = V[3 * k + o[0]]; v1[k] = V[3 * k + o[1]]; u0[k] = B[3 * k + o[0]]; u1[k] = B[3 * k + o[1]]; }
+  cross3(v0, v1, v2);
+  const double n0 = norm3(u0);
+  if (!(n0 > noise) || !(n0 > 1e-300)) return false;                   // coincident points
+  for (int k = 0; k < 3; ++k) u0[k] /= n0;
+  const double d01 = dot3(u0, u1);
+  for (int k = 0; k < 3; ++k) u1[k] -= d01 * u0[k];
+  const double n1 = norm3(u1);
+  if (!(n1 > 1e-12 * n0 + noise)) return false;                        // collinear points
+  for (int k = 0; k < 3; ++k) u1[k] /= n1;
+  cross3(u0, u1, u2);
+  // H = U S V^T  with U's columns u_i, V's columns v_i (both right-handed)  =>  R = V U^T
+  for (int a = 0; a < 3; ++a)
+    for (int b = 0; b < 3; ++b) R[3 * a + b] = v0[a] * u0[b] + v1[a] * u1[b] + v2[a] * u2[b];
+  double Rp[3];
+  mat3_vec(R, pb, Rp);
+  for (int k = 0; k < 3; ++k) t[k] = qb[k] - Rp[k];
+  return true;
+}
+
 // ------------------------------------------------------------------------------------------------
 // real roots of a polynomial  c[0] + c[1] x + ... + c[deg] x^deg,  deg <= 10
 // Roots of p are bracketed by the roots of p' (recursively down to a quadratic) plus a Cauchy

@@ -147,6 +147,7 @@ SIGNATURES = {
                                       c_float, ctypes.c_ulonglong, c_vp, c_vp, c_vp, c_vp]),
     "mfr_host_five_point": (c_int, [c_vp, c_vp, c_vp]),
     "mfr_host_p3p": (c_int, [c_vp, c_vp, c_vp, c_vp]),
+    "mfr_host_kabsch": (c_int, [ctypes.c_double, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "mfr_host_poly_real_roots": (c_int, [c_vp, c_int, c_vp]),
     "mfr_host_decompose_essential": (c_int, [c_vp, c_vp, c_vp, c_vp]),
     "mfr_host_ransac_satisfied": (c_int, [ctypes.c_double, c_int, c_int, c_int, c_int, c_int]),

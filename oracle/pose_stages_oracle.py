@@ -655,3 +655,163 @@ def pnp_final(res, Xw, uv, K1, thr):
     if out["failed"]:
         out["mask"] = np.zeros(len(Xw), bool)
     return out
+
+
+# ------------------------------------------------------------------------------------------------ Procrustes
+def procrustes_state(seed, pair, h):
+    return (seed ^ (0xC2B2AE3D27D4EB4F * (pair + 1)) ^ (0x9E3779B97F4A7C15 * (h + 1))) & M64
+
+
+def kabsch_sums(p, q):
+    """Moment sums (n, sum p [3], sum q [3], sum p q^T [9]) of p, q [n, 3]."""
+    return float(len(p)), p.sum(0), q.sum(0), (p[:, :, None] * q[:, None, :]).sum(0).ravel()
+
+
+def kabsch(n, sp, sq, spq):
+    """kabsch_from_sums through its host hook mfr_host_kabsch: (R [3, 3], t [3]) or None."""
+    R, t = np.zeros(9), np.zeros(3)
+    c = lambda a: np.ascontiguousarray(a, np.float64)
+    sp, sq, spq = c(sp), c(sq), c(spq)
+    if not _lib().mfr_host_kabsch(float(n), _p(sp), _p(sq), _p(spq), _p(R), _p(t)):
+        return None
+    return R.reshape(3, 3), t
+
+
+def procrustes_prepare(kpts0, kpts1, depth0, depth1, K0, K1, dmin0, dmin1):
+    """procrustes_prepare_kernel for one pair: both keypoints truncated toward zero and inside both images, valid iff
+    depth > dmin on both sides, in order. Returns (vidx, X0 [n, 3], X1 [n, 3]) float64 camera points."""
+    H, W = depth0.shape
+    i0, i1 = np.asarray(kpts0, np.float32).astype(np.int32), np.asarray(kpts1, np.float32).astype(np.int32)
+    inside = ((i0[:, 0] >= 0) & (i0[:, 0] < W) & (i0[:, 1] >= 0) & (i0[:, 1] < H) &
+              (i1[:, 0] >= 0) & (i1[:, 0] < W) & (i1[:, 1] >= 0) & (i1[:, 1] < H))
+    z0 = np.zeros(len(i0), np.float32); z1 = np.zeros(len(i0), np.float32)
+    z0[inside] = depth0[i0[inside, 1], i0[inside, 0]]; z1[inside] = depth1[i1[inside, 1], i1[inside, 0]]
+    vidx = np.nonzero(inside & (z0 > dmin0) & (z1 > dmin1))[0]
+    return (vidx, backproject(inverse_K_f32(K0), i0[vidx], z0[vidx]), backproject(inverse_K_f32(K1), i1[vidx], z1[vidx]))
+
+
+def procrustes_count_bound(R, t, X0, X1, max_dist):
+    """(lo, hi) [N] bool: the points procrustes_hyp_kernel's float32 test (R, t, X0, X1 rounded to float32, three fmaf
+    per component, a subtraction, d2 = fmaf(dx, dx, fmaf(dy, dy, dz * dz)) < float32 max_dist^2) must count (lo) and may
+    count (hi). Each component's error is at most 4 u of the sum of the magnitudes it is made of, d2's at most 3 u of
+    d2 on top of the propagated component errors."""
+    R32 = np.asarray(R, np.float32).astype(np.float64).reshape(3, 3)
+    t32 = np.asarray(t, np.float32).astype(np.float64)
+    P = np.asarray(X0, np.float32).astype(np.float64)
+    Q = np.asarray(X1, np.float32).astype(np.float64)
+    d = P @ R32.T + t32 - Q
+    dd = 4 * U32 * (np.abs(P) @ np.abs(R32).T + np.abs(t32) + np.abs(Q))
+    e = (d * d).sum(1)
+    de = (2 * np.abs(d) * dd + dd * dd).sum(1) + 3 * U32 * (e + (2 * np.abs(d) * dd + dd * dd).sum(1))
+    thr2 = float(np.float32(np.float32(max_dist) * np.float32(max_dist)))
+    return e + de < thr2, ~(e - de >= thr2)
+
+
+def procrustes_hypotheses(X0, X1, num_hyp, seed, pair):
+    """Every Procrustes hypothesis of one pair in the kernel's order: list over blocks of lists of (warp, lane, R, t)
+    for the 3-point samples whose Kabsch model exists."""
+    N = len(X0)
+    out = []
+    for b in range(-(-num_hyp // HYP_PER_BLOCK)):
+        cands = []
+        for th in range(HYP_PER_BLOCK):
+            h = b * HYP_PER_BLOCK + th
+            if h >= num_hyp:
+                break
+            idx = sample_distinct(procrustes_state(seed, pair, h), N, 3)
+            m = kabsch(*kabsch_sums(X0[idx], X1[idx]))
+            if m is not None:
+                cands.append((th >> 5, th & 31) + m)
+        out.append(cands)
+    return out
+
+
+def procrustes_final(res, X0, X1, max_dist):
+    """procrustes_final_kernel for one pair from its block records: the first valid block with the lowest cost, then
+    two refits on the inliers (d^2 < max_dist^2 in float64) and a final count. Returns dict(failed, R, t, n, near) where
+    ``near`` counts points within 1e-12 (relative) of the threshold in any round."""
+    thr2 = float(np.float32(max_dist)) ** 2
+    b = pnp_winner(res) if len(X0) >= 3 else None
+    if b is None:
+        return {"failed": True, "n": 0, "near": 0}
+    R = np.asarray(res[b]["model"][:9], np.float64).reshape(3, 3)
+    t = np.asarray(res[b]["model"][9:], np.float64)
+    near = 0
+    for rnd in range(3):
+        d2 = ((X0 @ R.T + t - X1) ** 2).sum(1)
+        inl = d2 < thr2
+        near += int((np.abs(d2 - thr2) <= 1e-12 * thr2).sum())
+        if rnd < 2:
+            m = kabsch(*kabsch_sums(X0[inl], X1[inl]))
+            if m is not None:
+                R, t = m
+    n = int(inl.sum())
+    return {"failed": n < 3, "R": R, "t": t, "n": n, "near": near, "record": b}
+
+
+# ------------------------------------------------------------------------------------------------ ICP
+def icp_clouds(depth0, depth1, K0, K1):
+    """The clouds icp_assoc_kernel lifts: every pixel with depth > 0, through the float32 inverse of K, row-major.
+    Returns (X0 [n0, 3], X1 [n1, 3]) float64."""
+    H, W = depth0.shape
+    vv, uu = np.mgrid[0:H, 0:W]
+    uv = np.stack([uu.ravel(), vv.ravel()], 1)
+    m0, m1 = depth0.ravel() > 0, depth1.ravel() > 0
+    return (backproject(inverse_K_f32(K0), uv[m0], depth0.ravel()[m0]),
+            backproject(inverse_K_f32(K1), uv[m1], depth1.ravel()[m1]))
+
+
+def icp_assoc(X0, X1, R, t, max_dist, tree=None):
+    """One association pass of icp_assoc_kernel, exact: the nearest target point within D (float64 of the float32
+    max_dist) of every transformed source point by cKDTree. Source points at z <= D + 1 mm in camera 1 are not
+    associated, as in the kernel. Returns dict(n, sums [16] = (sum p, sum q, sum p q^T), sse, rmse, near, P, Q, ok)
+    with ``near`` the count of points whose distance lies within 1e-9 (relative) of D."""
+    from scipy.spatial import cKDTree
+    D = float(np.float32(max_dist))
+    tree = cKDTree(X1) if tree is None else tree
+    P = X0 @ np.asarray(R, np.float64).reshape(3, 3).T + np.asarray(t, np.float64)
+    front = P[:, 2] > D + 1e-3
+    d, j = tree.query(P, k=1, distance_upper_bound=D * (1 + 1e-9))
+    fin = np.isfinite(d)
+    near = int((fin & front & (np.abs(d - D) <= 1e-9 * D)).sum())
+    ok = fin & front & (d < D)
+    Pm, Qm = P[ok], X1[j[ok]]
+    n = int(ok.sum())
+    sse = float((((Pm - Qm) ** 2).sum(1)).sum())
+    _, sp, sq, spq = kabsch_sums(Pm, Qm)
+    return {"n": n, "sums": np.concatenate([sp, sq, spq]), "sse": sse, "rmse": np.sqrt(sse / n) if n else 0.0,
+            "near": near, "ok": ok}
+
+
+def icp_update(state_prev, a, n_src, it, rel_fit, rel_rmse):
+    """icp_update_kernel for one pair: state_prev = (R [3, 3], t [3], fitness, rmse) of the previous pass, a = icp_assoc
+    at R, t. Returns (R, t, fitness, rmse, stop): stop when it > 0 and both changes are below the criteria, when n < 3,
+    or when Kabsch fails; otherwise the Kabsch update composed onto the pose."""
+    R, t, fit0, rmse0 = state_prev
+    n = a["n"]
+    fit = n / n_src if n_src > 0 else 0.0
+    rmse = a["rmse"]
+    if (it > 0 and abs(fit0 - fit) < rel_fit and abs(rmse0 - rmse) < rel_rmse) or n < 3:
+        return R, t, fit, rmse, True
+    m = kabsch(n, a["sums"][:3], a["sums"][3:6], a["sums"][6:])
+    if m is None:
+        return R, t, fit, rmse, True
+    Ru, tu = m
+    return Ru @ R, Ru @ t + tu, fit, rmse, False
+
+
+def icp_loop(X0, X1, R, t, max_dist, max_iter=30, rel_fit=1e-4, rel_rmse=1e-4):
+    """mfr_icp_refine restated: passes it = 0 .. max_iter of association + update (the last pass only evaluates).
+    Returns (R, t, fitness, rmse, stop pass, converged flag)."""
+    from scipy.spatial import cKDTree
+    tree = cKDTree(X1)
+    R, t = np.asarray(R, np.float64).reshape(3, 3), np.asarray(t, np.float64)
+    fit, rmse = 0.0, 0.0
+    for it in range(max_iter + 1):
+        last = it == max_iter
+        a = icp_assoc(X0, X1, R, t, max_dist, tree)
+        R, t, fit, rmse, stop = icp_update((R, t, fit, rmse), a, len(X0), it, 1e300 if last else rel_fit,
+                                           1e300 if last else rel_rmse)
+        if stop:
+            return R, t, fit, rmse, it, True
+    return R, t, fit, rmse, max_iter, False

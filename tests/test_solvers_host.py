@@ -111,3 +111,70 @@ def test_decompose_essential():
         assert min(np.abs(R1.reshape(3, 3) - R).max(), np.abs(R2.reshape(3, 3) - R).max()) < 1e-9
         assert min(np.abs(tt - tn).max(), np.abs(tt + tn).max()) < 1e-9
         assert abs(np.linalg.det(R1.reshape(3, 3)) - 1) < 1e-9 and abs(np.linalg.det(R2.reshape(3, 3)) - 1) < 1e-9
+
+
+def _kabsch(p, q):
+    """mfr_host_kabsch on the moment sums of p, q [n, 3]: (ok, R, t)."""
+    sp, sq = np.ascontiguousarray(p.sum(0)), np.ascontiguousarray(q.sum(0))
+    spq = np.ascontiguousarray((p[:, :, None] * q[:, None, :]).sum(0).ravel())
+    R, t = np.zeros(9), np.zeros(3)
+    ok = L.mfr_host_kabsch(float(len(p)), P(sp), P(sq), P(spq), P(R), P(t))
+    return ok, R.reshape(3, 3), t
+
+
+def _kabsch_bar(p, q):
+    """Error bound of a rotation from the moment sums: the sums carry a rounding error of a few ulps of their scale
+    (n |pb| |qb| for a cloud far from the origin), which moves the singular vectors by that over the gap between the
+    second and third singular values of the centred H."""
+    pb, qb = p.mean(0), q.mean(0)
+    spq = (p[:, :, None] * q[:, None, :]).sum(0)
+    scale = len(p) * np.linalg.norm(pb) * np.linalg.norm(qb) + np.linalg.norm(spq)
+    s = np.linalg.svd((p - pb).T @ (q - qb), compute_uv=False)
+    return 16 * np.finfo(float).eps * scale / (s[1] - s[2])
+
+
+def test_kabsch_matches_svd_where_htH_is_weakest():
+    """kabsch_from_sums (the Procrustes hypotheses and refit, every ICP update) against SVD-based Kabsch
+    (pose_solver_oracle.kabsch) on the inputs that break an eigen-decomposition of H^T H: exactly three points,
+    near-collinear samples, a cloud 80 m away with a 5 cm spread, a reflection optimum."""
+    from oracle import pose_solver_oracle as po
+    rng = np.random.default_rng(4)
+    cases = []
+    for off, spread, n in [(0.0, 1.0, 3), (3.0, 0.5, 3), (80.0, 0.05, 3), (80.0, 0.05, 10), (80.0, 0.05, 1000),
+                           (0.0, 1.0, 1000)]:
+        cases += [(f"cloud {off} m / {spread} m / n {n}", rng.normal(0, spread, (n, 3)) + [0.0, 0.0, off])]
+    for off in (0.0, 3.0, 80.0):
+        for eps in (1e-3, 1e-4):
+            d = rng.normal(0, 1, 3)
+            cases += [(f"near-collinear {off} m / {eps}", np.outer(rng.normal(0, 1, 6), d) + [0.0, 0.0, off] +
+                       rng.normal(0, eps, (6, 3)))]
+    for name, p in cases:
+        R0, t0 = synth.random_pose(rng)
+        q = p @ R0.T + t0
+        ok, R, t = _kabsch(p, q)
+        Ro, to = po.kabsch(p, q)
+        bar = _kabsch_bar(p, q)
+        assert ok == 1, name
+        assert np.abs(R @ R.T - np.eye(3)).max() < 1e-14 and np.linalg.det(R) > 0, name
+        assert np.abs(R - Ro).max() <= bar, (name, np.abs(R - Ro).max(), bar)
+        assert np.abs(t - to).max() <= bar * (1 + np.abs(p).max()) + 1e-14 * np.abs(to).max(), name
+    # the least-squares optimum over O(3) is a reflection: both return the rotation that flips the weakest direction
+    p = rng.normal(0, 1, (8, 3)) * [3.0, 2.0, 0.5]
+    q = p * [1.0, 1.0, -1.0] + rng.normal(0, 0.01, (8, 3))
+    ok, R, t = _kabsch(p, q)
+    Ro, to = po.kabsch(p, q)
+    assert ok == 1 and abs(np.linalg.det(R) - 1) < 1e-14 and np.abs(R - Ro).max() <= _kabsch_bar(p, q)
+
+
+def test_kabsch_rejects_degenerate_sums():
+    """Coincident points (at any distance from the origin, where the centred sums are rounding noise of a large
+    scale), exactly collinear points and fewer than three points give false."""
+    rng = np.random.default_rng(5)
+    for off in (0.0, 0.5, 3.0, 80.0, 1000.0):
+        R0, t0 = synth.random_pose(rng)
+        p = np.tile(rng.normal(0, 1, 3) + [0.0, 0.0, off], (5, 1))
+        assert _kabsch(p, p @ R0.T + t0)[0] == 0, ("coincident", off)
+        p = np.outer(rng.normal(0, 1, 7), rng.normal(0, 1, 3)) + [0.0, 0.0, off]
+        assert _kabsch(p, p @ R0.T + t0)[0] == 0, ("collinear", off)
+    p = rng.normal(0, 1, (2, 3))
+    assert _kabsch(p, p)[0] == 0
